@@ -1019,6 +1019,54 @@ __device__ __noinline__ void f_matvec_cols(int W, int ld, int rows, int cols, in
 
 #endif
 
+// End of a Newton iteration, column c: dx~ = -r~x - (W^T dv)_c, x~ += alpha dx~, r~x = x~ + (W^T v)_c + p~
+// (each with the rounding of the separate passes it replaces).
+__device__ __forceinline__ void f_cols2_out(int c, double wdv, double wv, int xt, int rxt, int pt, double alpha) {
+    QPB_SMEM;
+    const double dx = -qsm[rxt + c] - wdv;
+    const double x = fma(alpha, dx, qsm[xt + c]);
+    qsm[xt + c] = x;
+    qsm[rxt + c] = (x + wv) + qsm[pt + c];
+}
+// W^T dv and W^T v side by side (each W element read once) with the row split and summation order of the default
+// f_matvec_cols; partial sums in p0/p1 (dv) and p2/p3 (v). Ends with a block barrier.
+__device__ __noinline__ void f_matvec_cols2(int W, int ld, int rows, int cols, int dv, int v, int p0, int p1, int p2,
+                                            int p3, int xt, int rxt, int pt, double alpha) {
+    QPB_SMEM;
+    const int tid = threadIdx.x;
+    const int half = kNT / 2;
+    const int gidx = tid / half, c = tid - gidx * half;
+    const int chunk = (rows + 1) >> 1;
+    for (int c0 = 0; c0 < cols; c0 += half) {
+        const int cc = c0 + c;
+        if (cc < cols) {
+            const int r0 = gidx * chunk, r1 = min(rows, r0 + chunk);
+            const double* Wp = qsm + W + cc;
+            double s0 = 0.0, s1 = 0.0, s2 = 0.0, s3 = 0.0, u0 = 0.0, u1 = 0.0, u2 = 0.0, u3 = 0.0;
+            int r = r0;
+#pragma unroll 1
+            for (; r + 3 < r1; r += 4) {
+                const double w0 = Wp[(r + 0) * ld], w1 = Wp[(r + 1) * ld], w2 = Wp[(r + 2) * ld], w3 = Wp[(r + 3) * ld];
+                s0 = fma(w0, qsm[dv + r + 0], s0); u0 = fma(w0, qsm[v + r + 0], u0);
+                s1 = fma(w1, qsm[dv + r + 1], s1); u1 = fma(w1, qsm[v + r + 1], u1);
+                s2 = fma(w2, qsm[dv + r + 2], s2); u2 = fma(w2, qsm[v + r + 2], u2);
+                s3 = fma(w3, qsm[dv + r + 3], s3); u3 = fma(w3, qsm[v + r + 3], u3);
+            }
+#pragma unroll 1
+            for (; r < r1; ++r) {
+                const double w0 = Wp[r * ld];
+                s0 = fma(w0, qsm[dv + r], s0); u0 = fma(w0, qsm[v + r], u0);
+            }
+            qsm[(gidx ? p1 : p0) + cc] = (s0 + s1) + (s2 + s3);
+            qsm[(gidx ? p3 : p2) + cc] = (u0 + u1) + (u2 + u3);
+        }
+    }
+    __syncthreads();
+    for (int cc = tid; cc < cols; cc += kNT)
+        f_cols2_out(cc, qsm[p0 + cc] + qsm[p1 + cc], qsm[p2 + cc] + qsm[p3 + cc], xt, rxt, pt, alpha);
+    __syncthreads();
+}
+
 // || L x ||^2 partial sums (packed lower L in shared memory): 4 lanes per row, rows paired (r, n-1-r) so that every
 // lane group streams n + 1 entries. Returns this thread's partial (lane l == 0 of a group); sum over the block after.
 __device__ __noinline__ double f_tri_norm2(int Lp, int n, int x) {
@@ -1058,13 +1106,15 @@ __device__ __noinline__ double f_tri_norm2(int Lp, int n, int x) {
 __device__ __forceinline__ double2 ldg2(const double* p) { return __ldg(reinterpret_cast<const double2*>(p)); }
 
 // y1 = W x1 (, y2 = W x2). 8 lanes per row (lane j: 16-byte column pairs 2j + 16k), kNT/8 rows per pass, two passes
-// (14 loads) in flight per thread.
+// (14 loads) in flight per thread. Row groups are numbered from the LAST warp, so a partial last pass (rows 96-99 at
+// C2 with 192 threads) falls to the highest warps: warp 0 already carries the partial pass of g_tri_norm2, which
+// shares this phase in the forward kernel.
 template <bool kTwo>
 __device__ __forceinline__ void g_matvec_rows_impl(const double* __restrict__ Wg, int ld, int rows, int cols, int x1,
                                                    int x2, int y1, int y2) {
     QPB_SMEM;
-    const int tid = threadIdx.x, j = tid & 7, rg = tid >> 3;
     constexpr int kRG = kNT / 8;                             // row groups per pass (8 lanes per row)
+    const int tid = threadIdx.x, j = tid & 7, rg = kRG - 1 - (tid >> 3);
 #pragma unroll 1
     for (int rb = 0; rb < rows; rb += 2 * kRG) {             // warp-uniform trip count
         const int r0 = rb + rg, r1 = r0 + kRG;
@@ -1168,6 +1218,51 @@ __device__ __noinline__ void g_matvec_cols(const double* __restrict__ Wg, int ld
                 if (b >= 0) r1 += qsm[b + c + 1];
                 qsm[out + c + 1] = r1;
             }
+        }
+    }
+    __syncthreads();
+}
+
+// W^T dv and W^T v side by side, each W element loaded once, with the lane/row pairing and shuffle tree of
+// g_matvec_cols; the owning lane finishes its columns with f_cols2_out. Ends with a block barrier.
+__device__ __noinline__ void g_matvec_cols2(const double* __restrict__ Wg, int ld, int rows, int cols, int dv, int v,
+                                            int xt, int rxt, int pt, double alpha) {
+    QPB_SMEM;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, g = lane >> 3, cq = lane & 7;
+#pragma unroll 1
+    for (int c0 = 0; c0 < cols; c0 += 16 * (kNT / 32)) {     // warp-uniform trip count
+        const int c = c0 + 16 * warp + 2 * cq;
+        const bool okc = c < cols;
+        const double* pc = Wg + (okc ? c : 0);
+        double s0 = 0.0, s1 = 0.0, u0 = 0.0, u1 = 0.0;       // W^T dv, W^T v
+#pragma unroll 1
+        for (int rb = g; rb < rows; rb += 4 * 13) {
+            double2 w[13];
+#pragma unroll
+            for (int k = 0; k < 13; ++k) {
+                const int r = rb + 4 * k;
+                w[k] = (r < rows) ? ldg2(pc + (size_t)r * ld) : make_double2(0.0, 0.0);
+            }
+#pragma unroll
+            for (int k = 0; k < 13; ++k) {
+                const int r = rb + 4 * k;
+                if (r < rows) {
+                    const double dr = qsm[dv + r], vr = qsm[v + r];
+                    s0 = fma(w[k].x, dr, s0);
+                    s1 = fma(w[k].y, dr, s1);
+                    u0 = fma(w[k].x, vr, u0);
+                    u1 = fma(w[k].y, vr, u1);
+                }
+            }
+        }
+        __syncwarp();
+        s0 += __shfl_xor_sync(0xffffffffu, s0, 8);  s1 += __shfl_xor_sync(0xffffffffu, s1, 8);
+        u0 += __shfl_xor_sync(0xffffffffu, u0, 8);  u1 += __shfl_xor_sync(0xffffffffu, u1, 8);
+        s0 += __shfl_xor_sync(0xffffffffu, s0, 16); s1 += __shfl_xor_sync(0xffffffffu, s1, 16);
+        u0 += __shfl_xor_sync(0xffffffffu, u0, 16); u1 += __shfl_xor_sync(0xffffffffu, u1, 16);
+        if (g == 0 && okc) {
+            f_cols2_out(c, s0, u0, xt, rxt, pt, alpha);
+            if (c + 1 < cols) f_cols2_out(c + 1, s1, u1, xt, rxt, pt, alpha);
         }
     }
     __syncthreads();

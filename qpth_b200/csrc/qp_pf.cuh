@@ -394,19 +394,16 @@ __device__ __forceinline__ void pf_chol_setup(int S, int nts, int kb0, int kend,
 // ---- substitutions (order n = 8 nts <= kNT: thread tid owns entry tid) ----------------------------------------------
 // Running right-hand side over block columns [kb, ke):  b_i -= P_ik b_k  for every row below block k. In place.
 // Ends with a block barrier; afterwards b holds the running right-hand side of ALL rows.
-// Only the warps that own rows (tid < n) run the sweep, on a named barrier of their own (id 3); the others go straight
-// to the closing block barrier.
+// Every block step ends with a block barrier. Measured slower on H100 at C2: synchronising only the row-owning warps on
+// a named barrier, and one warp running the whole sweep (four rows per lane, __syncwarp between steps) at about 1.8x
+// the cycles per sweep in the latency-mode kernel; prefetching that warp's next P rows into registers spilled in the
+// three-per-SM build and was slower still.
 __device__ __noinline__ void pf_fwd(int S, int n, int kb, int ke, int b) {
     QPB_SMEM;
     const int tid = threadIdx.x;
     const double* M = qsm + S;
     const bool mine = tid < n;
-#ifndef QPB_PF_SWEEPBAR
-#define QPB_PF_SWEEPBAR 0  // A/B knob: 1 = the sweeps synchronise the row-owning warps only (named barrier 3): measured slightly
-                           // SLOWER than the whole-block barrier; 0 = the whole block
-#endif
-    const int nwp = QPB_PF_SWEEPBAR ? ((n + 31) >> 5) : (kNT / 32);   // participating warps
-    if ((tid >> 5) < nwp) {
+    {
         const int ro = pf_rowoff(mine ? tid : 0);
         double acc = mine ? qsm[b + tid] : 0.0;
         double row[8];
@@ -426,7 +423,7 @@ __device__ __noinline__ void pf_fwd(int S, int n, int kb, int ke, int b) {
                 if (tid < k0 + 16) qsm[b + tid] = acc;           // block k+1 becomes final
                 else if (k + 1 < ke) f_ld8(M + ro + k0 + 8, row);  // next step's P row (static data: no hazard)
             }
-            named_bar_sync(3, 32 * nwp);
+            __syncthreads();
         }
         if (mine && tid >= 8 * ke + 8 && kb < ke) qsm[b + tid] = acc;   // rows not yet published (partial sweeps only)
     }
@@ -475,8 +472,7 @@ __device__ __noinline__ void pf_bwd(int S, int n, int c, int w) {
     const int tid = threadIdx.x;
     const double* M = qsm + S;
     const int nts = n >> 3;
-    const int nwp = QPB_PF_SWEEPBAR ? ((n + 31) >> 5) : (kNT / 32);   // participating warps (see pf_fwd)
-    if ((tid >> 5) < nwp) {
+    {
         double acc = (tid < n) ? qsm[c + tid] : 0.0;
         if (tid >= n - 8 && tid < n) qsm[w + tid] = acc;
         double col[8];
@@ -488,7 +484,7 @@ __device__ __noinline__ void pf_bwd(int S, int n, int c, int w) {
                 for (int r = 0; r < 8; ++r) col[r] = Pc[r * ldi];
             }
         }
-        named_bar_sync(3, 32 * nwp);
+        __syncthreads();
 #pragma unroll 1
         for (int i = nts - 1; i > 0; --i) {
             const int i0 = 8 * i;
@@ -509,7 +505,7 @@ __device__ __noinline__ void pf_bwd(int S, int n, int c, int w) {
                     for (int r = 0; r < 8; ++r) col[r] = Pc[r * ldm];
                 }
             }
-            named_bar_sync(3, 32 * nwp);
+            __syncthreads();
         }
     }
     __syncthreads();

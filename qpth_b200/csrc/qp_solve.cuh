@@ -178,6 +178,15 @@ __device__ __forceinline__ void mv_rows2(const KDims& D, const FCtx& C, int x1, 
     if (kCoop) g_matvec_rows2(C.Wg, D.ldw, D.ms, D.n, x1, x2, y1, y2);
     else f_matvec_rows2(C.L.W, D.ldw, D.ms, D.n, x1, x2, y1, y2);
 }
+// One pass over W for the end of a Newton iteration (v, s already updated; ends with a block barrier):
+//   dx~ = -r~x - W^T dv,   x~ += alpha dx~,   r~x = x~ + W^T v + p~   (the next iteration's residual).
+// p0 .. p3: partial-sum scratch of the shared-memory pass.
+template <bool kCoop>
+__device__ __forceinline__ void mv_cols2(const KDims& D, const FCtx& C, int dv, int v, int p0, int p1, int p2, int p3,
+                                         int xt, int rxt, int pt, double alpha) {
+    if (kCoop) g_matvec_cols2(C.Wg, D.ldw, D.ms, D.n, dv, v, xt, rxt, pt, alpha);
+    else f_matvec_cols2(C.L.W, D.ldw, D.ms, D.n, dv, v, p0, p1, p2, p3, xt, rxt, pt, alpha);
+}
 template <bool kCoop>
 __device__ __forceinline__ void mv_cols(const KDims& D, const FCtx& C, int v, int p0, int p1, int out, int a, double sa,
                                         int b, double sgn) {
@@ -333,12 +342,15 @@ k_forward_fast(KDims D, const double* __restrict__ p, int64_t sp, const double* 
         iters_run = it + 1;
         // ---- residuals (batch.py:94-107)
         QPB_TICK(3);
-        mv_cols<kCoop>(D, C, v, t0, t1, rxt, xt, 1.0, pt, 1.0);      // r~x = x~ + p~ + W^T [y;z]
+        // r~x = x~ + p~ + W^T [y;z]: here at the initial point; later iterations get it from the previous one's mv_cols2
+        if (it == 0) mv_cols<kCoop>(D, C, v, t0, t1, rxt, xt, 1.0, pt, 1.0);
         QPB_TICK(4);
+        double acc[4] = {0.0, 0.0, 0.0, 0.0};                   // |ry|^2, |rz|^2, |L r~x|^2, s.z
         mv_rows2<kCoop>(D, C, xt, rxt, rv, hW);                      // W x~ , W r~x
+        // chol(Q) pass in the same phase as the W row pass (it needs r~x only): their load latencies overlap
+        acc[2] = kCoop ? g_tri_norm2(C.Lg, n, rxt) : f_tri_norm2(C.L.Lp, n, rxt);
         __syncthreads();
         QPB_TICK(5);
-        double acc[4] = {0.0, 0.0, 0.0, 0.0};                   // |ry|^2, |rz|^2, |L r~x|^2, s.z
         _Pragma("unroll 1") for (int i = tid; i < ms; i += kNT) {
             const double r = qsm[rv + i] - qsm[hb + i] + ((i >= ep) ? qsm[s + i] : 0.0);
             qsm[rv + i] = r;
@@ -346,8 +358,6 @@ k_forward_fast(KDims D, const double* __restrict__ p, int64_t sp, const double* 
             else { acc[1] = fma(r, r, acc[1]); acc[3] = fma(qsm[s + i], qsm[v + i], acc[3]); }
         }
         QPB_TICK(6);
-        acc[2] = kCoop ? g_tri_norm2(C.Lg, n, rxt) : f_tri_norm2(C.L.Lp, n, rxt);
-        QPB_TICK(7);
         f_reduce_sum4(acc, C.L.red + rtog); rtog ^= (QPB_RED1 ? 4 * qpb::fast::kFastStride : 0);
         QPB_TICK(8);
         const double mu = fabs(acc[3] / dm);
@@ -449,20 +459,18 @@ k_forward_fast(KDims D, const double* __restrict__ p, int64_t sp, const double* 
                 mn[1] = fmin(mn[1], step_candidate(qsm[s + i], dsi));
             }
         }
-        __syncthreads();
         QPB_TICK(14);
-        mv_cols<kCoop>(D, C, w, t0, t1, hW, rxt, -1.0, -1, -1.0);     // dx~ = -r~x - W^T dv  (in hW)
-        QPB_TICK(15);
+        // the step length does not depend on dx~: v and s move first, then one pass over W gives dx~, x~ and the next
+        // iteration's r~x (none after the last iteration: nothing reads x~ then)
         f_reduce_min2(mn, C.L.red + rtog); rtog ^= (QPB_RED1 ? 4 * qpb::fast::kFastStride : 0);
-        {
-            const double alpha = fmin(0.999 * fmin(f_step_fix(mn[0]), f_step_fix(mn[1])), 1.0);
-            _Pragma("unroll 1") for (int i = tid; i < n; i += kNT) qsm[xt + i] = fma(alpha, qsm[hW + i], qsm[xt + i]);
-            _Pragma("unroll 1") for (int i = tid; i < ms; i += kNT) {
-                qsm[v + i] = fma(alpha, qsm[w + i], qsm[v + i]);
-                if (i >= ep) qsm[s + i] = fma(alpha, qsm[ds + i], qsm[s + i]);
-            }
+        const double alpha = fmin(0.999 * fmin(f_step_fix(mn[0]), f_step_fix(mn[1])), 1.0);
+        _Pragma("unroll 1") for (int i = tid; i < ms; i += kNT) {
+            qsm[v + i] = fma(alpha, qsm[w + i], qsm[v + i]);
+            if (i >= ep) qsm[s + i] = fma(alpha, qsm[ds + i], qsm[s + i]);
         }
         __syncthreads();
+        if (it + 1 < maxIter) mv_cols2<kCoop>(D, C, w, v, t0, t1, hW, dsa, xt, rxt, pt, alpha);   // (t0, t1, hW, dsa dead)
+        QPB_TICK(15);
     }
 
     // ---- outputs: x = L^-T x~_best, y, z, s of the returned iterate (batch.py:205-207)
