@@ -2,8 +2,9 @@
 //   -DQPB_NT=192 -DQPB_ALT_CTAS=3   three QPs per SM (112 registers, <= 76.8 KB of shared memory per QP; W, chol(Q) from L2)
 //   -DQPB_NT=512 -DQPB_ALT_CTAS=1   large problems (order 136 .. 256, e.g. nz = nineq = 200): 15 update warps instead of 7
 // Same source, same arithmetic as the 256-thread build in qp_kernels.cu; only the thread count (compile-time constant
-// kNT of qp_fast.cuh) and the launch bounds differ. Exports qpb200_alt<NT>_{forward,backward,solve_kkt}: internal entry
-// points that qpb200_forward / qpb200_backward / qpb200_solve_kkt (qp_kernels.cu) dispatch to; not part of the public header.
+// kNT of qp_fast.cuh) and the launch bounds differ. Exports qpb200_alt<NT>_{forward,backward,solve_kkt} (and, at 192
+// threads, qpb200_alt192_setup: k_setup_pf of qp_setup_pf.cuh): internal entry points that qpb200_forward /
+// qpb200_backward / qpb200_solve_kkt / qpb200_pre_factor_kkt (qp_kernels.cu) dispatch to; not part of the public header.
 #include <cuda_runtime.h>
 #include <math.h>
 #include <stdint.h>
@@ -20,6 +21,7 @@
 #define QPB_NS_CAT(a, b) QPB_NS_CAT2(a, b)
 #define qpb QPB_NS_CAT(qpb_nt, QPB_NT)
 #include "qp_solve.cuh"
+#include "qp_setup_pf.cuh"
 
 extern "C" void qpb200_internal_cuda_error(int err, const char* what);   // (qp_kernels.cu) records the message, per thread
 
@@ -117,6 +119,23 @@ int QPB_ALT_NAME(_solve_kkt)(const qpb200_plan* plan, size_t smem, int nbatch, c
         D, d, rx, rs, rz, ry, nullptr, nullptr, nullptr, nullptr, Lfac, Wfac, Kfac, sF, dx, ds, dz, dy, O);
     return alt_check_launch();
 }
+
+#if QPB_NT == 192
+// pre_factor_kkt with the footprint of the three-per-SM forward / backward CTAs (throughput mode): any of an SM's three
+// slots can then hold a setup, forward or backward CTA of the pipeline
+int QPB_ALT_NAME(_setup)(const qpb200_plan* plan, size_t smem, int nsys, const double* Q, int64_t sQ, const double* G,
+                         int64_t sG, const double* A, int64_t sA, double reg, double* Lfac, double* Wfac, double* Kfac,
+                         int* spd_flag, void* stream) {
+    static size_t g_setup[16];
+    cudaStream_t st = (cudaStream_t)stream;
+    KDims D = alt_dims(plan);
+    D.reg = reg;
+    int rc = alt_set_smem(k_setup_pf<kMin>, smem, g_setup);
+    if (rc) return rc;
+    k_setup_pf<kMin><<<nsys, qpb::fast::kNT, smem, st>>>(D, Q, sQ, G, sG, A, sA, Lfac, Wfac, Kfac, spd_flag);
+    return alt_check_launch();
+}
+#endif
 
 // (the batch-mean reductions of qpb200_backward stay in qp_kernels.cu: this is only the per-QP kernel)
 int QPB_ALT_NAME(_backward)(const qpb200_plan* plan, size_t smem, int nbatch, const double* dl_dzhat, const double* zhat,

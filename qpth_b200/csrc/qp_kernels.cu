@@ -871,193 +871,9 @@ k_setup_fast(KDims D, const double* __restrict__ Q, int64_t sQ, const double* __
 #endif
 }
 
-// ---------------------------------------------------------------------------------------------
-// k_setup_pf: pre_factor_kkt (batch.py:375-429) on the product-form machinery, sized to share an SM.
-//   1. lower triangle of Q -> staircase in shared memory; pf_chol factors it IN PRODUCT FORM (T_k, P_ik) and emits the
-//      plain factor L (packed lower, true diagonal) to global memory as its tiles appear;
-//   2. W = [A; 0; G] L^-T one 8-row tile at a time (a warp stages the tile, sweeps the running right-hand side
-//      tile(i) -= tile(k) P_ik^T, finalises tile(k) T_k^T, all DMMA) straight to global memory;
-//   3. K = W W^T (DMMA, operands re-read from L2: W was written by this CTA) into the staircase that held chol(Q);
-//   4. equality block: the first neq_pad columns of K factored in product form by the same pf_chol (kend), K -> global.
-// Shared memory: staircase of order max(nz_pad, ms_pad) + panel scratch + 4 tile buffers: 88 KB at C2 (two systems per
-// SM; k_setup_fast holds Q and W side by side: 181 KB, one per SM), 220 KB at nz = nineq = 200 (where the only other
-// setup kernel works from global scratch on one CTA).
-// ---------------------------------------------------------------------------------------------
-namespace fk {
-constexpr int kSetupStage = 6;          // row tiles of [A; G] staged at a time (one warp each); fewer if shared memory is short
-struct PLayout { int SQ, pan, aug, tab, stage, ldt, nts, nstage, total; };
-__host__ __device__ inline PLayout setup_pf_layout(const KDims& D) {
-    PLayout L;
-    const int np = (D.n + 7) & ~7;
-    const int ord = np > D.msp ? np : D.msp;
-    L.nts = ord >> 3;
-    L.SQ = 0;
-    L.pan = qpb::pf::pf_elems(L.nts) - 8 * qpb::pf::kPanLd;   // (its first 8 rows are never touched: overlap the staircase)
-    L.aug = L.pan + (ord + 8) * qpb::pf::kPanLd;
-    L.tab = L.aug + ord;
-    L.stage = L.tab + ((qpb::pf::pf_tab_doubles(L.nts) + 1) & ~1);
-    L.ldt = np + 4;
-    const int room = (kMaxSmem / 8 - L.stage) / (8 * L.ldt);
-    L.nstage = room < 1 ? 1 : (room > kSetupStage ? kSetupStage : room);
-    L.total = L.stage + L.nstage * 8 * L.ldt;
-    return L;
-}
-}  // namespace fk
-
-__global__ void __launch_bounds__(kThreads, 2)
-k_setup_pf(KDims D, const double* __restrict__ Q, int64_t sQ, const double* __restrict__ G, int64_t sG,
-           const double* __restrict__ A, int64_t sA, double* __restrict__ Lfac, double* __restrict__ Wfac,
-           double* __restrict__ Kfac, int* __restrict__ spd_flag) {
-    using namespace fk;
-    using namespace qpb::pf;
-    QPB_SMEM;
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const int g = lane >> 2, q = lane & 3;
-    const int sys = blockIdx.x;
-    const int n = D.n, m = D.m, e = D.e, ep = D.ep, ms = D.ms, msp = D.msp;
-    const PLayout PL = setup_pf_layout(D);
-    const int np = (n + 7) & ~7, ntq = np >> 3, nts = msp >> 3;
-    const double* Qg = Q + (int64_t)sys * sQ;
-    const double* Gg = G + (int64_t)sys * sG;
-    const double* Ag = (e > 0) ? (A + (int64_t)sys * sA) : nullptr;
-    double* Lg = Lfac + (int64_t)sys * D.lp;
-    double* Wg = Wfac + (int64_t)sys * ms * D.ldw;
-    double* Kg = Kfac + (int64_t)sys * pf_elems(nts);
-    double* SQ = qsm + PL.SQ;
-    __shared__ int s_flag;
-    if (tid == 0) s_flag = 0;
-#ifdef QPB_TIMING
-    if (threadIdx.x == 0) { for (int i = 0; i < 128; ++i) s_tim[i] = 0; s_tim[128] = clock64(); s_tim2 = s_tim[128]; }
-    __syncthreads();
-#endif
-    // ---- 1. Q (lower triangle, identity padded, + eps I in the regularised variant) -> staircase
-    for (int r = warp; r < np; r += kThreads / 32) {
-        const int off = pf_rowoff(r), len = 8 * (r >> 3) + 8;
-        for (int c = lane; c < len; c += 32) {
-            double v = (r == c) ? 1.0 : 0.0;
-            if (r < n && c < n) v = Qg[(int64_t)r * n + c] + ((r == c) ? D.reg : 0.0);
-            SQ[off + c] = v;
-        }
-    }
-    for (int i = tid; i < (PL.nts << 3); i += kThreads) qsm[PL.aug + i] = 0.0;
-    pf_build_tab(PL.tab, PL.nts);
-    __syncthreads();
-    QPB_TICK(34);   // staging
-    pf_chol_setup(PL.SQ, ntq, 0, ntq, PL.aug, PL.pan, PL.tab, Lg, n);
-    QPB_TICK(35);   // chol(Q)
-    // SPD check (qp.py:81-85): every reciprocal pivot (diagonal of the T_k) must be a positive finite number
-    for (int i = tid; i < n; i += kThreads) {
-        const double ri = SQ[pf_rowoff(i) + i];
-        if (!(ri > 0.0) || isinf(ri)) s_flag = 1;
-    }
-    if (tid == 0 && (D.lp > n * (n + 1) / 2)) Lg[D.lp - 1] = 0.0;
-    // ---- 2. W = [A; 0; G] L^-T, kSetupStage row tiles at a time (warps 0 .. kSetupStage-1)
-    for (int rt0 = 0; rt0 < nts; rt0 += PL.nstage) {
-        const int rt = rt0 + warp;
-        if (warp < PL.nstage && rt < nts) {
-            double* T = qsm + PL.stage + warp * 8 * PL.ldt;
-            for (int rr = 0; rr < 8; ++rr) {                 // stage the tile: 8 rows of [A; 0; G; 0], zero padded to np columns
-                const int r = 8 * rt + rr;
-                const double* src = nullptr;
-                if (r < e) src = Ag + (int64_t)r * n;
-                else if (r >= ep && r < ms) src = Gg + (int64_t)(r - ep) * n;
-                for (int c = lane; c < np; c += 32) T[rr * PL.ldt + c] = (src != nullptr && c < n) ? src[c] : 0.0;
-            }
-            __syncwarp();
-            const int wrow = 8 * rt + g;                     // this lane's row of W
-            for (int k = 0; k < ntq; ++k) {
-                const int k0 = 8 * k;
-                const double a0 = T[g * PL.ldt + k0 + q], a1 = T[g * PL.ldt + k0 + q + 4];
-                // running right-hand side: tile(i) -= tile(k) P_ik^T  (B[kk][nn] = P_ik[nn][kk]), two tiles in flight
-                for (int i = k + 1; i < ntq; i += 2) {
-                    const bool two = i + 1 < ntq;
-                    const int r1 = pf_rowoff(8 * i + g) + k0 + q, r2 = pf_rowoff(8 * (two ? i + 1 : i) + g) + k0 + q;
-                    double* c1 = T + g * PL.ldt + 8 * i + 2 * q;
-                    double* c2 = T + g * PL.ldt + 8 * (two ? i + 1 : i) + 2 * q;
-                    double2 v1 = *reinterpret_cast<const double2*>(c1);
-                    double2 v2 = *reinterpret_cast<const double2*>(c2);
-                    const double b10 = SQ[r1], b11 = SQ[r1 + 4], b20 = SQ[r2], b21 = SQ[r2 + 4];
-                    dmma884(v1.x, v1.y, -a0, b10);
-                    if (two) dmma884(v2.x, v2.y, -a0, b20);
-                    dmma884(v1.x, v1.y, -a1, b11);
-                    if (two) dmma884(v2.x, v2.y, -a1, b21);
-                    *reinterpret_cast<double2*>(c1) = v1;
-                    if (two) *reinterpret_cast<double2*>(c2) = v2;
-                }
-                // y_k = tile(k) T_k^T  (B[kk][nn] = T_k[nn][kk]) -> W
-                const int rk = pf_rowoff(k0 + g) + k0;
-                const double bT0 = (q <= g) ? SQ[rk + q] : 0.0, bT1 = (q + 4 <= g) ? SQ[rk + q + 4] : 0.0;
-                double d0 = 0.0, d1 = 0.0;
-                dmma884(d0, d1, a0, bT0);
-                dmma884(d0, d1, a1, bT1);
-                if (wrow < ms) {
-                    double* wr = Wg + (int64_t)wrow * D.ldw + k0 + 2 * q;
-                    if (k0 + 2 * q < n) wr[0] = d0;
-                    if (k0 + 2 * q + 1 < n) wr[1] = d1;
-                }
-                __syncwarp();                                // the tiles of block column k+1 are complete before they are read as A
-            }
-            if (wrow < ms && q == 0)
-                for (int c = n; c < D.ldw; ++c) Wg[(int64_t)wrow * D.ldw + c] = 0.0;   // (padding columns of the W layout)
-        }
-    }
-    __syncthreads();                                         // W is in global memory (visible to the block), chol(Q) is dead
-    QPB_TICK(37);   // W
-    if (tid == 0) spd_flag[sys] = s_flag;
-    // ---- 3. K = W W^T -> staircase (lower tiles), unit diagonal on dummy / pad rows, + eps on the real equality rows
-    {
-        const int T2 = nts * (nts + 1) / 2;
-        for (int t = warp; t < T2; t += kThreads / 32) {
-            int ti = (int)((sqrtf(8.0f * (float)t + 1.0f) - 1.0f) * 0.5f);
-            while (ti * (ti + 1) / 2 > t) --ti;
-            while ((ti + 1) * (ti + 2) / 2 <= t) ++ti;
-            const int tj = t - ti * (ti + 1) / 2;
-            const int ra = 8 * ti + g, rb = 8 * tj + g;
-            const double* pa = Wg + (int64_t)(ra < ms ? ra : 0) * D.ldw + q;
-            const double* pb = Wg + (int64_t)(rb < ms ? rb : 0) * D.ldw + q;
-            const bool oka = ra < ms, okb = rb < ms;
-            double c0 = 0.0, c1 = 0.0, e0 = 0.0, e1 = 0.0;   // two accumulator chains
-            // W comes back from L2 (written by this CTA in step 2): 28 loads in flight per lane, then their 14 DMMAs
-#pragma unroll 1
-            for (int kk0 = 0; kk0 < np; kk0 += 56) {
-                double x0[7], y0[7], x1[7], y1[7];
-#pragma unroll
-                for (int u = 0; u < 7; ++u) {
-                    const int kk = kk0 + 8 * u;
-                    x0[u] = (oka && kk + q < n) ? pa[kk] : 0.0;
-                    y0[u] = (okb && kk + q < n) ? pb[kk] : 0.0;
-                    x1[u] = (oka && kk + 4 + q < n) ? pa[kk + 4] : 0.0;
-                    y1[u] = (okb && kk + 4 + q < n) ? pb[kk + 4] : 0.0;
-                }
-#pragma unroll
-                for (int u = 0; u < 7; ++u) {
-                    if (kk0 + 8 * u < np) {                  // (warp-uniform)
-                        dmma884(c0, c1, x0[u], y0[u]);
-                        dmma884(e0, e1, x1[u], y1[u]);
-                    }
-                }
-            }
-            const int rr = 8 * ti + g, cc = 8 * tj + 2 * q;
-            double v0 = c0 + e0, v1 = c1 + e1;
-            if (rr == cc && ((rr >= e && rr < ep) || rr >= ms)) v0 += 1.0;
-            if (rr == cc + 1 && ((rr >= e && rr < ep) || rr >= ms)) v1 += 1.0;
-            if (rr == cc && rr < e) v0 += D.reg;
-            if (rr == cc + 1 && rr < e) v1 += D.reg;
-            *reinterpret_cast<double2*>(SQ + pf_rowoff(rr) + cc) = make_double2(v0, v1);
-        }
-    }
-    __syncthreads();
-    QPB_TICK(39);   // K = W W^T
-    // ---- 4. equality block in product form (columns [0, ep)), then K -> global
-    if (ep > 0) pf_chol_setup(PL.SQ, nts, 0, ep >> 3, PL.aug, PL.pan, PL.tab, nullptr, 0);
-    __syncthreads();
-    QPB_TICK(45);   // equality block
-    for (int i = tid; i < pf_elems(nts); i += kThreads) Kg[i] = SQ[i];
-    QPB_TICK(46);   // write K
-#ifdef QPB_TIMING
-    if (tid == 0 && sys == 0) for (int i = 0; i < 128; ++i) g_tim[i] = s_tim[i];
-#endif
-}
+}  // namespace
+#include "qp_setup_pf.cuh"
+namespace {
 
 // ---------------------------------------------------------------------------------------------
 // OptNet parameterisation either side of the path (example-cls-layer.ipynb:125-129; SURVEY 8f.3):
@@ -1188,6 +1004,8 @@ extern "C" {
                                   double*, double*, void*);
 QPB_ALT_DECL(192)
 QPB_ALT_DECL(512)
+int qpb200_alt192_setup(const qpb200_plan*, size_t, int, const double*, int64_t, const double*, int64_t, const double*,
+                        int64_t, double, double*, double*, double*, int*, void*);
 int qpb200_alt512_forward_res(const qpb200_plan*, size_t, int, const double*, int64_t, const double*, int64_t,
                               const double*, int64_t, const double*, const double*, const double*, int, double, double,
                               double, int, int, double*, double*, double*, double*, int*, double*, double*, void*);
@@ -1317,14 +1135,18 @@ int qpb200_plan_init(int nz, int nineq, int neq, qpb200_plan* plan) {
             }
             plan->K_elems = (int64_t)qpb::pf::pf_elems(msp >> 3);
             plan->solve_scratch_elems = 0;                   // the factor lives in shared memory: no per-QP global workspace
-            // pre_factor_kkt on the same machinery (k_setup_pf) whenever its shared memory fits
+            // pre_factor_kkt on the same machinery (k_setup_pf) whenever its shared memory fits. In throughput mode
+            // (pf_three) pre_factor_impl runs its 192-thread build wherever it fits the three-per-SM slot; the choice
+            // below is the latency-mode one: the 256-thread build is faster than the global-scratch setup at
+            // nz = nineq = 200, but a lone CTA of it is slower than k_setup_fast at C2 - so it is the default only where
+            // there is no fast setup or the problem is small (nz <= 64: it wins at C3)
             const int64_t spf = (int64_t)fk::setup_pf_layout(D).total * 8;
-            // faster than the global-scratch setup at nz = nineq = 200, but slower than k_setup_fast at C2 (even at two per
-            // SM) - so it is the default only where there is no fast setup or the problem is small
             const char* esp = getenv("QPB200_SETUP_PF");     // development / A-B knob: "0" never, "1" wherever it fits
-            // (nz <= 64: the 6-warp W sweep covers the whole of [A; G] in one or two rounds and it wins at C3)
             const bool want_spf = (esp != nullptr) ? (esp[0] == '1') : (!setup_fast_ok || nz <= 64);
-            plan->setup_pf = (spf <= kMaxSmem && want_spf) ? 1 : 0;
+            // (room for one more row tile of [A; G]: the shapes this choice has been measured on. Beyond them, e.g.
+            // nz = 211, latency mode keeps the generic setup.)
+            const bool spf_fits = spf + 64 * (int64_t)(((nz + 7) & ~7) + 4) <= kMaxSmem;
+            plan->setup_pf = (spf_fits && want_spf) ? 1 : 0;
             plan->setup_pf_smem_bytes = spf;
             if (plan->setup_pf) plan->setup_scratch_elems = 0;
         }
@@ -1360,10 +1182,14 @@ static int pre_factor_impl(const qpb200_plan* plan, int nsys, const double* Q, i
         if (rc) return rc;
         k_setup<true, true><<<nsys, kTinyThreads, plan->setup_smem_bytes, st>>>(D, Q, sQ, G, sG, A, sA, Lfac, Wfac, Kfac,
                                                                                  spd_flag, nullptr, 0, 0);
+    } else if (plan->pf && plan->pf_three && plan->pf3_ok && plan->setup_pf_smem_bytes <= plan->pf3_smem_bytes) {
+        // throughput mode: the setup CTA fits a three-per-SM slot like the forward / backward CTAs around it
+        return qpb200_alt192_setup(plan, (size_t)plan->setup_pf_smem_bytes, nsys, Q, sQ, G, sG, A, sA, reg, Lfac, Wfac, Kfac,
+                                   spd_flag, stream);
     } else if (plan->pf && plan->setup_pf) {
-        int rc = set_smem(k_setup_pf, plan->setup_pf_smem_bytes);
+        int rc = set_smem(k_setup_pf<2>, plan->setup_pf_smem_bytes);
         if (rc) return rc;
-        k_setup_pf<<<nsys, kThreads, plan->setup_pf_smem_bytes, st>>>(D, Q, sQ, G, sG, A, sA, Lfac, Wfac, Kfac, spd_flag);
+        k_setup_pf<2><<<nsys, kThreads, plan->setup_pf_smem_bytes, st>>>(D, Q, sQ, G, sG, A, sA, Lfac, Wfac, Kfac, spd_flag);
     } else if (plan->setup_fast) {
         int rc = set_smem(k_setup_fast, plan->setup_smem_bytes);
         if (rc) return rc;

@@ -142,17 +142,21 @@ __device__ __forceinline__ void pf_build_tab(int tabo, int nts) {
 // update. Named barrier 1: T_k published (chain arrives, update warps wait); named barrier 2: panel complete (chain
 // arrives, update warps wait); one __syncthreads per step. blockDim.x == kNT.
 // kSetup (pre_factor_kkt, k_setup_pf): stop after block column kend - 1 (the trailing block keeps the Schur complement)
-// and, when Lg != nullptr, emit the plain factor L (rows < ln; packed lower, TRUE diagonal) to global memory as it appears.
-__device__ __forceinline__ void pf_emit_diag(double* Lg, int ln, int k, const double (&Lk)[36]) {
+// and, when Lg != nullptr, emit the plain factor L (rows < ln; packed lower) to global memory: the update warps store
+// the off-diagonal tiles L_ik as they appear, the chain warp parks the strictly lower part of each L_kk in the strict
+// upper triangle of its diagonal tile (pf_park_lower8), which k_setup_pf copies out after the factorization. The chain
+// warp thus issues 16 shared stores per step instead of 36 global stores and 8 divisions on the critical path.
+// Row r of L_kk (r entries) goes to tile row 7 - r, columns 8 - r .. 7 (r free slots); 16-byte stores where aligned.
+__device__ __forceinline__ void pf_park_lower8(double* M, int k, const double (&Lk)[36]) {
+    double* Mb = M + (32 * k + 64) * k + 8 * k;
+    const int ldk = 8 * k + 12;
 #pragma unroll
-    for (int r = 0; r < 8; ++r) {
-        const int R = 8 * k + r;
-        if (R < ln) {
-            double* row = Lg + ((int64_t)R * (R + 1)) / 2 + 8 * k;
+    for (int r = 1; r < 8; ++r) {
+        double* d = Mb + (7 - r) * ldk + 8 - r;
+        if (r & 1) d[0] = Lk[QPB_LIDX(r, 0)];
 #pragma unroll
-            for (int c = 0; c < r; ++c) row[c] = Lk[QPB_LIDX(r, c)];
-            row[r] = 1.0 / Lk[QPB_LIDX(r, r)];
-        }
+        for (int c = r & 1; c + 1 < r; c += 2)
+            *reinterpret_cast<double2*>(d + c) = make_double2(Lk[QPB_LIDX(r, c)], Lk[QPB_LIDX(r, c + 1)]);
     }
 }
 template <bool kSetup>
@@ -167,7 +171,7 @@ __device__ __noinline__ void pf_chol_chain_t(int S, int nts, int kb0, int kend, 
     __syncwarp();
     pf_factor8(Lk);
     pf_inv8_col(Lk, lane & 7, Tc);
-    if (kSetup && Lg != nullptr && lane == 0) pf_emit_diag(Lg, ln, kb0, Lk);
+    if (kSetup && Lg != nullptr) pf_park_lower8(M, kb0, Lk);
 #pragma unroll 1
     for (int k = kb0; k < (kSetup ? kend : nts); ++k) {
         const int k0 = 8 * k;
@@ -208,7 +212,7 @@ __device__ __noinline__ void pf_chol_chain_t(int S, int nts, int kb0, int kend, 
                 __syncwarp();
                 pf_factor8(Lk);                              // F_{k+1}
                 pf_inv8_col(Lk, lane & 7, Tc);               // T_{k+1}
-                if (kSetup && Lg != nullptr && lane == 0) pf_emit_diag(Lg, ln, k + 1, Lk);
+                if (kSetup && Lg != nullptr) pf_park_lower8(M, k + 1, Lk);
             }
             if (k < 16) QPB_TICK(80 + k);   // F_{k+1}
         } else {
