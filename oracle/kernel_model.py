@@ -36,9 +36,11 @@ def _chol(S):
     return np.tril(L)
 
 
-def setup(Q, G, A):
+def setup(Q, G, A, reg=0.0):
+    """reg > 0: the regularised factorization of pre_factor_kkt_reg, chol(Q + reg I) and chol(A~ A~^T + reg I)."""
     n = Q.shape[0]
     e = A.shape[0]
+    Q = Q + reg * np.eye(n) if reg > 0 else Q
     try:
         L = np.linalg.cholesky(Q)
         ok = True
@@ -49,7 +51,7 @@ def setup(Q, G, A):
     R = Gt @ Gt.T
     if e > 0:
         At = _tri(L, A.T).T
-        L11 = _chol(At @ At.T)
+        L11 = _chol(At @ At.T + reg * np.eye(e))
         L21 = _tri(L11, (Gt @ At.T).T).T
         R = R - L21 @ L21.T
         f.update(At=At, L11=L11, L21=L21)
@@ -76,6 +78,16 @@ def _solve_kkt(f, L22, d, t, rs, rz, ry):
     return dxt, ds, wz, wy
 
 
+def kkt_solve(Q, G, A, d, rx, rs, rz, ry, reg=0.0):
+    """solve_kkt[_reg] for one system in the original variables: (dx, ds, dz, dy) of
+    [Q+r 0 G' A'; 0 D+r I 0; G I -r 0; A 0 0 -r] [dx ds dz dy] = -[rx rs rz ry], r = reg (dy None without A)."""
+    f = setup(Q, G, A, reg)
+    dt = d + reg
+    L22 = _chol(f["R"] + np.diag(1.0 / dt + reg))
+    dxt, ds, dz, dy = _solve_kkt(f, L22, dt, _tri(f["L"], rx), rs, rz, ry if f["e"] > 0 else None)
+    return _tri(f["L"], dxt, trans=True), ds, dz, dy
+
+
 def _step(v, dv):
     a = -v / dv
     a = np.where(dv > 0, np.inf, a)          # the fill value max(1.0, a.max()) (batch.py:212) is >= every entry
@@ -83,17 +95,30 @@ def _step(v, dv):
     return 1.0 if st == np.inf else st       # every dv > 0: the fill is max(1.0, negative) = 1.0 at nBatch=1
 
 
-def solve_one(Q, p, G, h, A, b, eps=1e-12, notImprovedLim=3, maxIter=20, stall_tol=np.inf, use_eps=True, tie=1.0, noise=None):
+def solve_one(Q, p, G, h, A, b, eps=1e-12, notImprovedLim=3, maxIter=20, stall_tol=np.inf, use_eps=True, tie=1.0, noise=None,
+              trace=None, kkt_log=None):
+    """trace: a list that receives the kernels' per-iteration trace row [||rz|| + ||ry||, ||L r~x||, mu, resid]
+    (qp_solve.cuh, what verbose=1 prints). kkt_log: a list that receives every KKT solve in the original variables,
+    dict(d, rx, rs, rz, ry, dx, ds, dz, dy) for  K [dx ds dz dy] = -[rx rs rz ry]  (the initial point, then the affine
+    and the corrector direction of each iteration)."""
     m, n = G.shape
     f = setup(Q, G, A)
     e = f["e"]
     L, Gt = f["L"], f["Gt"]
     At = f.get("At")
     pt = _tri(L, p)
+
+    def solve(L22, d, t, rs, rz, ry):
+        out = _solve_kkt(f, L22, d, t, rs, rz, ry)
+        if kkt_log is not None:
+            kkt_log.append(dict(d=d.copy(), rx=L @ t, rs=rs.copy(), rz=rz.copy(), ry=None if ry is None else ry.copy(),
+                                dx=_tri(L, out[0], trans=True), ds=out[1], dz=out[2], dy=out[3]))
+        return out
+
     with np.errstate(all="ignore"):
         d = np.ones(m)
         L22 = _chol(f["R"] + np.diag(1.0 / d))
-        xt, s, z, y = _solve_kkt(f, L22, d, pt, np.zeros(m), -h, -b if e > 0 else None)
+        xt, s, z, y = solve(L22, d, pt, np.zeros(m), -h, -b if e > 0 else None)
         if s.min() < 0:
             s = s - (s.min() - 1)
         if z.min() < 0:
@@ -107,10 +132,13 @@ def solve_one(Q, p, G, h, A, b, eps=1e-12, notImprovedLim=3, maxIter=20, stall_t
             rz = Gt @ xt + s - h
             ry = At @ xt - b if e > 0 else None
             mu = abs((s * z).sum() / m)
-            resid = np.linalg.norm(rz) + (np.linalg.norm(ry) if e > 0 else 0.0) \
-                + np.linalg.norm(L @ rxt) + m * mu
+            pri = np.linalg.norm(rz) + (np.linalg.norm(ry) if e > 0 else 0.0)
+            dual = np.linalg.norm(L @ rxt)
+            resid = pri + dual + m * mu
             if noise is not None:
                 resid = resid + abs(noise.randn()) * 3e-13
+            if trace is not None:
+                trace.append([pri, dual, mu, resid])
             d = z / s
             L22 = _chol(f["R"] + np.diag(1.0 / d))
             if best is None:
@@ -132,12 +160,11 @@ def solve_one(Q, p, G, h, A, b, eps=1e-12, notImprovedLim=3, maxIter=20, stall_t
                 break
             if not np.isfinite(resid):
                 break        # every later iterate is NaN too; `best` cannot change (batch.py:126)
-            dxa, dsa, dza, dya = _solve_kkt(f, L22, d, rxt, z, rz, ry)
+            dxa, dsa, dza, dya = solve(L22, d, rxt, z, rz, ry)
             alpha = min(_step(z, dza), _step(s, dsa), 1.0)
             sig = (((s + alpha * dsa) * (z + alpha * dza)).sum() / (s * z).sum()) ** 3
             rs_c = (-mu * sig + dsa * dza) / s
-            dxc, dsc, dzc, dyc = _solve_kkt(f, L22, d, np.zeros(n), rs_c, np.zeros(m),
-                                            np.zeros(e) if e > 0 else None)
+            dxc, dsc, dzc, dyc = solve(L22, d, np.zeros(n), rs_c, np.zeros(m), np.zeros(e) if e > 0 else None)
             dx, ds, dz = dxa + dxc, dsa + dsc, dza + dzc
             alpha = min(0.999 * min(_step(z, dz), _step(s, ds)), 1.0)
             xt = xt + alpha * dx; s = s + alpha * ds; z = z + alpha * dz

@@ -102,7 +102,7 @@ def plan_for(nz, nineq, neq, two=None):
     # QPB200_PF (development / A-B knob read by qpb200_plan_init: "0" never, "1" product-form kernels wherever they fit,
     # "2" = "1" + the two-QPs-per-SM variant by default)
     key = (nz, nineq, neq, os.environ.get("QPB200_PF"), os.environ.get("QPB200_MAXQPS"), os.environ.get("QPB200_NT512"),
-           os.environ.get("QPB200_SETUP_PF"),
+           os.environ.get("QPB200_SETUP_PF"), os.environ.get("QPB200_COOP"),
            None if two is None else bool(two))
     if key not in _plans:
         p = Plan()

@@ -398,7 +398,7 @@ k_forward(KDims D, const double* __restrict__ p, int64_t sp, const double* __res
         __syncthreads();
     }
 
-    double best = 0.0, ret_resid = 0.0;
+    double best = 0.0;
     int nNot = 0, it = 0, iters_run = 0;
     const double dm = (double)m;
     for (it = 0; it < maxIter; ++it) {
@@ -438,7 +438,6 @@ k_forward(KDims D, const double* __restrict__ p, int64_t sp, const double* __res
         // to within noise while mu keeps shrinking 1000x per step; among iterates within best_tie of the
         // minimum the LATEST is kept, so the backward pass's 1e-8 clamps (qp.py:148) see converged duals.
         if (improved || resid < best_tie * best) {
-            ret_resid = resid;
             for (int i = tid; i < n; i += nt) VEC(V_BXT)[i] = xt[i];
             for (int i = tid; i < ms; i += nt) { VEC(V_BS)[i] = s[i]; VEC(V_BV)[i] = v[i]; }
         }
@@ -536,7 +535,7 @@ k_forward(KDims D, const double* __restrict__ p, int64_t sp, const double* __res
         for (int i = tid; i < e; i += nt) nus[(int64_t)qp * e + i] = VEC(V_BV)[i];
     if (tid == 0) {
         iters_out[qp] = iters_run;
-        resid_out[qp] = ret_resid;
+        resid_out[qp] = best;          // the minimum over the iterations, as the reference reports (batch.py:126-142)
     }
 }
 

@@ -335,7 +335,7 @@ k_forward_fast(KDims D, const double* __restrict__ p, int64_t sp, const double* 
         __syncthreads();
     }
 
-    double best = 0.0, ret_resid = 0.0;
+    double best = 0.0;
     int nNot = 0, iters_run = 0;
     const double dm = (double)m;
     for (int it = 0; it < maxIter; ++it) {
@@ -370,7 +370,6 @@ k_forward_fast(KDims D, const double* __restrict__ p, int64_t sp, const double* 
         const bool improved = (it == 0) || (resid < best);
         if (improved) { best = resid; nNot = 0; } else { ++nNot; }
         if (improved || resid < best_tie * best) {
-            ret_resid = resid;
             _Pragma("unroll 1") for (int i = tid; i < n; i += kNT) qsm[FV(F_BXT) + i] = qsm[xt + i];
             _Pragma("unroll 1") for (int i = tid; i < ms; i += kNT) { qsm[FV(F_BS) + i] = qsm[s + i]; qsm[FV(F_BV) + i] = qsm[v + i]; }
         }
@@ -492,7 +491,7 @@ k_forward_fast(KDims D, const double* __restrict__ p, int64_t sp, const double* 
         _Pragma("unroll 1") for (int i = tid; i < e; i += kNT) nus[(int64_t)qp * e + i] = qsm[FV(F_BV) + i];
     if (tid == 0) {
         iters_out[qp] = iters_run;
-        resid_out[qp] = ret_resid;
+        resid_out[qp] = best;          // the minimum over the iterations, as the reference reports (batch.py:126-142)
     }
 #ifdef QPB_TIMING
     QPB_TICK(16);

@@ -62,3 +62,38 @@ def jobs():
     for name, cfg in EQ_ONLY.items():
         out.append((name, "eq_only", cfg, {}, None))
     return out
+
+
+# Per-family tests (tests/kernel_families.py): the families with dispatch branches that had never run before them.
+KKT_B = 3
+KKT_VARIANTS = [(shared, reg) for shared in (False, True) for reg in (0.0, 1e-7)]
+TRAJ_B = 2
+TRAJ_RUNS = [(it, eps) for eps in (1e-12, 1e-6) for it in (1, 2, 3, 5, 20)]
+
+
+def kkt_job_name(fam, shape, shared, reg):
+    return "kkt_%s_%dx%dx%d_%s_%s" % ((fam,) + tuple(shape) + ("shared" if shared else "batched", "reg" if reg else "plain"))
+
+
+def traj_job_name(fam, shape, unbatched, it, eps):
+    return "traj_%s_%dx%dx%d_%s_it%d_eps%g" % ((fam,) + tuple(shape) + ("unbatched" if unbatched else "batched", it, eps))
+
+
+def family_kkt_jobs():
+    from tests.kernel_families import cases
+    return [(kkt_job_name(fam, s, shared, reg), "call",
+             ("kkt_on_gpu", dict(fam=fam, shape=s, B=KKT_B, shared=shared, reg=reg)), {}, None)
+            for fam, s in cases(child=True) for shared, reg in KKT_VARIANTS]
+
+
+def family_trajectory_jobs():
+    from tests.kernel_families import FAMILIES, cases
+    out = []
+    for fam, s in cases(child=True, forward=True):
+        unb = [False] + ([True] if s == FAMILIES[fam]["shapes"][0] else [])
+        for u in unb:
+            for it, eps in TRAJ_RUNS:
+                out.append((traj_job_name(fam, s, u, it, eps), "call",
+                            ("trajectory_on_gpu", dict(fam=fam, shape=s, B=TRAJ_B, unbatched=u, maxIter=it, eps=eps)),
+                            {}, None))
+    return out

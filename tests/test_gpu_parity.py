@@ -168,7 +168,7 @@ def test_all_solve_kernel_families_agree(family, monkeypatch):
         monkeypatch.setenv("QPB200_PF", "0")
         monkeypatch.setenv("QPB200_COOP", "1" if family == "r1_coop" else "0")
         plan = _lib.plan_for(100, 100, 0, two=False)
-        assert plan.pf == 0 and plan.fast == 1 and plan.coop_ok == 1
+        assert plan.pf == 0 and plan.fast == 1 and plan.coop_ok == 1 and plan.coop == (family == "r1_coop")
     else:
         monkeypatch.setenv("QPB200_MAXQPS", "2" if family == "pf_two" else "3")
         monkeypatch.setattr(qpmod, "MODE", "latency" if family == "pf_one" else "throughput")
