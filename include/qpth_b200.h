@@ -166,6 +166,46 @@ int qpb200_solve_kkt_reg(const qpb200_plan* plan, int nbatch,
                          double* dx, double* ds, double* dz, double* dy,
                          double* scratch, void* stream);
 
+/* ---- Box QPs (qpth_b200/box.py BoxQPFunction): min 1/2 z' diag(q) z + p'z  s.t.  A z = b,  lb <= z <= ub -------------
+ * The dense equivalent is Q = diag(q), G = [-I; I] (only the sides given: lb rows first), h = [-lb; ub]; lam and slacks
+ * are laid out as [lb rows; ub rows] (nineq = (has_lb + has_ub) * nz). The inequality block of the KKT system is
+ * eliminated in closed form (H = q + G'DG diagonal, M = A H^-1 A' of order neq), so there is no pre_factor_kkt: every
+ * call takes q and A themselves. Strides as above (0 = shared); lb / ub may be NULL for an absent side. */
+typedef struct qpb200_box_plan {
+    int nz, neq, neq_pad, nineq;
+    int has_lb, has_ub;
+    int threads;            /* CTA size (one CTA per QP) */
+    int64_t smem_bytes;     /* dynamic shared memory per CTA: A, the factor of M and every vector */
+    int ok;                 /* 1: the box kernels cover this shape (neq_pad <= threads, smem_bytes <= 227 KB); 0: the entry
+                             *    points below return QPB200_ERR_TOO_LARGE and the dense path is the one to use          */
+} qpb200_box_plan;
+
+int qpb200_box_plan_init(int nz, int neq, int has_lb, int has_ub, qpb200_box_plan* plan);
+
+/* forward (batch.py:47-207) with the structured solve; outputs and exit rules as qpb200_forward. spd_flag[B] (may be
+ * NULL): 1 where some q_i <= 0 ('Q is not SPD.'). */
+int qpb200_box_forward(const qpb200_box_plan* plan, int nbatch, const double* q, int64_t sq, const double* p, int64_t sp,
+                       const double* A, int64_t sA, const double* b, int64_t sb, const double* lb, int64_t slb,
+                       const double* ub, int64_t sub, double eps, double stall_tol, double best_tie, int notImprovedLim,
+                       int maxIter, double* zhat, double* lam, double* slacks, double* nus, int* iters,
+                       double* best_resid, double* trace, int* spd_flag, void* stream);
+
+/* backward: dq = dx o z (the diagonal of QPFunction's dQ), dp = dx, dlb = dlam_lb, dub = -dlam_ub, dA = dnu z' + nu dx',
+ * db = -dnu; mean_X = 1 writes the batch mean as one un-batched tensor. Any gradient may be NULL. dxv (B,nz), dlamv
+ * (B,nineq), dnuv (B,neq) are caller-provided work buffers that receive dx, dlam, dnu. */
+int qpb200_box_backward(const qpb200_box_plan* plan, int nbatch, const double* q, int64_t sq, const double* A,
+                        int64_t sA, const double* dl_dzhat, const double* zhat, const double* lam, const double* slacks,
+                        const double* nus, double* dq, int mean_q, double* dp, int mean_p, double* dlb, int mean_lb,
+                        double* dub, int mean_ub, double* dA, int mean_A, double* db, int mean_b, double* dxv,
+                        double* dlamv, double* dnuv, void* stream);
+
+/* The structured factor and solve for caller-supplied d (B,nineq) and right-hand sides (the counterpart of
+ * qpb200_solve_kkt):  [diag(q) 0 G' A'; 0 D I 0; G I 0 0; A 0 0 0] [dx ds dz dy] = -[rx rs rz ry].
+ * ry / dy may be NULL when neq == 0. */
+int qpb200_box_solve_kkt(const qpb200_box_plan* plan, int nbatch, const double* q, int64_t sq, const double* A,
+                         int64_t sA, const double* d, const double* rx, const double* rs, const double* rz,
+                         const double* ry, double* dx, double* ds, double* dz, double* dy, void* stream);
+
 /* Measurement aid: launches blocks x threads threads each issuing 8*iters dependent-chain-free fp64 FMAs
  * (2*8*iters*blocks*threads flops); out needs blocks*threads doubles. bench.py times it with CUDA
  * events to obtain the fp64 roofline denominator on the box it runs on. */

@@ -1,6 +1,7 @@
 """qpth_b200 — H100-native batched differentiable QP layer (drop-in for qpth.qp.QPFunction)."""
 from .qp import QPFunction, QPSolvers   # noqa: F401
 from .solution import QPSolutionFunction, cvxpy_forward   # noqa: F401
+from .box import BoxQPFunction   # noqa: F401
 
 __version__ = "0.1.0"
 

@@ -32,6 +32,15 @@ class Plan(ctypes.Structure):
     ]
 
 
+class BoxPlan(ctypes.Structure):
+    """Mirror of `qpb200_box_plan` (include/qpth_b200.h)."""
+    _fields_ = [
+        ("nz", ctypes.c_int), ("neq", ctypes.c_int), ("neq_pad", ctypes.c_int), ("nineq", ctypes.c_int),
+        ("has_lb", ctypes.c_int), ("has_ub", ctypes.c_int), ("threads", ctypes.c_int),
+        ("smem_bytes", ctypes.c_int64), ("ok", ctypes.c_int),
+    ]
+
+
 # symbol -> (restype, argtypes); also the list tests use to check every declared export exists
 _I, _L, _D, _P = ctypes.c_int, ctypes.c_int64, ctypes.c_double, ctypes.c_void_p
 SIGNATURES = {
@@ -55,6 +64,13 @@ SIGNATURES = {
     "qpb200_copy_lower": (_I, [_P, _P, _I, _I, _I, _I, _P]),
     "qpb200_qp_host": (_I, [_I, _I, _I, _I, _I, _P, _P, _P, _P, _P, _P, _P, _D, _I, _I,
                             _P, _P, _P, _P, _P, _P, _P, _P]),
+    "qpb200_box_plan_init": (_I, [_I, _I, _I, _I, ctypes.POINTER(BoxPlan)]),
+    "qpb200_box_forward": (_I, [ctypes.POINTER(BoxPlan), _I, _P, _L, _P, _L, _P, _L, _P, _L, _P, _L, _P, _L,
+                                _D, _D, _D, _I, _I, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
+    "qpb200_box_backward": (_I, [ctypes.POINTER(BoxPlan), _I, _P, _L, _P, _L, _P, _P, _P, _P, _P,
+                                 _P, _I, _P, _I, _P, _I, _P, _I, _P, _I, _P, _I, _P, _P, _P, _P]),
+    "qpb200_box_solve_kkt": (_I, [ctypes.POINTER(BoxPlan), _I, _P, _L, _P, _L, _P, _P, _P, _P, _P,
+                                  _P, _P, _P, _P, _P]),
 }
 
 _lib = None
@@ -115,6 +131,19 @@ def plan_for(nz, nineq, neq, two=None):
             p.pf_two = 1 if (two and p.pf2_ok and not p.pf_three) else 0
         _plans[key] = p
     return _plans[key]
+
+
+_box_plans = {}
+
+
+def box_plan_for(nz, neq, has_lb, has_ub):
+    """Plan of the box-QP kernels for a shape (cached; no device work). plan.ok: the kernels cover it."""
+    key = (nz, neq, bool(has_lb), bool(has_ub))
+    if key not in _box_plans:
+        p = BoxPlan()
+        check(load().qpb200_box_plan_init(nz, neq, int(bool(has_lb)), int(bool(has_ub)), ctypes.byref(p)))
+        _box_plans[key] = p
+    return _box_plans[key]
 
 
 _sm_count = {}

@@ -28,14 +28,15 @@ def up_to_date():
 
 
 # (source, extra defines, object suffix): the 256-thread build of every kernel + the 192- and 512-thread builds of the
-# product-form solve kernels (three QPs per SM; large orders)
+# product-form solve kernels (three QPs per SM; large orders) + the 128-thread box-QP kernels (BoxQPFunction)
 UNITS = [("qp_kernels.cu", [], "main"),
          ("qp_alt.cu", ["-DQPB_NT=192", "-DQPB_ALT_CTAS=3"], "alt192"),
-         ("qp_alt.cu", ["-DQPB_NT=512", "-DQPB_ALT_CTAS=1"], "alt512")]
+         ("qp_alt.cu", ["-DQPB_NT=512", "-DQPB_ALT_CTAS=1"], "alt512"),
+         ("qp_box.cu", ["-DQPB_NT=128"], "box")]
 
 
 def build(force=False, verbose=False, extra=(), out=None):
-    """Compile the three translation units in parallel and link them into one shared library."""
+    """Compile the translation units in parallel and link them into one shared library."""
     out = out or OUT
     if not force and out == OUT and up_to_date():
         return out

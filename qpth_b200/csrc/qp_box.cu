@@ -1,0 +1,573 @@
+// qp_box.cu - the structured solver of BoxQPFunction: diagonal Q = diag(q), inequality rows G = [-I; I] (the sides
+// given: "lb rows" then "ub rows", h = [-lb; ub]) and dense equality rows A z = b. The inequality block of the KKT
+// system (batch.py:349-372) is eliminated in closed form:
+//     H = q + G'DG (diagonal),  r = rx + G'(D rz - rs),  M = A H^-1 A'  (order neq, SPD for full-row-rank A),
+//     M dy = ry - A H^-1 r,  dx = -H^-1 (r + A'dy),  dz = D (G dx + rz) - rs,  ds = (-rs - dz) / D,
+// so a Newton iteration factors an order-neq matrix (no chol(Q), no W, no K template) and everything else is
+// elementwise or one pass over A. M is factored by the product-form Cholesky of qp_pf.cuh (pf_chol on a staircase of
+// order neq_pad) and solved with pf_fwd / pf_diag / pf_bwd; the predictor and the corrector share one factor.
+// oracle/box_model.py is the numpy model of exactly this arithmetic.
+//
+// One 128-thread CTA per QP; A (neq x nz, row stride nz | 1), the factor of M and every vector live in shared memory.
+// The kernels cover neq_pad <= 128 (the substitutions own one row per thread) and a footprint within the 227 KB an
+// H100 CTA may use (qpb200_box_plan.ok); BoxQPFunction runs the dense kernels on the dense equivalent otherwise.
+#include <cuda_runtime.h>
+#include <math.h>
+#include <stdint.h>
+#include <string.h>
+
+#include <mutex>
+
+#include "../../include/qpth_b200.h"
+#ifndef QPB_NT
+#define QPB_NT 128
+#endif
+// the device functions of the headers have external linkage (host stubs): give this build its own namespace
+#define qpb qpb_box
+#include "qp_pf.cuh"
+
+extern "C" void qpb200_internal_cuda_error(int err, const char* what);   // (qp_kernels.cu) records the message, per thread
+
+namespace {
+
+using namespace qpb::pf;
+constexpr int kBoxNT = qpb::fast::kNT;
+constexpr int kBoxMaxSmem = 232448;        // H100: 227 KB of dynamic shared memory per CTA
+
+// ---- shared-memory layout (doubles; every offset a multiple of 8, i.e. 64-byte aligned) ------------------------------
+struct BoxDims {
+    int n, m, e, ep, nlb;    // nz, inequality rows (nlb lb rows then ub rows), neq, neq_pad, nz if lb given else 0
+    int lda;                 // row stride of A in shared memory (odd: the row-wise passes are bank-conflict free)
+    // offsets
+    int A, S, pan, tab, red;
+    int q, p, x, rx, r, hinv, dxa, dx, bx;                   // length n
+    int h, s, z, d, rz, dsa, dza, ds, dz, bs, bz, rsc;       // length m
+    int b, y, ry, rhs, t, dya, dy, by;                       // length ep
+    int total;               // doubles
+};
+
+__host__ __device__ inline int r8(int v) { return (v + 7) & ~7; }
+
+__host__ __device__ inline BoxDims box_dims(int n, int e, int has_lb, int has_ub) {
+    BoxDims D;
+    D.n = n; D.e = e; D.ep = r8(e); D.nlb = has_lb ? n : 0; D.m = (has_lb ? n : 0) + (has_ub ? n : 0);
+    D.lda = n | 1;
+    const int nts = D.ep >> 3;
+    int o = 0;
+    D.A = o; o += r8(e * D.lda);
+    D.S = o; o += r8(pf_elems(nts));
+    D.pan = o; o += (e > 0) ? r8((8 * nts + 8) * kPanLd) : 0;
+    D.tab = o; o += r8(pf_tab_doubles(nts));
+    D.red = o; o += 4 * qpb::kRedStride;
+    const int nn = r8(n), mm = r8(D.m), ee = D.ep;
+    int* vn[] = {&D.q, &D.p, &D.x, &D.rx, &D.r, &D.hinv, &D.dxa, &D.dx, &D.bx};
+    for (int* v : vn) { *v = o; o += nn; }
+    int* vm[] = {&D.h, &D.s, &D.z, &D.d, &D.rz, &D.dsa, &D.dza, &D.ds, &D.dz, &D.bs, &D.bz, &D.rsc};
+    for (int* v : vm) { *v = o; o += mm; }
+    int* ve[] = {&D.b, &D.y, &D.ry, &D.rhs, &D.t, &D.dya, &D.dy, &D.by};
+    for (int* v : ve) { *v = o; o += ee; }
+    D.total = o;
+    return D;
+}
+
+// inequality row i is sign(i) * e_var(i)
+__device__ __forceinline__ int bvar(const BoxDims& D, int i) { return i < D.nlb ? i : i - D.nlb; }
+__device__ __forceinline__ double bsgn(const BoxDims& D, int i) { return i < D.nlb ? -1.0 : 1.0; }
+
+// G'v of a length-m shared vector at column j (the lb row and/or the ub row of variable j)
+__device__ __forceinline__ double gt_col(const BoxDims& D, const double* v, int j) {
+    double a = 0.0;
+    if (D.nlb) a -= v[j];
+    if (D.m > D.nlb) a += v[D.nlb + j];
+    return a;
+}
+
+// hinv = 1 / (q + G'DG) for the d currently in shared memory; with A, M = A H^-1 A' into the staircase (lower tiles,
+// identity rows beyond neq). Ends with a block barrier.
+__device__ __noinline__ void box_form(const BoxDims& D) {
+    QPB_SMEM;
+    const int tid = threadIdx.x;
+    for (int j = tid; j < D.n; j += kBoxNT) {
+        double hj = qsm[D.q + j];
+        if (D.nlb) hj += qsm[D.d + j];
+        if (D.m > D.nlb) hj += qsm[D.d + D.nlb + j];
+        qsm[D.hinv + j] = 1.0 / hj;
+    }
+    __syncthreads();
+    if (D.e == 0) return;
+    const int ep = D.ep, n = D.n, lda = D.lda;
+    const int tot = (ep * (ep + 1)) / 2;
+    const double* A = qsm + D.A;
+    const double* hv = qsm + D.hinv;
+    for (int t = tid; t < tot; t += kBoxNT) {
+        int r = (int)((sqrt(8.0 * t + 1.0) - 1.0) * 0.5);
+        while ((r * (r + 1)) / 2 > t) --r;
+        while (((r + 1) * (r + 2)) / 2 <= t) ++r;
+        const int c = t - (r * (r + 1)) / 2;
+        double v;
+        if (r < D.e) {
+            const double* ar = A + r * lda;
+            const double* ac = A + c * lda;
+            double s0 = 0.0, s1 = 0.0;
+            int k = 0;
+            for (; k + 1 < n; k += 2) {
+                s0 = fma(ar[k] * hv[k], ac[k], s0);
+                s1 = fma(ar[k + 1] * hv[k + 1], ac[k + 1], s1);
+            }
+            if (k < n) s0 = fma(ar[k] * hv[k], ac[k], s0);
+            v = s0 + s1;
+        } else {
+            v = (r == c) ? 1.0 : 0.0;
+        }
+        qsm[D.S + pf_rowoff(r) + c] = v;
+    }
+    __syncthreads();
+}
+
+// The structured KKT solve with the H / M of the last box_form:
+//   K [dx ds dz dy] = -[rx rs rz ry];  rs, rz, ry may be -1 (zero). fresh: M was just formed and is factored here
+// (with the right-hand side carried along), else the existing factor is reused. Ends with a block barrier.
+__device__ __noinline__ void box_solve(const BoxDims& D, bool fresh, int rx, int rs, int rz, int ry,
+                                       int dx, int ds, int dz, int dy) {
+    QPB_SMEM;
+    const int tid = threadIdx.x;
+    const int n = D.n, m = D.m, e = D.e, ep = D.ep, lda = D.lda;
+    // r = rx + G'(D rz - rs), kept as H^-1 r in D.r
+    for (int j = tid; j < n; j += kBoxNT) {
+        double a = qsm[rx + j];
+        if (D.nlb) {
+            const double t = ((rz >= 0) ? qsm[D.d + j] * qsm[rz + j] : 0.0) - ((rs >= 0) ? qsm[rs + j] : 0.0);
+            a -= t;
+        }
+        if (m > D.nlb) {
+            const int i = D.nlb + j;
+            const double t = ((rz >= 0) ? qsm[D.d + i] * qsm[rz + i] : 0.0) - ((rs >= 0) ? qsm[rs + i] : 0.0);
+            a += t;
+        }
+        qsm[D.r + j] = a * qsm[D.hinv + j];
+    }
+    __syncthreads();
+    if (e > 0) {
+        // rhs = ry - A H^-1 r: one warp per row, lanes over the columns
+        const int lane = tid & 31, warp = tid >> 5;
+        for (int i = warp; i < ep; i += kBoxNT / 32) {
+            double a = 0.0;
+            if (i < e)
+                for (int k = lane; k < n; k += 32) a = fma(qsm[D.A + i * lda + k], qsm[D.r + k], a);
+            a = qpb::warp_sum(a);
+            if (lane == 0) qsm[D.rhs + i] = (i < e) ? (((ry >= 0) ? qsm[ry + i] : 0.0) - a) : 0.0;
+        }
+        __syncthreads();
+        const int nts = ep >> 3;
+        if (fresh) {
+            pf_chol(D.S, nts, 0, D.rhs, D.pan, D.tab);       // the factor, and the forward sweep of the right-hand side
+            __syncthreads();
+        } else {
+            pf_fwd(D.S, ep, 0, nts - 1, D.rhs);
+        }
+        pf_diag(D.S, ep, D.rhs, D.t, D.rhs);
+        pf_bwd(D.S, ep, D.rhs, dy);
+    }
+    // dx = -H^-1 r - H^-1 A'dy
+    for (int j = tid; j < n; j += kBoxNT) {
+        double a = 0.0;
+        for (int i = 0; i < e; ++i) a = fma(qsm[D.A + i * lda + j], qsm[dy + i], a);
+        qsm[dx + j] = -qsm[D.r + j] - a * qsm[D.hinv + j];
+    }
+    __syncthreads();
+    for (int i = tid; i < m; i += kBoxNT) {
+        const double di = qsm[D.d + i];
+        const double rsi = (rs >= 0) ? qsm[rs + i] : 0.0;
+        const double dzi = di * (bsgn(D, i) * qsm[dx + bvar(D, i)] + ((rz >= 0) ? qsm[rz + i] : 0.0)) - rsi;
+        qsm[dz + i] = dzi;
+        qsm[ds + i] = (-rsi - dzi) / di;
+    }
+    __syncthreads();
+}
+
+// q, A (shared / per QP), b (nullptr in the backward and KKT kernels): staged once per CTA; the staircase tile table
+__device__ __forceinline__ void box_stage(const BoxDims& D, const double* q, const double* A, const double* b) {
+    QPB_SMEM;
+    const int tid = threadIdx.x;
+    for (int j = tid; j < D.n; j += kBoxNT) qsm[D.q + j] = q[j];
+    for (int t = tid; t < D.e * D.n; t += kBoxNT) {
+        const int i = t / D.n, j = t - i * D.n;
+        qsm[D.A + i * D.lda + j] = A[t];
+    }
+    for (int i = tid; i < D.ep; i += kBoxNT) qsm[D.b + i] = (b != nullptr && i < D.e) ? b[i] : 0.0;   // (b: forward only)
+    if (D.e > 0) pf_build_tab(D.tab, D.ep >> 3);
+    __syncthreads();
+}
+
+__device__ __forceinline__ double box_step(double v, double dv) { return (dv > 0.0) ? INFINITY : (-v / dv); }
+__device__ __forceinline__ double box_step_fix(double v) { return (isinf(v) && v > 0.0) ? 1.0 : v; }
+
+// forward (batch.py:47-207) with the structured solve, one CTA per QP; the loop of k_forward_fast (qp_solve.cuh).
+// Three CTAs per SM (at most 168 registers; about 48 KB of shared memory per QP at nz = 64, neq = 40): four (128
+// registers) spill.
+__global__ void __launch_bounds__(kBoxNT, 3)
+k_box_forward(BoxDims D, const double* __restrict__ q, int64_t sq, const double* __restrict__ p, int64_t sp,
+              const double* __restrict__ A, int64_t sA, const double* __restrict__ b, int64_t sb,
+              const double* __restrict__ lb, int64_t slb, const double* __restrict__ ub, int64_t sub, double eps,
+              double stall_tol, double best_tie, int notImprovedLim, int maxIter, double* __restrict__ zhat,
+              double* __restrict__ lam, double* __restrict__ slacks, double* __restrict__ nus, int* __restrict__ iters_out,
+              double* __restrict__ resid_out, double* __restrict__ trace, int* __restrict__ spd_flag) {
+    QPB_SMEM;
+    const int tid = threadIdx.x, qp = blockIdx.x;
+    const int n = D.n, m = D.m, e = D.e, ep = D.ep;
+    const double* qg = q + (int64_t)qp * sq;
+    box_stage(D, qg, A + (int64_t)qp * sA, (e > 0) ? b + (int64_t)qp * sb : nullptr);
+    {
+        int bad = 0;
+        for (int j = tid; j < n; j += kBoxNT) {
+            qsm[D.p + j] = p[(int64_t)qp * sp + j];
+            bad |= !(qsm[D.q + j] > 0.0);
+        }
+        bad = __syncthreads_or(bad);
+        if (tid == 0 && spd_flag != nullptr) spd_flag[qp] = bad;
+    }
+    for (int i = tid; i < m; i += kBoxNT) {
+        qsm[D.h + i] = (i < D.nlb) ? -lb[(int64_t)qp * slb + i] : ub[(int64_t)qp * sub + i - D.nlb];
+        qsm[D.d + i] = 1.0;
+        qsm[D.rz + i] = -qsm[D.h + i];
+    }
+    for (int i = tid; i < ep; i += kBoxNT) { qsm[D.ry + i] = -qsm[D.b + i]; qsm[D.y + i] = 0.0; }
+    __syncthreads();
+
+    // ---- initial point: solve_kkt(p, 0, -h, -b) with d = 1   (batch.py:61-67)
+    box_form(D);
+    box_solve(D, true, D.p, -1, D.rz, D.ry, D.x, D.s, D.z, D.y);
+    {
+        double mn[2] = {INFINITY, INFINITY};
+        for (int i = tid; i < m; i += kBoxNT) { mn[0] = fmin(mn[0], qsm[D.s + i]); mn[1] = fmin(mn[1], qsm[D.z + i]); }
+        qpb::block_reduce<2, true>(mn, qsm + D.red, tid, kBoxNT);
+        for (int i = tid; i < m; i += kBoxNT) {                  // slacks and duals >= 1 (batch.py:77-87)
+            if (mn[0] < 0.0) qsm[D.s + i] -= mn[0] - 1.0;
+            if (mn[1] < 0.0) qsm[D.z + i] -= mn[1] - 1.0;
+        }
+        __syncthreads();
+    }
+
+    double best = 0.0;
+    int nNot = 0, iters_run = 0;
+    const double dm = (double)m;
+    for (int it = 0; it < maxIter; ++it) {
+        iters_run = it + 1;
+        // ---- residuals (batch.py:94-107)
+        double acc[4] = {0.0, 0.0, 0.0, 0.0};                   // |ry|^2, |rz|^2, |rx|^2, s.z
+        for (int j = tid; j < n; j += kBoxNT) {
+            double a = 0.0;
+            for (int i = 0; i < e; ++i) a = fma(qsm[D.A + i * D.lda + j], qsm[D.y + i], a);
+            const double r = fma(qsm[D.q + j], qsm[D.x + j], qsm[D.p + j]) + gt_col(D, qsm + D.z, j) + a;
+            qsm[D.rx + j] = r;
+            acc[2] = fma(r, r, acc[2]);
+        }
+        for (int i = tid; i < m; i += kBoxNT) {
+            const double r = bsgn(D, i) * qsm[D.x + bvar(D, i)] + qsm[D.s + i] - qsm[D.h + i];
+            qsm[D.rz + i] = r;
+            acc[1] = fma(r, r, acc[1]);
+            acc[3] = fma(qsm[D.s + i], qsm[D.z + i], acc[3]);
+        }
+        {
+            const int lane = tid & 31, warp = tid >> 5;
+            for (int i = warp; i < ep; i += kBoxNT / 32) {
+                double a = 0.0;
+                if (i < e)
+                    for (int k = lane; k < n; k += 32) a = fma(qsm[D.A + i * D.lda + k], qsm[D.x + k], a);
+                a = qpb::warp_sum(a);
+                const double r = (i < e) ? a - qsm[D.b + i] : 0.0;
+                if (lane == 0) { qsm[D.ry + i] = r; acc[0] = fma(r, r, acc[0]); }
+            }
+        }
+        qpb::block_reduce<4, false>(acc, qsm + D.red, tid, kBoxNT);
+        const double mu = fabs(acc[3] / dm);
+        const double resid = sqrt(acc[1]) + sqrt(acc[0]) + sqrt(acc[2]) + dm * mu;
+        if (trace != nullptr && tid == 0) {                     // what verbose=1 prints (batch.py:115-117)
+            double* tr = trace + ((int64_t)qp * maxIter + it) * 4;
+            tr[0] = sqrt(acc[1]) + sqrt(acc[0]); tr[1] = sqrt(acc[2]); tr[2] = mu; tr[3] = resid;
+        }
+        // ---- best-iterate tracking and exit tests (batch.py:118-143), per QP
+        const bool improved = (it == 0) || (resid < best);
+        if (improved) { best = resid; nNot = 0; } else { ++nNot; }
+        if (improved || resid < best_tie * best) {
+            for (int j = tid; j < n; j += kBoxNT) qsm[D.bx + j] = qsm[D.x + j];
+            for (int i = tid; i < m; i += kBoxNT) { qsm[D.bs + i] = qsm[D.s + i]; qsm[D.bz + i] = qsm[D.z + i]; }
+            for (int i = tid; i < e; i += kBoxNT) qsm[D.by + i] = qsm[D.y + i];
+        }
+        if ((nNot == notImprovedLim && best < stall_tol) || best < eps || mu > 1e32) break;
+        if (!(resid == resid) || isinf(resid)) break;
+        // ---- d = z/s, H, M; the affine direction (batch.py:109-113,150) factors M
+        for (int i = tid; i < m; i += kBoxNT) qsm[D.d + i] = qsm[D.z + i] / qsm[D.s + i];
+        __syncthreads();
+        box_form(D);
+        box_solve(D, true, D.rx, D.z, D.rz, D.ry, D.dxa, D.dsa, D.dza, D.dya);
+        // ---- affine step length and sigma (batch.py:160-168)
+        double mn[2] = {INFINITY, INFINITY};
+        for (int i = tid; i < m; i += kBoxNT) {
+            mn[0] = fmin(mn[0], box_step(qsm[D.z + i], qsm[D.dza + i]));
+            mn[1] = fmin(mn[1], box_step(qsm[D.s + i], qsm[D.dsa + i]));
+        }
+        qpb::block_reduce<2, true>(mn, qsm + D.red, tid, kBoxNT);
+        {
+            const double alpha = fmin(fmin(box_step_fix(mn[0]), box_step_fix(mn[1])), 1.0);
+            double sm[2] = {0.0, 0.0};
+            for (int i = tid; i < m; i += kBoxNT) {
+                sm[0] = fma(qsm[D.s + i] + alpha * qsm[D.dsa + i], qsm[D.z + i] + alpha * qsm[D.dza + i], sm[0]);
+                sm[1] = fma(qsm[D.s + i], qsm[D.z + i], sm[1]);
+            }
+            qpb::block_reduce<2, false>(sm, qsm + D.red, tid, kBoxNT);
+            const double sr = sm[0] / sm[1];
+            const double sig = sr * sr * sr;
+            // ---- corrector right-hand side (batch.py:170-181): rs = (-mu sig + dsa dza) / s, rx = rz = ry = 0
+            for (int i = tid; i < m; i += kBoxNT)
+                qsm[D.rsc + i] = (-mu * sig + qsm[D.dsa + i] * qsm[D.dza + i]) / qsm[D.s + i];
+            for (int j = tid; j < n; j += kBoxNT) qsm[D.rx + j] = 0.0;
+            __syncthreads();
+        }
+        box_solve(D, false, D.rx, D.rsc, -1, -1, D.dx, D.ds, D.dz, D.dy);
+        // ---- combined direction, step length, update (batch.py:185-203)
+        mn[0] = INFINITY; mn[1] = INFINITY;
+        for (int i = tid; i < m; i += kBoxNT) {
+            const double dzi = qsm[D.dza + i] + qsm[D.dz + i], dsi = qsm[D.dsa + i] + qsm[D.ds + i];
+            qsm[D.dz + i] = dzi;
+            qsm[D.ds + i] = dsi;
+            mn[0] = fmin(mn[0], box_step(qsm[D.z + i], dzi));
+            mn[1] = fmin(mn[1], box_step(qsm[D.s + i], dsi));
+        }
+        qpb::block_reduce<2, true>(mn, qsm + D.red, tid, kBoxNT);
+        const double alpha = fmin(0.999 * fmin(box_step_fix(mn[0]), box_step_fix(mn[1])), 1.0);
+        for (int j = tid; j < n; j += kBoxNT) qsm[D.x + j] = fma(alpha, qsm[D.dxa + j] + qsm[D.dx + j], qsm[D.x + j]);
+        for (int i = tid; i < m; i += kBoxNT) {
+            qsm[D.s + i] = fma(alpha, qsm[D.ds + i], qsm[D.s + i]);
+            qsm[D.z + i] = fma(alpha, qsm[D.dz + i], qsm[D.z + i]);
+        }
+        for (int i = tid; i < e; i += kBoxNT) qsm[D.y + i] = fma(alpha, qsm[D.dya + i] + qsm[D.dy + i], qsm[D.y + i]);
+        __syncthreads();
+    }
+    __syncthreads();
+    for (int j = tid; j < n; j += kBoxNT) zhat[(int64_t)qp * n + j] = qsm[D.bx + j];
+    for (int i = tid; i < m; i += kBoxNT) {
+        lam[(int64_t)qp * m + i] = qsm[D.bz + i];
+        slacks[(int64_t)qp * m + i] = qsm[D.bs + i];
+    }
+    if (nus != nullptr)
+        for (int i = tid; i < e; i += kBoxNT) nus[(int64_t)qp * e + i] = qsm[D.by + i];
+    if (tid == 0) { iters_out[qp] = iters_run; resid_out[qp] = best; }
+}
+
+// QPFunctionFn.backward (qp.py:128-182) for the box QP: d from the clamped duals (qp.py:148), one factor of M and one
+// solve per QP, then dq = dx o z, dp = dx, dlb = dlam_lb, dub = -dlam_ub, dA = dnu z' + nu dx', db = -dnu. dxv, dlamv
+// and dnuv always receive dx, dlam, dnu (the batch means read them); a gradient whose mean flag is set is skipped here.
+struct BoxGrads {
+    double *dq, *dp, *dlb, *dub, *dA, *db;
+    int mq, mp, mlb, mub, mA, mb;
+};
+
+__global__ void __launch_bounds__(kBoxNT, 4)
+k_box_backward(BoxDims D, const double* __restrict__ q, int64_t sq, const double* __restrict__ A, int64_t sA,
+               const double* __restrict__ dl, const double* __restrict__ zhat, const double* __restrict__ lam,
+               const double* __restrict__ slacks, const double* __restrict__ nus, BoxGrads O,
+               double* __restrict__ dxv, double* __restrict__ dlamv, double* __restrict__ dnuv) {
+    QPB_SMEM;
+    const int tid = threadIdx.x, qp = blockIdx.x;
+    const int n = D.n, m = D.m, e = D.e;
+    box_stage(D, q + (int64_t)qp * sq, A + (int64_t)qp * sA, nullptr);
+    for (int j = tid; j < n; j += kBoxNT) qsm[D.rx + j] = dl[(int64_t)qp * n + j];
+    for (int i = tid; i < m; i += kBoxNT)
+        qsm[D.d + i] = fmax(lam[(int64_t)qp * m + i], 1e-8) / fmax(slacks[(int64_t)qp * m + i], 1e-8);
+    __syncthreads();
+    box_form(D);
+    box_solve(D, true, D.rx, -1, -1, -1, D.dx, D.ds, D.dz, D.dy);
+    for (int j = tid; j < n; j += kBoxNT) {
+        const double dx = qsm[D.dx + j], z = zhat[(int64_t)qp * n + j];
+        dxv[(int64_t)qp * n + j] = dx;
+        if (O.dq && !O.mq) O.dq[(int64_t)qp * n + j] = dx * z;
+        if (O.dp && !O.mp) O.dp[(int64_t)qp * n + j] = dx;
+    }
+    for (int i = tid; i < m; i += kBoxNT) {
+        const double dz = qsm[D.dz + i];
+        dlamv[(int64_t)qp * m + i] = dz;
+        if (i < D.nlb) { if (O.dlb && !O.mlb) O.dlb[(int64_t)qp * n + i] = dz; }
+        else if (O.dub && !O.mub) O.dub[(int64_t)qp * n + i - D.nlb] = -dz;
+    }
+    for (int i = tid; i < e; i += kBoxNT) {
+        dnuv[(int64_t)qp * e + i] = qsm[D.dy + i];
+        if (O.db && !O.mb) O.db[(int64_t)qp * e + i] = -qsm[D.dy + i];
+    }
+    if (O.dA && !O.mA)
+        for (int t = tid; t < e * n; t += kBoxNT) {
+            const int i = t / n, j = t - i * n;
+            O.dA[(int64_t)qp * e * n + t] = fma(qsm[D.dy + i], zhat[(int64_t)qp * n + j],
+                                                nus[(int64_t)qp * e + i] * qsm[D.dx + j]);
+        }
+}
+
+// qpb200_box_solve_kkt: the structured factor and solve for caller-given d and right-hand sides (all vectors (B, len))
+__global__ void __launch_bounds__(kBoxNT)
+k_box_kkt(BoxDims D, const double* __restrict__ q, int64_t sq, const double* __restrict__ A, int64_t sA,
+          const double* __restrict__ d, const double* __restrict__ rx, const double* __restrict__ rs,
+          const double* __restrict__ rz, const double* __restrict__ ry, double* __restrict__ dx, double* __restrict__ ds,
+          double* __restrict__ dz, double* __restrict__ dy) {
+    QPB_SMEM;
+    const int tid = threadIdx.x, qp = blockIdx.x;
+    const int n = D.n, m = D.m, e = D.e;
+    box_stage(D, q + (int64_t)qp * sq, A + (int64_t)qp * sA, nullptr);
+    for (int j = tid; j < n; j += kBoxNT) qsm[D.rx + j] = rx[(int64_t)qp * n + j];
+    for (int i = tid; i < m; i += kBoxNT) {
+        qsm[D.d + i] = d[(int64_t)qp * m + i];
+        qsm[D.rsc + i] = rs[(int64_t)qp * m + i];
+        qsm[D.rz + i] = rz[(int64_t)qp * m + i];
+    }
+    for (int i = tid; i < e; i += kBoxNT) qsm[D.ry + i] = ry[(int64_t)qp * e + i];
+    __syncthreads();
+    box_form(D);
+    box_solve(D, true, D.rx, D.rsc, D.rz, D.ry, D.dx, D.ds, D.dz, D.dy);
+    for (int j = tid; j < n; j += kBoxNT) dx[(int64_t)qp * n + j] = qsm[D.dx + j];
+    for (int i = tid; i < m; i += kBoxNT) {
+        ds[(int64_t)qp * m + i] = qsm[D.ds + i];
+        dz[(int64_t)qp * m + i] = qsm[D.dz + i];
+    }
+    if (dy != nullptr)
+        for (int i = tid; i < e; i += kBoxNT) dy[(int64_t)qp * e + i] = qsm[D.dy + i];
+}
+
+// batch means of the gradients of un-batched inputs (qp.py:159-177)
+// out[c] = scale / B * sum_b u[b * su + c] (* x[b * len + c] when x != null)
+__global__ void k_box_mean_vec(int B, int len, const double* __restrict__ u, int64_t su, const double* __restrict__ x,
+                               double scale, double* __restrict__ out) {
+    const int c = blockIdx.x * blockDim.x + threadIdx.x;
+    if (c >= len) return;
+    double s0 = 0.0, s1 = 0.0;
+    int bb = 0;
+    for (; bb + 1 < B; bb += 2) {
+        s0 += x ? u[(int64_t)bb * su + c] * x[(int64_t)bb * len + c] : u[(int64_t)bb * su + c];
+        s1 += x ? u[(int64_t)(bb + 1) * su + c] * x[(int64_t)(bb + 1) * len + c] : u[(int64_t)(bb + 1) * su + c];
+    }
+    if (bb < B) s0 += x ? u[(int64_t)bb * su + c] * x[(int64_t)bb * len + c] : u[(int64_t)bb * su + c];
+    out[c] = (s0 + s1) * scale / (double)B;
+}
+// dA mean: out[r][c] = 1/B sum_b (dnu[b][r] z[b][c] + nu[b][r] dx[b][c]); one thread per entry, a block per 128 columns
+__global__ void k_box_mean_outer(int B, int rows, int cols, const double* __restrict__ dnu, const double* __restrict__ z,
+                                 const double* __restrict__ nu, const double* __restrict__ dx, double* __restrict__ out) {
+    const int c = blockIdx.x * blockDim.x + threadIdx.x, r = blockIdx.y;
+    if (c >= cols) return;
+    double s = 0.0;
+    for (int bb = 0; bb < B; ++bb)
+        s = fma(dnu[(int64_t)bb * rows + r], z[(int64_t)bb * cols + c], fma(nu[(int64_t)bb * rows + r], dx[(int64_t)bb * cols + c], s));
+    out[(int64_t)r * cols + c] = s / (double)B;
+}
+
+std::mutex g_mu;
+template <typename K>
+int box_set_smem(K kernel, size_t bytes, size_t* cur) {      // cur: per-kernel high-water mark (device 0..15)
+    int dev = 0;
+    cudaError_t err = cudaGetDevice(&dev);
+    if (err != cudaSuccess) { qpb200_internal_cuda_error((int)err, "cudaGetDevice"); return QPB200_ERR_CUDA; }
+    std::lock_guard<std::mutex> lock(g_mu);
+    if (dev < 16 && cur[dev] >= bytes) return QPB200_OK;
+    err = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
+    if (err != cudaSuccess) { qpb200_internal_cuda_error((int)err, "cudaFuncSetAttribute"); return QPB200_ERR_CUDA; }
+    if (dev < 16) cur[dev] = bytes;
+    return QPB200_OK;
+}
+int box_check_launch(const char* what) {
+    cudaError_t err = cudaGetLastError();
+    if (err != cudaSuccess) { qpb200_internal_cuda_error((int)err, what); return QPB200_ERR_CUDA; }
+    return QPB200_OK;
+}
+size_t g_fwd[16], g_bwd[16], g_kkt[16];
+
+int box_plan_check(const qpb200_box_plan* P) {
+    if (P == nullptr || !P->ok) return P == nullptr ? QPB200_ERR_BAD_ARG : QPB200_ERR_TOO_LARGE;
+    return QPB200_OK;
+}
+BoxDims plan_dims(const qpb200_box_plan* P) { return box_dims(P->nz, P->neq, P->has_lb, P->has_ub); }
+
+}  // namespace
+
+extern "C" {
+
+int qpb200_box_plan_init(int nz, int neq, int has_lb, int has_ub, qpb200_box_plan* plan) {
+    if (plan == nullptr || nz <= 0 || neq < 0) return QPB200_ERR_BAD_ARG;
+    if (!has_lb && !has_ub) return QPB200_ERR_NO_CONSTRAINTS;
+    if (nz > 4096 || neq > 4096) return QPB200_ERR_TOO_LARGE;
+    memset(plan, 0, sizeof(*plan));
+    plan->nz = nz; plan->neq = neq; plan->neq_pad = r8(neq);
+    plan->has_lb = has_lb ? 1 : 0; plan->has_ub = has_ub ? 1 : 0;
+    plan->nineq = (plan->has_lb + plan->has_ub) * nz;
+    plan->threads = kBoxNT;
+    const BoxDims D = box_dims(nz, neq, plan->has_lb, plan->has_ub);
+    plan->smem_bytes = (int64_t)D.total * 8;
+    plan->ok = (plan->neq_pad <= kBoxNT && plan->smem_bytes <= kBoxMaxSmem) ? 1 : 0;
+    return QPB200_OK;
+}
+
+int qpb200_box_forward(const qpb200_box_plan* plan, int nbatch, const double* q, int64_t sq, const double* p, int64_t sp,
+                       const double* A, int64_t sA, const double* b, int64_t sb, const double* lb, int64_t slb,
+                       const double* ub, int64_t sub, double eps, double stall_tol, double best_tie, int notImprovedLim,
+                       int maxIter, double* zhat, double* lam, double* slacks, double* nus, int* iters,
+                       double* best_resid, double* trace, int* spd_flag, void* stream) {
+    int rc = box_plan_check(plan);
+    if (rc) return rc;
+    if (nbatch <= 0 || maxIter < 1 || !q || !p || !zhat || !lam || !slacks || !iters || !best_resid) return QPB200_ERR_BAD_ARG;
+    if ((plan->has_lb && !lb) || (plan->has_ub && !ub) || (plan->neq > 0 && (!A || !b || !nus))) return QPB200_ERR_BAD_ARG;
+    const BoxDims D = plan_dims(plan);
+    rc = box_set_smem(k_box_forward, (size_t)plan->smem_bytes, g_fwd);
+    if (rc) return rc;
+    k_box_forward<<<nbatch, kBoxNT, (size_t)plan->smem_bytes, (cudaStream_t)stream>>>(
+        D, q, sq, p, sp, A, sA, b, sb, lb, slb, ub, sub, eps, stall_tol, best_tie, notImprovedLim, maxIter, zhat, lam,
+        slacks, nus, iters, best_resid, trace, spd_flag);
+    return box_check_launch("k_box_forward");
+}
+
+int qpb200_box_backward(const qpb200_box_plan* plan, int nbatch, const double* q, int64_t sq, const double* A,
+                        int64_t sA, const double* dl_dzhat, const double* zhat, const double* lam, const double* slacks,
+                        const double* nus, double* dq, int mean_q, double* dp, int mean_p, double* dlb, int mean_lb,
+                        double* dub, int mean_ub, double* dA, int mean_A, double* db, int mean_b, double* dxv,
+                        double* dlamv, double* dnuv, void* stream) {
+    int rc = box_plan_check(plan);
+    if (rc) return rc;
+    if (nbatch <= 0 || !q || !dl_dzhat || !zhat || !lam || !slacks || !dxv || !dlamv) return QPB200_ERR_BAD_ARG;
+    if (plan->neq > 0 && (!A || !nus || !dnuv)) return QPB200_ERR_BAD_ARG;
+    if ((dlb && !plan->has_lb) || (dub && !plan->has_ub)) return QPB200_ERR_BAD_ARG;
+    const BoxDims D = plan_dims(plan);
+    const int n = D.n, m = D.m, e = D.e;
+    BoxGrads O;
+    O.dq = dq; O.dp = dp; O.dlb = dlb; O.dub = dub; O.dA = e > 0 ? dA : nullptr; O.db = e > 0 ? db : nullptr;
+    O.mq = mean_q; O.mp = mean_p; O.mlb = mean_lb; O.mub = mean_ub; O.mA = mean_A; O.mb = mean_b;
+    rc = box_set_smem(k_box_backward, (size_t)plan->smem_bytes, g_bwd);
+    if (rc) return rc;
+    cudaStream_t st = (cudaStream_t)stream;
+    k_box_backward<<<nbatch, kBoxNT, (size_t)plan->smem_bytes, st>>>(D, q, sq, A, sA, dl_dzhat, zhat, lam, slacks, nus,
+                                                                     O, dxv, dlamv, dnuv);
+    rc = box_check_launch("k_box_backward");
+    if (rc) return rc;
+    const int TB = 128;
+    if (dq && mean_q) k_box_mean_vec<<<(n + TB - 1) / TB, TB, 0, st>>>(nbatch, n, dxv, n, zhat, 1.0, dq);
+    if (dp && mean_p) k_box_mean_vec<<<(n + TB - 1) / TB, TB, 0, st>>>(nbatch, n, dxv, n, nullptr, 1.0, dp);
+    if (dlb && mean_lb) k_box_mean_vec<<<(n + TB - 1) / TB, TB, 0, st>>>(nbatch, n, dlamv, m, nullptr, 1.0, dlb);
+    if (dub && mean_ub)
+        k_box_mean_vec<<<(n + TB - 1) / TB, TB, 0, st>>>(nbatch, n, dlamv + D.nlb, m, nullptr, -1.0, dub);
+    if (e > 0) {
+        if (dA && mean_A) k_box_mean_outer<<<dim3((n + TB - 1) / TB, e), TB, 0, st>>>(nbatch, e, n, dnuv, zhat, nus, dxv, dA);
+        if (db && mean_b) k_box_mean_vec<<<(e + TB - 1) / TB, TB, 0, st>>>(nbatch, e, dnuv, e, nullptr, -1.0, db);
+    }
+    return box_check_launch("k_box_mean");
+}
+
+int qpb200_box_solve_kkt(const qpb200_box_plan* plan, int nbatch, const double* q, int64_t sq, const double* A,
+                         int64_t sA, const double* d, const double* rx, const double* rs, const double* rz,
+                         const double* ry, double* dx, double* ds, double* dz, double* dy, void* stream) {
+    int rc = box_plan_check(plan);
+    if (rc) return rc;
+    if (nbatch <= 0 || !q || !d || !rx || !rs || !rz || !dx || !ds || !dz) return QPB200_ERR_BAD_ARG;
+    if (plan->neq > 0 && (!A || !ry || !dy)) return QPB200_ERR_BAD_ARG;
+    const BoxDims D = plan_dims(plan);
+    rc = box_set_smem(k_box_kkt, (size_t)plan->smem_bytes, g_kkt);
+    if (rc) return rc;
+    k_box_kkt<<<nbatch, kBoxNT, (size_t)plan->smem_bytes, (cudaStream_t)stream>>>(D, q, sq, A, sA, d, rx, rs, rz, ry,
+                                                                                   dx, ds, dz, dy);
+    return box_check_launch("k_box_kkt");
+}
+
+}  // extern "C"

@@ -176,36 +176,43 @@ def solve_forward(Q_, p_, G_, h_, A_, b_, eps=1e-12, verbose=0, notImprovedLim=3
             float(eps), float(STALL_TOL), float(BEST_TIE), int(notImprovedLim), int(maxIter),
             _ptr(st.zhat), _ptr(st.lam), _ptr(st.slacks), _ptr(st.nus),
             _ptr(st.iters), _ptr(st.best_resid), _ptr(st.trace), _ptr(st.scratch), _stream()))
-        # One host read for both diagnostics (the reference syncs many times per iteration):
-        # 'Q is not SPD.' (qp.py:81-85) and the inaccurate-solution banner, printed iff
-        # best resids max > 1 and verbose >= 0 (batch.py:141-142,205-206).
-        if check_Q_spd or verbose >= 0:
-            flags = torch.stack([spd.any(), (st.best_resid.max() > 1.)])
-            if LAZY_CHECKS:
-                # the two flags travel to a pinned host buffer asynchronously; they are examined (and 'Q is not SPD.' raised,
-                # the banner printed) at the next QPFunction call, in this call's backward, or by flush_checks()
-                host = torch.empty(2, dtype=flags.dtype).pin_memory()
-                host.copy_(flags, non_blocking=True)
-                ev = torch.cuda.Event()
-                ev.record()
-                _pending.append((ev, host, bool(check_Q_spd), verbose >= 0))
-            else:
-                bad_spd, inacc = flags.tolist()
-                if check_Q_spd and bad_spd:
-                    raise RuntimeError('Q is not SPD.')
-                if verbose >= 0 and inacc:
-                    print(INACC_ERR)
-        if verbose == 1:
-            # batch.py:115-117: per-iteration batch means; a QP that has already stopped contributes
-            # the values of its last iteration (in the reference every QP runs every iteration)
-            tr = st.trace.cpu()
-            for i in range(int(st.iters.max())):
-                row = tr[:, i, :]
-                last = tr[torch.arange(nBatch), (st.iters.cpu().long() - 1).clamp(min=0), :]
-                row = torch.where(torch.isnan(row), last, row)
-                print('iter: {}, pri_resid: {:.5e}, dual_resid: {:.5e}, mu: {:.5e}'.format(
-                    i, row[:, 0].mean(), row[:, 1].mean(), row[:, 2].mean()))
+        diagnostics(spd, st, check_Q_spd, verbose)
     return st
+
+
+def diagnostics(spd, st, check_Q_spd, verbose):
+    """After a forward: 'Q is not SPD.' from the device flags `spd`, the inaccurate-solution banner from st.best_resid,
+    and at verbose == 1 the per-iteration lines from st.trace / st.iters."""
+    # One host read for both diagnostics (the reference syncs many times per iteration):
+    # 'Q is not SPD.' (qp.py:81-85) and the inaccurate-solution banner, printed iff
+    # best resids max > 1 and verbose >= 0 (batch.py:141-142,205-206).
+    if check_Q_spd or verbose >= 0:
+        flags = torch.stack([spd.any(), (st.best_resid.max() > 1.)])
+        if LAZY_CHECKS:
+            # the two flags travel to a pinned host buffer asynchronously; they are examined (and 'Q is not SPD.' raised,
+            # the banner printed) at the next QPFunction call, in this call's backward, or by flush_checks()
+            host = torch.empty(2, dtype=flags.dtype).pin_memory()
+            host.copy_(flags, non_blocking=True)
+            ev = torch.cuda.Event()
+            ev.record()
+            _pending.append((ev, host, bool(check_Q_spd), verbose >= 0))
+        else:
+            bad_spd, inacc = flags.tolist()
+            if check_Q_spd and bad_spd:
+                raise RuntimeError('Q is not SPD.')
+            if verbose >= 0 and inacc:
+                print(INACC_ERR)
+    if verbose == 1:
+        # batch.py:115-117: per-iteration batch means; a QP that has already stopped contributes
+        # the values of its last iteration (in the reference every QP runs every iteration)
+        nBatch = st.iters.shape[0]
+        tr = st.trace.cpu()
+        for i in range(int(st.iters.max())):
+            row = tr[:, i, :]
+            last = tr[torch.arange(nBatch), (st.iters.cpu().long() - 1).clamp(min=0), :]
+            row = torch.where(torch.isnan(row), last, row)
+            print('iter: {}, pri_resid: {:.5e}, dual_resid: {:.5e}, mu: {:.5e}'.format(
+                i, row[:, 0].mean(), row[:, 1].mean(), row[:, 2].mean()))
 
 
 def solve_backward(st, dl_dzhat, mean_flags, want):
