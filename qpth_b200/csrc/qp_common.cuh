@@ -11,7 +11,7 @@ struct KDims {
     int lp;          // doubles in the packed lower factor L (rounded up to even)
     double reg;      // regularisation eps of the iterative-refinement KKT variant (batch.py:244-310); 0 on the QPFunction path
 };
-constexpr int kTabDoubles = 24;   // 96 uint16 tile-table entries for chol_v2
+constexpr int kTabDoubles = 24;   // 96 uint16 tile-table entries for f_chol (build_tile_table)
 
 __host__ __device__ inline int ld_for(int c) {
     int v = c < 4 ? 4 : c;
@@ -26,7 +26,8 @@ enum Vec {
 };
 constexpr int kRedDoubles = 4 * 32;
 
-// vector slots + reduction scratch + 2 mbarriers (16 B)
+// vector slots + reduction scratch + 2 mbarriers (16 B) + 24 unused doubles: the `fits` and `tiny` tests of
+// qpb200_plan_init are calibrated on this size, and shrinking it would move their boundaries
 __host__ __device__ inline size_t solve_vec_doubles(int vl) { return (size_t)V_COUNT * vl + kRedDoubles + 2 + 24; }
 
 // Global-scratch fallback of the K -> S copy (shared-memory mode uses one TMA bulk copy instead).

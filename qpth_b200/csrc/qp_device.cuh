@@ -132,15 +132,13 @@ __device__ __forceinline__ double tri_norm2_partial(const double* Lp, int n, con
 
 // Block-wide reductions of N values. `red` is shared scratch of >= N * kRedStride doubles (up to 16 warps).
 constexpr int kRedStride = 16;
-// Every thread returns with the reduced values. Two barriers per call (one with kGuard = false).
-template <int N, bool kMin, bool kGuard = true, int kStride = kRedStride>
+// Every thread returns with the reduced values. Two barriers per call.
+template <int N, bool kMin, int kStride = kRedStride>
 __device__ __forceinline__ void block_reduce(double (&v)[N], double* red, int tid, int nt) {
     const int lane = tid & 31, warp = tid >> 5, nw = nt >> 5;
 #pragma unroll
     for (int k = 0; k < N; ++k) v[k] = kMin ? warp_min(v[k]) : warp_sum(v[k]);
-    // protect scratch from the previous call's readers (kGuard = false: the caller alternates between two scratch areas,
-    // so the previous call's readers use the other one and the call before that is fenced by the previous call's barrier)
-    if (kGuard) __syncthreads();
+    __syncthreads();                                         // protect scratch from the previous call's readers
     if (lane == 0) {
 #pragma unroll
         for (int k = 0; k < N; ++k) red[k * kStride + warp] = v[k];
@@ -341,323 +339,18 @@ __device__ __forceinline__ void chol_partial(double* A, int ld, int nsq, int c0,
     }
 }
 
-// =============================================================================================
-// Cholesky v2 (shared-memory mode, nt == 256, at most 13 tile rows): register-resident trailing matrix.
-//   * warp 0 owns the diagonal 8x8 tiles, warps 1..7 the off-diagonal ones (column-major round robin), as DMMA
-//     accumulator fragments held in registers for the whole factorization: a panel update is 4 LDS + 2 DMMA
-//     per tile, no read-modify-write of the matrix in shared memory;
-//   * look-ahead: in the update phase of panel k warp 0 first brings diagonal tile k+1 up to date, factors it
-//     (and inverts it: T = L_kk^-1) while the other warps finish the trailing update;
-//   * the panel step is a multiplication by T (no substitution chain): row <- row * T^T;
-//   * the right-hand side rides along as one extra row (aug), so L^-1 rhs falls out of the factorization.
-// Storage on exit: L in the lower triangle of A, 1/diag in dinv, and the strictly-lower part of every
-// T = L_kk^-1 transposed into the (otherwise unused) upper part of its diagonal block.
-// =============================================================================================
-constexpr int kCholMaxTiles = 13;       // tile rows supported by chol_v2 (order <= 104)
-constexpr int kCholMaxOff = 13;         // off-diagonal tiles per update warp (6 or 7 update warps)
-
-// Factor the 8x8 diagonal block at (k0,k0) (nb valid rows/cols) redundantly in every lane of one warp,
-// invert it, and write L (lower), T^T (upper) and dinv.
-__device__ __forceinline__ void factor_diag8(double* A, int ld, int k0, int nb, double* dinv, int lane) {
-    double Lk[36], T[36], rinv[8];
-#pragma unroll
-    for (int r = 0; r < 8; ++r)
-#pragma unroll
-        for (int c = 0; c <= r; ++c)
-            Lk[QPB_LIDX(r, c)] = (r < nb && c < nb) ? A[(k0 + r) * ld + k0 + c] : (r == c ? 1.0 : 0.0);
-#pragma unroll
-    for (int c = 0; c < 8; ++c) {
-        const double piv = Lk[QPB_LIDX(c, c)];
-        const double ri = rsqrt(piv);
-        rinv[c] = ri;
-        Lk[QPB_LIDX(c, c)] = piv * ri;
-#pragma unroll
-        for (int r = c + 1; r < 8; ++r) Lk[QPB_LIDX(r, c)] *= ri;
-#pragma unroll
-        for (int r = c + 1; r < 8; ++r)
-#pragma unroll
-            for (int cc = c + 1; cc <= r; ++cc)
-                Lk[QPB_LIDX(r, cc)] = fma(-Lk[QPB_LIDX(r, c)], Lk[QPB_LIDX(cc, c)], Lk[QPB_LIDX(r, cc)]);
-    }
-#pragma unroll
-    for (int c = 0; c < 8; ++c) {
-        T[QPB_LIDX(c, c)] = rinv[c];
-#pragma unroll
-        for (int r = c + 1; r < 8; ++r) {
-            double sacc = 0.0;
-#pragma unroll
-            for (int j = c; j < r; ++j) sacc = fma(Lk[QPB_LIDX(r, j)], T[QPB_LIDX(j, c)], sacc);
-            T[QPB_LIDX(r, c)] = -rinv[r] * sacc;
-        }
-    }
-    int e = 0;
-#pragma unroll
-    for (int r = 0; r < 8; ++r)
-#pragma unroll
-        for (int c = 0; c <= r; ++c) {
-            if (r < nb && lane == (e & 31)) A[(k0 + r) * ld + k0 + c] = Lk[QPB_LIDX(r, c)];
-            ++e;
-        }
-#pragma unroll
-    for (int r = 1; r < 8; ++r)
-#pragma unroll
-        for (int c = 0; c < r; ++c) {
-            if (r < nb && lane == (e & 31)) A[(k0 + c) * ld + k0 + r] = T[QPB_LIDX(r, c)];
-            ++e;
-        }
-#pragma unroll
-    for (int c = 0; c < 8; ++c) {
-        if (c < nb && lane == (e & 31)) dinv[k0 + c] = rinv[c];
-        ++e;
-    }
-}
-
-// Load T = L_kk^-1 (8x8 lower, virtual identity beyond nb) from its transposed home in the upper triangle.
-__device__ __forceinline__ void load_T8(const double* A, int ld, int k0, int nb, const double* dinv, double (&T)[36]) {
-#pragma unroll
-    for (int r = 0; r < 8; ++r) {
-        T[QPB_LIDX(r, r)] = (r < nb) ? dinv[k0 + r] : 1.0;
-#pragma unroll
-        for (int c = 0; c < r; ++c) T[QPB_LIDX(r, c)] = (r < nb) ? A[(k0 + c) * ld + k0 + r] : 0.0;
-    }
-}
+// Tile table of the register-resident Cholesky f_chol (qp_fast.cuh).
+constexpr int kCholMaxTiles = 13;       // tile rows supported by f_chol (order <= 104)
+constexpr int kCholMaxOff = 13;         // off-diagonal tiles per update warp of f_chol (6 update warps)
 
 // tab[idx] = (ti << 8) | tj for the off-diagonal tiles (ti > tj) enumerated column by column.
-// The table holds 96 entries (kTabDoubles): orders above 13 tile rows never use it (generic kernels, chol_partial) and
-// must not write it (r2b: compute-sanitizer caught the overflow at ms = 128).
+// The table holds 96 entries (kTabDoubles): orders above 13 tile rows must not write it.
 __device__ __forceinline__ void build_tile_table(uint16_t* tab, int nts, int tid) {
     if (nts > kCholMaxTiles) return;
     if (tid < nts - 1) {
         const int tj = tid;
         const int base = tj * (nts - 1) - (tj * (tj - 1)) / 2;
         for (int ti = tj + 1; ti < nts; ++ti) tab[base + ti - tj - 1] = (uint16_t)((ti << 8) | tj);
-    }
-}
-
-// Factor columns [c0, n) of the n x n lower matrix A (columns < c0 already factored and applied), with the
-// right-hand side `aug` (length n) carried along. Requires blockDim.x == 256 and (n - c0 + 7)/8 <= 13.
-__device__ __forceinline__ void chol_v2(double* A, int ld, int n, int c0, double* aug, double* dinv,
-                                        const uint16_t* tab, int tid) {
-    const int lane = tid & 31, warp = tid >> 5;
-    const int g = lane >> 2, q = lane & 3;
-    const int nts = (n - c0 + 7) >> 3;
-    const int noff = (nts * (nts - 1)) / 2;
-    double C[kCholMaxTiles][2];
-    // ---- owned tiles -> registers
-    if (warp == 0) {
-#pragma unroll
-        for (int s = 0; s < kCholMaxTiles; ++s) {
-            const int r = c0 + 8 * s + g, cc = c0 + 8 * s + 2 * q;
-            const bool ok = s < nts && r < n;
-            C[s][0] = (ok && cc < n) ? A[r * ld + cc] : 0.0;
-            C[s][1] = (ok && cc + 1 < n) ? A[r * ld + cc + 1] : 0.0;
-        }
-        factor_diag8(A, ld, c0, min(8, n - c0), dinv, lane);
-    } else {
-#pragma unroll
-        for (int s = 0; s < kCholMaxOff; ++s) {
-            const int idx = s * 7 + warp - 1;
-            const bool have = idx < noff;
-            const int tt = have ? tab[idx] : 0;
-            const int r = c0 + 8 * (tt >> 8) + g, cc = c0 + 8 * (tt & 255) + 2 * q;
-            const bool ok = have && r < n;
-            C[s][0] = (ok && cc < n) ? A[r * ld + cc] : 0.0;
-            C[s][1] = (ok && cc + 1 < n) ? A[r * ld + cc + 1] : 0.0;
-        }
-    }
-    __syncthreads();
-    for (int k = 0; k < nts; ++k) {
-        const int k0 = c0 + 8 * k;
-        const int nb = min(8, n - k0);
-        // ---- phase A: panel rows below the diagonal block (and the aug row) times T^T
-        {
-            const int nbelow = n - k0 - nb;
-            if (tid <= nbelow) {
-                double T[36], a[8], o[8];
-                load_T8(A, ld, k0, nb, dinv, T);
-                double* rowp = (tid < nbelow) ? (A + (k0 + nb + tid) * ld + k0) : (aug + k0);
-#pragma unroll
-                for (int c = 0; c < 8; ++c) a[c] = (c < nb) ? rowp[c] : 0.0;
-#pragma unroll
-                for (int c = 0; c < 8; ++c) {
-                    double acc = a[c] * T[QPB_LIDX(c, c)];
-#pragma unroll
-                    for (int j = 0; j < c; ++j) acc = fma(a[j], T[QPB_LIDX(c, j)], acc);
-                    o[c] = acc;
-                }
-#pragma unroll
-                for (int c = 0; c < 8; ++c)
-                    if (c < nb) rowp[c] = o[c];
-            }
-        }
-        __syncthreads();
-        if (k + 1 >= nts) break;
-        // ---- phase B: trailing update with panel k (registers), look-ahead factorization of block k+1
-        if (warp == 0) {
-#pragma unroll
-            for (int s = 1; s < kCholMaxTiles; ++s) {
-                if (s == k + 1) {
-                    const int r = c0 + 8 * s + g;
-                    const bool ok = r < n;
-                    const double a0 = ok ? A[r * ld + k0 + q] : 0.0, a1 = ok ? A[r * ld + k0 + 4 + q] : 0.0;
-                    dmma884(C[s][0], C[s][1], -a0, a0);
-                    dmma884(C[s][0], C[s][1], -a1, a1);
-                    const int cc = c0 + 8 * s + 2 * q;
-                    if (ok && cc < n) A[r * ld + cc] = C[s][0];
-                    if (ok && cc + 1 < n) A[r * ld + cc + 1] = C[s][1];
-                }
-            }
-            __syncwarp();
-            factor_diag8(A, ld, k0 + 8, min(8, n - k0 - 8), dinv, lane);
-#pragma unroll
-            for (int s = 2; s < kCholMaxTiles; ++s) {
-                if (s > k + 1 && s < nts) {
-                    const int r = c0 + 8 * s + g;
-                    const bool ok = r < n;
-                    const double a0 = ok ? A[r * ld + k0 + q] : 0.0, a1 = ok ? A[r * ld + k0 + 4 + q] : 0.0;
-                    dmma884(C[s][0], C[s][1], -a0, a0);
-                    dmma884(C[s][0], C[s][1], -a1, a1);
-                }
-            }
-        } else {
-#pragma unroll
-            for (int s = 0; s < kCholMaxOff; ++s) {
-                const int idx = s * 7 + warp - 1;
-                if (idx < noff) {
-                    const int tt = tab[idx];
-                    const int ti = tt >> 8, tj = tt & 255;
-                    if (tj > k) {
-                        const int ra = c0 + 8 * ti + g, rb = c0 + 8 * tj + g;
-                        const bool aok = ra < n, bok = rb < n;
-                        const double a0 = aok ? A[ra * ld + k0 + q] : 0.0, a1 = aok ? A[ra * ld + k0 + 4 + q] : 0.0;
-                        const double b0 = bok ? A[rb * ld + k0 + q] : 0.0, b1 = bok ? A[rb * ld + k0 + 4 + q] : 0.0;
-                        dmma884(C[s][0], C[s][1], -a0, b0);
-                        dmma884(C[s][0], C[s][1], -a1, b1);
-                        if (tj == k + 1) {          // this tile belongs to the next panel: publish it
-                            const int cc = c0 + 8 * tj + 2 * q;
-                            if (aok && cc < n) A[ra * ld + cc] = C[s][0];
-                            if (aok && cc + 1 < n) A[ra * ld + cc + 1] = C[s][1];
-                        }
-                    }
-                }
-            }
-            if (warp == 7) {                        // right-hand side: aug[j] -= P[j][:] . y
-                double y[8];
-#pragma unroll
-                for (int c = 0; c < 8; ++c) y[c] = aug[k0 + c];
-                for (int j = k0 + 8 + lane; j < n; j += 32) {
-                    const double* pr = A + j * ld + k0;
-                    double acc = aug[j];
-#pragma unroll
-                    for (int c = 0; c < 8; ++c) acc = fma(-pr[c], y[c], acc);
-                    aug[j] = acc;
-                }
-            }
-        }
-        __syncthreads();
-    }
-}
-
-// Invert an ALREADY FACTORED 8x8 diagonal block in place of its upper triangle (T^T), every lane redundantly.
-__device__ __forceinline__ void invert_diag8(double* A, int ld, int k0, int nb, int lane) {
-    double Lk[36], T[36], rinv[8];
-#pragma unroll
-    for (int r = 0; r < 8; ++r)
-#pragma unroll
-        for (int c = 0; c <= r; ++c)
-            Lk[QPB_LIDX(r, c)] = (r < nb && c < nb) ? A[(k0 + r) * ld + k0 + c] : (r == c ? 1.0 : 0.0);
-#pragma unroll
-    for (int c = 0; c < 8; ++c) rinv[c] = 1.0 / Lk[QPB_LIDX(c, c)];
-#pragma unroll
-    for (int c = 0; c < 8; ++c) {
-        T[QPB_LIDX(c, c)] = rinv[c];
-#pragma unroll
-        for (int r = c + 1; r < 8; ++r) {
-            double sacc = 0.0;
-#pragma unroll
-            for (int j = c; j < r; ++j) sacc = fma(Lk[QPB_LIDX(r, j)], T[QPB_LIDX(j, c)], sacc);
-            T[QPB_LIDX(r, c)] = -rinv[r] * sacc;
-        }
-    }
-    int e = 0;
-#pragma unroll
-    for (int r = 1; r < 8; ++r)
-#pragma unroll
-        for (int c = 0; c < r; ++c) {
-            if (r < nb && lane == (e & 31)) A[(k0 + c) * ld + k0 + r] = T[QPB_LIDX(r, c)];
-            ++e;
-        }
-}
-
-// Triangular solves that use the inverted diagonal blocks left behind by chol_v2 / invert_diag8
-// (a block step is a product with T, not a substitution chain). Same contracts as trsv_fwd / trsv_bwd.
-__device__ __forceinline__ void trsv_fwd_T(const double* A, int ld, int n, int kbeg, int kend,
-                                           const double* dinv, double* b, double* u, int tid, int nt) {
-    for (int k0 = kbeg; k0 < kend; k0 += 8) {
-        const int nb = min(8, kend - k0);
-        const int nbelow = n - k0 - nb;
-        if (tid < nbelow || tid == 0) {
-            double T[36], r[8], y[8];
-            load_T8(A, ld, k0, nb, dinv, T);
-#pragma unroll
-            for (int c = 0; c < 8; ++c) r[c] = (c < nb) ? b[k0 + c] : 0.0;
-#pragma unroll
-            for (int c = 0; c < 8; ++c) {
-                double acc = r[c] * T[QPB_LIDX(c, c)];
-#pragma unroll
-                for (int j = 0; j < c; ++j) acc = fma(r[j], T[QPB_LIDX(c, j)], acc);
-                y[c] = acc;
-            }
-            if (tid == 0) {
-#pragma unroll
-                for (int c = 0; c < 8; ++c)
-                    if (c < nb) u[k0 + c] = y[c];
-            }
-            for (int t = tid; t < nbelow; t += nt) {
-                const double* rowp = A + (k0 + nb + t) * ld + k0;
-                double acc = b[k0 + nb + t];
-#pragma unroll
-                for (int c = 0; c < 8; ++c)
-                    if (c < nb) acc = fma(-rowp[c], y[c], acc);
-                b[k0 + nb + t] = acc;
-            }
-        }
-        __syncthreads();
-    }
-}
-
-__device__ __forceinline__ void trsv_bwd_T(const double* A, int ld, int n, const double* dinv, double* u,
-                                           double* w, int tid, int nt) {
-    const int nblk = (n + 7) >> 3;
-    for (int kb = nblk - 1; kb >= 0; --kb) {
-        const int k0 = kb * 8;
-        const int nb = min(8, n - k0);
-        if (tid < k0 || tid == 0) {
-            double T[36], r[8], y[8];
-            load_T8(A, ld, k0, nb, dinv, T);
-#pragma unroll
-            for (int c = 0; c < 8; ++c) r[c] = (c < nb) ? u[k0 + c] : 0.0;
-#pragma unroll
-            for (int c = 0; c < 8; ++c) {                     // y = T^T r
-                double acc = r[c] * T[QPB_LIDX(c, c)];
-#pragma unroll
-                for (int j = c + 1; j < 8; ++j) acc = fma(r[j], T[QPB_LIDX(j, c)], acc);
-                y[c] = acc;
-            }
-            if (tid == 0) {
-#pragma unroll
-                for (int c = 0; c < 8; ++c)
-                    if (c < nb) w[k0 + c] = y[c];
-            }
-            for (int i = tid; i < k0; i += nt) {
-                double acc = u[i];
-#pragma unroll
-                for (int c = 0; c < 8; ++c)
-                    if (c < nb) acc = fma(-A[(k0 + c) * ld + i], y[c], acc);
-                u[i] = acc;
-            }
-        }
-        __syncthreads();
     }
 }
 

@@ -86,38 +86,7 @@ __device__ __forceinline__ double f_rsqrt(double x) {
 }
 
 // In-register factorization of an 8x8 block (lower triangle in Lk): on exit strictly lower = L, diagonal = 1/L_cc.
-// Columns are eliminated in PAIRS: with a = A_cc, b = A_c+1,c, e = A_c+1,c+1 the second pivot is det / a,
-// det = a e - b^2, so 1/L_c+1,c+1 = rsqrt(det) * sqrt(a) and the two rsqrt (the longest link of the chain: MUFU +
-// 4 dependent fp64 ops) run side by side: ~100 cycles per pair instead of 2 x 72.
-#ifndef QPB_CHAIN_V2
-#define QPB_CHAIN_V2 0   // no gain in A/B runs, kept for reference
-#endif
 __device__ __forceinline__ void f_factor8_regs(double (&Lk)[36]) {
-#if QPB_CHAIN_V2
-#pragma unroll
-    for (int c = 0; c < 8; c += 2) {
-        const double a = Lk[QPB_LIDX(c, c)], b = Lk[QPB_LIDX(c + 1, c)], e = Lk[QPB_LIDX(c + 1, c + 1)];
-        const double r1 = f_rsqrt(a);
-        const double det = fma(a, e, -(b * b));
-        const double r2 = f_rsqrt(det) * (a * r1);
-        const double l10 = b * r1;
-        Lk[QPB_LIDX(c, c)] = r1;
-        Lk[QPB_LIDX(c + 1, c)] = l10;
-        Lk[QPB_LIDX(c + 1, c + 1)] = r2;
-#pragma unroll
-        for (int r = c + 2; r < 8; ++r) {
-            const double l1 = Lk[QPB_LIDX(r, c)] * r1;
-            Lk[QPB_LIDX(r, c)] = l1;
-            Lk[QPB_LIDX(r, c + 1)] = fma(-l1, l10, Lk[QPB_LIDX(r, c + 1)]) * r2;
-        }
-#pragma unroll
-        for (int r = c + 2; r < 8; ++r)
-#pragma unroll
-            for (int cc = c + 2; cc <= r; ++cc)
-                Lk[QPB_LIDX(r, cc)] = fma(-Lk[QPB_LIDX(r, c + 1)], Lk[QPB_LIDX(cc, c + 1)],
-                                          fma(-Lk[QPB_LIDX(r, c)], Lk[QPB_LIDX(cc, c)], Lk[QPB_LIDX(r, cc)]));
-    }
-#else
 #pragma unroll
     for (int c = 0; c < 8; ++c) {
         const double ri = f_rsqrt(Lk[QPB_LIDX(c, c)]);
@@ -130,23 +99,6 @@ __device__ __forceinline__ void f_factor8_regs(double (&Lk)[36]) {
             for (int cc = c + 1; cc <= r; ++cc)
                 Lk[QPB_LIDX(r, cc)] = fma(-Lk[QPB_LIDX(r, c)], Lk[QPB_LIDX(cc, c)], Lk[QPB_LIDX(r, cc)]);
     }
-#endif
-}
-// Row-scaled copy of a factored block, Ls[r][c] = L[r][c] / L[r][r] (c < r): with it the substitution
-// a <- a * L_kk^-T has ONE dependent FMA per entry instead of a multiply and an FMA (72 vs 140 cycles for 8).
-__device__ __forceinline__ void f_scale_rows8(const double (&Lk)[36], double (&Ls)[28]) {
-#pragma unroll
-    for (int r = 1; r < 8; ++r)
-#pragma unroll
-        for (int c = 0; c < r; ++c) Ls[QPB_LIDX(r - 1, c)] = Lk[QPB_LIDX(r, c)] * Lk[QPB_LIDX(r, r)];
-}
-__device__ __forceinline__ void f_row_solve8_scaled(double (&a)[8], const double (&Lk)[36], const double (&Ls)[28]) {
-#pragma unroll
-    for (int c = 0; c < 8; ++c) a[c] *= Lk[QPB_LIDX(c, c)];
-#pragma unroll
-    for (int c = 0; c < 8; ++c)
-#pragma unroll
-        for (int c2 = c + 1; c2 < 8; ++c2) a[c2] = fma(-a[c], Ls[QPB_LIDX(c2 - 1, c)], a[c2]);
 }
 __device__ __forceinline__ void f_store_lower8(double* Mb, int ld, const double (&Lk)[36]) {
 #pragma unroll
@@ -155,37 +107,6 @@ __device__ __forceinline__ void f_store_lower8(double* Mb, int ld, const double 
         for (int c = 0; c <= r; c += 2)      // the odd tail writes one element of the (unused) upper part
             *reinterpret_cast<double2*>(Mb + r * ld + c) =
                 make_double2(Lk[QPB_LIDX(r, c)], (c + 1 <= r) ? Lk[QPB_LIDX(r, c + 1)] : 0.0);
-}
-
-// Factor the 8x8 block at Mb redundantly in every lane of the calling warp; lane 0 writes it back
-// (strictly lower = L, diagonal = rsqrt(pivot)).
-__device__ __noinline__ void f_factor8(int Mb_off, int ld) {
-    QPB_SMEM;
-    double* Mb = qsm + Mb_off;
-    double Lk[36];
-    f_load_lower8(Mb, ld, Lk);
-    __syncwarp();
-#pragma unroll
-    for (int c = 0; c < 8; ++c) {
-        const double ri = rsqrt(Lk[QPB_LIDX(c, c)]);
-        Lk[QPB_LIDX(c, c)] = ri;
-#pragma unroll
-        for (int r = c + 1; r < 8; ++r) Lk[QPB_LIDX(r, c)] *= ri;
-#pragma unroll
-        for (int r = c + 1; r < 8; ++r)
-#pragma unroll
-            for (int cc = c + 1; cc <= r; ++cc)
-                Lk[QPB_LIDX(r, cc)] = fma(-Lk[QPB_LIDX(r, c)], Lk[QPB_LIDX(cc, c)], Lk[QPB_LIDX(r, cc)]);
-    }
-    if ((threadIdx.x & 31) == 0) {
-#pragma unroll
-        for (int r = 0; r < 8; ++r)
-#pragma unroll
-            for (int c = 0; c <= r; c += 2)      // the odd tail writes one element of the (unused) upper part
-                *reinterpret_cast<double2*>(Mb + r * ld + c) =
-                    make_double2(Lk[QPB_LIDX(r, c)], (c + 1 <= r) ? Lk[QPB_LIDX(r, c + 1)] : 0.0);
-    }
-    __syncwarp();
 }
 
 // a <- a * L_kk^-T by substitution (Lk: strictly lower = L, diagonal = reciprocal).
@@ -237,9 +158,6 @@ __device__ __noinline__ void f_chol_chain(int A, int ld, int n, int c0) {
     const int nts = (n - c0) >> 3;
     double* M = qsm + A;
     double Lk[36];                                           // the current diagonal block stays in registers
-#if QPB_CHAIN_V2
-    double Ls[28];                                           // its row-scaled copy (for s_k)
-#endif
     // k = -1 is the prologue step (F_0 only): ONE instance of the unrolled 8x8 factorization in the code.
     for (int k = -1; k < nts; ++k) {
         const int k0 = c0 + 8 * k;
@@ -249,11 +167,7 @@ __device__ __noinline__ void f_chol_chain(int A, int ld, int n, int c0) {
                 double a[8];
                 double* rowp = M + (k0 + 8 + lane) * ld + k0;
                 f_ld8(rowp, a);
-#if QPB_CHAIN_V2
-                f_row_solve8_scaled(a, Lk, Ls);
-#else
                 f_row_solve8(a, Lk);
-#endif
                 f_st8(rowp, a);
             }
             __syncwarp();
@@ -275,9 +189,6 @@ __device__ __noinline__ void f_chol_chain(int A, int ld, int n, int c0) {
             __syncwarp();                                                             // all lanes have read the tile
             f_factor8_regs(Lk);                                                       // F_{k+1}
             if (lane == 0) f_store_lower8(M + (k0 + 8) * ld + k0 + 8, ld, Lk);
-#if QPB_CHAIN_V2
-            f_scale_rows8(Lk, Ls);
-#endif
             if (k >= 0) QPB_TICK(80 + k);   // F_{k+1}, per step
         }
         QPB_TICK(26);
@@ -460,358 +371,6 @@ __device__ __noinline__ void f_trsv_bwd(int A, int ld, int n, int u, int w) {
     }
 }
 
-// ---- substitution on 16-row blocks with INVERTED diagonal blocks ---------------------------------------------
-// Round-1 accounting: the three substitutions of a Newton iteration were a large share of it,
-// 13 block steps each, every thread redoing the same 8 x 8 substitution chain (8 dependent mul+fma links) before its
-// own row update. Here the factorization is followed by f_invert16 (X_k = L_kk^-1 for the 16 x 16 diagonal blocks,
-// ~500 cycles, all blocks in parallel) and a block step becomes  y_k = X_k b_k  (a dot product per lane, every warp
-// computes it for itself: no barrier between it and the row update) followed by the row update: 7 steps instead of
-// 13, one block barrier per step, no dependent chain inside a step.
-// Storage: X_k's strictly lower part TRANSPOSED in the (otherwise unused) upper triangle of its diagonal block,
-// X_k[i][j] (i > j) at M[(k0 + j) * ld + k0 + i]; its diagonal is the reciprocal diagonal already there.
-#ifndef QPB_TRSV16
-#define QPB_TRSV16 0     // inversion + three solves were slower than the 8-row chain in A/B runs
-#endif
-
-// All 16 x 16 diagonal blocks of the factored n x n matrix at A (n multiple of 8, n <= 256). One half-warp per
-// block, lane c = column c of X_k by forward substitution held in registers. Call with all threads after the
-// factorization's last barrier; the caller synchronises afterwards.
-__device__ __noinline__ void f_invert16(int A, int ld, int n) {
-    QPB_SMEM;
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const int c = lane & 15;
-    const int blk = warp + (kNT / 32) * (lane >> 4);
-    const int k0 = 16 * blk;
-    if (k0 < n) {
-        const int bs = min(16, n - k0);
-        double* M = qsm + A + k0 * ld + k0;
-        double x[16];
-#pragma unroll
-        for (int i = 0; i < 16; ++i) {
-            const int ii = (i < bs) ? i : (bs - 1);          // (rows past a short last block: results discarded)
-            const double* Di = M + ii * ld;
-            double sacc = 0.0;
-#pragma unroll
-            for (int k = 0; k < i; k += 2) {
-                const double2 v = *reinterpret_cast<const double2*>(Di + k);
-                sacc = fma(v.x, x[k], sacc);
-                if (k + 1 < i) sacc = fma(v.y, x[k + 1], sacc);
-            }
-            const double di = Di[ii];
-            x[i] = (i == c) ? di : ((i > c && i < bs) ? -di * sacc : 0.0);
-        }
-        double* xr = M + c * ld;                             // row c of the block: X[i][c] goes to column i > c
-#pragma unroll
-        for (int i = 1; i < 16; ++i)
-            if (i > c && i < bs) xr[i] = x[i];
-    }
-}
-
-// L y = b over all blocks (u = y, b destroyed, b != u); ys: 16 doubles of scratch per warp.
-__device__ __noinline__ void f_trsv16_fwd(int A, int ld, int n, int b, int u, int ys) {
-    QPB_SMEM;
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const int c = lane & 15, hf = lane >> 4;
-    const double* M = qsm + A;
-    double* yw = qsm + ys + 16 * warp;
-#pragma unroll 1
-    for (int k0 = 0; k0 < n; k0 += 16) {
-        const int bs = min(16, n - k0);
-        // (a) y_k = X_k b_k, every warp for itself: lane (c, hf) sums j in [8 hf, 8 hf + 8), j <= c
-        {
-            const double* Xc = M + k0 * ld + k0 + c;         // X[c][j] at Xc[j * ld]  (j <= c; j == c: the diagonal)
-            const double* bk = qsm + b + k0 + 8 * hf;
-            double s0 = 0.0, s1 = 0.0;
-#pragma unroll
-            for (int jj = 0; jj < 8; jj += 2) {
-                const int j = 8 * hf + jj;
-                const double2 bv = *reinterpret_cast<const double2*>(bk + jj);
-                const double x0 = (j <= c && c < bs) ? Xc[j * ld] : 0.0;
-                const double x1 = (j + 1 <= c && c < bs) ? Xc[(j + 1) * ld] : 0.0;
-                s0 = fma(x0, (j <= c && c < bs) ? bv.x : 0.0, s0);
-                s1 = fma(x1, (j + 1 <= c && c < bs) ? bv.y : 0.0, s1);
-            }
-            double y = s0 + s1;
-            y += __shfl_xor_sync(0xffffffffu, y, 16);
-            if (hf == 0) {
-                yw[c] = y;
-                if (warp == 0 && c < bs) qsm[u + k0 + c] = y;
-            }
-        }
-        __syncwarp();
-        // (b) rows below the block: b_i -= L[i][k0 .. k0+15] . y_k, two lanes per row (8 columns each)
-        if (bs == 16) {
-            const int pr = tid & 1;
-#pragma unroll 1
-            for (int ib = k0 + 16; ib < n; ib += kNT / 2) {                // block-uniform trip count (shuffle inside)
-                const int i = ib + (tid >> 1);
-                const bool ok = i < n;
-                const double* Li = M + (ok ? i : k0) * ld + k0 + 8 * pr;
-                const double* yy = yw + 8 * pr;
-                double s0 = 0.0, s1 = 0.0;
-#pragma unroll
-                for (int jj = 0; jj < 8; jj += 2) {
-                    const double2 lv = *reinterpret_cast<const double2*>(Li + jj);
-                    const double2 yv = *reinterpret_cast<const double2*>(yy + jj);
-                    s0 = fma(lv.x, yv.x, s0);
-                    s1 = fma(lv.y, yv.y, s1);
-                }
-                double sacc = s0 + s1;
-                sacc += __shfl_xor_sync(0xffffffffu, sacc, 1);
-                if (ok && pr == 0) qsm[b + i] -= sacc;
-            }
-        }
-        __syncthreads();
-    }
-}
-
-// L^T w = u over all blocks (u destroyed, u != w).
-__device__ __noinline__ void f_trsv16_bwd(int A, int ld, int n, int u, int w, int ys) {
-    QPB_SMEM;
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const int c = lane & 15, hf = lane >> 4;
-    const double* M = qsm + A;
-    double* yw = qsm + ys + 16 * warp;
-#pragma unroll 1
-    for (int k0 = ((n - 1) >> 4) << 4; k0 >= 0; k0 -= 16) {
-        const int bs = min(16, n - k0);
-        // (a) w_k = X_k^T u_k: w_c = sum_{i >= c} X[i][c] u_i, X[i][c] at row (k0 + c), column k0 + i (contiguous in i)
-        {
-            const double* Xr = M + (k0 + c) * ld + k0 + 8 * hf;
-            const double* uk = qsm + u + k0 + 8 * hf;
-            double s0 = 0.0, s1 = 0.0;
-            if (c < bs) {
-#pragma unroll
-                for (int jj = 0; jj < 8; jj += 2) {
-                    const int i = 8 * hf + jj;
-                    if (i + 1 >= c && i < bs) {              // (bs is a multiple of 8: i < bs covers i + 1 too)
-                        const double2 xv = *reinterpret_cast<const double2*>(Xr + jj);
-                        const double2 uv = *reinterpret_cast<const double2*>(uk + jj);
-                        s0 = fma((i >= c) ? xv.x : 0.0, (i >= c) ? uv.x : 0.0, s0);
-                        s1 = fma(xv.y, uv.y, s1);
-                    }
-                }
-            }
-            double y = s0 + s1;
-            y += __shfl_xor_sync(0xffffffffu, y, 16);
-            if (hf == 0) {
-                yw[c] = (c < bs) ? y : 0.0;
-                if (warp == 0 && c < bs) qsm[w + k0 + c] = y;
-            }
-        }
-        __syncwarp();
-        // (b) rows above the block: u_i -= sum_c L[k0 + c][i] w_c, two lanes per row (8 block rows each)
-        {
-            const int pr = tid & 1;
-#pragma unroll 1
-            for (int ib = 0; ib < k0; ib += kNT / 2) {                     // block-uniform trip count (shuffle inside)
-                const int i = ib + (tid >> 1);
-                const bool ok = i < k0;
-                const double* Lc = M + (k0 + 8 * pr) * ld + (ok ? i : 0);
-                const double* yy = yw + 8 * pr;
-                double s0 = 0.0, s1 = 0.0;
-                if (8 * pr < bs) {
-#pragma unroll
-                    for (int jj = 0; jj < 8; jj += 2) {
-                        s0 = fma(Lc[jj * ld], yy[jj], s0);
-                        s1 = fma(Lc[(jj + 1) * ld], yy[jj + 1], s1);
-                    }
-                }
-                double sacc = s0 + s1;
-                sacc += __shfl_xor_sync(0xffffffffu, sacc, 1);
-                if (ok && pr == 0) qsm[u + i] -= sacc;
-            }
-        }
-        __syncthreads();
-    }
-}
-
-// ---- product form of the factor: substitution without an intra-block chain -------------------------------
-// f_to_pform rewrites a factored matrix (diagonal blocks: strictly lower = L, diagonal = 1/L_cc) as
-//   T_k  = L_kk^-1      strictly lower part stored TRANSPOSED in the upper triangle of diagonal tile k
-//                       (T_k[j][c] at tile[c][j], j > c; its diagonal is the reciprocal diagonal already there),
-//   P_ik = L_ik T_k     in place of every tile below the diagonal.
-// Then   L y = b   :  y_k = T_k b_k,  b_i -= P_ik b_k  (b = running right-hand side), and
-//        L^T w = u :  u'_k = T_k^T u_k,  w_k = u'_k - sum_{i>k} P_ik^T w_i,
-// i.e. one 8-term dot product per thread and block step; the 8-long substitution chain of f_trsv_* (8 x (mul + fma)
-// dependent, redone by every thread) is gone and y_k is off the critical path. Costs one pass over the factor
-// (36 FMAs per row and block) per factorization; pays for itself with the three solves that follow.
-#ifndef QPB_PFORM
-#define QPB_PFORM 0      // in A/B runs the conversion pass cost what the chain-free solves saved
-#endif
-
-// Upper triangle incl. diagonal of the 8x8 tile at Mb: T[QPB_LIDX(j, c)] = Mb[c][j], j >= c  (= T_k[j][c]).
-__device__ __forceinline__ void f_load_upper8(const double* Mb, int ld, double (&T)[36]) {
-#pragma unroll
-    for (int c = 0; c < 8; ++c)
-#pragma unroll
-        for (int j = c & ~1; j < 8; j += 2) {
-            const double2 v = *reinterpret_cast<const double2*>(Mb + c * ld + j);
-            if (j >= c) T[QPB_LIDX(j, c)] = v.x;
-            T[QPB_LIDX(j + 1, c)] = v.y;
-        }
-}
-
-// All blocks of the n x n factor at A (n multiple of 8, n <= 8 * 32). Call with all threads; ends with a barrier.
-__device__ __noinline__ void f_to_pform(int A, int ld, int n) {
-    QPB_SMEM;
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    double* M = qsm + A;
-    const int nts = n >> 3;
-    // (i) T_k: 8 lanes per diagonal block, lane c computes column c of T_k (zeros above the diagonal of T).
-    // Reads touch the lower triangle only, writes the strictly upper one: no hazard between the lanes of a block.
-    if (tid < 8 * nts) {
-        const int k0 = tid & ~7, c = tid & 7;
-        double* Mb = M + k0 * ld + k0;
-        double Lk[36], Tc[8];
-#pragma unroll
-        for (int r = 0; r < 8; ++r)
-#pragma unroll
-            for (int cc = 0; cc <= r; cc += 2) {
-                if (cc + 1 <= r) {
-                    const double2 v = *reinterpret_cast<const double2*>(Mb + r * ld + cc);
-                    Lk[QPB_LIDX(r, cc)] = v.x; Lk[QPB_LIDX(r, cc + 1)] = v.y;
-                } else {
-                    Lk[QPB_LIDX(r, cc)] = Mb[r * ld + cc];
-                }
-            }
-#pragma unroll
-        for (int r = 0; r < 8; ++r) {
-            double sacc = 0.0;
-#pragma unroll
-            for (int j = 0; j < r; ++j) sacc = fma(Lk[QPB_LIDX(r, j)], Tc[j], sacc);
-            Tc[r] = (r < c) ? 0.0 : ((r == c) ? Lk[QPB_LIDX(r, r)] : -Lk[QPB_LIDX(r, r)] * sacc);
-        }
-#pragma unroll
-        for (int r = 1; r < 8; ++r)
-            if (r > c) Mb[c * ld + r] = Tc[r];
-    }
-    __syncthreads();
-    QPB_TICK(17);   // T_k blocks
-    // (ii) P_ik = L_ik T_k on the fp64 tensor pipe: one 8x8 tile = 2 DMMAs, tiles dealt round-robin to the warps.
-    // (The FMA version - one row per lane, T_k reloaded per work item - was LSU-bound.)
-    {
-        const int g = lane >> 2, q = lane & 3;
-        int item = 0;
-        const double zero = (double)(n >> 20);               // 0.0 the compiler cannot fold: the accumulator is a register, not RZ
-#pragma unroll 1
-        for (int k = 0; k + 1 < nts; ++k) {
-            const int k0 = 8 * k;
-            const double* Tb = M + (k0 + g) * ld + k0;                         // row g of diagonal tile k
-            // B fragment: T_k[kk][g], kk = q (slice 0), q + 4 (slice 1); T_k[kk][nn] = tile[nn][kk] for kk >= nn
-            const double b0 = (q >= g) ? Tb[q] : 0.0, b1 = (q + 4 >= g) ? Tb[q + 4] : 0.0;
-#pragma unroll 1
-            for (int ti = k + 1; ti < nts; ++ti, ++item) {
-                if ((item & 7) != warp) continue;
-                double* rowp = M + (8 * ti + g) * ld + k0;
-                const double a0 = rowp[q], a1 = rowp[q + 4];
-                double d0 = zero, d1 = zero;                                 // (a register, not RZ: see `zero` above)
-                dmma884(d0, d1, a0, b0);
-                dmma884(d0, d1, a1, b1);
-                *reinterpret_cast<double2*>(rowp + 2 * q) = make_double2(d0, d1);
-            }
-            if (k == 0) QPB_TICK(29);   // first block column (12 of the 78 tiles)
-        }
-    }
-    QPB_TICK(25);   // P conversion, before its barrier
-    __syncthreads();
-}
-
-// L y = b over ALL blocks of a product-form factor: u = y. Thread tid owns entry tid of the running right-hand
-// side in a register; a block of 8 entries is published to b[] when it becomes final, and y_k = T_k b_k is taken
-// for all blocks at once after the sweep (the b_k stay in place). b destroyed, b != u. One barrier per block
-// step; the P row of the NEXT step is fetched before it.
-// (First version: 8 "solver" threads computed y_k inside every step - 8 dependent LDS->FMA links, longer than the
-// row update it was supposed to hide behind.)
-__device__ __noinline__ void f_ptrsv_fwd(int A, int ld, int n, int b, int u) {
-    QPB_SMEM;
-    const int tid = threadIdx.x;
-    const double* M = qsm + A;
-    const bool mine = tid >= 8 && tid < n;
-    double acc = mine ? qsm[b + tid] : 0.0;
-    double row[8];
-    if (mine) f_ld8(M + tid * ld, row);
-#pragma unroll 1
-    for (int k0 = 0; k0 + 8 < n; k0 += 8) {
-        if (tid >= k0 + 8 && tid < n) {
-            double y[8];
-            f_ld8(qsm + b + k0, y);
-            double s1 = row[1] * y[1];
-            acc = fma(-row[0], y[0], acc); s1 = fma(row[3], y[3], s1);
-            acc = fma(-row[2], y[2], acc); s1 = fma(row[5], y[5], s1);
-            acc = fma(-row[4], y[4], acc); s1 = fma(row[7], y[7], s1);
-            acc = fma(-row[6], y[6], acc);
-            acc -= s1;
-            if (tid < k0 + 16) qsm[b + tid] = acc;
-            else f_ld8(M + tid * ld + k0 + 8, row);          // next step's P row (static data: no hazard)
-        }
-        __syncthreads();
-    }
-    QPB_TICK(27);   // ptrsv_fwd sweep
-    if (tid < n) {                                           // y = blockdiag(T_k) b: T_k[r][c] = tile[c][r], c <= r
-        const int k0 = tid & ~7, r = tid & 7;
-        double y[8], t[8];
-        f_ld8(qsm + b + k0, y);
-        const double* Tb = M + k0 * ld + k0 + r;
-#pragma unroll
-        for (int c = 0; c < 8; ++c) t[c] = Tb[c * ld];       // column r of the tile (rows > r hold L: masked below)
-        double s0 = 0.0, s1 = 0.0;
-#pragma unroll
-        for (int c = 0; c < 8; c += 2) {
-            s0 = fma((c <= r) ? t[c] : 0.0, y[c], s0);
-            s1 = fma((c + 1 <= r) ? t[c + 1] : 0.0, y[c + 1], s1);
-        }
-        qsm[u + tid] = s0 + s1;
-    }
-    __syncthreads();
-}
-
-// L^T w = u for a product-form factor. Thread tid owns w[tid]. u is only read. u != w.
-__device__ __noinline__ void f_ptrsv_bwd(int A, int ld, int n, int u, int w) {
-    QPB_SMEM;
-    const int tid = threadIdx.x;
-    const double* M = qsm + A;
-    double acc = 0.0;
-    if (tid < n) {                                           // u'_k = T_k^T u_k: row c of the (upper-stored) tile
-        const int k0 = tid & ~7, c = tid & 7;
-        double t[8], uu[8];
-        f_ld8(M + (k0 + c) * ld + k0, t);
-        f_ld8(qsm + u + k0, uu);
-        double s1 = 0.0;
-#pragma unroll
-        for (int r = 0; r < 8; r += 2) {
-            acc = fma((r >= c) ? t[r] : 0.0, uu[r], acc);
-            s1 = fma((r + 1 >= c) ? t[r + 1] : 0.0, uu[r + 1], s1);
-        }
-        acc += s1;
-        if (tid >= n - 8) qsm[w + tid] = acc;
-    }
-    double col[8];
-    if (tid < n - 8) {
-#pragma unroll
-        for (int c = 0; c < 8; ++c) col[c] = M[(n - 8 + c) * ld + tid];
-    }
-    __syncthreads();
-    for (int k0 = n - 8; k0 > 0; k0 -= 8) {
-        if (tid < k0) {
-            double y[8];
-            f_ld8(qsm + w + k0, y);
-            double s1 = col[1] * y[1];
-            acc = fma(-col[0], y[0], acc); s1 = fma(col[3], y[3], s1);
-            acc = fma(-col[2], y[2], acc); s1 = fma(col[5], y[5], s1);
-            acc = fma(-col[4], y[4], acc); s1 = fma(col[7], y[7], s1);
-            acc = fma(-col[6], y[6], acc);
-            acc -= s1;
-            if (tid >= k0 - 8) qsm[w + tid] = acc;
-            else {
-#pragma unroll
-                for (int c = 0; c < 8; ++c) col[c] = M[(k0 - 8 + c) * ld + tid];
-            }
-        }
-        __syncthreads();
-    }
-}
-
 // Invert a factored 8x8 diagonal block (strictly lower = L, diagonal = 1/L_cc): T = L_kk^-1. T's strictly
 // lower part is written TRANSPOSED into the (unused) upper triangle of the block; its diagonal is the
 // reciprocal diagonal already there. One lane does the work (pre_factor_kkt only; off the Newton loop).
@@ -931,56 +490,6 @@ __device__ __noinline__ void f_matvec_rows2(int W, int ld, int rows, int cols, i
 __device__ __noinline__ void f_matvec_rows1(int W, int ld, int rows, int cols, int x1, int y1) {
     f_matvec_rows_impl<false>(W, ld, rows, cols, x1, 0, y1, 0);
 }
-#ifndef QPB_MVCOLS2
-#define QPB_MVCOLS2 0    // A/B knob: 1 = f_matvec_cols with two columns per thread (LDS.128) and as many row groups as fit
-#endif
-#if QPB_MVCOLS2
-// out[c] = sa * a[c] + sgn * (W^T v)[c] (+ b[c] if b >= 0). A warp owns 16 columns: lane = (row group g, column pair cq),
-// one LDS.128 per row (a quarter-warp reads 128 contiguous bytes: no bank conflicts), the four row groups are summed with
-// two shuffles. Half the shared-memory loads of the one-column-per-thread version and no partial-sum vectors (p0, p1 unused).
-__device__ __noinline__ void f_matvec_cols(int W, int ld, int rows, int cols, int v, int p0, int p1, int out,
-                                           int a, double sa, int b, double sgn) {
-    QPB_SMEM;
-    (void)p0; (void)p1;
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, g = lane >> 3, cq = lane & 7;
-#pragma unroll 1
-    for (int c0 = 0; c0 < cols; c0 += 16 * (kNT / 32)) {     // warp-uniform trip count
-        const int c = c0 + 16 * warp + 2 * cq;
-        const bool okc = c < cols;
-        const double* Wp = qsm + W + (okc ? c : 0);
-        double s0 = 0.0, s1 = 0.0, t0 = 0.0, t1 = 0.0;
-        int r = g;
-#pragma unroll 2
-        for (; r + 4 < rows; r += 8) {
-            const double2 w0 = *reinterpret_cast<const double2*>(Wp + r * ld);
-            const double2 w1 = *reinterpret_cast<const double2*>(Wp + (r + 4) * ld);
-            const double v0 = qsm[v + r], v1 = qsm[v + r + 4];
-            s0 = fma(w0.x, v0, s0); s1 = fma(w0.y, v0, s1);
-            t0 = fma(w1.x, v1, t0); t1 = fma(w1.y, v1, t1);
-        }
-        if (r < rows) {
-            const double2 w0 = *reinterpret_cast<const double2*>(Wp + r * ld);
-            const double v0 = qsm[v + r];
-            s0 = fma(w0.x, v0, s0); s1 = fma(w0.y, v0, s1);
-        }
-        s0 += t0; s1 += t1;
-        __syncwarp();
-        s0 += __shfl_xor_sync(0xffffffffu, s0, 8);  s1 += __shfl_xor_sync(0xffffffffu, s1, 8);
-        s0 += __shfl_xor_sync(0xffffffffu, s0, 16); s1 += __shfl_xor_sync(0xffffffffu, s1, 16);
-        if (g == 0 && okc) {
-            double r0 = sa * qsm[a + c] + sgn * s0;
-            if (b >= 0) r0 += qsm[b + c];
-            qsm[out + c] = r0;
-            if (c + 1 < cols) {
-                double r1 = sa * qsm[a + c + 1] + sgn * s1;
-                if (b >= 0) r1 += qsm[b + c + 1];
-                qsm[out + c + 1] = r1;
-            }
-        }
-    }
-    __syncthreads();
-}
-#else
 // out[c] = a[c] + sgn * (W^T v)[c] (+ b[c] if b >= 0). Two row groups, partial sums in p0/p1.
 __device__ __noinline__ void f_matvec_cols(int W, int ld, int rows, int cols, int v, int p0, int p1, int out,
                                            int a, double sa, int b, double sgn) {
@@ -1017,8 +526,6 @@ __device__ __noinline__ void f_matvec_cols(int W, int ld, int rows, int cols, in
     __syncthreads();
 }
 
-#endif
-
 // End of a Newton iteration, column c: dx~ = -r~x - (W^T dv)_c, x~ += alpha dx~, r~x = x~ + (W^T v)_c + p~
 // (each with the rounding of the separate passes it replaces).
 __device__ __forceinline__ void f_cols2_out(int c, double wdv, double wv, int xt, int rxt, int pt, double alpha) {
@@ -1028,7 +535,7 @@ __device__ __forceinline__ void f_cols2_out(int c, double wdv, double wv, int xt
     qsm[xt + c] = x;
     qsm[rxt + c] = (x + wv) + qsm[pt + c];
 }
-// W^T dv and W^T v side by side (each W element read once) with the row split and summation order of the default
+// W^T dv and W^T v side by side (each W element read once) with the row split and summation order of
 // f_matvec_cols; partial sums in p0/p1 (dv) and p2/p3 (v). Ends with a block barrier.
 __device__ __noinline__ void f_matvec_cols2(int W, int ld, int rows, int cols, int dv, int v, int p0, int p1, int p2,
                                             int p3, int xt, int rxt, int pt, double alpha) {
@@ -1310,21 +817,18 @@ __device__ __noinline__ double g_tri_norm2(const double* __restrict__ Lg, int n,
     return acc;
 }
 
-#ifndef QPB_RED1
-#define QPB_RED1 0       // A/B knob: 1 = one barrier per block reduction (callers alternate between two scratch halves)
-#endif
 constexpr int kFastStride = (kNT / 32 <= 8) ? 8 : 16;       // per-value stride of the fast kernels' reduction scratch
 __device__ __noinline__ void f_reduce_sum4(double (&v)[4], int red) {
     QPB_SMEM;
-    block_reduce<4, false, !QPB_RED1, kFastStride>(v, qsm + red, (int)threadIdx.x, kNT);
+    block_reduce<4, false, kFastStride>(v, qsm + red, (int)threadIdx.x, kNT);
 }
 __device__ __noinline__ void f_reduce_sum2(double (&v)[2], int red) {
     QPB_SMEM;
-    block_reduce<2, false, !QPB_RED1, kFastStride>(v, qsm + red, (int)threadIdx.x, kNT);
+    block_reduce<2, false, kFastStride>(v, qsm + red, (int)threadIdx.x, kNT);
 }
 __device__ __noinline__ void f_reduce_min2(double (&v)[2], int red) {
     QPB_SMEM;
-    block_reduce<2, true, !QPB_RED1, kFastStride>(v, qsm + red, (int)threadIdx.x, kNT);
+    block_reduce<2, true, kFastStride>(v, qsm + red, (int)threadIdx.x, kNT);
 }
 
 }  // namespace fast

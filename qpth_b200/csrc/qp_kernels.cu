@@ -37,24 +37,6 @@ constexpr int kThreads = 256;
 constexpr int kTinyThreads = 32;        // tiny problems: one warp per QP (generic shared-memory kernels, 32-thread CTAs)
 constexpr int kTinyCtasPerSm = 16;
 constexpr int kTinyMax = 32;            // nz and ms_pad up to this size take the one-warp-per-QP path
-#ifndef QPB_COOP_DEFAULT
-#define QPB_COOP_DEFAULT 0     // the co-resident kernels lost in A/B runs (128-register cap spills
-                               // the register-resident Cholesky, L2 passes cost 3x the shared-memory ones); opt-in only
-#endif
-constexpr int kCoopDefault = QPB_COOP_DEFAULT;
-#ifndef QPB_TINY_DEFAULT
-#define QPB_TINY_DEFAULT 1
-#endif
-constexpr int kTinyDefault = QPB_TINY_DEFAULT;
-#ifndef QPB_PF_DEFAULT
-#define QPB_PF_DEFAULT 1       // product-form kernels: 0 = only for shapes without a fast kernel, 1 = wherever they fit
-                               // (never slower than the round-1 kernels in A/B runs at C2, C3 and C4)
-#endif
-constexpr int kPfDefault = QPB_PF_DEFAULT;
-#ifndef QPB_PF_TWO_DEFAULT
-#define QPB_PF_TWO_DEFAULT 0   // 1: prefer the two-QPs-per-SM product-form kernels (W, L from L2) where they fit
-#endif
-constexpr int kPfTwoDefault = QPB_PF_TWO_DEFAULT;
 constexpr int kMaxSmem = 232448 - 1024;   // 227 KB opt-in limit per CTA on sm_90, minus static smem slack
 
 }  // namespace
@@ -194,7 +176,6 @@ struct Ctx {
     double* vec;        // vector slots
     double* red;        // reduction scratch
     uint64_t* bar;      // [0]: W + L staged, [1]: K -> LS copies       (shared-memory mode only)
-    uint16_t* tab;      // chol_v2 tile table
     const double* Kg;   // K template in global memory (row stride lds)
     uint32_t kphase;    // parity of the next K copy completion
     bool kpending;
@@ -245,14 +226,12 @@ __device__ __forceinline__ Ctx make_ctx(const KDims& D, double* smem, double* gs
         c.vec = Lp + D.lp;
         c.red = c.vec + (size_t)V_COUNT * D.vl;
         c.bar = reinterpret_cast<uint64_t*>(c.red + kRedDoubles);
-        c.tab = reinterpret_cast<uint16_t*>(c.red + kRedDoubles + 2);
         c.W = W;
         c.Lp = Lp;
         if (tid == 0) {
             mbar_init(c.bar, 1);
             mbar_init(c.bar + 1, 1);
         }
-        build_tile_table(c.tab, (D.ms - D.ep + 7) >> 3, tid);
         __syncthreads();
         if (tid < 32) {
             const uint32_t wb = (uint32_t)(D.ms * D.ldw * 8), lb = (uint32_t)(D.lp * 8);
@@ -270,7 +249,6 @@ __device__ __forceinline__ Ctx make_ctx(const KDims& D, double* smem, double* gs
         c.vec = smem;
         c.red = c.vec + (size_t)V_COUNT * D.vl;
         c.bar = nullptr;
-        c.tab = nullptr;
         c.kpending = true;
     }
     return c;
@@ -280,7 +258,7 @@ __device__ __forceinline__ Ctx make_ctx(const KDims& D, double* smem, double* gs
 
 // factor_kkt + the forward half of solve_kkt: on entry V_AUG holds -h_full (length ms) and V_D holds d.
 // On exit V_W holds w = -S^-1 h_full. Destroys V_AUG, V_T0.
-template <bool kSmem, bool kV2>
+template <bool kSmem>
 __device__ __forceinline__ void factor_and_solve(const KDims& D, Ctx& C, int tid, int nt) {
     double* aug = VEC(V_AUG);
     wait_K<kSmem>(D, C, tid, nt);
@@ -289,32 +267,20 @@ __device__ __forceinline__ void factor_and_solve(const KDims& D, Ctx& C, int tid
     const FullIdx at{D.lds};
     if (D.ep > 0) {
         // equality block: forward-substitute the first ep entries with the pre-factored L11 / L21
-        if (kV2) trsv_fwd_T(C.LS, D.lds, D.ms, 0, D.ep, VEC(V_DINV), aug, VEC(V_T0), tid, nt);
-        else trsv_fwd(C.LS, at, D.ms, 0, D.ep, VEC(V_DINV), aug, VEC(V_T0), tid, nt);
+        trsv_fwd(C.LS, at, D.ms, 0, D.ep, VEC(V_DINV), aug, VEC(V_T0), tid, nt);
         for (int i = tid; i < D.ep; i += nt) aug[i] = VEC(V_T0)[i];
         __syncthreads();
     }
-    if (kV2) {
-        chol_v2(C.LS, D.lds, D.ms, D.ep, aug, VEC(V_DINV), C.tab, tid);
-        trsv_bwd_T(C.LS, D.lds, D.ms, VEC(V_DINV), aug, VEC(V_W), tid, nt);
-    } else {
-        chol_partial(C.LS, D.lds, D.ms, D.ep, D.ms, aug, 0, 1, VEC(V_DINV), nullptr, tid, nt);
-        trsv_bwd(C.LS, at, D.ms, VEC(V_DINV), aug, VEC(V_W), tid, nt);
-    }
+    chol_partial(C.LS, D.lds, D.ms, D.ep, D.ms, aug, 0, 1, VEC(V_DINV), nullptr, tid, nt);
+    trsv_bwd(C.LS, at, D.ms, VEC(V_DINV), aug, VEC(V_W), tid, nt);
 }
 
 // Solve with the factor already in LS: rhs in V_T1 (destroyed) -> result in `out`.
-template <bool kV2>
 __device__ __forceinline__ void solve_with_factor(const KDims& D, const Ctx& C, double* out, int tid,
                                                   int nt) {
-    if (kV2) {
-        trsv_fwd_T(C.LS, D.lds, D.ms, 0, D.ms, VEC(V_DINV), VEC(V_T1), VEC(V_T0), tid, nt);
-        trsv_bwd_T(C.LS, D.lds, D.ms, VEC(V_DINV), VEC(V_T0), out, tid, nt);
-    } else {
-        const FullIdx at{D.lds};
-        trsv_fwd(C.LS, at, D.ms, 0, D.ms, VEC(V_DINV), VEC(V_T1), VEC(V_T0), tid, nt);
-        trsv_bwd(C.LS, at, D.ms, VEC(V_DINV), VEC(V_T0), out, tid, nt);
-    }
+    const FullIdx at{D.lds};
+    trsv_fwd(C.LS, at, D.ms, 0, D.ms, VEC(V_DINV), VEC(V_T1), VEC(V_T0), tid, nt);
+    trsv_bwd(C.LS, at, D.ms, VEC(V_DINV), VEC(V_T0), out, tid, nt);
 }
 
 // x~ = L^-1 x: V_T1 (destroyed) -> dst.  x = L^-T x~: u (destroyed) -> out.
@@ -334,7 +300,7 @@ __device__ __forceinline__ void load_dinvs(const KDims& D, const Ctx& C, int tid
 // ---------------------------------------------------------------------------------------------
 // k_forward: the PDIPM loop (batch.py:47-207), per-QP semantics.
 // ---------------------------------------------------------------------------------------------
-template <bool kSmem, bool kV2, bool kTiny = false>
+template <bool kSmem, bool kTiny = false>
 __global__ void __launch_bounds__(kTiny ? kTinyThreads : kThreads, kTiny ? kTinyCtasPerSm : 1)
 k_forward(KDims D, const double* __restrict__ p, int64_t sp, const double* __restrict__ h,
           int64_t sh, const double* __restrict__ b, int64_t sb, const double* __restrict__ Lfac,
@@ -377,7 +343,7 @@ k_forward(KDims D, const double* __restrict__ p, int64_t sp, const double* __res
     __syncthreads();
     for (int i = tid; i < ms; i += nt) aug[i] = -(hW[i] + hb[i]);
     __syncthreads();
-    factor_and_solve<kSmem, kV2>(D, C, tid, nt);
+    factor_and_solve<kSmem>(D, C, tid, nt);
     issue_K<kSmem>(D, C, tid);
     finish_dxt(C.W, D.ldw, ms, n, w, pt, xt, part, D.vl, tid, nt);   // x~ = -p~ - W^T w
     {
@@ -456,7 +422,7 @@ k_forward(KDims D, const double* __restrict__ p, int64_t sp, const double* __res
             aug[i] = -hfull;
         }
         __syncthreads();
-        factor_and_solve<kSmem, kV2>(D, C, tid, nt);                 // w = [dy_aff; dz_aff]
+        factor_and_solve<kSmem>(D, C, tid, nt);                      // w = [dy_aff; dz_aff]
         // ---- affine step length and sigma (batch.py:160-168)
         double mn[2] = {INFINITY, INFINITY};
         for (int i = ep + tid; i < ms; i += nt) {
@@ -491,7 +457,7 @@ k_forward(KDims D, const double* __restrict__ p, int64_t sp, const double* __res
             }
             __syncthreads();
         }
-        solve_with_factor<kV2>(D, C, wc, tid, nt);                   // wc = [dy_cor; dz_cor]
+        solve_with_factor(D, C, wc, tid, nt);                        // wc = [dy_cor; dz_cor]
         issue_K<kSmem>(D, C, tid);                              // next factor_kkt's copy of K overlaps the rest
         // ---- combined direction, step length, update (batch.py:185-203)
         mn[0] = INFINITY; mn[1] = INFINITY;
@@ -545,7 +511,7 @@ k_forward(KDims D, const double* __restrict__ p, int64_t sp, const double* __res
 // other right-hand sides zero, fused gradient outer products for batched inputs.
 // ---------------------------------------------------------------------------------------------
 
-template <bool kSmem, bool kV2, bool kBackward, bool kTiny = false>
+template <bool kSmem, bool kBackward, bool kTiny = false>
 __global__ void __launch_bounds__(kTiny ? kTinyThreads : kThreads, kTiny ? kTinyCtasPerSm : 1)
 k_solve_kkt(KDims D, const double* __restrict__ d_in, const double* __restrict__ rx_in,
             const double* __restrict__ rs_in, const double* __restrict__ rz_in,
@@ -594,7 +560,7 @@ k_solve_kkt(KDims D, const double* __restrict__ d_in, const double* __restrict__
     __syncthreads();
     for (int i = tid; i < ms; i += nt) aug[i] = -(VEC(V_C2)[i] + hW[i]);
     __syncthreads();
-    factor_and_solve<kSmem, kV2>(D, C, tid, nt);                     // w = [dy; dz]
+    factor_and_solve<kSmem>(D, C, tid, nt);                          // w = [dy; dz]
     finish_dxt(C.W, D.ldw, ms, n, w, t, dxt, part, D.vl, tid, nt);
     unwhiten(D, C, dxt, VEC(V_XT), tid, nt);                    // dx = L^-T dx~
     const double* dx = VEC(V_XT);
@@ -1064,7 +1030,7 @@ int qpb200_plan_init(int nz, int nineq, int neq, qpb200_plan* plan) {
     const bool setup_fast_ok = fast_ok && nz <= 8 * kCholMaxTiles && (int64_t)SL.total * 8 <= kMaxSmem;
     // tiny problems (the sizes of the reference's own tests and prof scripts, test.py:99-187 nz = 10): a 256-thread
     // CTA per QP is 8 warps synchronising over a handful of rows; one warp per QP and 16 QPs per SM instead
-    const bool tiny = kTinyDefault && fits && nz <= kTinyMax && msp <= kTinyMax;
+    const bool tiny = fits && nz <= kTinyMax && msp <= kTinyMax;
     plan->tiny = tiny ? 1 : 0;
     plan->pf = 0; plan->pf_global = 0; plan->pf_smem_bytes = 0; plan->pf2_ok = 0; plan->pf2_smem_bytes = 0; plan->pf_two = 0; plan->pf3_ok = 0; plan->pf3_smem_bytes = 0; plan->pf_three = 0; plan->pf_threads = 256; plan->setup_pf = 0; plan->setup_pf_smem_bytes = 0;
     if (tiny) {
@@ -1081,7 +1047,9 @@ int qpb200_plan_init(int nz, int nineq, int neq, qpb200_plan* plan) {
     // CTA), the packed L must fit the S workspace it visits, W rows must be 16-byte aligned (ld is even by construction)
     plan->coop_smem_bytes = coop_doubles * 8;
     plan->coop_ok = (fast_ok && coop_doubles * 8 <= (232448 / 2 - 1024 - 64) && plan->L_elems <= (int64_t)msp * plan->lds) ? 1 : 0;
-    plan->coop = plan->coop_ok ? kCoopDefault : 0;
+    // opt-in only (QPB200_COOP): the co-resident kernels lost in A/B runs (the 128-register cap spills the
+    // register-resident Cholesky, L2 passes cost 3x the shared-memory ones)
+    plan->coop = 0;
     plan->smem_resident = (fast_ok || fits) ? 1 : 0;
     if (setup_fits && (fast_ok || fits)) {
         plan->setup_smem_bytes = setup_fast_ok ? (int64_t)SL.total * 8 : (setup_mat + setup_vec) * 8;
@@ -1103,15 +1071,14 @@ int qpb200_plan_init(int nz, int nineq, int neq, qpb200_plan* plan) {
         const int64_t pf_glb = (int64_t)fk::fast_smem_doubles(D, true, true) * 8;
         const bool shape_ok = msp <= kThreads && (msp - plan->neq_pad) / 8 >= 1;
         const bool res_ok = shape_ok && pf_res <= kMaxSmem, glb_ok = shape_ok && pf_glb <= kMaxSmem;
-        int want = kPfDefault;                               // 0: only where there is no fast kernel; 1: wherever possible
+        // wherever they fit: never slower than the round-1 kernels in A/B runs at C2, C3 and C4
         const char* env = getenv("QPB200_PF");               // development / A-B knob: "0" never, "1" wherever possible,
-        if (env != nullptr && env[0] == '0') want = -1;      // "2" = "1" + two QPs per SM (W, L from L2) where that fits
-        if (env != nullptr && (env[0] == '1' || env[0] == '2' || env[0] == '3')) want = 1;
+        const bool want = !(env != nullptr && env[0] == '0'); // "2" = "1" + two QPs per SM (W, L from L2) where that fits
         // co-residency: every CTA also costs the 1 KB the hardware reserves, out of 228 KB per SM
         const bool two_ok = glb_ok && 2 * (pf_glb + 1024) <= 233472;
         const bool three_ok = glb_ok && 3 * (pf_glb + 1024) <= 233472 && msp <= 192;   // 192-thread CTAs: one row per thread
-        const bool want_two = (env != nullptr && env[0] == '2') || (env == nullptr && kPfTwoDefault);
-        const bool use = (want == 1 && (res_ok || glb_ok)) || (want == 0 && !fast_ok && (res_ok || glb_ok));
+        const bool want_two = env != nullptr && env[0] == '2';
+        const bool use = want && (res_ok || glb_ok);
         if (use) {
             plan->pf = 1;
             plan->pf_global = res_ok ? 0 : 1;
@@ -1221,18 +1188,18 @@ int qpb200_forward(const qpb200_plan* plan, int nbatch, const double* p, int64_t
     if (plan->neq > 0 && (!b || !nus)) return QPB200_ERR_BAD_ARG;
     cudaStream_t st = (cudaStream_t)stream;
     KDims D = dims_of(plan);
-#define QPB_LAUNCH_FWD(KS, KV, SCR, SCRN)                                                              \
+#define QPB_LAUNCH_FWD(KS, SCR, SCRN)                                                                   \
     do {                                                                                                \
-        int rc = set_smem(k_forward<KS, KV>, plan->solve_smem_bytes);                                   \
+        int rc = set_smem(k_forward<KS>, plan->solve_smem_bytes);                                       \
         if (rc) return rc;                                                                              \
-        k_forward<KS, KV><<<nbatch, kThreads, plan->solve_smem_bytes, st>>>(                            \
+        k_forward<KS><<<nbatch, kThreads, plan->solve_smem_bytes, st>>>(                                \
             D, p, sp, h, sh, b, sb, Lfac, Wfac, Kfac, sF, eps, stall_tol, best_tie, notImprovedLim,     \
             maxIter, zhat, lam, slacks, nus, iters, best_resid, trace, SCR, SCRN);                      \
     } while (0)
     if (plan->tiny) {
-        int rc = set_smem(k_forward<true, false, true>, plan->solve_smem_bytes);
+        int rc = set_smem(k_forward<true, true>, plan->solve_smem_bytes);
         if (rc) return rc;
-        k_forward<true, false, true><<<nbatch, kTinyThreads, plan->solve_smem_bytes, st>>>(
+        k_forward<true, true><<<nbatch, kTinyThreads, plan->solve_smem_bytes, st>>>(
             D, p, sp, h, sh, b, sb, Lfac, Wfac, Kfac, sF, eps, stall_tol, best_tie, notImprovedLim, maxIter, zhat, lam,
             slacks, nus, iters, best_resid, trace, nullptr, 0);
     } else if (plan->pf) {
@@ -1274,10 +1241,10 @@ int qpb200_forward(const qpb200_plan* plan, int nbatch, const double* p, int64_t
             D, p, sp, h, sh, b, sb, Lfac, Wfac, Kfac, sF, eps, stall_tol, best_tie, notImprovedLim, maxIter,
             zhat, lam, slacks, nus, iters, best_resid, trace);
     } else if (plan->smem_resident) {
-        QPB_LAUNCH_FWD(true, false, nullptr, 0);
+        QPB_LAUNCH_FWD(true, nullptr, 0);
     } else {
         if (!scratch) return QPB200_ERR_BAD_ARG;
-        QPB_LAUNCH_FWD(false, false, scratch, plan->solve_scratch_elems);
+        QPB_LAUNCH_FWD(false, scratch, plan->solve_scratch_elems);
     }
 #undef QPB_LAUNCH_FWD
     CK(cudaGetLastError());
@@ -1316,18 +1283,18 @@ static int solve_kkt_impl(const qpb200_plan* plan, int nbatch, const double* d, 
     D.reg = reg;
     BwdOut O;
     memset(&O, 0, sizeof(O));
-#define QPB_LAUNCH_KKT(KS, KV, SCR, SCRN)                                                              \
+#define QPB_LAUNCH_KKT(KS, SCR, SCRN)                                                                   \
     do {                                                                                                \
-        int rc = set_smem(k_solve_kkt<KS, KV, false>, plan->solve_smem_bytes);                          \
+        int rc = set_smem(k_solve_kkt<KS, false>, plan->solve_smem_bytes);                              \
         if (rc) return rc;                                                                              \
-        k_solve_kkt<KS, KV, false><<<nbatch, kThreads, plan->solve_smem_bytes, st>>>(                   \
+        k_solve_kkt<KS, false><<<nbatch, kThreads, plan->solve_smem_bytes, st>>>(                       \
             D, d, rx, rs, rz, ry, nullptr, nullptr, nullptr, nullptr, Lfac, Wfac, Kfac, sF, dx, ds, dz, \
             dy, O, SCR, SCRN);                                                                          \
     } while (0)
     if (plan->tiny) {
-        int rc = set_smem(k_solve_kkt<true, false, false, true>, plan->solve_smem_bytes);
+        int rc = set_smem(k_solve_kkt<true, false, true>, plan->solve_smem_bytes);
         if (rc) return rc;
-        k_solve_kkt<true, false, false, true><<<nbatch, kTinyThreads, plan->solve_smem_bytes, st>>>(
+        k_solve_kkt<true, false, true><<<nbatch, kTinyThreads, plan->solve_smem_bytes, st>>>(
             D, d, rx, rs, rz, ry, nullptr, nullptr, nullptr, nullptr, Lfac, Wfac, Kfac, sF, dx, ds, dz, dy, O, nullptr, 0);
     } else if (plan->pf) {
 #define QPB_LAUNCH_PF(KG, K2)                                                                           \
@@ -1359,10 +1326,10 @@ static int solve_kkt_impl(const qpb200_plan* plan, int nbatch, const double* d, 
         k_kkt_fast<false, false><<<nbatch, kThreads, plan->solve_smem_bytes, st>>>(
             D, d, rx, rs, rz, ry, nullptr, nullptr, nullptr, nullptr, Lfac, Wfac, Kfac, sF, dx, ds, dz, dy, O);
     } else if (plan->smem_resident) {
-        QPB_LAUNCH_KKT(true, false, nullptr, 0);
+        QPB_LAUNCH_KKT(true, nullptr, 0);
     } else {
         if (!scratch) return QPB200_ERR_BAD_ARG;
-        QPB_LAUNCH_KKT(false, false, scratch, plan->solve_scratch_elems);
+        QPB_LAUNCH_KKT(false, scratch, plan->solve_scratch_elems);
     }
 #undef QPB_LAUNCH_KKT
     CK(cudaGetLastError());
@@ -1385,18 +1352,18 @@ int qpb200_backward(const qpb200_plan* plan, int nbatch, const double* dl_dzhat,
     BwdOut O;
     O.dQ = dQ; O.dp = dp; O.dG = dG; O.dh = dh; O.dA = dA; O.db = db;
     O.mQ = mean_Q; O.mp = mean_p; O.mG = mean_G; O.mh = mean_h; O.mA = mean_A; O.mb = mean_b;
-#define QPB_LAUNCH_BWD(KS, KV, SCR, SCRN)                                                              \
+#define QPB_LAUNCH_BWD(KS, SCR, SCRN)                                                                   \
     do {                                                                                                \
-        int rc = set_smem(k_solve_kkt<KS, KV, true>, plan->solve_smem_bytes);                           \
+        int rc = set_smem(k_solve_kkt<KS, true>, plan->solve_smem_bytes);                               \
         if (rc) return rc;                                                                              \
-        k_solve_kkt<KS, KV, true><<<nbatch, kThreads, plan->solve_smem_bytes, st>>>(                    \
+        k_solve_kkt<KS, true><<<nbatch, kThreads, plan->solve_smem_bytes, st>>>(                        \
             D, nullptr, dl_dzhat, nullptr, nullptr, nullptr, zhat, lam, slacks, nus, Lfac, Wfac, Kfac,  \
             sF, dxv, nullptr, dlamv, dnuv, O, SCR, SCRN);                                               \
     } while (0)
     if (plan->tiny) {
-        int rc = set_smem(k_solve_kkt<true, false, true, true>, plan->solve_smem_bytes);
+        int rc = set_smem(k_solve_kkt<true, true, true>, plan->solve_smem_bytes);
         if (rc) return rc;
-        k_solve_kkt<true, false, true, true><<<nbatch, kTinyThreads, plan->solve_smem_bytes, st>>>(
+        k_solve_kkt<true, true, true><<<nbatch, kTinyThreads, plan->solve_smem_bytes, st>>>(
             D, nullptr, dl_dzhat, nullptr, nullptr, nullptr, zhat, lam, slacks, nus, Lfac, Wfac, Kfac, sF, dxv, nullptr,
             dlamv, dnuv, O, nullptr, 0);
     } else if (plan->pf) {
@@ -1436,10 +1403,10 @@ int qpb200_backward(const qpb200_plan* plan, int nbatch, const double* dl_dzhat,
             D, nullptr, dl_dzhat, nullptr, nullptr, nullptr, zhat, lam, slacks, nus, Lfac, Wfac, Kfac, sF, dxv,
             nullptr, dlamv, dnuv, O);
     } else if (plan->smem_resident) {
-        QPB_LAUNCH_BWD(true, false, nullptr, 0);
+        QPB_LAUNCH_BWD(true, nullptr, 0);
     } else {
         if (!scratch) return QPB200_ERR_BAD_ARG;
-        QPB_LAUNCH_BWD(false, false, scratch, plan->solve_scratch_elems);
+        QPB_LAUNCH_BWD(false, scratch, plan->solve_scratch_elems);
     }
 #undef QPB_LAUNCH_BWD
     CK(cudaGetLastError());

@@ -35,37 +35,7 @@ constexpr int kPanLd = 12;              // row stride of the panel scratch (8 us
 
 // In-register factorization of an 8x8 SPD block (lower triangle in Lk, every lane holds all of it): on exit strictly
 // lower = L, diagonal = 1 / L_cc. A non-positive pivot gives NaN/inf everywhere below it.
-#ifndef QPB_PF_PAIRS
-#define QPB_PF_PAIRS 0     // 1: eliminate the columns of the 8x8 block in pairs (two rsqrt side by side); A/B knob
-#endif
 __device__ __forceinline__ void pf_factor8(double (&Lk)[36]) {
-#if QPB_PF_PAIRS
-    // with a = A_cc, b = A_c+1,c, e = A_c+1,c+1: second pivot = det / a, det = a e - b^2, so 1/L_c+1,c+1 = rsqrt(det) sqrt(a)
-    // and the two rsqrt (the longest link of the chain) run side by side
-#pragma unroll
-    for (int c = 0; c < 8; c += 2) {
-        const double a = Lk[QPB_LIDX(c, c)], b = Lk[QPB_LIDX(c + 1, c)], e = Lk[QPB_LIDX(c + 1, c + 1)];
-        const double r1 = f_rsqrt(a);
-        const double det = fma(a, e, -(b * b));
-        const double r2 = f_rsqrt(det) * (a * r1);
-        const double l10 = b * r1;
-        Lk[QPB_LIDX(c, c)] = r1;
-        Lk[QPB_LIDX(c + 1, c)] = l10;
-        Lk[QPB_LIDX(c + 1, c + 1)] = r2;
-#pragma unroll
-        for (int r = c + 2; r < 8; ++r) {
-            const double l1 = Lk[QPB_LIDX(r, c)] * r1;
-            Lk[QPB_LIDX(r, c)] = l1;
-            Lk[QPB_LIDX(r, c + 1)] = fma(-l1, l10, Lk[QPB_LIDX(r, c + 1)]) * r2;
-        }
-#pragma unroll
-        for (int r = c + 2; r < 8; ++r)
-#pragma unroll
-            for (int cc = c + 2; cc <= r; ++cc)
-                Lk[QPB_LIDX(r, cc)] = fma(-Lk[QPB_LIDX(r, c + 1)], Lk[QPB_LIDX(cc, c + 1)],
-                                          fma(-Lk[QPB_LIDX(r, c)], Lk[QPB_LIDX(cc, c)], Lk[QPB_LIDX(r, cc)]));
-    }
-#else
 #pragma unroll
     for (int c = 0; c < 8; ++c) {
         const double ri = f_rsqrt(Lk[QPB_LIDX(c, c)]);
@@ -78,7 +48,6 @@ __device__ __forceinline__ void pf_factor8(double (&Lk)[36]) {
             for (int cc = c + 1; cc <= r; ++cc)
                 Lk[QPB_LIDX(r, cc)] = fma(-Lk[QPB_LIDX(r, c)], Lk[QPB_LIDX(cc, c)], Lk[QPB_LIDX(r, cc)]);
     }
-#endif
 }
 // Column c = lane & 7 of T = L^-1 from the factored block (every lane holds Lk; the lane dependence is in predicates
 // only, so the eight columns are computed side by side instead of one lane doing all 112 operations):
@@ -247,42 +216,6 @@ __device__ __noinline__ void pf_chol_update_t(int S, int nts, int kb0, int kend,
             const double bT0 = (q <= g) ? M[rg + q] : 0.0, bT1 = (q + 4 <= g) ? M[rg + q + 4] : 0.0;   // T[g][q], T[g][q+4]
             const double bP0 = (g <= q) ? M[rq] : 0.0, bP1 = (g <= q + 4) ? M[rq + ld4] : 0.0;        // T[q][g], T[q+4][g]
             // ---- S_k: panel tiles (i, k), i > k, dealt round-robin
-#ifndef QPB_PF_PANEL2
-#define QPB_PF_PANEL2 0    // A/B knob: 1 = two panel tiles in flight per warp
-#endif
-#if QPB_PF_PANEL2
-#pragma unroll 1
-            for (int i = k + 1 + uw; i < nts; i += 2 * nuw) {
-                const int i2 = i + nuw;
-                const bool two = i2 < nts;                   // (warp-uniform)
-                const int r1 = 8 * i + g, r2 = 8 * (two ? i2 : i) + g;
-                double* row1 = M + pf_rowoff(r1) + k0;
-                double* row2 = M + pf_rowoff(r2) + k0;
-                const double a10 = row1[q], a11 = row1[q + 4], a20 = row2[q], a21 = row2[q + 4];
-                double d0 = 0.0, d1 = 0.0, f0 = 0.0, f1 = 0.0;
-                dmma884(d0, d1, a10, bT0);
-                if (two) dmma884(f0, f1, a20, bT0);
-                dmma884(d0, d1, a11, bT1);
-                if (two) dmma884(f0, f1, a21, bT1);
-                if (kSetup && Lg != nullptr) {
-                    if (r1 < ln) { double* lrow = Lg + ((int64_t)r1 * (r1 + 1)) / 2 + k0 + 2 * q; lrow[0] = d0; lrow[1] = d1; }
-                    if (two && r2 < ln) { double* lrow = Lg + ((int64_t)r2 * (r2 + 1)) / 2 + k0 + 2 * q; lrow[0] = f0; lrow[1] = f1; }
-                }
-                double* pl1 = P + ((i == k + 1) ? (8 * nts + g) : r1) * kPanLd;
-                double* pl2 = P + r2 * kPanLd;               // (i2 > k + 1 always)
-                *reinterpret_cast<double2*>(pl1 + 2 * q) = make_double2(d0, d1);
-                if (two) *reinterpret_cast<double2*>(pl2 + 2 * q) = make_double2(f0, f1);
-                __syncwarp();
-                const double la0 = pl1[q], la1 = pl1[q + 4], lb0 = pl2[q], lb1 = pl2[q + 4];
-                double e0 = 0.0, e1 = 0.0, h0 = 0.0, h1 = 0.0;
-                dmma884(e0, e1, la0, bP0);
-                if (two) dmma884(h0, h1, lb0, bP0);
-                dmma884(e0, e1, la1, bP1);
-                if (two) dmma884(h0, h1, lb1, bP1);
-                *reinterpret_cast<double2*>(row1 + 2 * q) = make_double2(e0, e1);
-                if (two) *reinterpret_cast<double2*>(row2 + 2 * q) = make_double2(h0, h1);
-            }
-#else
 #pragma unroll 1
             for (int i = k + 1 + uw; i < nts; i += nuw) {
                 const int r = 8 * i + g;
@@ -305,7 +238,6 @@ __device__ __noinline__ void pf_chol_update_t(int S, int nts, int kb0, int kend,
                 dmma884(e0, e1, la1, bP1);
                 *reinterpret_cast<double2*>(row + 2 * q) = make_double2(e0, e1);
             }
-#endif
         }
         if (k < 16) QPB_TICK1(64 + k);      // S_k
         named_bar_sync(2, kNT);                               // every panel row of this step is in the scratch (the chain warp's too), every P_ik in place
@@ -330,20 +262,14 @@ __device__ __noinline__ void pf_chol_update_t(int S, int nts, int kb0, int kend,
             const int nact = ((nts - 1 - k) * (nts - k)) / 2 - 1;
             // a warp takes FOUR CONSECUTIVE table entries at a time: they mostly lie in one tile column, whose panel
             // fragment (the B operand) is then loaded once
-#ifndef QPB_PF_CHUNK
-#define QPB_PF_CHUNK 1     // A/B knob: 0 round-robin, 1 always four consecutive entries (best at C2, B = 8192 and C4
-                           // in A/B runs), 2 consecutive when plenty
-#endif
-            const bool chunked = (QPB_PF_CHUNK == 1) || (QPB_PF_CHUNK == 2 && nact >= 8 * nuw);
-            const int su = chunked ? 1 : nuw;
 #pragma unroll 1
-            for (int t0 = chunked ? 4 * uw : uw; t0 < nact; t0 += 4 * nuw) {
+            for (int t0 = 4 * uw; t0 < nact; t0 += 4 * nuw) {
                 int ti[4], tj[4];
                 bool ok[4];
 #pragma unroll
                 for (int u = 0; u < 4; ++u) {
-                    ok[u] = t0 + u * su < nact;
-                    const int e = tab[ok[u] ? t0 + u * su : t0];
+                    ok[u] = t0 + u < nact;
+                    const int e = tab[ok[u] ? t0 + u : t0];
                     ti[u] = nts - 1 - (e & 255);
                     tj[u] = nts - 1 - (e >> 8);
                 }

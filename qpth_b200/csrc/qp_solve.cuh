@@ -18,7 +18,7 @@ using namespace qpb::fast;
 enum FVec { F_PT = 0, F_XT, F_RXT, F_S, F_V, F_RV, F_HW, F_W, F_DSA, F_DS, F_D, F_BXT, F_BS, F_BV, F_HB,
             F_DINVL, F_AUG, F_T0, F_T1, F_DINV, F_COUNT };
 
-constexpr int kFastRed = (QPB_RED1 ? 2 : 1) * 4 * qpb::fast::kFastStride;   // reduction scratch of the fast kernels (block_reduce<4>, up to 16 warps; two halves with QPB_RED1)
+constexpr int kFastRed = 4 * qpb::fast::kFastStride;   // reduction scratch of the fast kernels (block_reduce<4>, up to 16 warps)
 struct FLayout {              // offsets in doubles into the dynamic shared array
     int W, LS, Lp, vec, red, bar, tab, pan;
     int vl;
@@ -195,8 +195,7 @@ __device__ __forceinline__ void mv_cols(const KDims& D, const FCtx& C, int v, in
 }
 
 // factor_kkt + first half of solve_kkt: F_AUG = -h_full (pad entries 0), F_D = d  ->  F_W = -S^-1 h_full
-// pform: rewrite the factor in product form (worth it when two more solves with the same factor follow)
-__device__ __forceinline__ void f_factor_and_solve(const KDims& D, FCtx& C, bool pform) {
+__device__ __forceinline__ void f_factor_and_solve(const KDims& D, FCtx& C) {
     QPB_SMEM;
     const int tid = threadIdx.x;
     f_wait_K(C);
@@ -209,23 +208,7 @@ __device__ __forceinline__ void f_factor_and_solve(const KDims& D, FCtx& C, bool
     }
     f_chol(C.L.LS, D.lds, D.msp, D.ep, FV(F_AUG), C.L.tab);
     QPB_TICK(32);   // (chol internals are 20..27)
-#if QPB_PFORM
-    if (pform) {
-        f_to_pform(C.L.LS, D.lds, D.msp);                      // T_k, P_ik: every later solve is chain-free
-        QPB_TICK(28);   // product-form conversion
-        f_ptrsv_bwd(C.L.LS, D.lds, D.msp, FV(F_AUG), FV(F_W));
-    } else
-#endif
-    {
-#if QPB_TRSV16
-        f_invert16(C.L.LS, D.lds, D.msp);
-        __syncthreads();
-        QPB_TICK(28);   // inverted 16 x 16 diagonal blocks
-        f_trsv16_bwd(C.L.LS, D.lds, D.msp, FV(F_AUG), FV(F_W), C.L.red);
-#else
-        f_trsv_bwd(C.L.LS, D.lds, D.msp, FV(F_AUG), FV(F_W));
-#endif
-    }
+    f_trsv_bwd(C.L.LS, D.lds, D.msp, FV(F_AUG), FV(F_W));
     QPB_TICK(33);   // backward substitution
 }
 
@@ -278,7 +261,6 @@ k_forward_fast(KDims D, const double* __restrict__ p, int64_t sp, const double* 
     __syncthreads();
 #endif
     FCtx C = f_make_ctx<kCoop, kPF>(D, qp, Lfac, Wfac, Kfac, sF);
-    int rtog = 0;                                               // which half of the reduction scratch the next block reduction uses
     QPB_TICK(0);
     const int pt = FV(F_PT), xt = FV(F_XT), rxt = FV(F_RXT), s = FV(F_S), v = FV(F_V), rv = FV(F_RV),
               hW = FV(F_HW), w = FV(F_W), dsa = FV(F_DSA), ds = FV(F_DS), d = FV(F_D), hb = FV(F_HB),
@@ -313,7 +295,7 @@ k_forward_fast(KDims D, const double* __restrict__ p, int64_t sp, const double* 
     __syncthreads();
     _Pragma("unroll 1") for (int i = tid; i < ms; i += kNT) qsm[aug + i] = -(qsm[hW + i] + qsm[hb + i]);
     __syncthreads();
-    if (kPF) f_factor_and_solve_pf(D, C); else f_factor_and_solve(D, C, false);
+    if (kPF) f_factor_and_solve_pf(D, C); else f_factor_and_solve(D, C);
     f_issue_K(D, C);
     mv_cols<kCoop>(D, C, w, t0, t1, xt, pt, -1.0, -1, -1.0);   // x~ = -p~ - W^T w
     {
@@ -327,7 +309,7 @@ k_forward_fast(KDims D, const double* __restrict__ p, int64_t sp, const double* 
                 mn[1] = fmin(mn[1], wi);
             }
         }
-        f_reduce_min2(mn, C.L.red + rtog); rtog ^= (QPB_RED1 ? 4 * qpb::fast::kFastStride : 0);
+        f_reduce_min2(mn, C.L.red);
         _Pragma("unroll 1") for (int i = ep + tid; i < ms; i += kNT) {               // slacks and duals >= 1 (batch.py:77-87)
             if (mn[0] < 0.0) qsm[s + i] -= mn[0] - 1.0;
             if (mn[1] < 0.0) qsm[v + i] -= mn[1] - 1.0;
@@ -358,7 +340,7 @@ k_forward_fast(KDims D, const double* __restrict__ p, int64_t sp, const double* 
             else { acc[1] = fma(r, r, acc[1]); acc[3] = fma(qsm[s + i], qsm[v + i], acc[3]); }
         }
         QPB_TICK(6);
-        f_reduce_sum4(acc, C.L.red + rtog); rtog ^= (QPB_RED1 ? 4 * qpb::fast::kFastStride : 0);
+        f_reduce_sum4(acc, C.L.red);
         QPB_TICK(8);
         const double mu = fabs(acc[3] / dm);
         const double resid = sqrt(acc[1]) + sqrt(acc[0]) + sqrt(acc[2]) + dm * mu;
@@ -387,7 +369,7 @@ k_forward_fast(KDims D, const double* __restrict__ p, int64_t sp, const double* 
         }
         __syncthreads();
         QPB_TICK(9);
-        if (kPF) f_factor_and_solve_pf(D, C); else f_factor_and_solve(D, C, true);   // w = [dy_aff; dz_aff]
+        if (kPF) f_factor_and_solve_pf(D, C); else f_factor_and_solve(D, C);   // w = [dy_aff; dz_aff]
         QPB_TICK(10);
         // ---- affine step length and sigma (batch.py:160-168)
         double mn[2] = {INFINITY, INFINITY};
@@ -398,7 +380,7 @@ k_forward_fast(KDims D, const double* __restrict__ p, int64_t sp, const double* 
             mn[0] = fmin(mn[0], step_candidate(qsm[v + i], dz));
             mn[1] = fmin(mn[1], step_candidate(qsm[s + i], dsi));
         }
-        f_reduce_min2(mn, C.L.red + rtog); rtog ^= (QPB_RED1 ? 4 * qpb::fast::kFastStride : 0);
+        f_reduce_min2(mn, C.L.red);
         {
             const double alpha = fmin(fmin(f_step_fix(mn[0]), f_step_fix(mn[1])), 1.0);
             double sm[2] = {0.0, 0.0};
@@ -406,7 +388,7 @@ k_forward_fast(KDims D, const double* __restrict__ p, int64_t sp, const double* 
                 sm[0] = fma(qsm[s + i] + alpha * qsm[dsa + i], qsm[v + i] + alpha * qsm[w + i], sm[0]);
                 sm[1] = fma(qsm[s + i], qsm[v + i], sm[1]);
             }
-            f_reduce_sum2(sm, C.L.red + rtog); rtog ^= (QPB_RED1 ? 4 * qpb::fast::kFastStride : 0);
+            f_reduce_sum2(sm, C.L.red);
             const double sr = sm[0] / sm[1];
             const double sig = sr * sr * sr;
             // ---- corrector right-hand side (batch.py:170-181)
@@ -428,19 +410,9 @@ k_forward_fast(KDims D, const double* __restrict__ p, int64_t sp, const double* 
             wc = hW;
             QPB_TICK(12);
         } else {
-#if QPB_PFORM
-        f_ptrsv_fwd(C.L.LS, D.lds, msp, t1, t0);
-        QPB_TICK(12);
-        f_ptrsv_bwd(C.L.LS, D.lds, msp, t0, t1);                 // t1 = [dy_cor; dz_cor]
-#elif QPB_TRSV16
-        f_trsv16_fwd(C.L.LS, D.lds, msp, t1, t0, C.L.red);
-        QPB_TICK(12);
-        f_trsv16_bwd(C.L.LS, D.lds, msp, t0, t1, C.L.red);       // t1 = [dy_cor; dz_cor]
-#else
-        f_trsv_fwd(C.L.LS, D.lds, msp, 0, msp, t1, t0);
-        QPB_TICK(12);
-        f_trsv_bwd(C.L.LS, D.lds, msp, t0, t1);                  // t1 = [dy_cor; dz_cor]
-#endif
+            f_trsv_fwd(C.L.LS, D.lds, msp, 0, msp, t1, t0);
+            QPB_TICK(12);
+            f_trsv_bwd(C.L.LS, D.lds, msp, t0, t1);              // t1 = [dy_cor; dz_cor]
         }
         QPB_TICK(13);
         f_issue_K(D, C);                                         // next factor_kkt's K copy overlaps the rest
@@ -461,7 +433,7 @@ k_forward_fast(KDims D, const double* __restrict__ p, int64_t sp, const double* 
         QPB_TICK(14);
         // the step length does not depend on dx~: v and s move first, then one pass over W gives dx~, x~ and the next
         // iteration's r~x (none after the last iteration: nothing reads x~ then)
-        f_reduce_min2(mn, C.L.red + rtog); rtog ^= (QPB_RED1 ? 4 * qpb::fast::kFastStride : 0);
+        f_reduce_min2(mn, C.L.red);
         const double alpha = fmin(0.999 * fmin(f_step_fix(mn[0]), f_step_fix(mn[1])), 1.0);
         _Pragma("unroll 1") for (int i = tid; i < ms; i += kNT) {
             qsm[v + i] = fma(alpha, qsm[w + i], qsm[v + i]);
@@ -551,7 +523,7 @@ k_kkt_fast(KDims D, const double* __restrict__ d_in, const double* __restrict__ 
     __syncthreads();
     _Pragma("unroll 1") for (int i = tid; i < ms; i += kNT) qsm[aug + i] = -(qsm[c2 + i] + qsm[hW + i]);
     __syncthreads();
-    if (kPF) f_factor_and_solve_pf(D, C); else f_factor_and_solve(D, C, false);   // w = [dy; dz]
+    if (kPF) f_factor_and_solve_pf(D, C); else f_factor_and_solve(D, C);   // w = [dy; dz]
     mv_cols<kCoop>(D, C, w, t0, t1, dxt, t, -1.0, -1, -1.0);
     if (kCoop && !C.lglobal) f_stage_L(D, C);                   // (mv_cols ended with a block barrier; no K copy in flight)
     f_unwhiten_x(D, C, dxt, dxo);                          // dx = L^-T dx~

@@ -1,16 +1,15 @@
 #!/bin/bash
-# Build A/B variants of the kernels (load one with QPB200_LIB=<path> or scripts/phase_timing.py's QPB200_TIMING_LIB).
-#   scripts/build_variants.sh real  "NAME:-DFLAG=1 -DOTHER=0" ...   -> build/variants/lib_NAME.so
-#   scripts/build_variants.sh timing "NAME:-DFLAG=1" ...            -> build/timing/t_NAME.so   (adds -DQPB_TIMING)
-# Flags: QPB_PFORM, QPB_VECWARP, QPB_VG_SMEM, QPB_CHAIN_V2, QPB_TIMING_REPEAT, QPB_TIMING_PROBES (see the kernel sources).
-# Every variant is the full three-unit library (qpth_b200/build.py): the flags reach all units.
+# Build cycle-accounting libraries (-DQPB_TIMING) for scripts/phase_timing.py, which loads one with QPB200_TIMING_LIB=<path>.
+#   scripts/build_variants.sh timing "NAME:[extra nvcc flags]" ...   -> build/timing/t_NAME.so
+# Every library is the full four-unit build (qpth_b200/build.py): the flags reach all units.
 set -e
 cd "$(dirname "$0")/.."
-kind=$1; shift
-if [ "$kind" = timing ]; then dir=build/timing; pre=t_; extra=-DQPB_TIMING; else dir=build/variants; pre=lib_; extra=; fi
+if [ "$1" != timing ]; then echo "usage: $0 timing NAME:[flags] ..." >&2; exit 2; fi
+shift
+dir=build/timing
 mkdir -p $dir
 for spec in "$@"; do
   name=${spec%%:*}; flags=${spec#*:}
-  ( python -c "import sys; from qpth_b200 import build; build.build(force=True, extra=sys.argv[2:], out=sys.argv[1])" $PWD/$dir/$pre$name.so $extra $flags 2>&1 | grep -E "error" || true; echo "built $dir/$pre$name.so [$flags]" ) &
+  ( python -c "import sys; from qpth_b200 import build; build.build(force=True, extra=sys.argv[2:], out=sys.argv[1])" $PWD/$dir/t_$name.so -DQPB_TIMING $flags 2>&1 | grep -E "error" || true; echo "built $dir/t_$name.so [$flags]" ) &
 done
 wait

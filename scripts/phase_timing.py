@@ -43,7 +43,7 @@ lib.qpb200_debug_timing(buf, 0)
 it = int(c[slow, 2])
 names = {0: "make_ctx (TMA staging)", 1: "load vectors", 2: "whiten (+ first K issue)", 3: "loop misc/update (prev)", 4: "matvec_cols (r~x, iteration 0)", 5: "matvec_rows2 + tri_norm2", 6: "residual elementwise", 8: "reduce_sum4",
          9: "best/exit/aug build", 10: "factor_and_solve tail", 11: "aff step, sigma, rhs", 12: "trsv_fwd (cor)", 13: "trsv_bwd (cor)", 14: "issue_K + combine", 15: "alpha, update, matvec_cols2 (dx~, next r~x)", 16: "exit: unwhiten + outputs",
-         24: "chol: diag tile k+1 update", 26: "chol: (chain) F_k+1 / end of step", 28: "invert16", 32: "chol exit", 33: "trsv_bwd (aff)",
+         24: "chol: diag tile k+1 update", 26: "chol: (chain) F_k+1 / end of step", 32: "chol exit", 33: "trsv_bwd (aff)",
          40: "[warp1] gap", 42: "[warp1] named barrier wait", 44: "[warp1] step barrier wait"}
 tot = sum(buf[i] for i in range(40)) + sum(buf[i] for i in range(80, 128))   # thread 0 owns slots 0..39 and 80..127 (per-step Cholesky slots); 40..79 are warp 1's
 print("slowest QP (%d): thread-0 slots sum to %d cycles = %.1f us @1.965 GHz (CTA duration by globaltimer: %.1f us); per iteration %.0f cycles" % (slow, tot, tot / 1965.0, dur[slow], tot / (it + 1)))
