@@ -178,6 +178,14 @@ typedef struct qpb200_box_plan {
     int64_t smem_bytes;     /* dynamic shared memory per CTA: A, the factor of M and every vector */
     int ok;                 /* 1: the box kernels cover this shape (neq_pad <= threads, smem_bytes <= 227 KB); 0: the entry
                              *    points below return QPB200_ERR_TOO_LARGE and the dense path is the one to use          */
+    /* Thread block cluster kernels (ok == 0 but neq_pad <= threads): one cluster of cl_ctas CTAs solves one QP, CTA r
+     * owning the variables [r cl_slice, (r + 1) cl_slice). cl_ctas is the smallest of 2, 4, 8 whose slice fits 227 KB
+     * (0: no cluster covers the shape). The entry points below use them whenever cl_ctas != 0, and return
+     * QPB200_ERR_TOO_LARGE if the device cannot make such a cluster resident. QPB200_BOX_CLUSTER=C (development knob)
+     * forces C on shapes with ok == 1 too. */
+    int cl_ctas;
+    int cl_slice;           /* variables per CTA (the last CTA may hold fewer) */
+    int64_t cl_smem_bytes;  /* dynamic shared memory per CTA */
 } qpb200_box_plan;
 
 int qpb200_box_plan_init(int nz, int neq, int has_lb, int has_ub, qpb200_box_plan* plan);

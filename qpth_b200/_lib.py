@@ -38,6 +38,7 @@ class BoxPlan(ctypes.Structure):
         ("nz", ctypes.c_int), ("neq", ctypes.c_int), ("neq_pad", ctypes.c_int), ("nineq", ctypes.c_int),
         ("has_lb", ctypes.c_int), ("has_ub", ctypes.c_int), ("threads", ctypes.c_int),
         ("smem_bytes", ctypes.c_int64), ("ok", ctypes.c_int),
+        ("cl_ctas", ctypes.c_int), ("cl_slice", ctypes.c_int), ("cl_smem_bytes", ctypes.c_int64),
     ]
 
 
@@ -137,8 +138,10 @@ _box_plans = {}
 
 
 def box_plan_for(nz, neq, has_lb, has_ub):
-    """Plan of the box-QP kernels for a shape (cached; no device work). plan.ok: the kernels cover it."""
-    key = (nz, neq, bool(has_lb), bool(has_ub))
+    """Plan of the box-QP kernels for a shape (cached; no device work). plan.ok: the one-CTA kernels cover it;
+    plan.cl_ctas: the cluster kernels do (QPB200_BOX_CLUSTER, a development knob read by qpb200_box_plan_init,
+    forces them: part of the key)."""
+    key = (nz, neq, bool(has_lb), bool(has_ub), os.environ.get("QPB200_BOX_CLUSTER"))
     if key not in _box_plans:
         p = BoxPlan()
         check(load().qpb200_box_plan_init(nz, neq, int(bool(has_lb)), int(bool(has_ub)), ctypes.byref(p)))

@@ -7,8 +7,10 @@ the same Mehrotra loop, exit rules (per QP, STALL_TOL, BEST_TIE), residuals, dia
 gradient conventions (batch mean for an input passed un-batched). What differs is the KKT solve: with Q diagonal and
 every row of G equal to +-e_i the inequality block is eliminated in closed form, so a Newton iteration factors only
 M = A H^-1 A' (order neq, H = q + G'DG diagonal) - nothing at all without equality constraints - and needs no
-pre_factor_kkt (csrc/qp_box.cu). Shapes the box kernels do not cover (qpb200_box_plan.ok == 0: neq > 128, or A and the
-vectors beyond 227 KB of shared memory) run the dense kernels on the dense equivalent instead.
+pre_factor_kkt (csrc/qp_box.cu). One CTA solves one QP where A and the vectors fit its 227 KB of shared memory
+(qpb200_box_plan.ok); past that, a thread block cluster of 2, 4 or 8 CTAs does, each CTA holding a slice of the
+variables (plan.cl_ctas; e.g. the capped-simplex projection over thousands of classes). Shapes neither covers
+(neq > 128, or beyond a cluster's pooled shared memory) run the dense kernels on the dense equivalent instead.
 
 The OptNet sudoku layer (Q = 0.1 I, G = -I, h = 0, a learned A) is one such problem; a differentiable projection
 min 1/2 ||z - v||^2 s.t. Az = b, lb <= z <= ub is another (q = 1, p = -v).
@@ -64,7 +66,8 @@ class _BoxSolved:
 
 
 def solve_box_forward(q_, p_, A_, b_, lb_, ub_, eps=1e-12, verbose=0, notImprovedLim=3, maxIter=20, check_Q_spd=True):
-    """The box kernels on the device. Returns _BoxSolved (dense = None), or None when plan.ok == 0."""
+    """The box kernels on the device (one CTA per QP, or a cluster of plan.cl_ctas CTAs per QP). Returns _BoxSolved
+    (dense = None), or None when neither covers the shape."""
     nBatch, nz, neq = check_box_shapes(q_, p_, A_, b_, lb_, ub_)
     if _qp._pending:
         _qp.flush_checks(wait=False)
@@ -73,7 +76,7 @@ def solve_box_forward(q_, p_, A_, b_, lb_, ub_, eps=1e-12, verbose=0, notImprove
     if not torch.cuda.is_available():
         raise _lib.QpthB200Error("qpth_b200: no CUDA device available (there is no CPU fallback).")
     plan = _lib.box_plan_for(nz, neq, lb_ is not None, ub_ is not None)
-    if not plan.ok:
+    if not (plan.ok or plan.cl_ctas):
         return None
     device = q_.device if q_.is_cuda else torch.device("cuda", torch.cuda.current_device())
     with torch.cuda.device(device):

@@ -10,13 +10,19 @@
 //
 // One 128-thread CTA per QP; A (neq x nz, row stride nz | 1), the factor of M and every vector live in shared memory.
 // The kernels cover neq_pad <= 128 (the substitutions own one row per thread) and a footprint within the 227 KB an
-// H100 CTA may use (qpb200_box_plan.ok); BoxQPFunction runs the dense kernels on the dense equivalent otherwise.
+// H100 CTA may use (qpb200_box_plan.ok). Past that, the cluster kernels (k_box_*_cl, below) split one QP's variables
+// over a thread block cluster of 2, 4 or 8 CTAs (qpb200_box_plan.cl_ctas); BoxQPFunction runs the dense kernels on the
+// dense equivalent only where neither covers the shape.
+#include <cooperative_groups.h>
 #include <cuda_runtime.h>
 #include <math.h>
 #include <stdint.h>
+#include <stdlib.h>
 #include <string.h>
 
+#include <map>
 #include <mutex>
+#include <utility>
 
 #include "../../include/qpth_b200.h"
 #ifndef QPB_NT
@@ -457,6 +463,476 @@ __global__ void k_box_mean_outer(int B, int rows, int cols, const double* __rest
     out[(int64_t)r * cols + c] = s / (double)B;
 }
 
+// ---- cluster kernels: one thread block cluster of C CTAs per QP (shapes beyond one CTA's shared memory) ---------------
+// CTA `rank` owns the variables [rank * slice, rank * slice + nloc) (the last slice may be partial or empty). In its own
+// shared memory it holds its columns of A, its entries of every length-nz vector and the lb / ub rows of those variables
+// (local row order: lb rows, then ub rows), laid out by box_dims(slice, ...) so that every CTA has the same footprint;
+// the length-neq_pad vectors are replicated. Behind that layout: the partial M (compact lower triangle) and two publish
+// buffers of the cluster reductions.
+//
+// INVARIANT: every CTA of a cluster executes the same sequence of cluster.sync() calls. A reduction is combined in rank
+// order (then warp order) from the partials every CTA publishes, so every CTA holds bit-identical sums and minima; M is
+// summed in rank order and factored redundantly by every CTA (same input, same code: bit-identical factor and dy, no
+// broadcast and no extra barrier), so y, mu, the residual and the step lengths are bit-identical too. Every branch that
+// reaches a cluster barrier (the exit tests, NaN and mu > 1e32 exits, best-iterate tracking, notImprovedLim, e > 0,
+// fresh) is decided from those values or from kernel arguments only; a CTA that branched on a value of its own would
+// deadlock its cluster.
+//
+// Publish buffers alternate: a CTA rewrites buffer (ph & 1) only after the cluster barrier of the reduction that
+// followed its previous use, and every CTA finishes reading a buffer before it arrives at that barrier. The partial M is
+// rewritten by the next cl_form only after the right-hand-side reduction of the solve that read it.
+namespace cg = cooperative_groups;
+constexpr int kClW = kBoxNT / 32;                          // warps per CTA: scalar partials are published per warp
+
+struct ClDims {
+    BoxDims L;               // layout of one slice (L.n = slice); counts are set per CTA in cl_local
+    int C, slice, ng, nlbg, mg;   // cluster size, variables per CTA, nz, lb rows, inequality rows (global)
+    int Mp, pub, pb;         // partial M (e (e + 1) / 2 doubles), publish buffers (two of pb doubles: ep + 4 kClW)
+    int total;               // doubles per CTA
+};
+
+__host__ __device__ inline ClDims cl_dims(int n, int e, int has_lb, int has_ub, int C) {
+    ClDims X;
+    X.C = C; X.slice = (n + C - 1) / C; X.ng = n;
+    X.nlbg = has_lb ? n : 0; X.mg = (has_lb ? n : 0) + (has_ub ? n : 0);
+    X.L = box_dims(X.slice, e, has_lb, has_ub);
+    int o = X.L.total;
+    X.Mp = o; o += r8((e * (e + 1)) / 2);
+    X.pb = r8(X.L.ep + 4 * kClW);
+    X.pub = o; o += 2 * X.pb;
+    X.total = o;
+    return X;
+}
+
+// this CTA's counts: nloc variables from j0
+__device__ __forceinline__ BoxDims cl_local(const ClDims& X, int rank, int& j0) {
+    BoxDims D = X.L;
+    j0 = rank * X.slice;
+    const int nloc = max(0, min(X.slice, X.ng - j0));
+    D.n = nloc;
+    D.nlb = X.nlbg ? nloc : 0;
+    D.m = (X.nlbg ? nloc : 0) + (X.mg > X.nlbg ? nloc : 0);
+    return D;
+}
+// global inequality row of local row i
+__device__ __forceinline__ int64_t cl_grow(const ClDims& X, const BoxDims& D, int j0, int i) {
+    return (i < D.nlb) ? (int64_t)(j0 + i) : (int64_t)(X.nlbg + j0 + i - D.nlb);
+}
+
+// Cluster-wide reduction of N scalars (sum or min) and, when vlen > 0, of the length-vlen vector the caller wrote to
+// qsm[buf(ph)] (vdst: where its sum goes). One cluster barrier; every thread returns with the combined scalars.
+// Ends with a block barrier when vlen > 0.
+__device__ __forceinline__ int cl_buf(const ClDims& X, int ph) { return X.pub + (ph & 1) * X.pb; }
+
+template <int N, bool kMin>
+__device__ __forceinline__ void cl_reduce(const ClDims& X, double (&v)[N], int& ph, int vlen, int vdst) {
+    QPB_SMEM;
+    cg::cluster_group cl = cg::this_cluster();
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int buf = cl_buf(X, ph), sc = buf + X.L.ep;
+#pragma unroll
+    for (int k = 0; k < N; ++k) v[k] = kMin ? qpb::warp_min(v[k]) : qpb::warp_sum(v[k]);
+    if (lane == 0) {
+#pragma unroll
+        for (int k = 0; k < N; ++k) qsm[sc + k * kClW + warp] = v[k];
+    }
+    cl.sync();
+#pragma unroll
+    for (int k = 0; k < N; ++k) v[k] = kMin ? INFINITY : 0.0;
+    for (int r = 0; r < X.C; ++r) {
+        const double* rp = cl.map_shared_rank(qsm + sc, r);
+#pragma unroll
+        for (int k = 0; k < N; ++k)
+#pragma unroll
+            for (int w = 0; w < kClW; ++w) v[k] = kMin ? fmin(v[k], rp[k * kClW + w]) : v[k] + rp[k * kClW + w];
+    }
+    if (vlen > 0) {
+        for (int i = tid; i < vlen; i += kBoxNT) {
+            double s = 0.0;
+            for (int r = 0; r < X.C; ++r) s += cl.map_shared_rank(qsm + buf, r)[i];
+            qsm[vdst + i] = s;
+        }
+        __syncthreads();
+    }
+    ++ph;
+}
+
+// hinv for this CTA's variables and its partial A_r H_r^-1 A_r' (rows < e) into X.Mp; summed by the next cl_solve.
+__device__ __noinline__ void cl_form(const ClDims& X, const BoxDims& D) {
+    QPB_SMEM;
+    const int tid = threadIdx.x;
+    for (int j = tid; j < D.n; j += kBoxNT) {
+        double hj = qsm[D.q + j];
+        if (D.nlb) hj += qsm[D.d + j];
+        if (D.m > D.nlb) hj += qsm[D.d + D.nlb + j];
+        qsm[D.hinv + j] = 1.0 / hj;
+    }
+    __syncthreads();
+    if (D.e == 0) return;
+    const int n = D.n, lda = D.lda;
+    const int tot = (D.e * (D.e + 1)) / 2;
+    const double* A = qsm + D.A;
+    const double* hv = qsm + D.hinv;
+    for (int t = tid; t < tot; t += kBoxNT) {
+        int r = (int)((sqrt(8.0 * t + 1.0) - 1.0) * 0.5);
+        while ((r * (r + 1)) / 2 > t) --r;
+        while (((r + 1) * (r + 2)) / 2 <= t) ++r;
+        const int c = t - (r * (r + 1)) / 2;
+        const double* ar = A + r * lda;
+        const double* ac = A + c * lda;
+        double s0 = 0.0, s1 = 0.0;
+        int k = 0;
+        for (; k + 1 < n; k += 2) {
+            s0 = fma(ar[k] * hv[k], ac[k], s0);
+            s1 = fma(ar[k + 1] * hv[k + 1], ac[k + 1], s1);
+        }
+        if (k < n) s0 = fma(ar[k] * hv[k], ac[k], s0);
+        qsm[X.Mp + t] = s0 + s1;
+    }
+}
+
+// box_solve on a cluster: rhs = ry - sum_r A_r H_r^-1 r_r (one cluster reduction; with fresh, the partial M of the last
+// cl_form is summed in the same barrier into the staircase and factored here, redundantly in every CTA). Ends with a
+// block barrier.
+__device__ __noinline__ void cl_solve(const ClDims& X, const BoxDims& D, int& ph, bool fresh, int rx, int rs, int rz,
+                                      int ry, int dx, int ds, int dz, int dy) {
+    QPB_SMEM;
+    const int tid = threadIdx.x;
+    const int n = D.n, m = D.m, e = D.e, ep = D.ep, lda = D.lda;
+    for (int j = tid; j < n; j += kBoxNT) {
+        double a = qsm[rx + j];
+        if (D.nlb) {
+            const double t = ((rz >= 0) ? qsm[D.d + j] * qsm[rz + j] : 0.0) - ((rs >= 0) ? qsm[rs + j] : 0.0);
+            a -= t;
+        }
+        if (m > D.nlb) {
+            const int i = D.nlb + j;
+            const double t = ((rz >= 0) ? qsm[D.d + i] * qsm[rz + i] : 0.0) - ((rs >= 0) ? qsm[rs + i] : 0.0);
+            a += t;
+        }
+        qsm[D.r + j] = a * qsm[D.hinv + j];
+    }
+    __syncthreads();
+    if (e > 0) {
+        cg::cluster_group cl = cg::this_cluster();
+        const int lane = tid & 31, warp = tid >> 5, buf = cl_buf(X, ph);
+        for (int i = warp; i < e; i += kBoxNT / 32) {
+            double a = 0.0;
+            for (int k = lane; k < n; k += 32) a = fma(qsm[D.A + i * lda + k], qsm[D.r + k], a);
+            a = qpb::warp_sum(a);
+            if (lane == 0) qsm[buf + i] = a;
+        }
+        cl.sync();                                           // the partials of A H^-1 r (and of M) are published
+        if (fresh) {
+            const int tot = (ep * (ep + 1)) / 2;
+            for (int t = tid; t < tot; t += kBoxNT) {
+                int r = (int)((sqrt(8.0 * t + 1.0) - 1.0) * 0.5);
+                while ((r * (r + 1)) / 2 > t) --r;
+                while (((r + 1) * (r + 2)) / 2 <= t) ++r;
+                const int c = t - (r * (r + 1)) / 2;
+                double v = 0.0;
+                if (r < e)
+                    for (int k = 0; k < X.C; ++k) v += cl.map_shared_rank(qsm + X.Mp, k)[t];
+                else
+                    v = (r == c) ? 1.0 : 0.0;
+                qsm[D.S + pf_rowoff(r) + c] = v;
+            }
+        }
+        for (int i = tid; i < ep; i += kBoxNT) {
+            double a = 0.0;
+            if (i < e)
+                for (int k = 0; k < X.C; ++k) a += cl.map_shared_rank(qsm + buf, k)[i];
+            qsm[D.rhs + i] = (i < e) ? (((ry >= 0) ? qsm[ry + i] : 0.0) - a) : 0.0;
+        }
+        ++ph;
+        __syncthreads();
+        const int nts = ep >> 3;
+        if (fresh) {
+            pf_chol(D.S, nts, 0, D.rhs, D.pan, D.tab);
+            __syncthreads();
+        } else {
+            pf_fwd(D.S, ep, 0, nts - 1, D.rhs);
+        }
+        pf_diag(D.S, ep, D.rhs, D.t, D.rhs);
+        pf_bwd(D.S, ep, D.rhs, dy);
+    }
+    for (int j = tid; j < n; j += kBoxNT) {
+        double a = 0.0;
+        for (int i = 0; i < e; ++i) a = fma(qsm[D.A + i * lda + j], qsm[dy + i], a);
+        qsm[dx + j] = -qsm[D.r + j] - a * qsm[D.hinv + j];
+    }
+    __syncthreads();
+    for (int i = tid; i < m; i += kBoxNT) {
+        const double di = qsm[D.d + i];
+        const double rsi = (rs >= 0) ? qsm[rs + i] : 0.0;
+        const double dzi = di * (bsgn(D, i) * qsm[dx + bvar(D, i)] + ((rz >= 0) ? qsm[rz + i] : 0.0)) - rsi;
+        qsm[dz + i] = dzi;
+        qsm[ds + i] = (-rsi - dzi) / di;
+    }
+    __syncthreads();
+}
+
+// q and this CTA's columns of A; b replicated (forward only); the staircase tile table
+__device__ __forceinline__ void cl_stage(const ClDims& X, const BoxDims& D, int j0, const double* q, const double* A,
+                                         const double* b) {
+    QPB_SMEM;
+    const int tid = threadIdx.x;
+    for (int j = tid; j < D.n; j += kBoxNT) qsm[D.q + j] = q[j0 + j];
+    for (int t = tid; t < D.e * D.n; t += kBoxNT) {
+        const int i = t / D.n, j = t - i * D.n;
+        qsm[D.A + i * D.lda + j] = A[(int64_t)i * X.ng + j0 + j];
+    }
+    for (int i = tid; i < D.ep; i += kBoxNT) qsm[D.b + i] = (b != nullptr && i < D.e) ? b[i] : 0.0;
+    if (D.e > 0) pf_build_tab(D.tab, D.ep >> 3);
+    __syncthreads();
+}
+
+// k_box_forward on a cluster (same Mehrotra loop, exit rules and outputs; see the invariant above). Rank 0 writes nus,
+// iters, best_resid, the trace rows and spd_flag; every CTA its slice of zhat, lam and slacks.
+__global__ void __launch_bounds__(kBoxNT, 1)
+k_box_forward_cl(ClDims X, const double* __restrict__ q, int64_t sq, const double* __restrict__ p, int64_t sp,
+                 const double* __restrict__ A, int64_t sA, const double* __restrict__ b, int64_t sb,
+                 const double* __restrict__ lb, int64_t slb, const double* __restrict__ ub, int64_t sub, double eps,
+                 double stall_tol, double best_tie, int notImprovedLim, int maxIter, double* __restrict__ zhat,
+                 double* __restrict__ lam, double* __restrict__ slacks, double* __restrict__ nus,
+                 int* __restrict__ iters_out, double* __restrict__ resid_out, double* __restrict__ trace,
+                 int* __restrict__ spd_flag) {
+    QPB_SMEM;
+    const int rank = (int)cg::this_cluster().block_rank();
+    const int tid = threadIdx.x, qp = blockIdx.x / X.C;
+    int j0, ph = 0;
+    const BoxDims D = cl_local(X, rank, j0);
+    const int n = D.n, m = D.m, e = D.e, ep = D.ep, N = X.ng;
+    cl_stage(X, D, j0, q + (int64_t)qp * sq, A + (int64_t)qp * sA, (e > 0) ? b + (int64_t)qp * sb : nullptr);
+    {
+        double bad[1] = {0.0};
+        for (int j = tid; j < n; j += kBoxNT) {
+            qsm[D.p + j] = p[(int64_t)qp * sp + j0 + j];
+            if (!(qsm[D.q + j] > 0.0)) bad[0] = 1.0;
+        }
+        cl_reduce<1, false>(X, bad, ph, 0, 0);
+        if (rank == 0 && tid == 0 && spd_flag != nullptr) spd_flag[qp] = bad[0] > 0.0;
+    }
+    for (int i = tid; i < m; i += kBoxNT) {
+        qsm[D.h + i] = (i < D.nlb) ? -lb[(int64_t)qp * slb + j0 + i] : ub[(int64_t)qp * sub + j0 + i - D.nlb];
+        qsm[D.d + i] = 1.0;
+        qsm[D.rz + i] = -qsm[D.h + i];
+    }
+    for (int i = tid; i < ep; i += kBoxNT) { qsm[D.ry + i] = -qsm[D.b + i]; qsm[D.y + i] = 0.0; }
+    __syncthreads();
+
+    // ---- initial point: solve_kkt(p, 0, -h, -b) with d = 1   (batch.py:61-67)
+    cl_form(X, D);
+    cl_solve(X, D, ph, true, D.p, -1, D.rz, D.ry, D.x, D.s, D.z, D.y);
+    {
+        double mn[2] = {INFINITY, INFINITY};
+        for (int i = tid; i < m; i += kBoxNT) { mn[0] = fmin(mn[0], qsm[D.s + i]); mn[1] = fmin(mn[1], qsm[D.z + i]); }
+        cl_reduce<2, true>(X, mn, ph, 0, 0);
+        for (int i = tid; i < m; i += kBoxNT) {                  // slacks and duals >= 1 (batch.py:77-87)
+            if (mn[0] < 0.0) qsm[D.s + i] -= mn[0] - 1.0;
+            if (mn[1] < 0.0) qsm[D.z + i] -= mn[1] - 1.0;
+        }
+        __syncthreads();
+    }
+
+    double best = 0.0;
+    int nNot = 0, iters_run = 0;
+    const double dm = (double)X.mg;
+    for (int it = 0; it < maxIter; ++it) {
+        iters_run = it + 1;
+        // ---- residuals (batch.py:94-107): A x is reduced with the scalars, ry and |ry|^2 are formed redundantly
+        double acc[4] = {0.0, 0.0, 0.0, 0.0};                   // |ry|^2, |rz|^2, |rx|^2, s.z
+        for (int j = tid; j < n; j += kBoxNT) {
+            double a = 0.0;
+            for (int i = 0; i < e; ++i) a = fma(qsm[D.A + i * D.lda + j], qsm[D.y + i], a);
+            const double r = fma(qsm[D.q + j], qsm[D.x + j], qsm[D.p + j]) + gt_col(D, qsm + D.z, j) + a;
+            qsm[D.rx + j] = r;
+            acc[2] = fma(r, r, acc[2]);
+        }
+        for (int i = tid; i < m; i += kBoxNT) {
+            const double r = bsgn(D, i) * qsm[D.x + bvar(D, i)] + qsm[D.s + i] - qsm[D.h + i];
+            qsm[D.rz + i] = r;
+            acc[1] = fma(r, r, acc[1]);
+            acc[3] = fma(qsm[D.s + i], qsm[D.z + i], acc[3]);
+        }
+        {
+            const int lane = tid & 31, warp = tid >> 5, buf = cl_buf(X, ph);
+            for (int i = warp; i < e; i += kBoxNT / 32) {
+                double a = 0.0;
+                for (int k = lane; k < n; k += 32) a = fma(qsm[D.A + i * D.lda + k], qsm[D.x + k], a);
+                a = qpb::warp_sum(a);
+                if (lane == 0) qsm[buf + i] = a;
+            }
+        }
+        cl_reduce<4, false>(X, acc, ph, e, D.ry);
+        for (int i = 0; i < e; ++i) {
+            const double r = qsm[D.ry + i] - qsm[D.b + i];
+            acc[0] = fma(r, r, acc[0]);
+        }
+        __syncthreads();                                         // every thread has read the sums of A x
+        for (int i = tid; i < ep; i += kBoxNT) qsm[D.ry + i] = (i < e) ? qsm[D.ry + i] - qsm[D.b + i] : 0.0;
+        const double mu = fabs(acc[3] / dm);
+        const double resid = sqrt(acc[1]) + sqrt(acc[0]) + sqrt(acc[2]) + dm * mu;
+        if (trace != nullptr && rank == 0 && tid == 0) {          // what verbose=1 prints (batch.py:115-117)
+            double* tr = trace + ((int64_t)qp * maxIter + it) * 4;
+            tr[0] = sqrt(acc[1]) + sqrt(acc[0]); tr[1] = sqrt(acc[2]); tr[2] = mu; tr[3] = resid;
+        }
+        // ---- best-iterate tracking and exit tests (batch.py:118-143), per QP: cluster-wide values only
+        const bool improved = (it == 0) || (resid < best);
+        if (improved) { best = resid; nNot = 0; } else { ++nNot; }
+        if (improved || resid < best_tie * best) {
+            for (int j = tid; j < n; j += kBoxNT) qsm[D.bx + j] = qsm[D.x + j];
+            for (int i = tid; i < m; i += kBoxNT) { qsm[D.bs + i] = qsm[D.s + i]; qsm[D.bz + i] = qsm[D.z + i]; }
+            for (int i = tid; i < e; i += kBoxNT) qsm[D.by + i] = qsm[D.y + i];
+        }
+        if ((nNot == notImprovedLim && best < stall_tol) || best < eps || mu > 1e32) break;
+        if (!(resid == resid) || isinf(resid)) break;
+        // ---- d = z/s, H, M; the affine direction (batch.py:109-113,150) factors M
+        for (int i = tid; i < m; i += kBoxNT) qsm[D.d + i] = qsm[D.z + i] / qsm[D.s + i];
+        __syncthreads();
+        cl_form(X, D);
+        cl_solve(X, D, ph, true, D.rx, D.z, D.rz, D.ry, D.dxa, D.dsa, D.dza, D.dya);
+        // ---- affine step length and sigma (batch.py:160-168)
+        double mn[2] = {INFINITY, INFINITY};
+        for (int i = tid; i < m; i += kBoxNT) {
+            mn[0] = fmin(mn[0], box_step(qsm[D.z + i], qsm[D.dza + i]));
+            mn[1] = fmin(mn[1], box_step(qsm[D.s + i], qsm[D.dsa + i]));
+        }
+        cl_reduce<2, true>(X, mn, ph, 0, 0);
+        {
+            const double alpha = fmin(fmin(box_step_fix(mn[0]), box_step_fix(mn[1])), 1.0);
+            double sm[2] = {0.0, 0.0};
+            for (int i = tid; i < m; i += kBoxNT) {
+                sm[0] = fma(qsm[D.s + i] + alpha * qsm[D.dsa + i], qsm[D.z + i] + alpha * qsm[D.dza + i], sm[0]);
+                sm[1] = fma(qsm[D.s + i], qsm[D.z + i], sm[1]);
+            }
+            cl_reduce<2, false>(X, sm, ph, 0, 0);
+            const double sr = sm[0] / sm[1];
+            const double sig = sr * sr * sr;
+            // ---- corrector right-hand side (batch.py:170-181): rs = (-mu sig + dsa dza) / s, rx = rz = ry = 0
+            for (int i = tid; i < m; i += kBoxNT)
+                qsm[D.rsc + i] = (-mu * sig + qsm[D.dsa + i] * qsm[D.dza + i]) / qsm[D.s + i];
+            for (int j = tid; j < n; j += kBoxNT) qsm[D.rx + j] = 0.0;
+            __syncthreads();
+        }
+        cl_solve(X, D, ph, false, D.rx, D.rsc, -1, -1, D.dx, D.ds, D.dz, D.dy);
+        // ---- combined direction, step length, update (batch.py:185-203)
+        mn[0] = INFINITY; mn[1] = INFINITY;
+        for (int i = tid; i < m; i += kBoxNT) {
+            const double dzi = qsm[D.dza + i] + qsm[D.dz + i], dsi = qsm[D.dsa + i] + qsm[D.ds + i];
+            qsm[D.dz + i] = dzi;
+            qsm[D.ds + i] = dsi;
+            mn[0] = fmin(mn[0], box_step(qsm[D.z + i], dzi));
+            mn[1] = fmin(mn[1], box_step(qsm[D.s + i], dsi));
+        }
+        cl_reduce<2, true>(X, mn, ph, 0, 0);
+        const double alpha = fmin(0.999 * fmin(box_step_fix(mn[0]), box_step_fix(mn[1])), 1.0);
+        for (int j = tid; j < n; j += kBoxNT) qsm[D.x + j] = fma(alpha, qsm[D.dxa + j] + qsm[D.dx + j], qsm[D.x + j]);
+        for (int i = tid; i < m; i += kBoxNT) {
+            qsm[D.s + i] = fma(alpha, qsm[D.ds + i], qsm[D.s + i]);
+            qsm[D.z + i] = fma(alpha, qsm[D.dz + i], qsm[D.z + i]);
+        }
+        for (int i = tid; i < e; i += kBoxNT) qsm[D.y + i] = fma(alpha, qsm[D.dya + i] + qsm[D.dy + i], qsm[D.y + i]);
+        __syncthreads();
+    }
+    __syncthreads();
+    for (int j = tid; j < n; j += kBoxNT) zhat[(int64_t)qp * N + j0 + j] = qsm[D.bx + j];
+    for (int i = tid; i < m; i += kBoxNT) {
+        const int64_t g = (int64_t)qp * X.mg + cl_grow(X, D, j0, i);
+        lam[g] = qsm[D.bz + i];
+        slacks[g] = qsm[D.bs + i];
+    }
+    if (rank == 0) {
+        if (nus != nullptr)
+            for (int i = tid; i < e; i += kBoxNT) nus[(int64_t)qp * e + i] = qsm[D.by + i];
+        if (tid == 0) { iters_out[qp] = iters_run; resid_out[qp] = best; }
+    }
+    cg::this_cluster().sync();       // no CTA exits while another may still read its publish buffers
+}
+
+// k_box_backward on a cluster: every CTA its slice of dx, dlam, dq, dp, dlb, dub and its columns of dA; rank 0 dnu, db
+__global__ void __launch_bounds__(kBoxNT, 1)
+k_box_backward_cl(ClDims X, const double* __restrict__ q, int64_t sq, const double* __restrict__ A, int64_t sA,
+                  const double* __restrict__ dl, const double* __restrict__ zhat, const double* __restrict__ lam,
+                  const double* __restrict__ slacks, const double* __restrict__ nus, BoxGrads O,
+                  double* __restrict__ dxv, double* __restrict__ dlamv, double* __restrict__ dnuv) {
+    QPB_SMEM;
+    const int rank = (int)cg::this_cluster().block_rank();
+    const int tid = threadIdx.x, qp = blockIdx.x / X.C;
+    int j0, ph = 0;
+    const BoxDims D = cl_local(X, rank, j0);
+    const int n = D.n, m = D.m, e = D.e, N = X.ng;
+    cl_stage(X, D, j0, q + (int64_t)qp * sq, A + (int64_t)qp * sA, nullptr);
+    for (int j = tid; j < n; j += kBoxNT) qsm[D.rx + j] = dl[(int64_t)qp * N + j0 + j];
+    for (int i = tid; i < m; i += kBoxNT) {
+        const int64_t g = (int64_t)qp * X.mg + cl_grow(X, D, j0, i);
+        qsm[D.d + i] = fmax(lam[g], 1e-8) / fmax(slacks[g], 1e-8);
+    }
+    __syncthreads();
+    cl_form(X, D);
+    cl_solve(X, D, ph, true, D.rx, -1, -1, -1, D.dx, D.ds, D.dz, D.dy);
+    for (int j = tid; j < n; j += kBoxNT) {
+        const int64_t g = (int64_t)qp * N + j0 + j;
+        const double dx = qsm[D.dx + j], z = zhat[g];
+        dxv[g] = dx;
+        if (O.dq && !O.mq) O.dq[g] = dx * z;
+        if (O.dp && !O.mp) O.dp[g] = dx;
+    }
+    for (int i = tid; i < m; i += kBoxNT) {
+        const double dz = qsm[D.dz + i];
+        dlamv[(int64_t)qp * X.mg + cl_grow(X, D, j0, i)] = dz;
+        if (i < D.nlb) { if (O.dlb && !O.mlb) O.dlb[(int64_t)qp * N + j0 + i] = dz; }
+        else if (O.dub && !O.mub) O.dub[(int64_t)qp * N + j0 + i - D.nlb] = -dz;
+    }
+    if (rank == 0)
+        for (int i = tid; i < e; i += kBoxNT) {
+            dnuv[(int64_t)qp * e + i] = qsm[D.dy + i];
+            if (O.db && !O.mb) O.db[(int64_t)qp * e + i] = -qsm[D.dy + i];
+        }
+    if (O.dA && !O.mA)
+        for (int t = tid; t < e * n; t += kBoxNT) {
+            const int i = t / n, j = t - i * n;
+            O.dA[((int64_t)qp * e + i) * N + j0 + j] = fma(qsm[D.dy + i], zhat[(int64_t)qp * N + j0 + j],
+                                                           nus[(int64_t)qp * e + i] * qsm[D.dx + j]);
+        }
+    cg::this_cluster().sync();
+}
+
+// k_box_kkt on a cluster
+__global__ void __launch_bounds__(kBoxNT, 1)
+k_box_kkt_cl(ClDims X, const double* __restrict__ q, int64_t sq, const double* __restrict__ A, int64_t sA,
+             const double* __restrict__ d, const double* __restrict__ rx, const double* __restrict__ rs,
+             const double* __restrict__ rz, const double* __restrict__ ry, double* __restrict__ dx,
+             double* __restrict__ ds, double* __restrict__ dz, double* __restrict__ dy) {
+    QPB_SMEM;
+    const int rank = (int)cg::this_cluster().block_rank();
+    const int tid = threadIdx.x, qp = blockIdx.x / X.C;
+    int j0, ph = 0;
+    const BoxDims D = cl_local(X, rank, j0);
+    const int n = D.n, m = D.m, e = D.e, N = X.ng;
+    cl_stage(X, D, j0, q + (int64_t)qp * sq, A + (int64_t)qp * sA, nullptr);
+    for (int j = tid; j < n; j += kBoxNT) qsm[D.rx + j] = rx[(int64_t)qp * N + j0 + j];
+    for (int i = tid; i < m; i += kBoxNT) {
+        const int64_t g = (int64_t)qp * X.mg + cl_grow(X, D, j0, i);
+        qsm[D.d + i] = d[g];
+        qsm[D.rsc + i] = rs[g];
+        qsm[D.rz + i] = rz[g];
+    }
+    for (int i = tid; i < e; i += kBoxNT) qsm[D.ry + i] = ry[(int64_t)qp * e + i];
+    __syncthreads();
+    cl_form(X, D);
+    cl_solve(X, D, ph, true, D.rx, D.rsc, D.rz, D.ry, D.dx, D.ds, D.dz, D.dy);
+    for (int j = tid; j < n; j += kBoxNT) dx[(int64_t)qp * N + j0 + j] = qsm[D.dx + j];
+    for (int i = tid; i < m; i += kBoxNT) {
+        const int64_t g = (int64_t)qp * X.mg + cl_grow(X, D, j0, i);
+        ds[g] = qsm[D.ds + i];
+        dz[g] = qsm[D.dz + i];
+    }
+    if (dy != nullptr && rank == 0)
+        for (int i = tid; i < e; i += kBoxNT) dy[(int64_t)qp * e + i] = qsm[D.dy + i];
+    cg::this_cluster().sync();
+}
+
 std::mutex g_mu;
 template <typename K>
 int box_set_smem(K kernel, size_t bytes, size_t* cur) {      // cur: per-kernel high-water mark (device 0..15)
@@ -476,12 +952,71 @@ int box_check_launch(const char* what) {
     return QPB200_OK;
 }
 size_t g_fwd[16], g_bwd[16], g_kkt[16];
+size_t g_cfwd[16], g_cbwd[16], g_ckkt[16];
 
 int box_plan_check(const qpb200_box_plan* P) {
-    if (P == nullptr || !P->ok) return P == nullptr ? QPB200_ERR_BAD_ARG : QPB200_ERR_TOO_LARGE;
+    if (P == nullptr) return QPB200_ERR_BAD_ARG;
+    if (P->cl_ctas != 0 && P->cl_ctas != 2 && P->cl_ctas != 4 && P->cl_ctas != 8) return QPB200_ERR_BAD_ARG;
+    if (!P->ok && !P->cl_ctas) return QPB200_ERR_TOO_LARGE;
     return QPB200_OK;
 }
 BoxDims plan_dims(const qpb200_box_plan* P) { return box_dims(P->nz, P->neq, P->has_lb, P->has_ub); }
+ClDims plan_cl_dims(const qpb200_box_plan* P) { return cl_dims(P->nz, P->neq, P->has_lb, P->has_ub, P->cl_ctas); }
+
+// Whether a cluster of C CTAs with `bytes` of shared memory each can be resident at all (cudaOccupancyMaxActiveClusters
+// > 0), checked once per (kernel, C, bytes, device): QPB200_ERR_TOO_LARGE if not.
+struct ClKey {
+    const void* k; int C; size_t bytes; int dev;
+    bool operator<(const ClKey& o) const {
+        if (k != o.k) return k < o.k;
+        if (C != o.C) return C < o.C;
+        if (bytes != o.bytes) return bytes < o.bytes;
+        return dev < o.dev;
+    }
+};
+std::map<ClKey, bool> g_cl_ok;
+
+template <typename K>
+int cl_prepare(K kernel, int C, size_t bytes, size_t* cur) {
+    int rc = box_set_smem(kernel, bytes, cur);
+    if (rc) return rc;
+    int dev = 0;
+    cudaError_t err = cudaGetDevice(&dev);
+    if (err != cudaSuccess) { qpb200_internal_cuda_error((int)err, "cudaGetDevice"); return QPB200_ERR_CUDA; }
+    const ClKey key{(const void*)kernel, C, bytes, dev};
+    std::lock_guard<std::mutex> lock(g_mu);
+    auto it = g_cl_ok.find(key);
+    if (it == g_cl_ok.end()) {
+        cudaLaunchConfig_t cfg = {};
+        cudaLaunchAttribute at[1];
+        at[0].id = cudaLaunchAttributeClusterDimension;
+        at[0].val.clusterDim.x = C; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
+        cfg.gridDim = dim3(C); cfg.blockDim = dim3(kBoxNT); cfg.dynamicSmemBytes = bytes;
+        cfg.attrs = at; cfg.numAttrs = 1;
+        int nclusters = 0;
+        err = cudaOccupancyMaxActiveClusters(&nclusters, (const void*)kernel, &cfg);
+        if (err != cudaSuccess) {
+            qpb200_internal_cuda_error((int)err, "cudaOccupancyMaxActiveClusters");
+            return QPB200_ERR_CUDA;
+        }
+        it = g_cl_ok.emplace(key, nclusters > 0).first;
+    }
+    return it->second ? QPB200_OK : QPB200_ERR_TOO_LARGE;
+}
+
+template <typename... KArgs, typename... Args>
+int cl_launch(const char* what, void (*kernel)(KArgs...), int C, int nbatch, size_t bytes, cudaStream_t st,
+              Args&&... args) {
+    cudaLaunchConfig_t cfg = {};
+    cudaLaunchAttribute at[1];
+    at[0].id = cudaLaunchAttributeClusterDimension;
+    at[0].val.clusterDim.x = C; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
+    cfg.gridDim = dim3((unsigned)nbatch * (unsigned)C); cfg.blockDim = dim3(kBoxNT); cfg.dynamicSmemBytes = bytes;
+    cfg.stream = st; cfg.attrs = at; cfg.numAttrs = 1;
+    const cudaError_t err = cudaLaunchKernelEx(&cfg, kernel, std::forward<Args>(args)...);
+    if (err != cudaSuccess) { qpb200_internal_cuda_error((int)err, what); return QPB200_ERR_CUDA; }
+    return box_check_launch(what);
+}
 
 }  // namespace
 
@@ -490,7 +1025,8 @@ extern "C" {
 int qpb200_box_plan_init(int nz, int neq, int has_lb, int has_ub, qpb200_box_plan* plan) {
     if (plan == nullptr || nz <= 0 || neq < 0) return QPB200_ERR_BAD_ARG;
     if (!has_lb && !has_ub) return QPB200_ERR_NO_CONSTRAINTS;
-    if (nz > 4096 || neq > 4096) return QPB200_ERR_TOO_LARGE;
+    // past every path: the dense kernels stop at 4096, and 8 CTAs of 227 KB hold fewer than 12000 variables
+    if (nz > 16384 || neq > 4096) return QPB200_ERR_TOO_LARGE;
     memset(plan, 0, sizeof(*plan));
     plan->nz = nz; plan->neq = neq; plan->neq_pad = r8(neq);
     plan->has_lb = has_lb ? 1 : 0; plan->has_ub = has_ub ? 1 : 0;
@@ -499,6 +1035,31 @@ int qpb200_box_plan_init(int nz, int neq, int has_lb, int has_ub, qpb200_box_pla
     const BoxDims D = box_dims(nz, neq, plan->has_lb, plan->has_ub);
     plan->smem_bytes = (int64_t)D.total * 8;
     plan->ok = (plan->neq_pad <= kBoxNT && plan->smem_bytes <= kBoxMaxSmem) ? 1 : 0;
+    // the cluster kernels: the smallest cluster whose slice fits, for shapes one CTA does not hold.
+    // QPB200_BOX_CLUSTER=C (development knob, C in {2, 4, 8}) forces them where that C fits.
+    if (plan->neq_pad <= kBoxNT) {
+        auto fits = [&](int C) {
+            return (int64_t)cl_dims(nz, neq, plan->has_lb, plan->has_ub, C).total * 8 <= kBoxMaxSmem;
+        };
+        const char* env = getenv("QPB200_BOX_CLUSTER");
+        const int forced = env ? atoi(env) : 0;
+        int C = 0;
+        if ((forced == 2 || forced == 4 || forced == 8) && fits(forced)) C = forced;
+        else if (!plan->ok)
+            for (int c = 2; c <= 8 && !C; c *= 2)
+                if (fits(c)) C = c;
+        if (C) {
+            const ClDims X = cl_dims(nz, neq, plan->has_lb, plan->has_ub, C);
+            plan->cl_ctas = C;
+            plan->cl_slice = X.slice;
+            plan->cl_smem_bytes = (int64_t)X.total * 8;
+        }
+    }
+    if (!plan->ok && !plan->cl_ctas) {          // only the dense kernels on the dense equivalent are left
+        qpb200_plan dp;
+        const int rc = qpb200_plan_init(nz, plan->nineq, neq, &dp);
+        if (rc == QPB200_ERR_TOO_LARGE) return rc;
+    }
     return QPB200_OK;
 }
 
@@ -511,6 +1072,15 @@ int qpb200_box_forward(const qpb200_box_plan* plan, int nbatch, const double* q,
     if (rc) return rc;
     if (nbatch <= 0 || maxIter < 1 || !q || !p || !zhat || !lam || !slacks || !iters || !best_resid) return QPB200_ERR_BAD_ARG;
     if ((plan->has_lb && !lb) || (plan->has_ub && !ub) || (plan->neq > 0 && (!A || !b || !nus))) return QPB200_ERR_BAD_ARG;
+    if (plan->cl_ctas) {
+        const ClDims X = plan_cl_dims(plan);
+        const size_t bytes = (size_t)X.total * 8;
+        rc = cl_prepare(k_box_forward_cl, X.C, bytes, g_cfwd);
+        if (rc) return rc;
+        return cl_launch("k_box_forward_cl", k_box_forward_cl, X.C, nbatch, bytes, (cudaStream_t)stream, X, q, sq, p,
+                         sp, A, sA, b, sb, lb, slb, ub, sub, eps, stall_tol, best_tie, notImprovedLim, maxIter, zhat,
+                         lam, slacks, nus, iters, best_resid, trace, spd_flag);
+    }
     const BoxDims D = plan_dims(plan);
     rc = box_set_smem(k_box_forward, (size_t)plan->smem_bytes, g_fwd);
     if (rc) return rc;
@@ -535,12 +1105,21 @@ int qpb200_box_backward(const qpb200_box_plan* plan, int nbatch, const double* q
     BoxGrads O;
     O.dq = dq; O.dp = dp; O.dlb = dlb; O.dub = dub; O.dA = e > 0 ? dA : nullptr; O.db = e > 0 ? db : nullptr;
     O.mq = mean_q; O.mp = mean_p; O.mlb = mean_lb; O.mub = mean_ub; O.mA = mean_A; O.mb = mean_b;
-    rc = box_set_smem(k_box_backward, (size_t)plan->smem_bytes, g_bwd);
-    if (rc) return rc;
     cudaStream_t st = (cudaStream_t)stream;
-    k_box_backward<<<nbatch, kBoxNT, (size_t)plan->smem_bytes, st>>>(D, q, sq, A, sA, dl_dzhat, zhat, lam, slacks, nus,
-                                                                     O, dxv, dlamv, dnuv);
-    rc = box_check_launch("k_box_backward");
+    if (plan->cl_ctas) {
+        const ClDims X = plan_cl_dims(plan);
+        const size_t bytes = (size_t)X.total * 8;
+        rc = cl_prepare(k_box_backward_cl, X.C, bytes, g_cbwd);
+        if (rc) return rc;
+        rc = cl_launch("k_box_backward_cl", k_box_backward_cl, X.C, nbatch, bytes, st, X, q, sq, A, sA, dl_dzhat, zhat,
+                       lam, slacks, nus, O, dxv, dlamv, dnuv);
+    } else {
+        rc = box_set_smem(k_box_backward, (size_t)plan->smem_bytes, g_bwd);
+        if (rc) return rc;
+        k_box_backward<<<nbatch, kBoxNT, (size_t)plan->smem_bytes, st>>>(D, q, sq, A, sA, dl_dzhat, zhat, lam, slacks,
+                                                                         nus, O, dxv, dlamv, dnuv);
+        rc = box_check_launch("k_box_backward");
+    }
     if (rc) return rc;
     const int TB = 128;
     if (dq && mean_q) k_box_mean_vec<<<(n + TB - 1) / TB, TB, 0, st>>>(nbatch, n, dxv, n, zhat, 1.0, dq);
@@ -562,6 +1141,14 @@ int qpb200_box_solve_kkt(const qpb200_box_plan* plan, int nbatch, const double* 
     if (rc) return rc;
     if (nbatch <= 0 || !q || !d || !rx || !rs || !rz || !dx || !ds || !dz) return QPB200_ERR_BAD_ARG;
     if (plan->neq > 0 && (!A || !ry || !dy)) return QPB200_ERR_BAD_ARG;
+    if (plan->cl_ctas) {
+        const ClDims X = plan_cl_dims(plan);
+        const size_t bytes = (size_t)X.total * 8;
+        rc = cl_prepare(k_box_kkt_cl, X.C, bytes, g_ckkt);
+        if (rc) return rc;
+        return cl_launch("k_box_kkt_cl", k_box_kkt_cl, X.C, nbatch, bytes, (cudaStream_t)stream, X, q, sq, A, sA, d, rx,
+                         rs, rz, ry, dx, ds, dz, dy);
+    }
     const BoxDims D = plan_dims(plan);
     rc = box_set_smem(k_box_kkt, (size_t)plan->smem_bytes, g_kkt);
     if (rc) return rc;
