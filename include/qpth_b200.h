@@ -182,7 +182,10 @@ typedef struct qpb200_box_plan {
      * owning the variables [r cl_slice, (r + 1) cl_slice). cl_ctas is the smallest of 2, 4, 8 whose slice fits 227 KB
      * (0: no cluster covers the shape). The entry points below use them whenever cl_ctas != 0, and return
      * QPB200_ERR_TOO_LARGE if the device cannot make such a cluster resident. QPB200_BOX_CLUSTER=C (development knob)
-     * forces C on shapes with ok == 1 too. */
+     * forces C on shapes with ok == 1 too.
+     * neq_pad > threads selects the distributed-M cluster kernels instead: M = A H^-1 A' is spread over the cluster by
+     * 8-row block rows (rank i mod C), cl_smem_bytes is the largest rank's share. They are chosen where the dense path
+     * rejects the shape or its order ms_pad exceeds 384 (the knob forces them on any neq_pad > threads shape C fits). */
     int cl_ctas;
     int cl_slice;           /* variables per CTA (the last CTA may hold fewer) */
     int64_t cl_smem_bytes;  /* dynamic shared memory per CTA */

@@ -139,8 +139,8 @@ _box_plans = {}
 
 def box_plan_for(nz, neq, has_lb, has_ub):
     """Plan of the box-QP kernels for a shape (cached; no device work). plan.ok: the one-CTA kernels cover it;
-    plan.cl_ctas: the cluster kernels do (QPB200_BOX_CLUSTER, a development knob read by qpb200_box_plan_init,
-    forces them: part of the key)."""
+    plan.cl_ctas: the cluster kernels do, with M distributed over the cluster when plan.neq_pad > 128
+    (QPB200_BOX_CLUSTER, a development knob read by qpb200_box_plan_init, forces them: part of the key)."""
     key = (nz, neq, bool(has_lb), bool(has_ub), os.environ.get("QPB200_BOX_CLUSTER"))
     if key not in _box_plans:
         p = BoxPlan()

@@ -9,8 +9,10 @@ every row of G equal to +-e_i the inequality block is eliminated in closed form,
 M = A H^-1 A' (order neq, H = q + G'DG diagonal) - nothing at all without equality constraints - and needs no
 pre_factor_kkt (csrc/qp_box.cu). One CTA solves one QP where A and the vectors fit its 227 KB of shared memory
 (qpb200_box_plan.ok); past that, a thread block cluster of 2, 4 or 8 CTAs does, each CTA holding a slice of the
-variables (plan.cl_ctas; e.g. the capped-simplex projection over thousands of classes). Shapes neither covers
-(neq > 128, or beyond a cluster's pooled shared memory) run the dense kernels on the dense equivalent instead.
+variables (plan.cl_ctas; e.g. the capped-simplex projection over thousands of classes). With more than 128 equality
+rows (the 9x9 sudoku layer: nz = 729, neq = 249) the cluster also distributes the factor of M (plan.cl_ctas with
+plan.neq_pad > 128), where the dense equivalent's order exceeds 384 or the dense kernels reject it. Shapes none of these
+covers run the dense kernels on the dense equivalent instead.
 
 The OptNet sudoku layer (Q = 0.1 I, G = -I, h = 0, a learned A) is one such problem; a differentiable projection
 min 1/2 ||z - v||^2 s.t. Az = b, lb <= z <= ub is another (q = 1, p = -v).

@@ -11,8 +11,9 @@
 // One 128-thread CTA per QP; A (neq x nz, row stride nz | 1), the factor of M and every vector live in shared memory.
 // The kernels cover neq_pad <= 128 (the substitutions own one row per thread) and a footprint within the 227 KB an
 // H100 CTA may use (qpb200_box_plan.ok). Past that, the cluster kernels (k_box_*_cl, below) split one QP's variables
-// over a thread block cluster of 2, 4 or 8 CTAs (qpb200_box_plan.cl_ctas); BoxQPFunction runs the dense kernels on the
-// dense equivalent only where neither covers the shape.
+// over a thread block cluster of 2, 4 or 8 CTAs (qpb200_box_plan.cl_ctas), and past neq_pad = 128 the distributed-M
+// kernels (k_box_*_dm) spread M over the cluster as well; BoxQPFunction runs the dense kernels on the dense equivalent
+// only where none covers the shape.
 #include <cooperative_groups.h>
 #include <cuda_runtime.h>
 #include <math.h>
@@ -933,6 +934,636 @@ k_box_kkt_cl(ClDims X, const double* __restrict__ q, int64_t sq, const double* _
     cg::this_cluster().sync();
 }
 
+// ---- distributed-M kernels: neq_pad > 128 on a cluster ---------------------------------------------------------------
+// Past neq_pad = 128 a full copy of M per CTA no longer fits (the staircase of order 256 alone is 272 KB). These kernels
+// keep the variable slices, the reductions, the Mehrotra loop and the invariant of the cluster kernels above, but M is
+// DISTRIBUTED: block row i of the staircase (8 rows, columns 0 .. 8i+7) lives on rank i mod C, which balances both the
+// storage and the trailing-update work. A is read from global memory (a shared A stays in L2 for the whole batch).
+//   form:     the full H^-1 is gathered from the slices; column chunks of A are staged through shared memory and every
+//             CTA forms its own block rows, M_ij = sum_v A_iv h_v A_jv, with DMMA 8x8x4.
+//   factor:   pf_chol's steps. F_k: the owner of block row k factors the diagonal tile and publishes T_k there. After a
+//             cluster barrier, S_k: every CTA forms L_ik (into its panel rows) and P_ik for its own block rows and
+//             sweeps its rows of the running right-hand side with b_k. After a second barrier, U_k: every CTA copies the
+//             panel rows of the other ranks that its trailing tiles need and updates its own tiles.
+//   sweeps:   forward (corrector): one barrier per block step, after which b_k is final on its owner. pf_diag: local.
+//             Backward: one barrier per block step; each CTA adds P_ik' w_i of its own block rows into a partial, and
+//             the owner of block k sums the partials in rank order. Then dy is gathered into every CTA.
+// dy is computed once, by the owners of its blocks, and copied: every CTA holds it bit for bit, so everything derived
+// from it is cluster-wide and the branch rule of the cluster kernels holds unchanged.
+struct DmDims {
+    ClDims X;                // slices and reductions; X.L.S: this CTA's block rows, X.L.pan: panel rows of all of M
+    int nts;                 // block rows of M
+    int hfull, Tk, cv, part, wpub, As;   // full H^-1, T_k and b_k, pf_diag output, backward partial, w blocks, A chunk
+    int total;               // doubles per CTA (the rank with the largest share of M)
+};
+constexpr int kDmKC = 16;                // columns of A per staged chunk
+constexpr int kDmLdA = kDmKC + 4;        // row stride of the chunk (== 4 mod 16: conflict-free DMMA fragment reads)
+constexpr int kDmDenseOrder = 384;       // dense order ms_pad past which they are chosen (H100: parity at 384, 2.2x at 504)
+
+// local offset of the li-th own block row (block i = rank + C li, 8 (8i + 12) doubles each) and own block-row count
+__host__ __device__ inline int dm_boff(int C, int rank, int li) { return 64 * rank * li + 32 * C * li * (li - 1) + 96 * li; }
+__host__ __device__ inline int dm_nblk(int nts, int C, int rank) { return rank < nts ? (nts - rank + C - 1) / C : 0; }
+// first own block row below block k
+__device__ __forceinline__ int dm_below(int C, int rank, int k) { return (k >= rank) ? (k - rank) / C + 1 : 0; }
+
+__host__ __device__ inline DmDims dm_dims(int n, int e, int has_lb, int has_ub, int C) {
+    DmDims Y;
+    ClDims& X = Y.X;
+    X.C = C; X.slice = (n + C - 1) / C; X.ng = n;
+    X.nlbg = has_lb ? n : 0; X.mg = (has_lb ? n : 0) + (has_ub ? n : 0);
+    BoxDims& D = X.L;
+    D.n = X.slice; D.e = e; D.ep = r8(e);
+    D.nlb = has_lb ? X.slice : 0; D.m = (has_lb ? X.slice : 0) + (has_ub ? X.slice : 0);
+    D.lda = 0; D.A = 0; D.tab = 0; D.red = 0;           // (A is not staged; no tile table, no block reductions)
+    Y.nts = D.ep >> 3;
+    int stair = 0;
+    for (int r = 0; r < C; ++r) {
+        const int s = dm_boff(C, r, dm_nblk(Y.nts, C, r));
+        stair = s > stair ? s : stair;
+    }
+    int o = 0;
+    D.S = o; o += r8(stair);
+    D.pan = o; o += 8 * Y.nts * kPanLd;
+    const int nn = r8(D.n), mm = r8(D.m), ee = D.ep;
+    int* vn[] = {&D.q, &D.p, &D.x, &D.rx, &D.r, &D.hinv, &D.dxa, &D.dx, &D.bx};
+    for (int* v : vn) { *v = o; o += nn; }
+    int* vm[] = {&D.h, &D.s, &D.z, &D.d, &D.rz, &D.dsa, &D.dza, &D.ds, &D.dz, &D.bs, &D.bz, &D.rsc};
+    for (int* v : vm) { *v = o; o += mm; }
+    int* ve[] = {&D.b, &D.y, &D.ry, &D.rhs, &D.t, &D.dya, &D.dy, &D.by};
+    for (int* v : ve) { *v = o; o += ee; }
+    D.total = o;
+    X.Mp = 0;
+    X.pb = r8(ee + 4 * kClW);
+    X.pub = o; o += 2 * X.pb;
+    Y.hfull = o; o += r8(n) + kDmKC;                     // zero past n: the last chunk reads it
+    Y.Tk = o; o += 72;                                   // T_k (64, upper part zero), then b_k (8)
+    Y.cv = o; o += ee;
+    Y.part = o; o += ee;
+    Y.wpub = o; o += ee;
+    Y.As = o; o += ee * kDmLdA;
+    X.total = Y.total = o;
+    return Y;
+}
+
+// hinv for this CTA's variables, the gathered full H^-1, and this CTA's block rows of M (identity rows beyond neq).
+// One cluster barrier; ends with a block barrier.
+__device__ __noinline__ void dm_form(const DmDims& Y, const BoxDims& D, int rank, const double* __restrict__ Ag) {
+    QPB_SMEM;
+    cg::cluster_group cl = cg::this_cluster();
+    const ClDims& X = Y.X;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, g = lane >> 2, q = lane & 3;
+    const int N = X.ng, e = D.e, C = X.C, nb = dm_nblk(Y.nts, C, rank);
+    for (int j = tid; j < D.n; j += kBoxNT) {
+        double hj = qsm[D.q + j];
+        if (D.nlb) hj += qsm[D.d + j];
+        if (D.m > D.nlb) hj += qsm[D.d + D.nlb + j];
+        qsm[D.hinv + j] = 1.0 / hj;
+    }
+    cl.sync();                                           // every slice of H^-1 is published
+    for (int v = tid; v < r8(N) + kDmKC; v += kBoxNT)
+        qsm[Y.hfull + v] = (v < N) ? cl.map_shared_rank(qsm + D.hinv, v / X.slice)[v % X.slice] : 0.0;
+    double* S = qsm + D.S;
+    const double* As = qsm + Y.As;
+    const double* hf = qsm + Y.hfull;
+    for (int v0 = 0; v0 < N; v0 += kDmKC) {
+        __syncthreads();                                 // the previous chunk is consumed (first: H^-1 is gathered)
+        for (int t = tid; t < D.ep * kDmKC; t += kBoxNT) {
+            const int r = t / kDmKC, c = t - r * kDmKC, v = v0 + c;
+            qsm[Y.As + r * kDmLdA + c] = (r < e && v < N) ? Ag[(int64_t)r * N + v] : 0.0;
+        }
+        __syncthreads();
+        // own tiles (i, j), j <= i, dealt round-robin over the warps (cnt is warp-uniform)
+        int cnt = 0;
+        for (int li = 0; li < nb; ++li) {
+            const int i = rank + C * li;
+            double* rowp = S + dm_boff(C, rank, li) + g * (8 * i + 12) + 2 * q;
+            const double* ai = As + (8 * i + g) * kDmLdA + q;
+            for (int j = 0; j <= i; ++j, ++cnt) {
+                if ((cnt & (kClW - 1)) != warp) continue;
+                double2 acc = (v0 == 0) ? make_double2(0.0, 0.0) : *reinterpret_cast<const double2*>(rowp + 8 * j);
+                const double* aj = As + (8 * j + g) * kDmLdA + q;
+#pragma unroll
+                for (int kk = 0; kk < kDmKC; kk += 4) qpb::dmma884(acc.x, acc.y, ai[kk] * hf[v0 + kk + q], aj[kk]);
+                *reinterpret_cast<double2*>(rowp + 8 * j) = acc;
+            }
+        }
+    }
+    __syncthreads();
+    for (int t = tid; t < 8 * nb; t += kBoxNT) {
+        const int li = t >> 3, i = rank + C * li, r = 8 * i + (t & 7);
+        if (r >= e) S[dm_boff(C, rank, li) + (t & 7) * (8 * i + 12) + r] = 1.0;
+    }
+    __syncthreads();
+}
+
+// pf_chol over the cluster, with the running right-hand side b (offset; this CTA's block rows are meaningful) carried
+// along. 2 nts - 1 cluster barriers; ends with a block barrier.
+__device__ __noinline__ void dm_chol(const DmDims& Y, const BoxDims& D, int rank, int b) {
+    QPB_SMEM;
+    cg::cluster_group cl = cg::this_cluster();
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, g = lane >> 2, q = lane & 3;
+    const int C = Y.X.C, nts = Y.nts, nb = dm_nblk(nts, C, rank);
+    double* S = qsm + D.S;
+    double* P = qsm + D.pan;
+    double* Tk = qsm + Y.Tk;
+#pragma unroll 1
+    for (int k = 0; k < nts; ++k) {
+        const int k0 = 8 * k, own = k % C, lk = k / C, ldk = 8 * k + 12;
+        if (rank == own && warp == 0) {                  // F_k
+            double* Mb = S + dm_boff(C, rank, lk) + k0;
+            double Lk[36], Tc[8];
+#pragma unroll
+            for (int r = 0; r < 8; ++r)
+#pragma unroll
+                for (int c = 0; c <= r; ++c) Lk[QPB_LIDX(r, c)] = Mb[r * ldk + c];
+            __syncwarp();
+            pf_factor8(Lk);
+            pf_inv8_col(Lk, lane & 7, Tc);
+            if (lane < 8) {
+#pragma unroll
+                for (int r = 0; r < 8; ++r)
+                    if (r >= lane) Mb[r * ldk + lane] = Tc[r];
+            }
+        }
+        cl.sync();                                       // T_k and b_k are final on their owner
+        {
+            const double* Mo = cl.map_shared_rank(S, own) + dm_boff(C, own, lk) + k0;
+            for (int t = tid; t < 64; t += kBoxNT) {
+                const int r = t >> 3, c = t & 7;
+                Tk[t] = (c <= r) ? Mo[r * ldk + c] : 0.0;
+            }
+            if (tid < 8) Tk[64 + tid] = cl.map_shared_rank(qsm + b, own)[k0 + tid];
+        }
+        __syncthreads();
+        const int lo = dm_below(C, rank, k);
+        {                                                // S_k: one own block row per warp
+            const double bT0 = Tk[g * 8 + q], bT1 = Tk[g * 8 + q + 4];      // T[g][q], T[g][q+4]
+            const double bP0 = Tk[q * 8 + g], bP1 = Tk[(q + 4) * 8 + g];    // T[q][g], T[q+4][g]
+#pragma unroll 1
+            for (int li = lo + warp; li < nb; li += kClW) {
+                const int i = rank + C * li;
+                double* row = S + dm_boff(C, rank, li) + g * (8 * i + 12) + k0;
+                const double a0 = row[q], a1 = row[q + 4];
+                double d0 = 0.0, d1 = 0.0;
+                qpb::dmma884(d0, d1, a0, bT0);
+                qpb::dmma884(d0, d1, a1, bT1);
+                double* pl = P + (8 * i + g) * kPanLd;
+                *reinterpret_cast<double2*>(pl + 2 * q) = make_double2(d0, d1);
+                __syncwarp();
+                const double la0 = pl[q], la1 = pl[q + 4];
+                double e0 = 0.0, e1 = 0.0;
+                qpb::dmma884(e0, e1, la0, bP0);
+                qpb::dmma884(e0, e1, la1, bP1);
+                *reinterpret_cast<double2*>(row + 2 * q) = make_double2(e0, e1);
+            }
+        }
+        __syncthreads();
+        for (int t = 8 * lo + tid; t < 8 * nb; t += kBoxNT) {       // b_r -= P[r][k0 .. k0+7] . b_k, own rows below k
+            const int li = t >> 3, i = rank + C * li, rr = t & 7;
+            const double* pr = S + dm_boff(C, rank, li) + rr * (8 * i + 12) + k0;
+            double s0 = qsm[b + 8 * i + rr], s1 = 0.0;
+#pragma unroll
+            for (int c = 0; c < 8; c += 2) { s0 = fma(-pr[c], Tk[64 + c], s0); s1 = fma(-pr[c + 1], Tk[65 + c], s1); }
+            qsm[b + 8 * i + rr] = s0 + s1;
+        }
+        if (k + 1 == nts) break;
+        cl.sync();                                       // every panel row of step k is written
+        const int nj = (nb > 0) ? rank + C * (nb - 1) - k : 0;       // block rows k+1 .. this CTA's last one
+        for (int t = tid; t < 64 * nj; t += kBoxNT) {
+            const int j = k + 1 + (t >> 6), o = (8 * j + ((t >> 3) & 7)) * kPanLd + (t & 7);
+            if (j % C != rank) P[o] = cl.map_shared_rank(P, j % C)[o];
+        }
+        __syncthreads();
+        int cnt = 0;                                     // U_k: own tiles (i, j), k < j <= i, round-robin
+#pragma unroll 1
+        for (int li = lo; li < nb; ++li) {
+            const int i = rank + C * li;
+            double* rowp = S + dm_boff(C, rank, li) + g * (8 * i + 12) + 2 * q;
+            const double la0 = P[(8 * i + g) * kPanLd + q], la1 = P[(8 * i + g) * kPanLd + q + 4];
+#pragma unroll 1
+            for (int j = k + 1; j <= i; ++j, ++cnt) {
+                if ((cnt & (kClW - 1)) != warp) continue;
+                double2 v = *reinterpret_cast<const double2*>(rowp + 8 * j);
+                const double* pb = P + (8 * j + g) * kPanLd + q;
+                qpb::dmma884(v.x, v.y, -la0, pb[0]);
+                qpb::dmma884(v.x, v.y, -la1, pb[4]);
+                *reinterpret_cast<double2*>(rowp + 8 * j) = v;
+            }
+        }
+        __syncthreads();
+    }
+    __syncthreads();
+}
+
+// pf_fwd over the cluster with an existing factor: b_i -= P_ik b_k. nts - 1 cluster barriers; ends with a block barrier.
+__device__ __noinline__ void dm_fwd(const DmDims& Y, const BoxDims& D, int rank, int b) {
+    QPB_SMEM;
+    cg::cluster_group cl = cg::this_cluster();
+    const int tid = threadIdx.x, C = Y.X.C, nts = Y.nts, nb = dm_nblk(nts, C, rank);
+    const double* S = qsm + D.S;
+#pragma unroll 1
+    for (int k = 0; k + 1 < nts; ++k) {
+        cl.sync();                                       // b_k is final on its owner
+        const double* bk = cl.map_shared_rank(qsm + b, k % C) + 8 * k;
+        for (int t = 8 * dm_below(C, rank, k) + tid; t < 8 * nb; t += kBoxNT) {
+            const int li = t >> 3, i = rank + C * li, rr = t & 7;
+            const double* pr = S + dm_boff(C, rank, li) + rr * (8 * i + 12) + 8 * k;
+            double s0 = qsm[b + 8 * i + rr], s1 = 0.0;
+#pragma unroll
+            for (int c = 0; c < 8; c += 2) { s0 = fma(-pr[c], bk[c], s0); s1 = fma(-pr[c + 1], bk[c + 1], s1); }
+            qsm[b + 8 * i + rr] = s0 + s1;
+        }
+    }
+    __syncthreads();
+}
+
+// pf_diag on this CTA's block rows: c_k = T_k^T (T_k b_k), with y a scratch vector. c != b (other CTAs may still read b).
+// Ends with a block barrier.
+__device__ __noinline__ void dm_diag(const DmDims& Y, const BoxDims& D, int rank, int b, int y, int c) {
+    QPB_SMEM;
+    const int tid = threadIdx.x, C = Y.X.C, nb = dm_nblk(Y.nts, C, rank);
+    const double* S = qsm + D.S;
+    for (int t = tid; t < 8 * nb; t += kBoxNT) {
+        const int li = t >> 3, i = rank + C * li, r = t & 7, ld = 8 * i + 12;
+        const double* Tr = S + dm_boff(C, rank, li) + r * ld + 8 * i;       // row r of T_k
+        double s0 = 0.0, s1 = 0.0;
+#pragma unroll
+        for (int cc = 0; cc < 8; cc += 2) {
+            s0 = fma((cc <= r) ? Tr[cc] : 0.0, (cc <= r) ? qsm[b + 8 * i + cc] : 0.0, s0);
+            s1 = fma((cc + 1 <= r) ? Tr[cc + 1] : 0.0, (cc + 1 <= r) ? qsm[b + 8 * i + cc + 1] : 0.0, s1);
+        }
+        qsm[y + 8 * i + r] = s0 + s1;
+    }
+    __syncthreads();
+    for (int t = tid; t < 8 * nb; t += kBoxNT) {
+        const int li = t >> 3, i = rank + C * li, r = t & 7, ld = 8 * i + 12;
+        const double* Tc = S + dm_boff(C, rank, li) + 8 * i + r;            // column r of T_k: T[j][r] at Tc[j ld]
+        double s0 = 0.0, s1 = 0.0;
+#pragma unroll
+        for (int j = 0; j < 8; j += 2) {
+            s0 = fma((j >= r) ? Tc[j * ld] : 0.0, (j >= r) ? qsm[y + 8 * i + j] : 0.0, s0);
+            s1 = fma((j + 1 >= r) ? Tc[(j + 1) * ld] : 0.0, (j + 1 >= r) ? qsm[y + 8 * i + j + 1] : 0.0, s1);
+        }
+        qsm[c + 8 * i + r] = s0 + s1;
+    }
+    __syncthreads();
+}
+
+// pf_bwd over the cluster: w_k = c_k - sum_{i>k} P_ik' w_i, then w gathered into every CTA (offset w, length ep).
+// nts + 1 cluster barriers; ends with a block barrier.
+__device__ __noinline__ void dm_bwd(const DmDims& Y, const BoxDims& D, int rank, int c, int w) {
+    QPB_SMEM;
+    cg::cluster_group cl = cg::this_cluster();
+    const int tid = threadIdx.x, C = Y.X.C, nts = Y.nts, ep = D.ep;
+    const double* S = qsm + D.S;
+    double* part = qsm + Y.part;
+    double* wp = qsm + Y.wpub;
+    for (int t = tid; t < ep; t += kBoxNT) part[t] = 0.0;
+#pragma unroll 1
+    for (int i = nts - 1; i >= 0; --i) {
+        cl.sync();                                       // every partial holds the block rows below i
+        if (rank == i % C) {                             // (CTA-uniform)
+            const int i0 = 8 * i, ld = 8 * i + 12;
+            if (tid < 8) {
+                double s = qsm[c + i0 + tid];
+                for (int r = 0; r < C; ++r) s -= cl.map_shared_rank(part, r)[i0 + tid];
+                wp[i0 + tid] = s;
+            }
+            __syncthreads();
+            const double* blk = S + dm_boff(C, rank, i / C);
+            for (int t = tid; t < i0; t += kBoxNT) {
+                double s0 = part[t], s1 = 0.0;
+#pragma unroll
+                for (int rr = 0; rr < 8; rr += 2) {
+                    s0 = fma(blk[rr * ld + t], wp[i0 + rr], s0);
+                    s1 = fma(blk[(rr + 1) * ld + t], wp[i0 + rr + 1], s1);
+                }
+                part[t] = s0 + s1;
+            }
+        }
+    }
+    cl.sync();                                           // every block of w is final on its owner
+    for (int t = tid; t < ep; t += kBoxNT) qsm[w + t] = cl.map_shared_rank(wp, (t >> 3) % C)[t];
+    __syncthreads();
+}
+
+// cl_solve with M distributed (Ag: this QP's A in global memory). Ends with a block barrier.
+__device__ __noinline__ void dm_solve(const DmDims& Y, const BoxDims& D, int rank, const double* __restrict__ Ag, int j0,
+                                      int& ph, bool fresh, int rx, int rs, int rz, int ry, int dx, int ds, int dz, int dy) {
+    QPB_SMEM;
+    cg::cluster_group cl = cg::this_cluster();
+    const ClDims& X = Y.X;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int n = D.n, m = D.m, e = D.e, ep = D.ep, N = X.ng;
+    for (int j = tid; j < n; j += kBoxNT) {
+        double a = qsm[rx + j];
+        if (D.nlb) {
+            const double t = ((rz >= 0) ? qsm[D.d + j] * qsm[rz + j] : 0.0) - ((rs >= 0) ? qsm[rs + j] : 0.0);
+            a -= t;
+        }
+        if (m > D.nlb) {
+            const int i = D.nlb + j;
+            const double t = ((rz >= 0) ? qsm[D.d + i] * qsm[rz + i] : 0.0) - ((rs >= 0) ? qsm[rs + i] : 0.0);
+            a += t;
+        }
+        qsm[D.r + j] = a * qsm[D.hinv + j];
+    }
+    __syncthreads();
+    const int buf = cl_buf(X, ph);
+    for (int i = warp; i < e; i += kClW) {
+        double a = 0.0;
+        for (int k = lane; k < n; k += 32) a = fma(Ag[(int64_t)i * N + j0 + k], qsm[D.r + k], a);
+        a = qpb::warp_sum(a);
+        if (lane == 0) qsm[buf + i] = a;
+    }
+    cl.sync();                                           // the partials of A H^-1 r are published
+    for (int i = tid; i < ep; i += kBoxNT) {
+        double a = 0.0;
+        if (i < e)
+            for (int k = 0; k < X.C; ++k) a += cl.map_shared_rank(qsm + buf, k)[i];
+        qsm[D.rhs + i] = (i < e) ? (((ry >= 0) ? qsm[ry + i] : 0.0) - a) : 0.0;
+    }
+    ++ph;
+    __syncthreads();
+    if (fresh) dm_chol(Y, D, rank, D.rhs);
+    else dm_fwd(Y, D, rank, D.rhs);
+    dm_diag(Y, D, rank, D.rhs, D.t, Y.cv);
+    dm_bwd(Y, D, rank, Y.cv, dy);
+    for (int j = tid; j < n; j += kBoxNT) {
+        double a = 0.0;
+        for (int i = 0; i < e; ++i) a = fma(Ag[(int64_t)i * N + j0 + j], qsm[dy + i], a);
+        qsm[dx + j] = -qsm[D.r + j] - a * qsm[D.hinv + j];
+    }
+    __syncthreads();
+    for (int i = tid; i < m; i += kBoxNT) {
+        const double di = qsm[D.d + i];
+        const double rsi = (rs >= 0) ? qsm[rs + i] : 0.0;
+        const double dzi = di * (bsgn(D, i) * qsm[dx + bvar(D, i)] + ((rz >= 0) ? qsm[rz + i] : 0.0)) - rsi;
+        qsm[dz + i] = dzi;
+        qsm[ds + i] = (-rsi - dzi) / di;
+    }
+    __syncthreads();
+}
+
+// q (this CTA's slice) and b (replicated; forward only)
+__device__ __forceinline__ void dm_stage(const BoxDims& D, int j0, const double* q, const double* b) {
+    QPB_SMEM;
+    const int tid = threadIdx.x;
+    for (int j = tid; j < D.n; j += kBoxNT) qsm[D.q + j] = q[j0 + j];
+    for (int i = tid; i < D.ep; i += kBoxNT) qsm[D.b + i] = (b != nullptr && i < D.e) ? b[i] : 0.0;
+    __syncthreads();
+}
+
+// k_box_forward_cl with M distributed (outputs as there)
+__global__ void __launch_bounds__(kBoxNT, 1)
+k_box_forward_dm(DmDims Y, const double* __restrict__ q, int64_t sq, const double* __restrict__ p, int64_t sp,
+                 const double* __restrict__ A, int64_t sA, const double* __restrict__ b, int64_t sb,
+                 const double* __restrict__ lb, int64_t slb, const double* __restrict__ ub, int64_t sub, double eps,
+                 double stall_tol, double best_tie, int notImprovedLim, int maxIter, double* __restrict__ zhat,
+                 double* __restrict__ lam, double* __restrict__ slacks, double* __restrict__ nus,
+                 int* __restrict__ iters_out, double* __restrict__ resid_out, double* __restrict__ trace,
+                 int* __restrict__ spd_flag) {
+    QPB_SMEM;
+    const ClDims& X = Y.X;
+    const int rank = (int)cg::this_cluster().block_rank();
+    const int tid = threadIdx.x, qp = blockIdx.x / X.C;
+    int j0, ph = 0;
+    const BoxDims D = cl_local(X, rank, j0);
+    const int n = D.n, m = D.m, e = D.e, ep = D.ep, N = X.ng;
+    const double* Ag = A + (int64_t)qp * sA;
+    dm_stage(D, j0, q + (int64_t)qp * sq, b + (int64_t)qp * sb);
+    {
+        double bad[1] = {0.0};
+        for (int j = tid; j < n; j += kBoxNT) {
+            qsm[D.p + j] = p[(int64_t)qp * sp + j0 + j];
+            if (!(qsm[D.q + j] > 0.0)) bad[0] = 1.0;
+        }
+        cl_reduce<1, false>(X, bad, ph, 0, 0);
+        if (rank == 0 && tid == 0 && spd_flag != nullptr) spd_flag[qp] = bad[0] > 0.0;
+    }
+    for (int i = tid; i < m; i += kBoxNT) {
+        qsm[D.h + i] = (i < D.nlb) ? -lb[(int64_t)qp * slb + j0 + i] : ub[(int64_t)qp * sub + j0 + i - D.nlb];
+        qsm[D.d + i] = 1.0;
+        qsm[D.rz + i] = -qsm[D.h + i];
+    }
+    for (int i = tid; i < ep; i += kBoxNT) { qsm[D.ry + i] = -qsm[D.b + i]; qsm[D.y + i] = 0.0; }
+    __syncthreads();
+
+    // ---- initial point: solve_kkt(p, 0, -h, -b) with d = 1   (batch.py:61-67)
+    dm_form(Y, D, rank, Ag);
+    dm_solve(Y, D, rank, Ag, j0, ph, true, D.p, -1, D.rz, D.ry, D.x, D.s, D.z, D.y);
+    {
+        double mn[2] = {INFINITY, INFINITY};
+        for (int i = tid; i < m; i += kBoxNT) { mn[0] = fmin(mn[0], qsm[D.s + i]); mn[1] = fmin(mn[1], qsm[D.z + i]); }
+        cl_reduce<2, true>(X, mn, ph, 0, 0);
+        for (int i = tid; i < m; i += kBoxNT) {                  // slacks and duals >= 1 (batch.py:77-87)
+            if (mn[0] < 0.0) qsm[D.s + i] -= mn[0] - 1.0;
+            if (mn[1] < 0.0) qsm[D.z + i] -= mn[1] - 1.0;
+        }
+        __syncthreads();
+    }
+
+    double best = 0.0;
+    int nNot = 0, iters_run = 0;
+    const double dm = (double)X.mg;
+    for (int it = 0; it < maxIter; ++it) {
+        iters_run = it + 1;
+        // ---- residuals (batch.py:94-107): A x is reduced with the scalars, ry and |ry|^2 are formed redundantly
+        double acc[4] = {0.0, 0.0, 0.0, 0.0};                   // |ry|^2, |rz|^2, |rx|^2, s.z
+        for (int j = tid; j < n; j += kBoxNT) {
+            double a = 0.0;
+            for (int i = 0; i < e; ++i) a = fma(Ag[(int64_t)i * N + j0 + j], qsm[D.y + i], a);
+            const double r = fma(qsm[D.q + j], qsm[D.x + j], qsm[D.p + j]) + gt_col(D, qsm + D.z, j) + a;
+            qsm[D.rx + j] = r;
+            acc[2] = fma(r, r, acc[2]);
+        }
+        for (int i = tid; i < m; i += kBoxNT) {
+            const double r = bsgn(D, i) * qsm[D.x + bvar(D, i)] + qsm[D.s + i] - qsm[D.h + i];
+            qsm[D.rz + i] = r;
+            acc[1] = fma(r, r, acc[1]);
+            acc[3] = fma(qsm[D.s + i], qsm[D.z + i], acc[3]);
+        }
+        {
+            const int lane = tid & 31, warp = tid >> 5, buf = cl_buf(X, ph);
+            for (int i = warp; i < e; i += kClW) {
+                double a = 0.0;
+                for (int k = lane; k < n; k += 32) a = fma(Ag[(int64_t)i * N + j0 + k], qsm[D.x + k], a);
+                a = qpb::warp_sum(a);
+                if (lane == 0) qsm[buf + i] = a;
+            }
+        }
+        cl_reduce<4, false>(X, acc, ph, e, D.ry);
+        for (int i = 0; i < e; ++i) {
+            const double r = qsm[D.ry + i] - qsm[D.b + i];
+            acc[0] = fma(r, r, acc[0]);
+        }
+        __syncthreads();                                         // every thread has read the sums of A x
+        for (int i = tid; i < ep; i += kBoxNT) qsm[D.ry + i] = (i < e) ? qsm[D.ry + i] - qsm[D.b + i] : 0.0;
+        const double mu = fabs(acc[3] / dm);
+        const double resid = sqrt(acc[1]) + sqrt(acc[0]) + sqrt(acc[2]) + dm * mu;
+        if (trace != nullptr && rank == 0 && tid == 0) {          // what verbose=1 prints (batch.py:115-117)
+            double* tr = trace + ((int64_t)qp * maxIter + it) * 4;
+            tr[0] = sqrt(acc[1]) + sqrt(acc[0]); tr[1] = sqrt(acc[2]); tr[2] = mu; tr[3] = resid;
+        }
+        // ---- best-iterate tracking and exit tests (batch.py:118-143), per QP: cluster-wide values only
+        const bool improved = (it == 0) || (resid < best);
+        if (improved) { best = resid; nNot = 0; } else { ++nNot; }
+        if (improved || resid < best_tie * best) {
+            for (int j = tid; j < n; j += kBoxNT) qsm[D.bx + j] = qsm[D.x + j];
+            for (int i = tid; i < m; i += kBoxNT) { qsm[D.bs + i] = qsm[D.s + i]; qsm[D.bz + i] = qsm[D.z + i]; }
+            for (int i = tid; i < e; i += kBoxNT) qsm[D.by + i] = qsm[D.y + i];
+        }
+        if ((nNot == notImprovedLim && best < stall_tol) || best < eps || mu > 1e32) break;
+        if (!(resid == resid) || isinf(resid)) break;
+        // ---- d = z/s, H, M; the affine direction (batch.py:109-113,150) factors M
+        for (int i = tid; i < m; i += kBoxNT) qsm[D.d + i] = qsm[D.z + i] / qsm[D.s + i];
+        __syncthreads();
+        dm_form(Y, D, rank, Ag);
+        dm_solve(Y, D, rank, Ag, j0, ph, true, D.rx, D.z, D.rz, D.ry, D.dxa, D.dsa, D.dza, D.dya);
+        // ---- affine step length and sigma (batch.py:160-168)
+        double mn[2] = {INFINITY, INFINITY};
+        for (int i = tid; i < m; i += kBoxNT) {
+            mn[0] = fmin(mn[0], box_step(qsm[D.z + i], qsm[D.dza + i]));
+            mn[1] = fmin(mn[1], box_step(qsm[D.s + i], qsm[D.dsa + i]));
+        }
+        cl_reduce<2, true>(X, mn, ph, 0, 0);
+        {
+            const double alpha = fmin(fmin(box_step_fix(mn[0]), box_step_fix(mn[1])), 1.0);
+            double sm[2] = {0.0, 0.0};
+            for (int i = tid; i < m; i += kBoxNT) {
+                sm[0] = fma(qsm[D.s + i] + alpha * qsm[D.dsa + i], qsm[D.z + i] + alpha * qsm[D.dza + i], sm[0]);
+                sm[1] = fma(qsm[D.s + i], qsm[D.z + i], sm[1]);
+            }
+            cl_reduce<2, false>(X, sm, ph, 0, 0);
+            const double sr = sm[0] / sm[1];
+            const double sig = sr * sr * sr;
+            // ---- corrector right-hand side (batch.py:170-181): rs = (-mu sig + dsa dza) / s, rx = rz = ry = 0
+            for (int i = tid; i < m; i += kBoxNT)
+                qsm[D.rsc + i] = (-mu * sig + qsm[D.dsa + i] * qsm[D.dza + i]) / qsm[D.s + i];
+            for (int j = tid; j < n; j += kBoxNT) qsm[D.rx + j] = 0.0;
+            __syncthreads();
+        }
+        dm_solve(Y, D, rank, Ag, j0, ph, false, D.rx, D.rsc, -1, -1, D.dx, D.ds, D.dz, D.dy);
+        // ---- combined direction, step length, update (batch.py:185-203)
+        mn[0] = INFINITY; mn[1] = INFINITY;
+        for (int i = tid; i < m; i += kBoxNT) {
+            const double dzi = qsm[D.dza + i] + qsm[D.dz + i], dsi = qsm[D.dsa + i] + qsm[D.ds + i];
+            qsm[D.dz + i] = dzi;
+            qsm[D.ds + i] = dsi;
+            mn[0] = fmin(mn[0], box_step(qsm[D.z + i], dzi));
+            mn[1] = fmin(mn[1], box_step(qsm[D.s + i], dsi));
+        }
+        cl_reduce<2, true>(X, mn, ph, 0, 0);
+        const double alpha = fmin(0.999 * fmin(box_step_fix(mn[0]), box_step_fix(mn[1])), 1.0);
+        for (int j = tid; j < n; j += kBoxNT) qsm[D.x + j] = fma(alpha, qsm[D.dxa + j] + qsm[D.dx + j], qsm[D.x + j]);
+        for (int i = tid; i < m; i += kBoxNT) {
+            qsm[D.s + i] = fma(alpha, qsm[D.ds + i], qsm[D.s + i]);
+            qsm[D.z + i] = fma(alpha, qsm[D.dz + i], qsm[D.z + i]);
+        }
+        for (int i = tid; i < e; i += kBoxNT) qsm[D.y + i] = fma(alpha, qsm[D.dya + i] + qsm[D.dy + i], qsm[D.y + i]);
+        __syncthreads();
+    }
+    __syncthreads();
+    for (int j = tid; j < n; j += kBoxNT) zhat[(int64_t)qp * N + j0 + j] = qsm[D.bx + j];
+    for (int i = tid; i < m; i += kBoxNT) {
+        const int64_t g = (int64_t)qp * X.mg + cl_grow(X, D, j0, i);
+        lam[g] = qsm[D.bz + i];
+        slacks[g] = qsm[D.bs + i];
+    }
+    if (rank == 0) {
+        for (int i = tid; i < e; i += kBoxNT) nus[(int64_t)qp * e + i] = qsm[D.by + i];
+        if (tid == 0) { iters_out[qp] = iters_run; resid_out[qp] = best; }
+    }
+    cg::this_cluster().sync();       // no CTA exits while another may still read its shared memory
+}
+
+// k_box_backward_cl with M distributed
+__global__ void __launch_bounds__(kBoxNT, 1)
+k_box_backward_dm(DmDims Y, const double* __restrict__ q, int64_t sq, const double* __restrict__ A, int64_t sA,
+                  const double* __restrict__ dl, const double* __restrict__ zhat, const double* __restrict__ lam,
+                  const double* __restrict__ slacks, const double* __restrict__ nus, BoxGrads O,
+                  double* __restrict__ dxv, double* __restrict__ dlamv, double* __restrict__ dnuv) {
+    QPB_SMEM;
+    const ClDims& X = Y.X;
+    const int rank = (int)cg::this_cluster().block_rank();
+    const int tid = threadIdx.x, qp = blockIdx.x / X.C;
+    int j0, ph = 0;
+    const BoxDims D = cl_local(X, rank, j0);
+    const int n = D.n, m = D.m, e = D.e, N = X.ng;
+    const double* Ag = A + (int64_t)qp * sA;
+    dm_stage(D, j0, q + (int64_t)qp * sq, nullptr);
+    for (int j = tid; j < n; j += kBoxNT) qsm[D.rx + j] = dl[(int64_t)qp * N + j0 + j];
+    for (int i = tid; i < m; i += kBoxNT) {
+        const int64_t g = (int64_t)qp * X.mg + cl_grow(X, D, j0, i);
+        qsm[D.d + i] = fmax(lam[g], 1e-8) / fmax(slacks[g], 1e-8);
+    }
+    __syncthreads();
+    dm_form(Y, D, rank, Ag);
+    dm_solve(Y, D, rank, Ag, j0, ph, true, D.rx, -1, -1, -1, D.dx, D.ds, D.dz, D.dy);
+    for (int j = tid; j < n; j += kBoxNT) {
+        const int64_t g = (int64_t)qp * N + j0 + j;
+        const double dx = qsm[D.dx + j], z = zhat[g];
+        dxv[g] = dx;
+        if (O.dq && !O.mq) O.dq[g] = dx * z;
+        if (O.dp && !O.mp) O.dp[g] = dx;
+    }
+    for (int i = tid; i < m; i += kBoxNT) {
+        const double dz = qsm[D.dz + i];
+        dlamv[(int64_t)qp * X.mg + cl_grow(X, D, j0, i)] = dz;
+        if (i < D.nlb) { if (O.dlb && !O.mlb) O.dlb[(int64_t)qp * N + j0 + i] = dz; }
+        else if (O.dub && !O.mub) O.dub[(int64_t)qp * N + j0 + i - D.nlb] = -dz;
+    }
+    if (rank == 0)
+        for (int i = tid; i < e; i += kBoxNT) {
+            dnuv[(int64_t)qp * e + i] = qsm[D.dy + i];
+            if (O.db && !O.mb) O.db[(int64_t)qp * e + i] = -qsm[D.dy + i];
+        }
+    if (O.dA && !O.mA)
+        for (int t = tid; t < e * n; t += kBoxNT) {
+            const int i = t / n, j = t - i * n;
+            O.dA[((int64_t)qp * e + i) * N + j0 + j] = fma(qsm[D.dy + i], zhat[(int64_t)qp * N + j0 + j],
+                                                           nus[(int64_t)qp * e + i] * qsm[D.dx + j]);
+        }
+    cg::this_cluster().sync();
+}
+
+// k_box_kkt_cl with M distributed
+__global__ void __launch_bounds__(kBoxNT, 1)
+k_box_kkt_dm(DmDims Y, const double* __restrict__ q, int64_t sq, const double* __restrict__ A, int64_t sA,
+             const double* __restrict__ d, const double* __restrict__ rx, const double* __restrict__ rs,
+             const double* __restrict__ rz, const double* __restrict__ ry, double* __restrict__ dx,
+             double* __restrict__ ds, double* __restrict__ dz, double* __restrict__ dy) {
+    QPB_SMEM;
+    const ClDims& X = Y.X;
+    const int rank = (int)cg::this_cluster().block_rank();
+    const int tid = threadIdx.x, qp = blockIdx.x / X.C;
+    int j0, ph = 0;
+    const BoxDims D = cl_local(X, rank, j0);
+    const int n = D.n, m = D.m, e = D.e, N = X.ng;
+    const double* Ag = A + (int64_t)qp * sA;
+    dm_stage(D, j0, q + (int64_t)qp * sq, nullptr);
+    for (int j = tid; j < n; j += kBoxNT) qsm[D.rx + j] = rx[(int64_t)qp * N + j0 + j];
+    for (int i = tid; i < m; i += kBoxNT) {
+        const int64_t g = (int64_t)qp * X.mg + cl_grow(X, D, j0, i);
+        qsm[D.d + i] = d[g];
+        qsm[D.rsc + i] = rs[g];
+        qsm[D.rz + i] = rz[g];
+    }
+    for (int i = tid; i < e; i += kBoxNT) qsm[D.ry + i] = ry[(int64_t)qp * e + i];
+    __syncthreads();
+    dm_form(Y, D, rank, Ag);
+    dm_solve(Y, D, rank, Ag, j0, ph, true, D.rx, D.rsc, D.rz, D.ry, D.dx, D.ds, D.dz, D.dy);
+    for (int j = tid; j < n; j += kBoxNT) dx[(int64_t)qp * N + j0 + j] = qsm[D.dx + j];
+    for (int i = tid; i < m; i += kBoxNT) {
+        const int64_t g = (int64_t)qp * X.mg + cl_grow(X, D, j0, i);
+        ds[g] = qsm[D.ds + i];
+        dz[g] = qsm[D.dz + i];
+    }
+    if (rank == 0)
+        for (int i = tid; i < e; i += kBoxNT) dy[(int64_t)qp * e + i] = qsm[D.dy + i];
+    cg::this_cluster().sync();
+}
+
 std::mutex g_mu;
 template <typename K>
 int box_set_smem(K kernel, size_t bytes, size_t* cur) {      // cur: per-kernel high-water mark (device 0..15)
@@ -953,6 +1584,7 @@ int box_check_launch(const char* what) {
 }
 size_t g_fwd[16], g_bwd[16], g_kkt[16];
 size_t g_cfwd[16], g_cbwd[16], g_ckkt[16];
+size_t g_dfwd[16], g_dbwd[16], g_dkkt[16];
 
 int box_plan_check(const qpb200_box_plan* P) {
     if (P == nullptr) return QPB200_ERR_BAD_ARG;
@@ -962,6 +1594,7 @@ int box_plan_check(const qpb200_box_plan* P) {
 }
 BoxDims plan_dims(const qpb200_box_plan* P) { return box_dims(P->nz, P->neq, P->has_lb, P->has_ub); }
 ClDims plan_cl_dims(const qpb200_box_plan* P) { return cl_dims(P->nz, P->neq, P->has_lb, P->has_ub, P->cl_ctas); }
+DmDims plan_dm_dims(const qpb200_box_plan* P) { return dm_dims(P->nz, P->neq, P->has_lb, P->has_ub, P->cl_ctas); }
 
 // Whether a cluster of C CTAs with `bytes` of shared memory each can be resident at all (cudaOccupancyMaxActiveClusters
 // > 0), checked once per (kernel, C, bytes, device): QPB200_ERR_TOO_LARGE if not.
@@ -1054,6 +1687,31 @@ int qpb200_box_plan_init(int nz, int neq, int has_lb, int has_ub, qpb200_box_pla
             plan->cl_slice = X.slice;
             plan->cl_smem_bytes = (int64_t)X.total * 8;
         }
+    } else {
+        // the distributed-M kernels (neq_pad > 128): the smallest cluster that holds its share of M, where the dense
+        // path rejects the shape or its order is past kDmDenseOrder (below it the dense kernels are faster).
+        // QPB200_BOX_CLUSTER=C forces them where that C fits.
+        auto fits = [&](int C) {
+            return (int64_t)dm_dims(nz, neq, plan->has_lb, plan->has_ub, C).total * 8 <= kBoxMaxSmem;
+        };
+        const char* env = getenv("QPB200_BOX_CLUSTER");
+        const int forced = env ? atoi(env) : 0;
+        int C = 0;
+        if ((forced == 2 || forced == 4 || forced == 8) && fits(forced)) {
+            C = forced;
+        } else {
+            qpb200_plan dp;
+            const int rc = qpb200_plan_init(nz, plan->nineq, neq, &dp);
+            if (rc == QPB200_ERR_TOO_LARGE || (rc == QPB200_OK && dp.ms_pad > kDmDenseOrder))
+                for (int c = 2; c <= 8 && !C; c *= 2)
+                    if (fits(c)) C = c;
+        }
+        if (C) {
+            const DmDims Y = dm_dims(nz, neq, plan->has_lb, plan->has_ub, C);
+            plan->cl_ctas = C;
+            plan->cl_slice = Y.X.slice;
+            plan->cl_smem_bytes = (int64_t)Y.total * 8;
+        }
     }
     if (!plan->ok && !plan->cl_ctas) {          // only the dense kernels on the dense equivalent are left
         qpb200_plan dp;
@@ -1072,6 +1730,15 @@ int qpb200_box_forward(const qpb200_box_plan* plan, int nbatch, const double* q,
     if (rc) return rc;
     if (nbatch <= 0 || maxIter < 1 || !q || !p || !zhat || !lam || !slacks || !iters || !best_resid) return QPB200_ERR_BAD_ARG;
     if ((plan->has_lb && !lb) || (plan->has_ub && !ub) || (plan->neq > 0 && (!A || !b || !nus))) return QPB200_ERR_BAD_ARG;
+    if (plan->cl_ctas && plan->neq_pad > kBoxNT) {
+        const DmDims Y = plan_dm_dims(plan);
+        const size_t bytes = (size_t)Y.total * 8;
+        rc = cl_prepare(k_box_forward_dm, Y.X.C, bytes, g_dfwd);
+        if (rc) return rc;
+        return cl_launch("k_box_forward_dm", k_box_forward_dm, Y.X.C, nbatch, bytes, (cudaStream_t)stream, Y, q, sq, p,
+                         sp, A, sA, b, sb, lb, slb, ub, sub, eps, stall_tol, best_tie, notImprovedLim, maxIter, zhat,
+                         lam, slacks, nus, iters, best_resid, trace, spd_flag);
+    }
     if (plan->cl_ctas) {
         const ClDims X = plan_cl_dims(plan);
         const size_t bytes = (size_t)X.total * 8;
@@ -1106,7 +1773,14 @@ int qpb200_box_backward(const qpb200_box_plan* plan, int nbatch, const double* q
     O.dq = dq; O.dp = dp; O.dlb = dlb; O.dub = dub; O.dA = e > 0 ? dA : nullptr; O.db = e > 0 ? db : nullptr;
     O.mq = mean_q; O.mp = mean_p; O.mlb = mean_lb; O.mub = mean_ub; O.mA = mean_A; O.mb = mean_b;
     cudaStream_t st = (cudaStream_t)stream;
-    if (plan->cl_ctas) {
+    if (plan->cl_ctas && plan->neq_pad > kBoxNT) {
+        const DmDims Y = plan_dm_dims(plan);
+        const size_t bytes = (size_t)Y.total * 8;
+        rc = cl_prepare(k_box_backward_dm, Y.X.C, bytes, g_dbwd);
+        if (rc) return rc;
+        rc = cl_launch("k_box_backward_dm", k_box_backward_dm, Y.X.C, nbatch, bytes, st, Y, q, sq, A, sA, dl_dzhat, zhat,
+                       lam, slacks, nus, O, dxv, dlamv, dnuv);
+    } else if (plan->cl_ctas) {
         const ClDims X = plan_cl_dims(plan);
         const size_t bytes = (size_t)X.total * 8;
         rc = cl_prepare(k_box_backward_cl, X.C, bytes, g_cbwd);
@@ -1141,6 +1815,14 @@ int qpb200_box_solve_kkt(const qpb200_box_plan* plan, int nbatch, const double* 
     if (rc) return rc;
     if (nbatch <= 0 || !q || !d || !rx || !rs || !rz || !dx || !ds || !dz) return QPB200_ERR_BAD_ARG;
     if (plan->neq > 0 && (!A || !ry || !dy)) return QPB200_ERR_BAD_ARG;
+    if (plan->cl_ctas && plan->neq_pad > kBoxNT) {
+        const DmDims Y = plan_dm_dims(plan);
+        const size_t bytes = (size_t)Y.total * 8;
+        rc = cl_prepare(k_box_kkt_dm, Y.X.C, bytes, g_dkkt);
+        if (rc) return rc;
+        return cl_launch("k_box_kkt_dm", k_box_kkt_dm, Y.X.C, nbatch, bytes, (cudaStream_t)stream, Y, q, sq, A, sA, d, rx,
+                         rs, rz, ry, dx, ds, dz, dy);
+    }
     if (plan->cl_ctas) {
         const ClDims X = plan_cl_dims(plan);
         const size_t bytes = (size_t)X.total * 8;
