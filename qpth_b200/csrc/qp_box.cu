@@ -8,12 +8,18 @@
 // order neq_pad) and solved with pf_fwd / pf_diag / pf_bwd; the predictor and the corrector share one factor.
 // oracle/box_model.py is the numpy model of exactly this arithmetic.
 //
-// One 128-thread CTA per QP; A (neq x nz, row stride nz | 1), the factor of M and every vector live in shared memory.
-// The kernels cover neq_pad <= 128 (the substitutions own one row per thread) and a footprint within the 227 KB an
-// H100 CTA may use (qpb200_box_plan.ok). Past that, the cluster kernels (k_box_*_cl, below) split one QP's variables
-// over a thread block cluster of 2, 4 or 8 CTAs (qpb200_box_plan.cl_ctas), and past neq_pad = 128 the distributed-M
-// kernels (k_box_*_dm) spread M over the cluster as well; BoxQPFunction runs the dense kernels on the dense equivalent
-// only where none covers the shape.
+// Three layouts run this solver, all with 128-thread CTAs:
+//   one CTA per QP (family OneCta): A (neq x nz, row stride nz | 1), the factor of M and every vector live in shared
+//            memory. neq_pad <= 128 (the substitutions own one row per thread) and a footprint within the 227 KB an
+//            H100 CTA may use (qpb200_box_plan.ok).
+//   a cluster per QP (family Cluster): past that, a thread block cluster of 2, 4 or 8 CTAs (qpb200_box_plan.cl_ctas),
+//            each CTA holding a slice of the variables; M is summed and factored redundantly in every CTA.
+//   distributed M (k_box_*_dm): past neq_pad = 128, M is distributed over the cluster as well and A is read from
+//            global memory.
+// BoxQPFunction runs the dense kernels on the dense equivalent only where none covers the shape. For the first two the
+// Mehrotra loop (k_box_forward<F>), the backward and KKT kernels and the structured solve (box_solve<F>) are written
+// once; a family supplies only what differs: its per-CTA context, its reductions, how A is staged, how M is formed and
+// solved.
 #include <cooperative_groups.h>
 #include <cuda_runtime.h>
 #include <math.h>
@@ -38,7 +44,9 @@ extern "C" void qpb200_internal_cuda_error(int err, const char* what);   // (qp_
 namespace {
 
 using namespace qpb::pf;
+namespace cg = cooperative_groups;
 constexpr int kBoxNT = qpb::fast::kNT;
+constexpr int kClW = kBoxNT / 32;          // warps per CTA: scalar partials are published per warp
 constexpr int kBoxMaxSmem = 232448;        // H100: 227 KB of dynamic shared memory per CTA
 
 // ---- shared-memory layout (doubles; every offset a multiple of 8, i.e. 64-byte aligned) ------------------------------
@@ -55,6 +63,18 @@ struct BoxDims {
 
 __host__ __device__ inline int r8(int v) { return (v + 7) & ~7; }
 
+// the n-, m- and ep-length vectors of D (counts set) from offset o; returns the end
+__host__ __device__ inline int box_vectors(BoxDims& D, int o) {
+    const int nn = r8(D.n), mm = r8(D.m), ee = D.ep;
+    int* vn[] = {&D.q, &D.p, &D.x, &D.rx, &D.r, &D.hinv, &D.dxa, &D.dx, &D.bx};
+    for (int* v : vn) { *v = o; o += nn; }
+    int* vm[] = {&D.h, &D.s, &D.z, &D.d, &D.rz, &D.dsa, &D.dza, &D.ds, &D.dz, &D.bs, &D.bz, &D.rsc};
+    for (int* v : vm) { *v = o; o += mm; }
+    int* ve[] = {&D.b, &D.y, &D.ry, &D.rhs, &D.t, &D.dya, &D.dy, &D.by};
+    for (int* v : ve) { *v = o; o += ee; }
+    return o;
+}
+
 __host__ __device__ inline BoxDims box_dims(int n, int e, int has_lb, int has_ub) {
     BoxDims D;
     D.n = n; D.e = e; D.ep = r8(e); D.nlb = has_lb ? n : 0; D.m = (has_lb ? n : 0) + (has_ub ? n : 0);
@@ -66,14 +86,7 @@ __host__ __device__ inline BoxDims box_dims(int n, int e, int has_lb, int has_ub
     D.pan = o; o += (e > 0) ? r8((8 * nts + 8) * kPanLd) : 0;
     D.tab = o; o += r8(pf_tab_doubles(nts));
     D.red = o; o += 4 * qpb::kRedStride;
-    const int nn = r8(n), mm = r8(D.m), ee = D.ep;
-    int* vn[] = {&D.q, &D.p, &D.x, &D.rx, &D.r, &D.hinv, &D.dxa, &D.dx, &D.bx};
-    for (int* v : vn) { *v = o; o += nn; }
-    int* vm[] = {&D.h, &D.s, &D.z, &D.d, &D.rz, &D.dsa, &D.dza, &D.ds, &D.dz, &D.bs, &D.bz, &D.rsc};
-    for (int* v : vm) { *v = o; o += mm; }
-    int* ve[] = {&D.b, &D.y, &D.ry, &D.rhs, &D.t, &D.dya, &D.dy, &D.by};
-    for (int* v : ve) { *v = o; o += ee; }
-    D.total = o;
+    D.total = box_vectors(D, o);
     return D;
 }
 
@@ -89,75 +102,139 @@ __device__ __forceinline__ double gt_col(const BoxDims& D, const double* v, int 
     return a;
 }
 
-// hinv = 1 / (q + G'DG) for the d currently in shared memory; with A, M = A H^-1 A' into the staircase (lower tiles,
-// identity rows beyond neq). Ends with a block barrier.
-__device__ __noinline__ void box_form(const BoxDims& D) {
+__device__ __forceinline__ double box_step(double v, double dv) { return (dv > 0.0) ? INFINITY : (-v / dv); }
+__device__ __forceinline__ double box_step_fix(double v) { return (isinf(v) && v > 0.0) ? 1.0 : v; }
+
+// hinv = 1 / (q + G'DG) for the local variables and the d currently in shared memory (no barrier)
+__device__ __forceinline__ void form_hinv(const BoxDims& D) {
     QPB_SMEM;
-    const int tid = threadIdx.x;
-    for (int j = tid; j < D.n; j += kBoxNT) {
+    for (int j = threadIdx.x; j < D.n; j += kBoxNT) {
         double hj = qsm[D.q + j];
         if (D.nlb) hj += qsm[D.d + j];
         if (D.m > D.nlb) hj += qsm[D.d + D.nlb + j];
         qsm[D.hinv + j] = 1.0 / hj;
     }
-    __syncthreads();
-    if (D.e == 0) return;
-    const int ep = D.ep, n = D.n, lda = D.lda;
-    const int tot = (ep * (ep + 1)) / 2;
-    const double* A = qsm + D.A;
-    const double* hv = qsm + D.hinv;
-    for (int t = tid; t < tot; t += kBoxNT) {
-        int r = (int)((sqrt(8.0 * t + 1.0) - 1.0) * 0.5);
-        while ((r * (r + 1)) / 2 > t) --r;
-        while (((r + 1) * (r + 2)) / 2 <= t) ++r;
-        const int c = t - (r * (r + 1)) / 2;
-        double v;
-        if (r < D.e) {
-            const double* ar = A + r * lda;
-            const double* ac = A + c * lda;
-            double s0 = 0.0, s1 = 0.0;
-            int k = 0;
-            for (; k + 1 < n; k += 2) {
-                s0 = fma(ar[k] * hv[k], ac[k], s0);
-                s1 = fma(ar[k + 1] * hv[k + 1], ac[k + 1], s1);
-            }
-            if (k < n) s0 = fma(ar[k] * hv[k], ac[k], s0);
-            v = s0 + s1;
-        } else {
-            v = (r == c) ? 1.0 : 0.0;
-        }
-        qsm[D.S + pf_rowoff(r) + c] = v;
-    }
-    __syncthreads();
 }
 
-// The structured KKT solve with the H / M of the last box_form:
-//   K [dx ds dz dy] = -[rx rs rz ry];  rs, rz, ry may be -1 (zero). fresh: M was just formed and is factored here
-// (with the right-hand side carried along), else the existing factor is reused. Ends with a block barrier.
-__device__ __noinline__ void box_solve(const BoxDims& D, bool fresh, int rx, int rs, int rz, int ry,
-                                       int dx, int ds, int dz, int dy) {
-    QPB_SMEM;
-    const int tid = threadIdx.x;
-    const int n = D.n, m = D.m, e = D.e, ep = D.ep, lda = D.lda;
-    // r = rx + G'(D rz - rs), kept as H^-1 r in D.r
-    for (int j = tid; j < n; j += kBoxNT) {
-        double a = qsm[rx + j];
-        if (D.nlb) {
-            const double t = ((rz >= 0) ? qsm[D.d + j] * qsm[rz + j] : 0.0) - ((rs >= 0) ? qsm[rs + j] : 0.0);
-            a -= t;
-        }
-        if (m > D.nlb) {
-            const int i = D.nlb + j;
-            const double t = ((rz >= 0) ? qsm[D.d + i] * qsm[rz + i] : 0.0) - ((rs >= 0) ? qsm[rs + i] : 0.0);
-            a += t;
-        }
-        qsm[D.r + j] = a * qsm[D.hinv + j];
+// row of entry t of a packed lower triangle (t = r (r + 1) / 2 + c)
+__device__ __forceinline__ int tri_row(int t) {
+    int r = (int)((sqrt(8.0 * t + 1.0) - 1.0) * 0.5);
+    while ((r * (r + 1)) / 2 > t) --r;
+    while (((r + 1) * (r + 2)) / 2 <= t) ++r;
+    return r;
+}
+
+// (A H^-1 A')_rc over the n shared columns of rows ar, ac (lda apart in shared memory)
+__device__ __forceinline__ double ahat(const double* ar, const double* ac, const double* hv, int n) {
+    double s0 = 0.0, s1 = 0.0;
+    int k = 0;
+    for (; k + 1 < n; k += 2) {
+        s0 = fma(ar[k] * hv[k], ac[k], s0);
+        s1 = fma(ar[k + 1] * hv[k + 1], ac[k + 1], s1);
     }
-    __syncthreads();
-    if (e > 0) {
+    if (k < n) s0 = fma(ar[k] * hv[k], ac[k], s0);
+    return s0 + s1;
+}
+
+// The factor of the staircase in D.S with the right-hand side D.rhs carried along (fresh), or its forward sweep with
+// the existing factor; then pf_diag and the backward sweep into dy.
+__device__ __forceinline__ void stair_solve(const BoxDims& D, bool fresh, int dy) {
+    const int nts = D.ep >> 3;
+    if (fresh) {
+        pf_chol(D.S, nts, 0, D.rhs, D.pan, D.tab);
+        __syncthreads();
+    } else {
+        pf_fwd(D.S, D.ep, 0, nts - 1, D.rhs);
+    }
+    pf_diag(D.S, D.ep, D.rhs, D.t, D.rhs);
+    pf_bwd(D.S, D.ep, D.rhs, dy);
+}
+
+// ---- the families -------------------------------------------------------------------------------------------------------
+// Each is the per-CTA context of one layout, built in the kernel from its parameter (F::Dims), and supplies:
+//   qp(), j0() (first local variable), ng() / mg() (nz and inequality rows of the whole QP), grow(i) (global
+//   inequality row of local row i), leader() (rank 0: writes the length-neq outputs, iters, best_resid, the trace and
+//   spd_flag), a(i, j) (A at local column j), reduce_sum / reduce_min, any (the SPD test), stage, form (H^-1 and M),
+//   ry_step (ry = A x - b, |ry|^2 into acc, and the reduction of acc), solve_mid (rhs = ry - A H^-1 r, factor or forward
+//   sweep, pf_diag, backward sweep to dy) and sync() (the closing cluster barrier).
+
+// One CTA per QP; j0 = 0 and leader() (rank 0) are compile-time facts.
+struct OneCta {
+    using Dims = BoxDims;
+    static constexpr int kMinFwd = 3, kMinBwd = 4, kMinKkt = 0;     // CTAs per SM (0: no bound)
+    BoxDims D;
+
+    __device__ explicit OneCta(const BoxDims& P) : D(P) {}
+    __device__ static int qp() { return blockIdx.x; }
+    __host__ __device__ static constexpr int j0() { return 0; }
+    __device__ int ng() const { return D.n; }
+    __device__ int mg() const { return D.m; }
+    __device__ static int64_t grow(int i) { return i; }
+    __host__ __device__ static constexpr bool leader() { return true; }
+    __device__ double a(int i, int j) const { QPB_SMEM; return qsm[D.A + i * D.lda + j]; }
+    template <int N> __device__ void reduce_sum(double (&v)[N]) {
+        QPB_SMEM;
+        qpb::block_reduce<N, false>(v, qsm + D.red, threadIdx.x, kBoxNT);
+    }
+    template <int N> __device__ void reduce_min(double (&v)[N]) {
+        QPB_SMEM;
+        qpb::block_reduce<N, true>(v, qsm + D.red, threadIdx.x, kBoxNT);
+    }
+    __device__ static int any(int v) { return __syncthreads_or(v); }
+    __device__ static void sync() {}
+
+    // q, A, b (nullptr in the backward and KKT kernels) of this QP; the staircase tile table
+    __device__ void stage(const double* q, const double* A, const double* b) const {
+        QPB_SMEM;
+        const int tid = threadIdx.x;
+        for (int j = tid; j < D.n; j += kBoxNT) qsm[D.q + j] = q[j];
+        for (int t = tid; t < D.e * D.n; t += kBoxNT) {
+            const int i = t / D.n, j = t - i * D.n;
+            qsm[D.A + i * D.lda + j] = A[t];
+        }
+        for (int i = tid; i < D.ep; i += kBoxNT) qsm[D.b + i] = (b != nullptr && i < D.e) ? b[i] : 0.0;
+        if (D.e > 0) pf_build_tab(D.tab, D.ep >> 3);
+        __syncthreads();
+    }
+
+    // H^-1; with A, M into the staircase (lower tiles, identity rows beyond neq). Ends with a block barrier.
+    __device__ __noinline__ void form() const {
+        QPB_SMEM;
+        form_hinv(D);
+        __syncthreads();
+        if (D.e == 0) return;
+        const int ep = D.ep, n = D.n, lda = D.lda;
+        const int tot = (ep * (ep + 1)) / 2;
+        for (int t = threadIdx.x; t < tot; t += kBoxNT) {
+            const int r = tri_row(t), c = t - (r * (r + 1)) / 2;
+            const double v = (r < D.e) ? ahat(qsm + D.A + r * lda, qsm + D.A + c * lda, qsm + D.hinv, n)
+                                       : ((r == c) ? 1.0 : 0.0);
+            qsm[D.S + pf_rowoff(r) + c] = v;
+        }
+        __syncthreads();
+    }
+
+    // ry = A x - b, one warp per row; |ry|^2 per warp before the block reduction
+    __device__ void ry_step(double (&acc)[4]) {
+        QPB_SMEM;
+        const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+        for (int i = warp; i < D.ep; i += kClW) {
+            double a = 0.0;
+            if (i < D.e)
+                for (int k = lane; k < D.n; k += 32) a = fma(qsm[D.A + i * D.lda + k], qsm[D.x + k], a);
+            a = qpb::warp_sum(a);
+            const double r = (i < D.e) ? a - qsm[D.b + i] : 0.0;
+            if (lane == 0) { qsm[D.ry + i] = r; acc[0] = fma(r, r, acc[0]); }
+        }
+        reduce_sum(acc);
+    }
+
+    __device__ void solve_mid(bool fresh, int ry, int dy) {
+        QPB_SMEM;
+        const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+        const int n = D.n, e = D.e, ep = D.ep, lda = D.lda;
         // rhs = ry - A H^-1 r: one warp per row, lanes over the columns
-        const int lane = tid & 31, warp = tid >> 5;
-        for (int i = warp; i < ep; i += kBoxNT / 32) {
+        for (int i = warp; i < ep; i += kClW) {
             double a = 0.0;
             if (i < e)
                 for (int k = lane; k < n; k += 32) a = fma(qsm[D.A + i * lda + k], qsm[D.r + k], a);
@@ -165,326 +242,19 @@ __device__ __noinline__ void box_solve(const BoxDims& D, bool fresh, int rx, int
             if (lane == 0) qsm[D.rhs + i] = (i < e) ? (((ry >= 0) ? qsm[ry + i] : 0.0) - a) : 0.0;
         }
         __syncthreads();
-        const int nts = ep >> 3;
-        if (fresh) {
-            pf_chol(D.S, nts, 0, D.rhs, D.pan, D.tab);       // the factor, and the forward sweep of the right-hand side
-            __syncthreads();
-        } else {
-            pf_fwd(D.S, ep, 0, nts - 1, D.rhs);
-        }
-        pf_diag(D.S, ep, D.rhs, D.t, D.rhs);
-        pf_bwd(D.S, ep, D.rhs, dy);
+        stair_solve(D, fresh, dy);
     }
-    // dx = -H^-1 r - H^-1 A'dy
-    for (int j = tid; j < n; j += kBoxNT) {
-        double a = 0.0;
-        for (int i = 0; i < e; ++i) a = fma(qsm[D.A + i * lda + j], qsm[dy + i], a);
-        qsm[dx + j] = -qsm[D.r + j] - a * qsm[D.hinv + j];
-    }
-    __syncthreads();
-    for (int i = tid; i < m; i += kBoxNT) {
-        const double di = qsm[D.d + i];
-        const double rsi = (rs >= 0) ? qsm[rs + i] : 0.0;
-        const double dzi = di * (bsgn(D, i) * qsm[dx + bvar(D, i)] + ((rz >= 0) ? qsm[rz + i] : 0.0)) - rsi;
-        qsm[dz + i] = dzi;
-        qsm[ds + i] = (-rsi - dzi) / di;
-    }
-    __syncthreads();
-}
-
-// q, A (shared / per QP), b (nullptr in the backward and KKT kernels): staged once per CTA; the staircase tile table
-__device__ __forceinline__ void box_stage(const BoxDims& D, const double* q, const double* A, const double* b) {
-    QPB_SMEM;
-    const int tid = threadIdx.x;
-    for (int j = tid; j < D.n; j += kBoxNT) qsm[D.q + j] = q[j];
-    for (int t = tid; t < D.e * D.n; t += kBoxNT) {
-        const int i = t / D.n, j = t - i * D.n;
-        qsm[D.A + i * D.lda + j] = A[t];
-    }
-    for (int i = tid; i < D.ep; i += kBoxNT) qsm[D.b + i] = (b != nullptr && i < D.e) ? b[i] : 0.0;   // (b: forward only)
-    if (D.e > 0) pf_build_tab(D.tab, D.ep >> 3);
-    __syncthreads();
-}
-
-__device__ __forceinline__ double box_step(double v, double dv) { return (dv > 0.0) ? INFINITY : (-v / dv); }
-__device__ __forceinline__ double box_step_fix(double v) { return (isinf(v) && v > 0.0) ? 1.0 : v; }
-
-// forward (batch.py:47-207) with the structured solve, one CTA per QP; the loop of k_forward_fast (qp_solve.cuh).
-// Three CTAs per SM (at most 168 registers; about 48 KB of shared memory per QP at nz = 64, neq = 40): four (128
-// registers) spill.
-__global__ void __launch_bounds__(kBoxNT, 3)
-k_box_forward(BoxDims D, const double* __restrict__ q, int64_t sq, const double* __restrict__ p, int64_t sp,
-              const double* __restrict__ A, int64_t sA, const double* __restrict__ b, int64_t sb,
-              const double* __restrict__ lb, int64_t slb, const double* __restrict__ ub, int64_t sub, double eps,
-              double stall_tol, double best_tie, int notImprovedLim, int maxIter, double* __restrict__ zhat,
-              double* __restrict__ lam, double* __restrict__ slacks, double* __restrict__ nus, int* __restrict__ iters_out,
-              double* __restrict__ resid_out, double* __restrict__ trace, int* __restrict__ spd_flag) {
-    QPB_SMEM;
-    const int tid = threadIdx.x, qp = blockIdx.x;
-    const int n = D.n, m = D.m, e = D.e, ep = D.ep;
-    const double* qg = q + (int64_t)qp * sq;
-    box_stage(D, qg, A + (int64_t)qp * sA, (e > 0) ? b + (int64_t)qp * sb : nullptr);
-    {
-        int bad = 0;
-        for (int j = tid; j < n; j += kBoxNT) {
-            qsm[D.p + j] = p[(int64_t)qp * sp + j];
-            bad |= !(qsm[D.q + j] > 0.0);
-        }
-        bad = __syncthreads_or(bad);
-        if (tid == 0 && spd_flag != nullptr) spd_flag[qp] = bad;
-    }
-    for (int i = tid; i < m; i += kBoxNT) {
-        qsm[D.h + i] = (i < D.nlb) ? -lb[(int64_t)qp * slb + i] : ub[(int64_t)qp * sub + i - D.nlb];
-        qsm[D.d + i] = 1.0;
-        qsm[D.rz + i] = -qsm[D.h + i];
-    }
-    for (int i = tid; i < ep; i += kBoxNT) { qsm[D.ry + i] = -qsm[D.b + i]; qsm[D.y + i] = 0.0; }
-    __syncthreads();
-
-    // ---- initial point: solve_kkt(p, 0, -h, -b) with d = 1   (batch.py:61-67)
-    box_form(D);
-    box_solve(D, true, D.p, -1, D.rz, D.ry, D.x, D.s, D.z, D.y);
-    {
-        double mn[2] = {INFINITY, INFINITY};
-        for (int i = tid; i < m; i += kBoxNT) { mn[0] = fmin(mn[0], qsm[D.s + i]); mn[1] = fmin(mn[1], qsm[D.z + i]); }
-        qpb::block_reduce<2, true>(mn, qsm + D.red, tid, kBoxNT);
-        for (int i = tid; i < m; i += kBoxNT) {                  // slacks and duals >= 1 (batch.py:77-87)
-            if (mn[0] < 0.0) qsm[D.s + i] -= mn[0] - 1.0;
-            if (mn[1] < 0.0) qsm[D.z + i] -= mn[1] - 1.0;
-        }
-        __syncthreads();
-    }
-
-    double best = 0.0;
-    int nNot = 0, iters_run = 0;
-    const double dm = (double)m;
-    for (int it = 0; it < maxIter; ++it) {
-        iters_run = it + 1;
-        // ---- residuals (batch.py:94-107)
-        double acc[4] = {0.0, 0.0, 0.0, 0.0};                   // |ry|^2, |rz|^2, |rx|^2, s.z
-        for (int j = tid; j < n; j += kBoxNT) {
-            double a = 0.0;
-            for (int i = 0; i < e; ++i) a = fma(qsm[D.A + i * D.lda + j], qsm[D.y + i], a);
-            const double r = fma(qsm[D.q + j], qsm[D.x + j], qsm[D.p + j]) + gt_col(D, qsm + D.z, j) + a;
-            qsm[D.rx + j] = r;
-            acc[2] = fma(r, r, acc[2]);
-        }
-        for (int i = tid; i < m; i += kBoxNT) {
-            const double r = bsgn(D, i) * qsm[D.x + bvar(D, i)] + qsm[D.s + i] - qsm[D.h + i];
-            qsm[D.rz + i] = r;
-            acc[1] = fma(r, r, acc[1]);
-            acc[3] = fma(qsm[D.s + i], qsm[D.z + i], acc[3]);
-        }
-        {
-            const int lane = tid & 31, warp = tid >> 5;
-            for (int i = warp; i < ep; i += kBoxNT / 32) {
-                double a = 0.0;
-                if (i < e)
-                    for (int k = lane; k < n; k += 32) a = fma(qsm[D.A + i * D.lda + k], qsm[D.x + k], a);
-                a = qpb::warp_sum(a);
-                const double r = (i < e) ? a - qsm[D.b + i] : 0.0;
-                if (lane == 0) { qsm[D.ry + i] = r; acc[0] = fma(r, r, acc[0]); }
-            }
-        }
-        qpb::block_reduce<4, false>(acc, qsm + D.red, tid, kBoxNT);
-        const double mu = fabs(acc[3] / dm);
-        const double resid = sqrt(acc[1]) + sqrt(acc[0]) + sqrt(acc[2]) + dm * mu;
-        if (trace != nullptr && tid == 0) {                     // what verbose=1 prints (batch.py:115-117)
-            double* tr = trace + ((int64_t)qp * maxIter + it) * 4;
-            tr[0] = sqrt(acc[1]) + sqrt(acc[0]); tr[1] = sqrt(acc[2]); tr[2] = mu; tr[3] = resid;
-        }
-        // ---- best-iterate tracking and exit tests (batch.py:118-143), per QP
-        const bool improved = (it == 0) || (resid < best);
-        if (improved) { best = resid; nNot = 0; } else { ++nNot; }
-        if (improved || resid < best_tie * best) {
-            for (int j = tid; j < n; j += kBoxNT) qsm[D.bx + j] = qsm[D.x + j];
-            for (int i = tid; i < m; i += kBoxNT) { qsm[D.bs + i] = qsm[D.s + i]; qsm[D.bz + i] = qsm[D.z + i]; }
-            for (int i = tid; i < e; i += kBoxNT) qsm[D.by + i] = qsm[D.y + i];
-        }
-        if ((nNot == notImprovedLim && best < stall_tol) || best < eps || mu > 1e32) break;
-        if (!(resid == resid) || isinf(resid)) break;
-        // ---- d = z/s, H, M; the affine direction (batch.py:109-113,150) factors M
-        for (int i = tid; i < m; i += kBoxNT) qsm[D.d + i] = qsm[D.z + i] / qsm[D.s + i];
-        __syncthreads();
-        box_form(D);
-        box_solve(D, true, D.rx, D.z, D.rz, D.ry, D.dxa, D.dsa, D.dza, D.dya);
-        // ---- affine step length and sigma (batch.py:160-168)
-        double mn[2] = {INFINITY, INFINITY};
-        for (int i = tid; i < m; i += kBoxNT) {
-            mn[0] = fmin(mn[0], box_step(qsm[D.z + i], qsm[D.dza + i]));
-            mn[1] = fmin(mn[1], box_step(qsm[D.s + i], qsm[D.dsa + i]));
-        }
-        qpb::block_reduce<2, true>(mn, qsm + D.red, tid, kBoxNT);
-        {
-            const double alpha = fmin(fmin(box_step_fix(mn[0]), box_step_fix(mn[1])), 1.0);
-            double sm[2] = {0.0, 0.0};
-            for (int i = tid; i < m; i += kBoxNT) {
-                sm[0] = fma(qsm[D.s + i] + alpha * qsm[D.dsa + i], qsm[D.z + i] + alpha * qsm[D.dza + i], sm[0]);
-                sm[1] = fma(qsm[D.s + i], qsm[D.z + i], sm[1]);
-            }
-            qpb::block_reduce<2, false>(sm, qsm + D.red, tid, kBoxNT);
-            const double sr = sm[0] / sm[1];
-            const double sig = sr * sr * sr;
-            // ---- corrector right-hand side (batch.py:170-181): rs = (-mu sig + dsa dza) / s, rx = rz = ry = 0
-            for (int i = tid; i < m; i += kBoxNT)
-                qsm[D.rsc + i] = (-mu * sig + qsm[D.dsa + i] * qsm[D.dza + i]) / qsm[D.s + i];
-            for (int j = tid; j < n; j += kBoxNT) qsm[D.rx + j] = 0.0;
-            __syncthreads();
-        }
-        box_solve(D, false, D.rx, D.rsc, -1, -1, D.dx, D.ds, D.dz, D.dy);
-        // ---- combined direction, step length, update (batch.py:185-203)
-        mn[0] = INFINITY; mn[1] = INFINITY;
-        for (int i = tid; i < m; i += kBoxNT) {
-            const double dzi = qsm[D.dza + i] + qsm[D.dz + i], dsi = qsm[D.dsa + i] + qsm[D.ds + i];
-            qsm[D.dz + i] = dzi;
-            qsm[D.ds + i] = dsi;
-            mn[0] = fmin(mn[0], box_step(qsm[D.z + i], dzi));
-            mn[1] = fmin(mn[1], box_step(qsm[D.s + i], dsi));
-        }
-        qpb::block_reduce<2, true>(mn, qsm + D.red, tid, kBoxNT);
-        const double alpha = fmin(0.999 * fmin(box_step_fix(mn[0]), box_step_fix(mn[1])), 1.0);
-        for (int j = tid; j < n; j += kBoxNT) qsm[D.x + j] = fma(alpha, qsm[D.dxa + j] + qsm[D.dx + j], qsm[D.x + j]);
-        for (int i = tid; i < m; i += kBoxNT) {
-            qsm[D.s + i] = fma(alpha, qsm[D.ds + i], qsm[D.s + i]);
-            qsm[D.z + i] = fma(alpha, qsm[D.dz + i], qsm[D.z + i]);
-        }
-        for (int i = tid; i < e; i += kBoxNT) qsm[D.y + i] = fma(alpha, qsm[D.dya + i] + qsm[D.dy + i], qsm[D.y + i]);
-        __syncthreads();
-    }
-    __syncthreads();
-    for (int j = tid; j < n; j += kBoxNT) zhat[(int64_t)qp * n + j] = qsm[D.bx + j];
-    for (int i = tid; i < m; i += kBoxNT) {
-        lam[(int64_t)qp * m + i] = qsm[D.bz + i];
-        slacks[(int64_t)qp * m + i] = qsm[D.bs + i];
-    }
-    if (nus != nullptr)
-        for (int i = tid; i < e; i += kBoxNT) nus[(int64_t)qp * e + i] = qsm[D.by + i];
-    if (tid == 0) { iters_out[qp] = iters_run; resid_out[qp] = best; }
-}
-
-// QPFunctionFn.backward (qp.py:128-182) for the box QP: d from the clamped duals (qp.py:148), one factor of M and one
-// solve per QP, then dq = dx o z, dp = dx, dlb = dlam_lb, dub = -dlam_ub, dA = dnu z' + nu dx', db = -dnu. dxv, dlamv
-// and dnuv always receive dx, dlam, dnu (the batch means read them); a gradient whose mean flag is set is skipped here.
-struct BoxGrads {
-    double *dq, *dp, *dlb, *dub, *dA, *db;
-    int mq, mp, mlb, mub, mA, mb;
 };
 
-__global__ void __launch_bounds__(kBoxNT, 4)
-k_box_backward(BoxDims D, const double* __restrict__ q, int64_t sq, const double* __restrict__ A, int64_t sA,
-               const double* __restrict__ dl, const double* __restrict__ zhat, const double* __restrict__ lam,
-               const double* __restrict__ slacks, const double* __restrict__ nus, BoxGrads O,
-               double* __restrict__ dxv, double* __restrict__ dlamv, double* __restrict__ dnuv) {
-    QPB_SMEM;
-    const int tid = threadIdx.x, qp = blockIdx.x;
-    const int n = D.n, m = D.m, e = D.e;
-    box_stage(D, q + (int64_t)qp * sq, A + (int64_t)qp * sA, nullptr);
-    for (int j = tid; j < n; j += kBoxNT) qsm[D.rx + j] = dl[(int64_t)qp * n + j];
-    for (int i = tid; i < m; i += kBoxNT)
-        qsm[D.d + i] = fmax(lam[(int64_t)qp * m + i], 1e-8) / fmax(slacks[(int64_t)qp * m + i], 1e-8);
-    __syncthreads();
-    box_form(D);
-    box_solve(D, true, D.rx, -1, -1, -1, D.dx, D.ds, D.dz, D.dy);
-    for (int j = tid; j < n; j += kBoxNT) {
-        const double dx = qsm[D.dx + j], z = zhat[(int64_t)qp * n + j];
-        dxv[(int64_t)qp * n + j] = dx;
-        if (O.dq && !O.mq) O.dq[(int64_t)qp * n + j] = dx * z;
-        if (O.dp && !O.mp) O.dp[(int64_t)qp * n + j] = dx;
-    }
-    for (int i = tid; i < m; i += kBoxNT) {
-        const double dz = qsm[D.dz + i];
-        dlamv[(int64_t)qp * m + i] = dz;
-        if (i < D.nlb) { if (O.dlb && !O.mlb) O.dlb[(int64_t)qp * n + i] = dz; }
-        else if (O.dub && !O.mub) O.dub[(int64_t)qp * n + i - D.nlb] = -dz;
-    }
-    for (int i = tid; i < e; i += kBoxNT) {
-        dnuv[(int64_t)qp * e + i] = qsm[D.dy + i];
-        if (O.db && !O.mb) O.db[(int64_t)qp * e + i] = -qsm[D.dy + i];
-    }
-    if (O.dA && !O.mA)
-        for (int t = tid; t < e * n; t += kBoxNT) {
-            const int i = t / n, j = t - i * n;
-            O.dA[(int64_t)qp * e * n + t] = fma(qsm[D.dy + i], zhat[(int64_t)qp * n + j],
-                                                nus[(int64_t)qp * e + i] * qsm[D.dx + j]);
-        }
-}
-
-// qpb200_box_solve_kkt: the structured factor and solve for caller-given d and right-hand sides (all vectors (B, len))
-__global__ void __launch_bounds__(kBoxNT)
-k_box_kkt(BoxDims D, const double* __restrict__ q, int64_t sq, const double* __restrict__ A, int64_t sA,
-          const double* __restrict__ d, const double* __restrict__ rx, const double* __restrict__ rs,
-          const double* __restrict__ rz, const double* __restrict__ ry, double* __restrict__ dx, double* __restrict__ ds,
-          double* __restrict__ dz, double* __restrict__ dy) {
-    QPB_SMEM;
-    const int tid = threadIdx.x, qp = blockIdx.x;
-    const int n = D.n, m = D.m, e = D.e;
-    box_stage(D, q + (int64_t)qp * sq, A + (int64_t)qp * sA, nullptr);
-    for (int j = tid; j < n; j += kBoxNT) qsm[D.rx + j] = rx[(int64_t)qp * n + j];
-    for (int i = tid; i < m; i += kBoxNT) {
-        qsm[D.d + i] = d[(int64_t)qp * m + i];
-        qsm[D.rsc + i] = rs[(int64_t)qp * m + i];
-        qsm[D.rz + i] = rz[(int64_t)qp * m + i];
-    }
-    for (int i = tid; i < e; i += kBoxNT) qsm[D.ry + i] = ry[(int64_t)qp * e + i];
-    __syncthreads();
-    box_form(D);
-    box_solve(D, true, D.rx, D.rsc, D.rz, D.ry, D.dx, D.ds, D.dz, D.dy);
-    for (int j = tid; j < n; j += kBoxNT) dx[(int64_t)qp * n + j] = qsm[D.dx + j];
-    for (int i = tid; i < m; i += kBoxNT) {
-        ds[(int64_t)qp * m + i] = qsm[D.ds + i];
-        dz[(int64_t)qp * m + i] = qsm[D.dz + i];
-    }
-    if (dy != nullptr)
-        for (int i = tid; i < e; i += kBoxNT) dy[(int64_t)qp * e + i] = qsm[D.dy + i];
-}
-
-// batch means of the gradients of un-batched inputs (qp.py:159-177)
-// out[c] = scale / B * sum_b u[b * su + c] (* x[b * len + c] when x != null)
-__global__ void k_box_mean_vec(int B, int len, const double* __restrict__ u, int64_t su, const double* __restrict__ x,
-                               double scale, double* __restrict__ out) {
-    const int c = blockIdx.x * blockDim.x + threadIdx.x;
-    if (c >= len) return;
-    double s0 = 0.0, s1 = 0.0;
-    int bb = 0;
-    for (; bb + 1 < B; bb += 2) {
-        s0 += x ? u[(int64_t)bb * su + c] * x[(int64_t)bb * len + c] : u[(int64_t)bb * su + c];
-        s1 += x ? u[(int64_t)(bb + 1) * su + c] * x[(int64_t)(bb + 1) * len + c] : u[(int64_t)(bb + 1) * su + c];
-    }
-    if (bb < B) s0 += x ? u[(int64_t)bb * su + c] * x[(int64_t)bb * len + c] : u[(int64_t)bb * su + c];
-    out[c] = (s0 + s1) * scale / (double)B;
-}
-// dA mean: out[r][c] = 1/B sum_b (dnu[b][r] z[b][c] + nu[b][r] dx[b][c]); one thread per entry, a block per 128 columns
-__global__ void k_box_mean_outer(int B, int rows, int cols, const double* __restrict__ dnu, const double* __restrict__ z,
-                                 const double* __restrict__ nu, const double* __restrict__ dx, double* __restrict__ out) {
-    const int c = blockIdx.x * blockDim.x + threadIdx.x, r = blockIdx.y;
-    if (c >= cols) return;
-    double s = 0.0;
-    for (int bb = 0; bb < B; ++bb)
-        s = fma(dnu[(int64_t)bb * rows + r], z[(int64_t)bb * cols + c], fma(nu[(int64_t)bb * rows + r], dx[(int64_t)bb * cols + c], s));
-    out[(int64_t)r * cols + c] = s / (double)B;
-}
-
-// ---- cluster kernels: one thread block cluster of C CTAs per QP (shapes beyond one CTA's shared memory) ---------------
+// ---- one thread block cluster of C CTAs per QP ------------------------------------------------------------------------
 // CTA `rank` owns the variables [rank * slice, rank * slice + nloc) (the last slice may be partial or empty). In its own
-// shared memory it holds its columns of A, its entries of every length-nz vector and the lb / ub rows of those variables
-// (local row order: lb rows, then ub rows), laid out by box_dims(slice, ...) so that every CTA has the same footprint;
-// the length-neq_pad vectors are replicated. Behind that layout: the partial M (compact lower triangle) and two publish
-// buffers of the cluster reductions.
-//
-// INVARIANT: every CTA of a cluster executes the same sequence of cluster.sync() calls. A reduction is combined in rank
-// order (then warp order) from the partials every CTA publishes, so every CTA holds bit-identical sums and minima; M is
-// summed in rank order and factored redundantly by every CTA (same input, same code: bit-identical factor and dy, no
-// broadcast and no extra barrier), so y, mu, the residual and the step lengths are bit-identical too. Every branch that
-// reaches a cluster barrier (the exit tests, NaN and mu > 1e32 exits, best-iterate tracking, notImprovedLim, e > 0,
-// fresh) is decided from those values or from kernel arguments only; a CTA that branched on a value of its own would
-// deadlock its cluster.
+// shared memory it holds its entries of every length-nz vector and the lb / ub rows of those variables (local row order:
+// lb rows, then ub rows), laid out as for slice variables so that every CTA has the same footprint; the length-neq_pad
+// vectors are replicated. A reduction is combined in rank order (then warp order) from the partials every CTA publishes,
+// so every CTA holds bit-identical sums and minima (see the invariant at k_box_forward).
 //
 // Publish buffers alternate: a CTA rewrites buffer (ph & 1) only after the cluster barrier of the reduction that
-// followed its previous use, and every CTA finishes reading a buffer before it arrives at that barrier. The partial M is
-// rewritten by the next cl_form only after the right-hand-side reduction of the solve that read it.
-namespace cg = cooperative_groups;
-constexpr int kClW = kBoxNT / 32;                          // warps per CTA: scalar partials are published per warp
-
+// followed its previous use, and every CTA finishes reading a buffer before it arrives at that barrier.
 struct ClDims {
     BoxDims L;               // layout of one slice (L.n = slice); counts are set per CTA in cl_local
     int C, slice, ng, nlbg, mg;   // cluster size, variables per CTA, nz, lb rows, inequality rows (global)
@@ -492,10 +262,15 @@ struct ClDims {
     int total;               // doubles per CTA
 };
 
-__host__ __device__ inline ClDims cl_dims(int n, int e, int has_lb, int has_ub, int C) {
-    ClDims X;
+// the variable slices of a cluster of C CTAs
+__host__ __device__ inline void cl_slices(ClDims& X, int n, int has_lb, int has_ub, int C) {
     X.C = C; X.slice = (n + C - 1) / C; X.ng = n;
     X.nlbg = has_lb ? n : 0; X.mg = (has_lb ? n : 0) + (has_ub ? n : 0);
+}
+
+__host__ __device__ inline ClDims cl_dims(int n, int e, int has_lb, int has_ub, int C) {
+    ClDims X;
+    cl_slices(X, n, has_lb, has_ub, C);
     X.L = box_dims(X.slice, e, has_lb, has_ub);
     int o = X.L.total;
     X.Mp = o; o += r8((e * (e + 1)) / 2);
@@ -504,6 +279,8 @@ __host__ __device__ inline ClDims cl_dims(int n, int e, int has_lb, int has_ub, 
     X.total = o;
     return X;
 }
+
+__device__ __forceinline__ int cl_buf(const ClDims& X, int ph) { return X.pub + (ph & 1) * X.pb; }
 
 // this CTA's counts: nloc variables from j0
 __device__ __forceinline__ BoxDims cl_local(const ClDims& X, int rank, int& j0) {
@@ -521,10 +298,8 @@ __device__ __forceinline__ int64_t cl_grow(const ClDims& X, const BoxDims& D, in
 }
 
 // Cluster-wide reduction of N scalars (sum or min) and, when vlen > 0, of the length-vlen vector the caller wrote to
-// qsm[buf(ph)] (vdst: where its sum goes). One cluster barrier; every thread returns with the combined scalars.
+// qsm[cl_buf(X, ph)] (vdst: where its sum goes). One cluster barrier; every thread returns with the combined scalars.
 // Ends with a block barrier when vlen > 0.
-__device__ __forceinline__ int cl_buf(const ClDims& X, int ph) { return X.pub + (ph & 1) * X.pb; }
-
 template <int N, bool kMin>
 __device__ __forceinline__ void cl_reduce(const ClDims& X, double (&v)[N], int& ph, int vlen, int vdst) {
     QPB_SMEM;
@@ -558,48 +333,135 @@ __device__ __forceinline__ void cl_reduce(const ClDims& X, double (&v)[N], int& 
     ++ph;
 }
 
-// hinv for this CTA's variables and its partial A_r H_r^-1 A_r' (rows < e) into X.Mp; summed by the next cl_solve.
-__device__ __noinline__ void cl_form(const ClDims& X, const BoxDims& D) {
-    QPB_SMEM;
-    const int tid = threadIdx.x;
-    for (int j = tid; j < D.n; j += kBoxNT) {
-        double hj = qsm[D.q + j];
-        if (D.nlb) hj += qsm[D.d + j];
-        if (D.m > D.nlb) hj += qsm[D.d + D.nlb + j];
-        qsm[D.hinv + j] = 1.0 / hj;
-    }
-    __syncthreads();
-    if (D.e == 0) return;
-    const int n = D.n, lda = D.lda;
-    const int tot = (D.e * (D.e + 1)) / 2;
-    const double* A = qsm + D.A;
-    const double* hv = qsm + D.hinv;
-    for (int t = tid; t < tot; t += kBoxNT) {
-        int r = (int)((sqrt(8.0 * t + 1.0) - 1.0) * 0.5);
-        while ((r * (r + 1)) / 2 > t) --r;
-        while (((r + 1) * (r + 2)) / 2 <= t) ++r;
-        const int c = t - (r * (r + 1)) / 2;
-        const double* ar = A + r * lda;
-        const double* ac = A + c * lda;
-        double s0 = 0.0, s1 = 0.0;
-        int k = 0;
-        for (; k + 1 < n; k += 2) {
-            s0 = fma(ar[k] * hv[k], ac[k], s0);
-            s1 = fma(ar[k + 1] * hv[k + 1], ac[k + 1], s1);
-        }
-        if (k < n) s0 = fma(ar[k] * hv[k], ac[k], s0);
-        qsm[X.Mp + t] = s0 + s1;
-    }
-}
+// A cluster per QP: every CTA holds its columns of A, forms its partial A_r H_r^-1 A_r' (compact lower triangle, X.Mp),
+// and sums the partials in rank order and factors M itself (same input, same code: bit-identical factor and dy, with no
+// broadcast and no extra barrier). The partial M is rewritten by the next form only after the right-hand-side reduction
+// of the solve that read it.
+struct Cluster {
+    using Dims = ClDims;
+    static constexpr int kMinFwd = 1, kMinBwd = 1, kMinKkt = 1;
+    ClDims X;
+    BoxDims D;               // this CTA's slice
+    int ph = 0;              // cluster reductions so far: selects the publish buffer
 
-// box_solve on a cluster: rhs = ry - sum_r A_r H_r^-1 r_r (one cluster reduction; with fresh, the partial M of the last
-// cl_form is summed in the same barrier into the staircase and factored here, redundantly in every CTA). Ends with a
-// block barrier.
-__device__ __noinline__ void cl_solve(const ClDims& X, const BoxDims& D, int& ph, bool fresh, int rx, int rs, int rz,
-                                      int ry, int dx, int ds, int dz, int dy) {
+    __device__ explicit Cluster(const ClDims& P) : X(P) {
+        int j0;
+        D = cl_local(X, rank(), j0);
+    }
+    __device__ int qp() const { return blockIdx.x / X.C; }
+    __device__ static int rank() { return (int)cg::this_cluster().block_rank(); }
+    __device__ int j0() const { return rank() * X.slice; }
+    __device__ int ng() const { return X.ng; }
+    __device__ int mg() const { return X.mg; }
+    __device__ int64_t grow(int i) const { return cl_grow(X, D, j0(), i); }
+    __device__ static bool leader() { return rank() == 0; }
+    template <int N> __device__ void reduce_sum(double (&v)[N]) { cl_reduce<N, false>(X, v, ph, 0, 0); }
+    template <int N> __device__ void reduce_min(double (&v)[N]) { cl_reduce<N, true>(X, v, ph, 0, 0); }
+    __device__ int any(int bad) {
+        double v[1] = {bad ? 1.0 : 0.0};
+        reduce_sum(v);
+        return v[0] > 0.0;
+    }
+    // no CTA exits while another may still read its shared memory
+    __device__ static void sync() { cg::this_cluster().sync(); }
+    __device__ double a(int i, int j) const { QPB_SMEM; return qsm[D.A + i * D.lda + j]; }
+
+    // q and this CTA's columns of A; b replicated (forward only); the staircase tile table
+    __device__ void stage(const double* q, const double* A, const double* b) const {
+        QPB_SMEM;
+        const int tid = threadIdx.x, j0 = this->j0();
+        for (int j = tid; j < D.n; j += kBoxNT) qsm[D.q + j] = q[j0 + j];
+        for (int t = tid; t < D.e * D.n; t += kBoxNT) {
+            const int i = t / D.n, j = t - i * D.n;
+            qsm[D.A + i * D.lda + j] = A[(int64_t)i * X.ng + j0 + j];
+        }
+        for (int i = tid; i < D.ep; i += kBoxNT) qsm[D.b + i] = (b != nullptr && i < D.e) ? b[i] : 0.0;
+        if (D.e > 0) pf_build_tab(D.tab, D.ep >> 3);
+        __syncthreads();
+    }
+
+    // H^-1 and the partial M (rows < e) into X.Mp; summed by the next solve
+    __device__ __noinline__ void form() const {
+        QPB_SMEM;
+        form_hinv(D);
+        __syncthreads();
+        if (D.e == 0) return;
+        const int tot = (D.e * (D.e + 1)) / 2;
+        for (int t = threadIdx.x; t < tot; t += kBoxNT) {
+            const int r = tri_row(t), c = t - (r * (r + 1)) / 2;
+            qsm[X.Mp + t] = ahat(qsm + D.A + r * D.lda, qsm + D.A + c * D.lda, qsm + D.hinv, D.n);
+        }
+    }
+
+    // this CTA's partials of A v (rows < e, its columns) into the publish buffer of the next reduction, a warp per row
+    __device__ void publish_av(int v) const {
+        QPB_SMEM;
+        const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, buf = cl_buf(X, ph);
+        for (int i = warp; i < D.e; i += kClW) {
+            double a = 0.0;
+            for (int k = lane; k < D.n; k += 32) a = fma(qsm[D.A + i * D.lda + k], qsm[v + k], a);
+            a = qpb::warp_sum(a);
+            if (lane == 0) qsm[buf + i] = a;
+        }
+    }
+
+    // ry = A x - b: A x is reduced with the scalars, ry and |ry|^2 are formed redundantly after the cluster reduction
+    __device__ void ry_step(double (&acc)[4]) {
+        QPB_SMEM;
+        const int e = D.e;
+        publish_av(D.x);
+        cl_reduce<4, false>(X, acc, ph, e, D.ry);
+        for (int i = 0; i < e; ++i) {
+            const double r = qsm[D.ry + i] - qsm[D.b + i];
+            acc[0] = fma(r, r, acc[0]);
+        }
+        __syncthreads();                                     // every thread has read the sums of A x
+        for (int i = threadIdx.x; i < D.ep; i += kBoxNT) qsm[D.ry + i] = (i < e) ? qsm[D.ry + i] - qsm[D.b + i] : 0.0;
+    }
+
+    // rhs = ry - sum_r A_r H_r^-1 r_r in one cluster barrier; fresh: the partial M of the last form is summed into the
+    // staircase in the same barrier
+    __device__ void solve_mid(bool fresh, int ry, int dy) {
+        QPB_SMEM;
+        cg::cluster_group cl = cg::this_cluster();
+        const int e = D.e, buf = cl_buf(X, ph);
+        publish_av(D.r);
+        cl.sync();
+        for (int i = threadIdx.x; i < D.ep; i += kBoxNT) {
+            double a = 0.0;
+            if (i < e)
+                for (int k = 0; k < X.C; ++k) a += cl.map_shared_rank(qsm + buf, k)[i];
+            qsm[D.rhs + i] = (i < e) ? (((ry >= 0) ? qsm[ry + i] : 0.0) - a) : 0.0;
+        }
+        ++ph;
+        if (fresh) {
+            const int tot = (D.ep * (D.ep + 1)) / 2;
+            for (int t = threadIdx.x; t < tot; t += kBoxNT) {
+                const int r = tri_row(t), c = t - (r * (r + 1)) / 2;
+                double v = 0.0;
+                if (r < e)
+                    for (int k = 0; k < X.C; ++k) v += cl.map_shared_rank(qsm + X.Mp, k)[t];
+                else
+                    v = (r == c) ? 1.0 : 0.0;
+                qsm[D.S + pf_rowoff(r) + c] = v;
+            }
+        }
+        __syncthreads();
+        stair_solve(D, fresh, dy);
+    }
+};
+
+// ---- the solver, written once over the families ------------------------------------------------------------------------
+// The structured KKT solve with the H / M of the last form:
+//   K [dx ds dz dy] = -[rx rs rz ry];  rs, rz, ry may be -1 (zero). fresh: M was just formed and is factored here
+// (with the right-hand side carried along), else the existing factor is reused. Ends with a block barrier.
+template <class F>
+__device__ __noinline__ void box_solve(F& f, bool fresh, int rx, int rs, int rz, int ry, int dx, int ds, int dz, int dy) {
     QPB_SMEM;
+    const BoxDims& D = f.D;
     const int tid = threadIdx.x;
-    const int n = D.n, m = D.m, e = D.e, ep = D.ep, lda = D.lda;
+    const int n = D.n, m = D.m, e = D.e;
+    // r = rx + G'(D rz - rs), kept as H^-1 r in D.r
     for (int j = tid; j < n; j += kBoxNT) {
         double a = qsm[rx + j];
         if (D.nlb) {
@@ -614,52 +476,11 @@ __device__ __noinline__ void cl_solve(const ClDims& X, const BoxDims& D, int& ph
         qsm[D.r + j] = a * qsm[D.hinv + j];
     }
     __syncthreads();
-    if (e > 0) {
-        cg::cluster_group cl = cg::this_cluster();
-        const int lane = tid & 31, warp = tid >> 5, buf = cl_buf(X, ph);
-        for (int i = warp; i < e; i += kBoxNT / 32) {
-            double a = 0.0;
-            for (int k = lane; k < n; k += 32) a = fma(qsm[D.A + i * lda + k], qsm[D.r + k], a);
-            a = qpb::warp_sum(a);
-            if (lane == 0) qsm[buf + i] = a;
-        }
-        cl.sync();                                           // the partials of A H^-1 r (and of M) are published
-        if (fresh) {
-            const int tot = (ep * (ep + 1)) / 2;
-            for (int t = tid; t < tot; t += kBoxNT) {
-                int r = (int)((sqrt(8.0 * t + 1.0) - 1.0) * 0.5);
-                while ((r * (r + 1)) / 2 > t) --r;
-                while (((r + 1) * (r + 2)) / 2 <= t) ++r;
-                const int c = t - (r * (r + 1)) / 2;
-                double v = 0.0;
-                if (r < e)
-                    for (int k = 0; k < X.C; ++k) v += cl.map_shared_rank(qsm + X.Mp, k)[t];
-                else
-                    v = (r == c) ? 1.0 : 0.0;
-                qsm[D.S + pf_rowoff(r) + c] = v;
-            }
-        }
-        for (int i = tid; i < ep; i += kBoxNT) {
-            double a = 0.0;
-            if (i < e)
-                for (int k = 0; k < X.C; ++k) a += cl.map_shared_rank(qsm + buf, k)[i];
-            qsm[D.rhs + i] = (i < e) ? (((ry >= 0) ? qsm[ry + i] : 0.0) - a) : 0.0;
-        }
-        ++ph;
-        __syncthreads();
-        const int nts = ep >> 3;
-        if (fresh) {
-            pf_chol(D.S, nts, 0, D.rhs, D.pan, D.tab);
-            __syncthreads();
-        } else {
-            pf_fwd(D.S, ep, 0, nts - 1, D.rhs);
-        }
-        pf_diag(D.S, ep, D.rhs, D.t, D.rhs);
-        pf_bwd(D.S, ep, D.rhs, dy);
-    }
+    if (e > 0) f.solve_mid(fresh, ry, dy);
+    // dx = -H^-1 r - H^-1 A'dy
     for (int j = tid; j < n; j += kBoxNT) {
         double a = 0.0;
-        for (int i = 0; i < e; ++i) a = fma(qsm[D.A + i * lda + j], qsm[dy + i], a);
+        for (int i = 0; i < e; ++i) a = fma(f.a(i, j), qsm[dy + i], a);
         qsm[dx + j] = -qsm[D.r + j] - a * qsm[D.hinv + j];
     }
     __syncthreads();
@@ -673,46 +494,39 @@ __device__ __noinline__ void cl_solve(const ClDims& X, const BoxDims& D, int& ph
     __syncthreads();
 }
 
-// q and this CTA's columns of A; b replicated (forward only); the staircase tile table
-__device__ __forceinline__ void cl_stage(const ClDims& X, const BoxDims& D, int j0, const double* q, const double* A,
-                                         const double* b) {
+// forward (batch.py:47-207) with the structured solve; the loop of k_forward_fast (qp_solve.cuh). Every CTA writes its
+// slice of zhat, lam and slacks; the leader nus, iters, best_resid, the trace rows and spd_flag. One CTA per QP: three
+// CTAs per SM (at most 168 registers; about 48 KB of shared memory per QP at nz = 64, neq = 40): four (128 registers)
+// spill.
+//
+// INVARIANT (Cluster, and the k_box_*_dm kernels, which repeat this loop): every CTA of a cluster executes the same
+// sequence of cluster.sync() calls. Every reduction leaves bit-identical sums and minima in every CTA, and so does every
+// solve (M is summed in rank order and factored redundantly, or dy is gathered from its owners), so y, mu, the residual
+// and the step lengths are bit-identical too. Every branch that reaches a cluster barrier (the exit tests, NaN and mu > 1e32 exits, best-iterate
+// tracking, notImprovedLim, e > 0, fresh) is decided from those values or from kernel arguments only; a CTA that branched
+// on a value of its own would deadlock its cluster.
+template <class F>
+__global__ void __launch_bounds__(kBoxNT, F::kMinFwd)
+k_box_forward(typename F::Dims P, const double* __restrict__ q, int64_t sq, const double* __restrict__ p, int64_t sp,
+              const double* __restrict__ A, int64_t sA, const double* __restrict__ b, int64_t sb,
+              const double* __restrict__ lb, int64_t slb, const double* __restrict__ ub, int64_t sub, double eps,
+              double stall_tol, double best_tie, int notImprovedLim, int maxIter, double* __restrict__ zhat,
+              double* __restrict__ lam, double* __restrict__ slacks, double* __restrict__ nus, int* __restrict__ iters_out,
+              double* __restrict__ resid_out, double* __restrict__ trace, int* __restrict__ spd_flag) {
     QPB_SMEM;
-    const int tid = threadIdx.x;
-    for (int j = tid; j < D.n; j += kBoxNT) qsm[D.q + j] = q[j0 + j];
-    for (int t = tid; t < D.e * D.n; t += kBoxNT) {
-        const int i = t / D.n, j = t - i * D.n;
-        qsm[D.A + i * D.lda + j] = A[(int64_t)i * X.ng + j0 + j];
-    }
-    for (int i = tid; i < D.ep; i += kBoxNT) qsm[D.b + i] = (b != nullptr && i < D.e) ? b[i] : 0.0;
-    if (D.e > 0) pf_build_tab(D.tab, D.ep >> 3);
-    __syncthreads();
-}
-
-// k_box_forward on a cluster (same Mehrotra loop, exit rules and outputs; see the invariant above). Rank 0 writes nus,
-// iters, best_resid, the trace rows and spd_flag; every CTA its slice of zhat, lam and slacks.
-__global__ void __launch_bounds__(kBoxNT, 1)
-k_box_forward_cl(ClDims X, const double* __restrict__ q, int64_t sq, const double* __restrict__ p, int64_t sp,
-                 const double* __restrict__ A, int64_t sA, const double* __restrict__ b, int64_t sb,
-                 const double* __restrict__ lb, int64_t slb, const double* __restrict__ ub, int64_t sub, double eps,
-                 double stall_tol, double best_tie, int notImprovedLim, int maxIter, double* __restrict__ zhat,
-                 double* __restrict__ lam, double* __restrict__ slacks, double* __restrict__ nus,
-                 int* __restrict__ iters_out, double* __restrict__ resid_out, double* __restrict__ trace,
-                 int* __restrict__ spd_flag) {
-    QPB_SMEM;
-    const int rank = (int)cg::this_cluster().block_rank();
-    const int tid = threadIdx.x, qp = blockIdx.x / X.C;
-    int j0, ph = 0;
-    const BoxDims D = cl_local(X, rank, j0);
-    const int n = D.n, m = D.m, e = D.e, ep = D.ep, N = X.ng;
-    cl_stage(X, D, j0, q + (int64_t)qp * sq, A + (int64_t)qp * sA, (e > 0) ? b + (int64_t)qp * sb : nullptr);
+    F f(P);
+    const BoxDims& D = f.D;
+    const int tid = threadIdx.x, qp = f.qp(), j0 = f.j0();
+    const int n = D.n, m = D.m, e = D.e, ep = D.ep;
+    f.stage(q + (int64_t)qp * sq, A + (int64_t)qp * sA, (e > 0) ? b + (int64_t)qp * sb : nullptr);
     {
-        double bad[1] = {0.0};
+        int bad = 0;
         for (int j = tid; j < n; j += kBoxNT) {
             qsm[D.p + j] = p[(int64_t)qp * sp + j0 + j];
-            if (!(qsm[D.q + j] > 0.0)) bad[0] = 1.0;
+            bad |= !(qsm[D.q + j] > 0.0);
         }
-        cl_reduce<1, false>(X, bad, ph, 0, 0);
-        if (rank == 0 && tid == 0 && spd_flag != nullptr) spd_flag[qp] = bad[0] > 0.0;
+        bad = f.any(bad);
+        if (f.leader() && tid == 0 && spd_flag != nullptr) spd_flag[qp] = bad;
     }
     for (int i = tid; i < m; i += kBoxNT) {
         qsm[D.h + i] = (i < D.nlb) ? -lb[(int64_t)qp * slb + j0 + i] : ub[(int64_t)qp * sub + j0 + i - D.nlb];
@@ -723,12 +537,12 @@ k_box_forward_cl(ClDims X, const double* __restrict__ q, int64_t sq, const doubl
     __syncthreads();
 
     // ---- initial point: solve_kkt(p, 0, -h, -b) with d = 1   (batch.py:61-67)
-    cl_form(X, D);
-    cl_solve(X, D, ph, true, D.p, -1, D.rz, D.ry, D.x, D.s, D.z, D.y);
+    f.form();
+    box_solve(f, true, D.p, -1, D.rz, D.ry, D.x, D.s, D.z, D.y);
     {
         double mn[2] = {INFINITY, INFINITY};
         for (int i = tid; i < m; i += kBoxNT) { mn[0] = fmin(mn[0], qsm[D.s + i]); mn[1] = fmin(mn[1], qsm[D.z + i]); }
-        cl_reduce<2, true>(X, mn, ph, 0, 0);
+        f.reduce_min(mn);
         for (int i = tid; i < m; i += kBoxNT) {                  // slacks and duals >= 1 (batch.py:77-87)
             if (mn[0] < 0.0) qsm[D.s + i] -= mn[0] - 1.0;
             if (mn[1] < 0.0) qsm[D.z + i] -= mn[1] - 1.0;
@@ -738,14 +552,14 @@ k_box_forward_cl(ClDims X, const double* __restrict__ q, int64_t sq, const doubl
 
     double best = 0.0;
     int nNot = 0, iters_run = 0;
-    const double dm = (double)X.mg;
+    const double dm = (double)f.mg();
     for (int it = 0; it < maxIter; ++it) {
         iters_run = it + 1;
-        // ---- residuals (batch.py:94-107): A x is reduced with the scalars, ry and |ry|^2 are formed redundantly
+        // ---- residuals (batch.py:94-107)
         double acc[4] = {0.0, 0.0, 0.0, 0.0};                   // |ry|^2, |rz|^2, |rx|^2, s.z
         for (int j = tid; j < n; j += kBoxNT) {
             double a = 0.0;
-            for (int i = 0; i < e; ++i) a = fma(qsm[D.A + i * D.lda + j], qsm[D.y + i], a);
+            for (int i = 0; i < e; ++i) a = fma(f.a(i, j), qsm[D.y + i], a);
             const double r = fma(qsm[D.q + j], qsm[D.x + j], qsm[D.p + j]) + gt_col(D, qsm + D.z, j) + a;
             qsm[D.rx + j] = r;
             acc[2] = fma(r, r, acc[2]);
@@ -756,25 +570,10 @@ k_box_forward_cl(ClDims X, const double* __restrict__ q, int64_t sq, const doubl
             acc[1] = fma(r, r, acc[1]);
             acc[3] = fma(qsm[D.s + i], qsm[D.z + i], acc[3]);
         }
-        {
-            const int lane = tid & 31, warp = tid >> 5, buf = cl_buf(X, ph);
-            for (int i = warp; i < e; i += kBoxNT / 32) {
-                double a = 0.0;
-                for (int k = lane; k < n; k += 32) a = fma(qsm[D.A + i * D.lda + k], qsm[D.x + k], a);
-                a = qpb::warp_sum(a);
-                if (lane == 0) qsm[buf + i] = a;
-            }
-        }
-        cl_reduce<4, false>(X, acc, ph, e, D.ry);
-        for (int i = 0; i < e; ++i) {
-            const double r = qsm[D.ry + i] - qsm[D.b + i];
-            acc[0] = fma(r, r, acc[0]);
-        }
-        __syncthreads();                                         // every thread has read the sums of A x
-        for (int i = tid; i < ep; i += kBoxNT) qsm[D.ry + i] = (i < e) ? qsm[D.ry + i] - qsm[D.b + i] : 0.0;
+        f.ry_step(acc);
         const double mu = fabs(acc[3] / dm);
         const double resid = sqrt(acc[1]) + sqrt(acc[0]) + sqrt(acc[2]) + dm * mu;
-        if (trace != nullptr && rank == 0 && tid == 0) {          // what verbose=1 prints (batch.py:115-117)
+        if (trace != nullptr && f.leader() && tid == 0) {       // what verbose=1 prints (batch.py:115-117)
             double* tr = trace + ((int64_t)qp * maxIter + it) * 4;
             tr[0] = sqrt(acc[1]) + sqrt(acc[0]); tr[1] = sqrt(acc[2]); tr[2] = mu; tr[3] = resid;
         }
@@ -791,15 +590,15 @@ k_box_forward_cl(ClDims X, const double* __restrict__ q, int64_t sq, const doubl
         // ---- d = z/s, H, M; the affine direction (batch.py:109-113,150) factors M
         for (int i = tid; i < m; i += kBoxNT) qsm[D.d + i] = qsm[D.z + i] / qsm[D.s + i];
         __syncthreads();
-        cl_form(X, D);
-        cl_solve(X, D, ph, true, D.rx, D.z, D.rz, D.ry, D.dxa, D.dsa, D.dza, D.dya);
+        f.form();
+        box_solve(f, true, D.rx, D.z, D.rz, D.ry, D.dxa, D.dsa, D.dza, D.dya);
         // ---- affine step length and sigma (batch.py:160-168)
         double mn[2] = {INFINITY, INFINITY};
         for (int i = tid; i < m; i += kBoxNT) {
             mn[0] = fmin(mn[0], box_step(qsm[D.z + i], qsm[D.dza + i]));
             mn[1] = fmin(mn[1], box_step(qsm[D.s + i], qsm[D.dsa + i]));
         }
-        cl_reduce<2, true>(X, mn, ph, 0, 0);
+        f.reduce_min(mn);
         {
             const double alpha = fmin(fmin(box_step_fix(mn[0]), box_step_fix(mn[1])), 1.0);
             double sm[2] = {0.0, 0.0};
@@ -807,7 +606,7 @@ k_box_forward_cl(ClDims X, const double* __restrict__ q, int64_t sq, const doubl
                 sm[0] = fma(qsm[D.s + i] + alpha * qsm[D.dsa + i], qsm[D.z + i] + alpha * qsm[D.dza + i], sm[0]);
                 sm[1] = fma(qsm[D.s + i], qsm[D.z + i], sm[1]);
             }
-            cl_reduce<2, false>(X, sm, ph, 0, 0);
+            f.reduce_sum(sm);
             const double sr = sm[0] / sm[1];
             const double sig = sr * sr * sr;
             // ---- corrector right-hand side (batch.py:170-181): rs = (-mu sig + dsa dza) / s, rx = rz = ry = 0
@@ -816,7 +615,7 @@ k_box_forward_cl(ClDims X, const double* __restrict__ q, int64_t sq, const doubl
             for (int j = tid; j < n; j += kBoxNT) qsm[D.rx + j] = 0.0;
             __syncthreads();
         }
-        cl_solve(X, D, ph, false, D.rx, D.rsc, -1, -1, D.dx, D.ds, D.dz, D.dy);
+        box_solve(f, false, D.rx, D.rsc, -1, -1, D.dx, D.ds, D.dz, D.dy);
         // ---- combined direction, step length, update (batch.py:185-203)
         mn[0] = INFINITY; mn[1] = INFINITY;
         for (int i = tid; i < m; i += kBoxNT) {
@@ -826,7 +625,7 @@ k_box_forward_cl(ClDims X, const double* __restrict__ q, int64_t sq, const doubl
             mn[0] = fmin(mn[0], box_step(qsm[D.z + i], dzi));
             mn[1] = fmin(mn[1], box_step(qsm[D.s + i], dsi));
         }
-        cl_reduce<2, true>(X, mn, ph, 0, 0);
+        f.reduce_min(mn);
         const double alpha = fmin(0.999 * fmin(box_step_fix(mn[0]), box_step_fix(mn[1])), 1.0);
         for (int j = tid; j < n; j += kBoxNT) qsm[D.x + j] = fma(alpha, qsm[D.dxa + j] + qsm[D.dx + j], qsm[D.x + j]);
         for (int i = tid; i < m; i += kBoxNT) {
@@ -837,41 +636,49 @@ k_box_forward_cl(ClDims X, const double* __restrict__ q, int64_t sq, const doubl
         __syncthreads();
     }
     __syncthreads();
-    for (int j = tid; j < n; j += kBoxNT) zhat[(int64_t)qp * N + j0 + j] = qsm[D.bx + j];
+    for (int j = tid; j < n; j += kBoxNT) zhat[(int64_t)qp * f.ng() + j0 + j] = qsm[D.bx + j];
     for (int i = tid; i < m; i += kBoxNT) {
-        const int64_t g = (int64_t)qp * X.mg + cl_grow(X, D, j0, i);
+        const int64_t g = (int64_t)qp * f.mg() + f.grow(i);
         lam[g] = qsm[D.bz + i];
         slacks[g] = qsm[D.bs + i];
     }
-    if (rank == 0) {
+    if (f.leader()) {
         if (nus != nullptr)
             for (int i = tid; i < e; i += kBoxNT) nus[(int64_t)qp * e + i] = qsm[D.by + i];
         if (tid == 0) { iters_out[qp] = iters_run; resid_out[qp] = best; }
     }
-    cg::this_cluster().sync();       // no CTA exits while another may still read its publish buffers
+    f.sync();
 }
 
-// k_box_backward on a cluster: every CTA its slice of dx, dlam, dq, dp, dlb, dub and its columns of dA; rank 0 dnu, db
-__global__ void __launch_bounds__(kBoxNT, 1)
-k_box_backward_cl(ClDims X, const double* __restrict__ q, int64_t sq, const double* __restrict__ A, int64_t sA,
-                  const double* __restrict__ dl, const double* __restrict__ zhat, const double* __restrict__ lam,
-                  const double* __restrict__ slacks, const double* __restrict__ nus, BoxGrads O,
-                  double* __restrict__ dxv, double* __restrict__ dlamv, double* __restrict__ dnuv) {
+// QPFunctionFn.backward (qp.py:128-182) for the box QP: d from the clamped duals (qp.py:148), one factor of M and one
+// solve per QP, then dq = dx o z, dp = dx, dlb = dlam_lb, dub = -dlam_ub, dA = dnu z' + nu dx', db = -dnu. dxv, dlamv
+// and dnuv always receive dx, dlam, dnu (the batch means read them); a gradient whose mean flag is set is skipped here.
+// Every CTA writes its slice of dx, dlam, dq, dp, dlb, dub and its columns of dA; the leader dnu and db.
+struct BoxGrads {
+    double *dq, *dp, *dlb, *dub, *dA, *db;
+    int mq, mp, mlb, mub, mA, mb;
+};
+
+template <class F>
+__global__ void __launch_bounds__(kBoxNT, F::kMinBwd)
+k_box_backward(typename F::Dims P, const double* __restrict__ q, int64_t sq, const double* __restrict__ A, int64_t sA,
+               const double* __restrict__ dl, const double* __restrict__ zhat, const double* __restrict__ lam,
+               const double* __restrict__ slacks, const double* __restrict__ nus, BoxGrads O,
+               double* __restrict__ dxv, double* __restrict__ dlamv, double* __restrict__ dnuv) {
     QPB_SMEM;
-    const int rank = (int)cg::this_cluster().block_rank();
-    const int tid = threadIdx.x, qp = blockIdx.x / X.C;
-    int j0, ph = 0;
-    const BoxDims D = cl_local(X, rank, j0);
-    const int n = D.n, m = D.m, e = D.e, N = X.ng;
-    cl_stage(X, D, j0, q + (int64_t)qp * sq, A + (int64_t)qp * sA, nullptr);
+    F f(P);
+    const BoxDims& D = f.D;
+    const int tid = threadIdx.x, qp = f.qp(), j0 = f.j0();
+    const int n = D.n, m = D.m, e = D.e, N = f.ng();
+    f.stage(q + (int64_t)qp * sq, A + (int64_t)qp * sA, nullptr);
     for (int j = tid; j < n; j += kBoxNT) qsm[D.rx + j] = dl[(int64_t)qp * N + j0 + j];
     for (int i = tid; i < m; i += kBoxNT) {
-        const int64_t g = (int64_t)qp * X.mg + cl_grow(X, D, j0, i);
+        const int64_t g = (int64_t)qp * f.mg() + f.grow(i);
         qsm[D.d + i] = fmax(lam[g], 1e-8) / fmax(slacks[g], 1e-8);
     }
     __syncthreads();
-    cl_form(X, D);
-    cl_solve(X, D, ph, true, D.rx, -1, -1, -1, D.dx, D.ds, D.dz, D.dy);
+    f.form();
+    box_solve(f, true, D.rx, -1, -1, -1, D.dx, D.ds, D.dz, D.dy);
     for (int j = tid; j < n; j += kBoxNT) {
         const int64_t g = (int64_t)qp * N + j0 + j;
         const double dx = qsm[D.dx + j], z = zhat[g];
@@ -881,11 +688,11 @@ k_box_backward_cl(ClDims X, const double* __restrict__ q, int64_t sq, const doub
     }
     for (int i = tid; i < m; i += kBoxNT) {
         const double dz = qsm[D.dz + i];
-        dlamv[(int64_t)qp * X.mg + cl_grow(X, D, j0, i)] = dz;
+        dlamv[(int64_t)qp * f.mg() + f.grow(i)] = dz;
         if (i < D.nlb) { if (O.dlb && !O.mlb) O.dlb[(int64_t)qp * N + j0 + i] = dz; }
         else if (O.dub && !O.mub) O.dub[(int64_t)qp * N + j0 + i - D.nlb] = -dz;
     }
-    if (rank == 0)
+    if (f.leader())
         for (int i = tid; i < e; i += kBoxNT) {
             dnuv[(int64_t)qp * e + i] = qsm[D.dy + i];
             if (O.db && !O.mb) O.db[(int64_t)qp * e + i] = -qsm[D.dy + i];
@@ -896,42 +703,42 @@ k_box_backward_cl(ClDims X, const double* __restrict__ q, int64_t sq, const doub
             O.dA[((int64_t)qp * e + i) * N + j0 + j] = fma(qsm[D.dy + i], zhat[(int64_t)qp * N + j0 + j],
                                                            nus[(int64_t)qp * e + i] * qsm[D.dx + j]);
         }
-    cg::this_cluster().sync();
+    f.sync();
 }
 
-// k_box_kkt on a cluster
-__global__ void __launch_bounds__(kBoxNT, 1)
-k_box_kkt_cl(ClDims X, const double* __restrict__ q, int64_t sq, const double* __restrict__ A, int64_t sA,
-             const double* __restrict__ d, const double* __restrict__ rx, const double* __restrict__ rs,
-             const double* __restrict__ rz, const double* __restrict__ ry, double* __restrict__ dx,
-             double* __restrict__ ds, double* __restrict__ dz, double* __restrict__ dy) {
+// qpb200_box_solve_kkt: the structured factor and solve for caller-given d and right-hand sides (all vectors (B, len))
+template <class F>
+__global__ void __launch_bounds__(kBoxNT, F::kMinKkt)
+k_box_kkt(typename F::Dims P, const double* __restrict__ q, int64_t sq, const double* __restrict__ A, int64_t sA,
+          const double* __restrict__ d, const double* __restrict__ rx, const double* __restrict__ rs,
+          const double* __restrict__ rz, const double* __restrict__ ry, double* __restrict__ dx, double* __restrict__ ds,
+          double* __restrict__ dz, double* __restrict__ dy) {
     QPB_SMEM;
-    const int rank = (int)cg::this_cluster().block_rank();
-    const int tid = threadIdx.x, qp = blockIdx.x / X.C;
-    int j0, ph = 0;
-    const BoxDims D = cl_local(X, rank, j0);
-    const int n = D.n, m = D.m, e = D.e, N = X.ng;
-    cl_stage(X, D, j0, q + (int64_t)qp * sq, A + (int64_t)qp * sA, nullptr);
+    F f(P);
+    const BoxDims& D = f.D;
+    const int tid = threadIdx.x, qp = f.qp(), j0 = f.j0();
+    const int n = D.n, m = D.m, e = D.e, N = f.ng();
+    f.stage(q + (int64_t)qp * sq, A + (int64_t)qp * sA, nullptr);
     for (int j = tid; j < n; j += kBoxNT) qsm[D.rx + j] = rx[(int64_t)qp * N + j0 + j];
     for (int i = tid; i < m; i += kBoxNT) {
-        const int64_t g = (int64_t)qp * X.mg + cl_grow(X, D, j0, i);
+        const int64_t g = (int64_t)qp * f.mg() + f.grow(i);
         qsm[D.d + i] = d[g];
         qsm[D.rsc + i] = rs[g];
         qsm[D.rz + i] = rz[g];
     }
     for (int i = tid; i < e; i += kBoxNT) qsm[D.ry + i] = ry[(int64_t)qp * e + i];
     __syncthreads();
-    cl_form(X, D);
-    cl_solve(X, D, ph, true, D.rx, D.rsc, D.rz, D.ry, D.dx, D.ds, D.dz, D.dy);
+    f.form();
+    box_solve(f, true, D.rx, D.rsc, D.rz, D.ry, D.dx, D.ds, D.dz, D.dy);
     for (int j = tid; j < n; j += kBoxNT) dx[(int64_t)qp * N + j0 + j] = qsm[D.dx + j];
     for (int i = tid; i < m; i += kBoxNT) {
-        const int64_t g = (int64_t)qp * X.mg + cl_grow(X, D, j0, i);
+        const int64_t g = (int64_t)qp * f.mg() + f.grow(i);
         ds[g] = qsm[D.ds + i];
         dz[g] = qsm[D.dz + i];
     }
-    if (dy != nullptr && rank == 0)
+    if (dy != nullptr && f.leader())
         for (int i = tid; i < e; i += kBoxNT) dy[(int64_t)qp * e + i] = qsm[D.dy + i];
-    cg::this_cluster().sync();
+    f.sync();
 }
 
 // ---- distributed-M kernels: neq_pad > 128 on a cluster ---------------------------------------------------------------
@@ -969,8 +776,7 @@ __device__ __forceinline__ int dm_below(int C, int rank, int k) { return (k >= r
 __host__ __device__ inline DmDims dm_dims(int n, int e, int has_lb, int has_ub, int C) {
     DmDims Y;
     ClDims& X = Y.X;
-    X.C = C; X.slice = (n + C - 1) / C; X.ng = n;
-    X.nlbg = has_lb ? n : 0; X.mg = (has_lb ? n : 0) + (has_ub ? n : 0);
+    cl_slices(X, n, has_lb, has_ub, C);
     BoxDims& D = X.L;
     D.n = X.slice; D.e = e; D.ep = r8(e);
     D.nlb = has_lb ? X.slice : 0; D.m = (has_lb ? X.slice : 0) + (has_ub ? X.slice : 0);
@@ -984,23 +790,17 @@ __host__ __device__ inline DmDims dm_dims(int n, int e, int has_lb, int has_ub, 
     int o = 0;
     D.S = o; o += r8(stair);
     D.pan = o; o += 8 * Y.nts * kPanLd;
-    const int nn = r8(D.n), mm = r8(D.m), ee = D.ep;
-    int* vn[] = {&D.q, &D.p, &D.x, &D.rx, &D.r, &D.hinv, &D.dxa, &D.dx, &D.bx};
-    for (int* v : vn) { *v = o; o += nn; }
-    int* vm[] = {&D.h, &D.s, &D.z, &D.d, &D.rz, &D.dsa, &D.dza, &D.ds, &D.dz, &D.bs, &D.bz, &D.rsc};
-    for (int* v : vm) { *v = o; o += mm; }
-    int* ve[] = {&D.b, &D.y, &D.ry, &D.rhs, &D.t, &D.dya, &D.dy, &D.by};
-    for (int* v : ve) { *v = o; o += ee; }
+    o = box_vectors(D, o);
     D.total = o;
     X.Mp = 0;
-    X.pb = r8(ee + 4 * kClW);
+    X.pb = r8(D.ep + 4 * kClW);
     X.pub = o; o += 2 * X.pb;
     Y.hfull = o; o += r8(n) + kDmKC;                     // zero past n: the last chunk reads it
     Y.Tk = o; o += 72;                                   // T_k (64, upper part zero), then b_k (8)
-    Y.cv = o; o += ee;
-    Y.part = o; o += ee;
-    Y.wpub = o; o += ee;
-    Y.As = o; o += ee * kDmLdA;
+    Y.cv = o; o += D.ep;
+    Y.part = o; o += D.ep;
+    Y.wpub = o; o += D.ep;
+    Y.As = o; o += D.ep * kDmLdA;
     X.total = Y.total = o;
     return Y;
 }
@@ -1247,7 +1047,7 @@ __device__ __noinline__ void dm_bwd(const DmDims& Y, const BoxDims& D, int rank,
     __syncthreads();
 }
 
-// cl_solve with M distributed (Ag: this QP's A in global memory). Ends with a block barrier.
+// box_solve<Cluster> with M distributed (Ag: this QP's A in global memory). Ends with a block barrier.
 __device__ __noinline__ void dm_solve(const DmDims& Y, const BoxDims& D, int rank, const double* __restrict__ Ag, int j0,
                                       int& ph, bool fresh, int rx, int rs, int rz, int ry, int dx, int ds, int dz, int dy) {
     QPB_SMEM;
@@ -1314,7 +1114,7 @@ __device__ __forceinline__ void dm_stage(const BoxDims& D, int j0, const double*
     __syncthreads();
 }
 
-// k_box_forward_cl with M distributed (outputs as there)
+// k_box_forward<Cluster> with M distributed (outputs as there)
 __global__ void __launch_bounds__(kBoxNT, 1)
 k_box_forward_dm(DmDims Y, const double* __restrict__ q, int64_t sq, const double* __restrict__ p, int64_t sp,
                  const double* __restrict__ A, int64_t sA, const double* __restrict__ b, int64_t sb,
@@ -1477,7 +1277,7 @@ k_box_forward_dm(DmDims Y, const double* __restrict__ q, int64_t sq, const doubl
     cg::this_cluster().sync();       // no CTA exits while another may still read its shared memory
 }
 
-// k_box_backward_cl with M distributed
+// k_box_backward<Cluster> with M distributed
 __global__ void __launch_bounds__(kBoxNT, 1)
 k_box_backward_dm(DmDims Y, const double* __restrict__ q, int64_t sq, const double* __restrict__ A, int64_t sA,
                   const double* __restrict__ dl, const double* __restrict__ zhat, const double* __restrict__ lam,
@@ -1527,7 +1327,7 @@ k_box_backward_dm(DmDims Y, const double* __restrict__ q, int64_t sq, const doub
     cg::this_cluster().sync();
 }
 
-// k_box_kkt_cl with M distributed
+// k_box_kkt<Cluster> with M distributed
 __global__ void __launch_bounds__(kBoxNT, 1)
 k_box_kkt_dm(DmDims Y, const double* __restrict__ q, int64_t sq, const double* __restrict__ A, int64_t sA,
              const double* __restrict__ d, const double* __restrict__ rx, const double* __restrict__ rs,
@@ -1564,17 +1364,47 @@ k_box_kkt_dm(DmDims Y, const double* __restrict__ q, int64_t sq, const double* _
     cg::this_cluster().sync();
 }
 
+// batch means of the gradients of un-batched inputs (qp.py:159-177)
+// out[c] = scale / B * sum_b u[b * su + c] (* x[b * len + c] when x != null)
+__global__ void k_box_mean_vec(int B, int len, const double* __restrict__ u, int64_t su, const double* __restrict__ x,
+                               double scale, double* __restrict__ out) {
+    const int c = blockIdx.x * blockDim.x + threadIdx.x;
+    if (c >= len) return;
+    double s0 = 0.0, s1 = 0.0;
+    int bb = 0;
+    for (; bb + 1 < B; bb += 2) {
+        s0 += x ? u[(int64_t)bb * su + c] * x[(int64_t)bb * len + c] : u[(int64_t)bb * su + c];
+        s1 += x ? u[(int64_t)(bb + 1) * su + c] * x[(int64_t)(bb + 1) * len + c] : u[(int64_t)(bb + 1) * su + c];
+    }
+    if (bb < B) s0 += x ? u[(int64_t)bb * su + c] * x[(int64_t)bb * len + c] : u[(int64_t)bb * su + c];
+    out[c] = (s0 + s1) * scale / (double)B;
+}
+// dA mean: out[r][c] = 1/B sum_b (dnu[b][r] z[b][c] + nu[b][r] dx[b][c]); one thread per entry, a block per 128 columns
+__global__ void k_box_mean_outer(int B, int rows, int cols, const double* __restrict__ dnu, const double* __restrict__ z,
+                                 const double* __restrict__ nu, const double* __restrict__ dx, double* __restrict__ out) {
+    const int c = blockIdx.x * blockDim.x + threadIdx.x, r = blockIdx.y;
+    if (c >= cols) return;
+    double s = 0.0;
+    for (int bb = 0; bb < B; ++bb)
+        s = fma(dnu[(int64_t)bb * rows + r], z[(int64_t)bb * cols + c], fma(nu[(int64_t)bb * rows + r], dx[(int64_t)bb * cols + c], s));
+    out[(int64_t)r * cols + c] = s / (double)B;
+}
+
 std::mutex g_mu;
+// cudaFuncAttributeMaxDynamicSharedMemorySize already set, per (kernel, device): its high-water mark
+std::map<std::pair<const void*, int>, size_t> g_smem;
+
 template <typename K>
-int box_set_smem(K kernel, size_t bytes, size_t* cur) {      // cur: per-kernel high-water mark (device 0..15)
+int box_set_smem(K kernel, size_t bytes) {
     int dev = 0;
     cudaError_t err = cudaGetDevice(&dev);
     if (err != cudaSuccess) { qpb200_internal_cuda_error((int)err, "cudaGetDevice"); return QPB200_ERR_CUDA; }
     std::lock_guard<std::mutex> lock(g_mu);
-    if (dev < 16 && cur[dev] >= bytes) return QPB200_OK;
+    size_t& cur = g_smem[{(const void*)kernel, dev}];
+    if (cur >= bytes) return QPB200_OK;
     err = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
     if (err != cudaSuccess) { qpb200_internal_cuda_error((int)err, "cudaFuncSetAttribute"); return QPB200_ERR_CUDA; }
-    if (dev < 16) cur[dev] = bytes;
+    cur = bytes;
     return QPB200_OK;
 }
 int box_check_launch(const char* what) {
@@ -1582,9 +1412,6 @@ int box_check_launch(const char* what) {
     if (err != cudaSuccess) { qpb200_internal_cuda_error((int)err, what); return QPB200_ERR_CUDA; }
     return QPB200_OK;
 }
-size_t g_fwd[16], g_bwd[16], g_kkt[16];
-size_t g_cfwd[16], g_cbwd[16], g_ckkt[16];
-size_t g_dfwd[16], g_dbwd[16], g_dkkt[16];
 
 int box_plan_check(const qpb200_box_plan* P) {
     if (P == nullptr) return QPB200_ERR_BAD_ARG;
@@ -1592,9 +1419,6 @@ int box_plan_check(const qpb200_box_plan* P) {
     if (!P->ok && !P->cl_ctas) return QPB200_ERR_TOO_LARGE;
     return QPB200_OK;
 }
-BoxDims plan_dims(const qpb200_box_plan* P) { return box_dims(P->nz, P->neq, P->has_lb, P->has_ub); }
-ClDims plan_cl_dims(const qpb200_box_plan* P) { return cl_dims(P->nz, P->neq, P->has_lb, P->has_ub, P->cl_ctas); }
-DmDims plan_dm_dims(const qpb200_box_plan* P) { return dm_dims(P->nz, P->neq, P->has_lb, P->has_ub, P->cl_ctas); }
 
 // Whether a cluster of C CTAs with `bytes` of shared memory each can be resident at all (cudaOccupancyMaxActiveClusters
 // > 0), checked once per (kernel, C, bytes, device): QPB200_ERR_TOO_LARGE if not.
@@ -1610,8 +1434,8 @@ struct ClKey {
 std::map<ClKey, bool> g_cl_ok;
 
 template <typename K>
-int cl_prepare(K kernel, int C, size_t bytes, size_t* cur) {
-    int rc = box_set_smem(kernel, bytes, cur);
+int cl_prepare(K kernel, int C, size_t bytes) {
+    int rc = box_set_smem(kernel, bytes);
     if (rc) return rc;
     int dev = 0;
     cudaError_t err = cudaGetDevice(&dev);
@@ -1651,6 +1475,30 @@ int cl_launch(const char* what, void (*kernel)(KArgs...), int C, int nbatch, siz
     return box_check_launch(what);
 }
 
+// Launches the kernel for the layout the plan selects: k1 (k_box_*<OneCta>) with one CTA per QP, or a cluster per QP
+// (cl_ctas): kc (k_box_*<Cluster>), or kd (k_box_*_dm) with M distributed past neq_pad = 128.
+template <class K1, class KC, class KD, class... Args>
+int box_launch(const char* what, const qpb200_box_plan* plan, int nbatch, void* stream, K1 k1, KC kc, KD kd,
+               Args... args) {
+    cudaStream_t st = (cudaStream_t)stream;
+    auto run = [&](auto kernel, const auto& P) {
+        const size_t bytes = (size_t)P.total * 8;
+        if (!plan->cl_ctas) {
+            const int rc = box_set_smem(kernel, bytes);
+            if (rc) return rc;
+            kernel<<<nbatch, kBoxNT, bytes, st>>>(P, args...);
+            return box_check_launch(what);
+        }
+        const int rc = cl_prepare(kernel, plan->cl_ctas, bytes);
+        if (rc) return rc;
+        return cl_launch(what, kernel, plan->cl_ctas, nbatch, bytes, st, P, args...);
+    };
+    const int n = plan->nz, e = plan->neq, lb = plan->has_lb, ub = plan->has_ub, C = plan->cl_ctas;
+    if (!C) return run(k1, box_dims(n, e, lb, ub));
+    if (plan->neq_pad > kBoxNT) return run(kd, dm_dims(n, e, lb, ub, C));
+    return run(kc, cl_dims(n, e, lb, ub, C));
+}
+
 }  // namespace
 
 extern "C" {
@@ -1668,50 +1516,33 @@ int qpb200_box_plan_init(int nz, int neq, int has_lb, int has_ub, qpb200_box_pla
     const BoxDims D = box_dims(nz, neq, plan->has_lb, plan->has_ub);
     plan->smem_bytes = (int64_t)D.total * 8;
     plan->ok = (plan->neq_pad <= kBoxNT && plan->smem_bytes <= kBoxMaxSmem) ? 1 : 0;
-    // the cluster kernels: the smallest cluster whose slice fits, for shapes one CTA does not hold.
-    // QPB200_BOX_CLUSTER=C (development knob, C in {2, 4, 8}) forces them where that C fits.
-    if (plan->neq_pad <= kBoxNT) {
-        auto fits = [&](int C) {
-            return (int64_t)cl_dims(nz, neq, plan->has_lb, plan->has_ub, C).total * 8 <= kBoxMaxSmem;
-        };
-        const char* env = getenv("QPB200_BOX_CLUSTER");
-        const int forced = env ? atoi(env) : 0;
-        int C = 0;
-        if ((forced == 2 || forced == 4 || forced == 8) && fits(forced)) C = forced;
-        else if (!plan->ok)
-            for (int c = 2; c <= 8 && !C; c *= 2)
-                if (fits(c)) C = c;
-        if (C) {
-            const ClDims X = cl_dims(nz, neq, plan->has_lb, plan->has_ub, C);
-            plan->cl_ctas = C;
-            plan->cl_slice = X.slice;
-            plan->cl_smem_bytes = (int64_t)X.total * 8;
-        }
-    } else {
-        // the distributed-M kernels (neq_pad > 128): the smallest cluster that holds its share of M, where the dense
-        // path rejects the shape or its order is past kDmDenseOrder (below it the dense kernels are faster).
-        // QPB200_BOX_CLUSTER=C forces them where that C fits.
-        auto fits = [&](int C) {
-            return (int64_t)dm_dims(nz, neq, plan->has_lb, plan->has_ub, C).total * 8 <= kBoxMaxSmem;
-        };
-        const char* env = getenv("QPB200_BOX_CLUSTER");
-        const int forced = env ? atoi(env) : 0;
-        int C = 0;
-        if ((forced == 2 || forced == 4 || forced == 8) && fits(forced)) {
-            C = forced;
-        } else {
-            qpb200_plan dp;
-            const int rc = qpb200_plan_init(nz, plan->nineq, neq, &dp);
-            if (rc == QPB200_ERR_TOO_LARGE || (rc == QPB200_OK && dp.ms_pad > kDmDenseOrder))
-                for (int c = 2; c <= 8 && !C; c *= 2)
-                    if (fits(c)) C = c;
-        }
-        if (C) {
-            const DmDims Y = dm_dims(nz, neq, plan->has_lb, plan->has_ub, C);
-            plan->cl_ctas = C;
-            plan->cl_slice = Y.X.slice;
-            plan->cl_smem_bytes = (int64_t)Y.total * 8;
-        }
+    // A cluster of C CTAs, the smallest whose slice fits: the cluster kernels for shapes one CTA does not hold; past
+    // neq_pad = 128 the distributed-M kernels, where the dense path rejects the shape or its order is past
+    // kDmDenseOrder (below it the dense kernels are faster). QPB200_BOX_CLUSTER=C (development knob, C in {2, 4, 8})
+    // forces them where that C fits.
+    const bool distm = plan->neq_pad > kBoxNT;
+    auto cl_for = [&](int C) -> ClDims {
+        return distm ? dm_dims(nz, neq, plan->has_lb, plan->has_ub, C).X : cl_dims(nz, neq, plan->has_lb, plan->has_ub, C);
+    };
+    auto fits = [&](int C) { return (int64_t)cl_for(C).total * 8 <= kBoxMaxSmem; };
+    auto wanted = [&]() {
+        if (!distm) return !plan->ok;
+        qpb200_plan dp;
+        const int rc = qpb200_plan_init(nz, plan->nineq, neq, &dp);
+        return rc == QPB200_ERR_TOO_LARGE || (rc == QPB200_OK && dp.ms_pad > kDmDenseOrder);
+    };
+    const char* env = getenv("QPB200_BOX_CLUSTER");
+    const int forced = env ? atoi(env) : 0;
+    int C = 0;
+    if ((forced == 2 || forced == 4 || forced == 8) && fits(forced)) C = forced;
+    else if (wanted())
+        for (int c = 2; c <= 8 && !C; c *= 2)
+            if (fits(c)) C = c;
+    if (C) {
+        const ClDims X = cl_for(C);
+        plan->cl_ctas = C;
+        plan->cl_slice = X.slice;
+        plan->cl_smem_bytes = (int64_t)X.total * 8;
     }
     if (!plan->ok && !plan->cl_ctas) {          // only the dense kernels on the dense equivalent are left
         qpb200_plan dp;
@@ -1730,31 +1561,9 @@ int qpb200_box_forward(const qpb200_box_plan* plan, int nbatch, const double* q,
     if (rc) return rc;
     if (nbatch <= 0 || maxIter < 1 || !q || !p || !zhat || !lam || !slacks || !iters || !best_resid) return QPB200_ERR_BAD_ARG;
     if ((plan->has_lb && !lb) || (plan->has_ub && !ub) || (plan->neq > 0 && (!A || !b || !nus))) return QPB200_ERR_BAD_ARG;
-    if (plan->cl_ctas && plan->neq_pad > kBoxNT) {
-        const DmDims Y = plan_dm_dims(plan);
-        const size_t bytes = (size_t)Y.total * 8;
-        rc = cl_prepare(k_box_forward_dm, Y.X.C, bytes, g_dfwd);
-        if (rc) return rc;
-        return cl_launch("k_box_forward_dm", k_box_forward_dm, Y.X.C, nbatch, bytes, (cudaStream_t)stream, Y, q, sq, p,
-                         sp, A, sA, b, sb, lb, slb, ub, sub, eps, stall_tol, best_tie, notImprovedLim, maxIter, zhat,
-                         lam, slacks, nus, iters, best_resid, trace, spd_flag);
-    }
-    if (plan->cl_ctas) {
-        const ClDims X = plan_cl_dims(plan);
-        const size_t bytes = (size_t)X.total * 8;
-        rc = cl_prepare(k_box_forward_cl, X.C, bytes, g_cfwd);
-        if (rc) return rc;
-        return cl_launch("k_box_forward_cl", k_box_forward_cl, X.C, nbatch, bytes, (cudaStream_t)stream, X, q, sq, p,
-                         sp, A, sA, b, sb, lb, slb, ub, sub, eps, stall_tol, best_tie, notImprovedLim, maxIter, zhat,
-                         lam, slacks, nus, iters, best_resid, trace, spd_flag);
-    }
-    const BoxDims D = plan_dims(plan);
-    rc = box_set_smem(k_box_forward, (size_t)plan->smem_bytes, g_fwd);
-    if (rc) return rc;
-    k_box_forward<<<nbatch, kBoxNT, (size_t)plan->smem_bytes, (cudaStream_t)stream>>>(
-        D, q, sq, p, sp, A, sA, b, sb, lb, slb, ub, sub, eps, stall_tol, best_tie, notImprovedLim, maxIter, zhat, lam,
-        slacks, nus, iters, best_resid, trace, spd_flag);
-    return box_check_launch("k_box_forward");
+    return box_launch("k_box_forward", plan, nbatch, stream, k_box_forward<OneCta>, k_box_forward<Cluster>,
+                      k_box_forward_dm, q, sq, p, sp, A, sA, b, sb, lb, slb, ub, sub, eps, stall_tol, best_tie,
+                      notImprovedLim, maxIter, zhat, lam, slacks, nus, iters, best_resid, trace, spd_flag);
 }
 
 int qpb200_box_backward(const qpb200_box_plan* plan, int nbatch, const double* q, int64_t sq, const double* A,
@@ -1767,40 +1576,20 @@ int qpb200_box_backward(const qpb200_box_plan* plan, int nbatch, const double* q
     if (nbatch <= 0 || !q || !dl_dzhat || !zhat || !lam || !slacks || !dxv || !dlamv) return QPB200_ERR_BAD_ARG;
     if (plan->neq > 0 && (!A || !nus || !dnuv)) return QPB200_ERR_BAD_ARG;
     if ((dlb && !plan->has_lb) || (dub && !plan->has_ub)) return QPB200_ERR_BAD_ARG;
-    const BoxDims D = plan_dims(plan);
-    const int n = D.n, m = D.m, e = D.e;
+    const int n = plan->nz, m = plan->nineq, e = plan->neq, nlb = plan->has_lb ? n : 0;
     BoxGrads O;
     O.dq = dq; O.dp = dp; O.dlb = dlb; O.dub = dub; O.dA = e > 0 ? dA : nullptr; O.db = e > 0 ? db : nullptr;
     O.mq = mean_q; O.mp = mean_p; O.mlb = mean_lb; O.mub = mean_ub; O.mA = mean_A; O.mb = mean_b;
-    cudaStream_t st = (cudaStream_t)stream;
-    if (plan->cl_ctas && plan->neq_pad > kBoxNT) {
-        const DmDims Y = plan_dm_dims(plan);
-        const size_t bytes = (size_t)Y.total * 8;
-        rc = cl_prepare(k_box_backward_dm, Y.X.C, bytes, g_dbwd);
-        if (rc) return rc;
-        rc = cl_launch("k_box_backward_dm", k_box_backward_dm, Y.X.C, nbatch, bytes, st, Y, q, sq, A, sA, dl_dzhat, zhat,
-                       lam, slacks, nus, O, dxv, dlamv, dnuv);
-    } else if (plan->cl_ctas) {
-        const ClDims X = plan_cl_dims(plan);
-        const size_t bytes = (size_t)X.total * 8;
-        rc = cl_prepare(k_box_backward_cl, X.C, bytes, g_cbwd);
-        if (rc) return rc;
-        rc = cl_launch("k_box_backward_cl", k_box_backward_cl, X.C, nbatch, bytes, st, X, q, sq, A, sA, dl_dzhat, zhat,
-                       lam, slacks, nus, O, dxv, dlamv, dnuv);
-    } else {
-        rc = box_set_smem(k_box_backward, (size_t)plan->smem_bytes, g_bwd);
-        if (rc) return rc;
-        k_box_backward<<<nbatch, kBoxNT, (size_t)plan->smem_bytes, st>>>(D, q, sq, A, sA, dl_dzhat, zhat, lam, slacks,
-                                                                         nus, O, dxv, dlamv, dnuv);
-        rc = box_check_launch("k_box_backward");
-    }
+    rc = box_launch("k_box_backward", plan, nbatch, stream, k_box_backward<OneCta>, k_box_backward<Cluster>,
+                    k_box_backward_dm, q, sq, A, sA, dl_dzhat, zhat, lam, slacks, nus, O, dxv, dlamv, dnuv);
     if (rc) return rc;
+    cudaStream_t st = (cudaStream_t)stream;
     const int TB = 128;
     if (dq && mean_q) k_box_mean_vec<<<(n + TB - 1) / TB, TB, 0, st>>>(nbatch, n, dxv, n, zhat, 1.0, dq);
     if (dp && mean_p) k_box_mean_vec<<<(n + TB - 1) / TB, TB, 0, st>>>(nbatch, n, dxv, n, nullptr, 1.0, dp);
     if (dlb && mean_lb) k_box_mean_vec<<<(n + TB - 1) / TB, TB, 0, st>>>(nbatch, n, dlamv, m, nullptr, 1.0, dlb);
     if (dub && mean_ub)
-        k_box_mean_vec<<<(n + TB - 1) / TB, TB, 0, st>>>(nbatch, n, dlamv + D.nlb, m, nullptr, -1.0, dub);
+        k_box_mean_vec<<<(n + TB - 1) / TB, TB, 0, st>>>(nbatch, n, dlamv + nlb, m, nullptr, -1.0, dub);
     if (e > 0) {
         if (dA && mean_A) k_box_mean_outer<<<dim3((n + TB - 1) / TB, e), TB, 0, st>>>(nbatch, e, n, dnuv, zhat, nus, dxv, dA);
         if (db && mean_b) k_box_mean_vec<<<(e + TB - 1) / TB, TB, 0, st>>>(nbatch, e, dnuv, e, nullptr, -1.0, db);
@@ -1815,28 +1604,8 @@ int qpb200_box_solve_kkt(const qpb200_box_plan* plan, int nbatch, const double* 
     if (rc) return rc;
     if (nbatch <= 0 || !q || !d || !rx || !rs || !rz || !dx || !ds || !dz) return QPB200_ERR_BAD_ARG;
     if (plan->neq > 0 && (!A || !ry || !dy)) return QPB200_ERR_BAD_ARG;
-    if (plan->cl_ctas && plan->neq_pad > kBoxNT) {
-        const DmDims Y = plan_dm_dims(plan);
-        const size_t bytes = (size_t)Y.total * 8;
-        rc = cl_prepare(k_box_kkt_dm, Y.X.C, bytes, g_dkkt);
-        if (rc) return rc;
-        return cl_launch("k_box_kkt_dm", k_box_kkt_dm, Y.X.C, nbatch, bytes, (cudaStream_t)stream, Y, q, sq, A, sA, d, rx,
-                         rs, rz, ry, dx, ds, dz, dy);
-    }
-    if (plan->cl_ctas) {
-        const ClDims X = plan_cl_dims(plan);
-        const size_t bytes = (size_t)X.total * 8;
-        rc = cl_prepare(k_box_kkt_cl, X.C, bytes, g_ckkt);
-        if (rc) return rc;
-        return cl_launch("k_box_kkt_cl", k_box_kkt_cl, X.C, nbatch, bytes, (cudaStream_t)stream, X, q, sq, A, sA, d, rx,
-                         rs, rz, ry, dx, ds, dz, dy);
-    }
-    const BoxDims D = plan_dims(plan);
-    rc = box_set_smem(k_box_kkt, (size_t)plan->smem_bytes, g_kkt);
-    if (rc) return rc;
-    k_box_kkt<<<nbatch, kBoxNT, (size_t)plan->smem_bytes, (cudaStream_t)stream>>>(D, q, sq, A, sA, d, rx, rs, rz, ry,
-                                                                                   dx, ds, dz, dy);
-    return box_check_launch("k_box_kkt");
+    return box_launch("k_box_kkt", plan, nbatch, stream, k_box_kkt<OneCta>, k_box_kkt<Cluster>, k_box_kkt_dm, q, sq,
+                      A, sA, d, rx, rs, rz, ry, dx, ds, dz, dy);
 }
 
 }  // extern "C"
