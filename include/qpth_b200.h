@@ -166,6 +166,40 @@ int qpb200_solve_kkt_reg(const qpb200_plan* plan, int nbatch,
                          double* dx, double* ds, double* dz, double* dy,
                          double* scratch, void* stream);
 
+/* Regularised QP solve (QPFunction kkt_solver=IR_UNOPT): QPs whose Q is only positive SEMIdefinite (LPs, low-rank
+ * quadratic terms) or whose equality rows are linearly dependent. The Newton loop and its exits, outputs and trace are
+ * those of qpb200_forward / qpb200_backward, but every KKT solve (initial point, each iteration's direction, the backward
+ * solve) uses the regularised system of the pair above, [Q+eI 0 G' A'; 0 D+eI I 0; G I -eI 0; A 0 0 -eI], followed by
+ * ir_steps refinement steps against the un-regularised one (0 <= ir_steps <= 8), and the residuals, best_resid and the
+ * trace are those of the TRUE problem (||Qx + p + G'z + A'y||, not Q + eps I). The loop is thus an inexact Newton method
+ * whose fixed point is the exact KKT point. In the forward pass the refinement is applied to each iteration's combined
+ * direction (the same correction as refining the affine and corrector directions one by one: it is linear); sigma uses
+ * the unrefined affine direction.
+ * The plan comes from qpb200_plan_init_reg: the product-form kernels with 256 threads and one QP per SM (W and chol(Q)
+ * in shared memory, or read from L2 when pf_global), on every shape they take, tiny ones included; it returns
+ * QPB200_ERR_TOO_LARGE for ms_pad > 256 or nineq == 0. The factors come from qpb200_pre_factor_kkt_reg with that plan
+ * and the same reg_eps; spd_flag is then 1 where a pivot of chol(Q + eps I) failed, i.e. Q has an eigenvalue below
+ * -eps. With rank-deficient A the duals nus and the gradients dA, db are not unique. scratch is unused (may be NULL). */
+int qpb200_plan_init_reg(int nz, int nineq, int neq, qpb200_plan* plan);
+int qpb200_forward_reg(const qpb200_plan* plan, int nbatch,
+                       const double* p, int64_t sp, const double* h, int64_t sh,
+                       const double* b, int64_t sb,
+                       const double* Lfac, const double* Wfac, const double* Kfac, int sF,
+                       double eps, double stall_tol, double best_tie, int notImprovedLim, int maxIter,
+                       double reg_eps, int ir_steps,
+                       double* zhat, double* lam, double* slacks, double* nus,
+                       int* iters, double* best_resid, double* trace, double* scratch, void* stream);
+int qpb200_backward_reg(const qpb200_plan* plan, int nbatch,
+                        const double* dl_dzhat,
+                        const double* zhat, const double* lam, const double* slacks, const double* nus,
+                        const double* Lfac, const double* Wfac, const double* Kfac, int sF,
+                        double reg_eps, int ir_steps,
+                        double* dQ, int mean_Q, double* dp, int mean_p,
+                        double* dG, int mean_G, double* dh, int mean_h,
+                        double* dA, int mean_A, double* db, int mean_b,
+                        double* dxv, double* dlamv, double* dnuv,
+                        double* scratch, void* stream);
+
 /* ---- Box QPs (qpth_b200/box.py BoxQPFunction): min 1/2 z' diag(q) z + p'z  s.t.  A z = b,  lb <= z <= ub -------------
  * The dense equivalent is Q = diag(q), G = [-I; I] (only the sides given: lb rows first), h = [-lb; ub]; lam and slacks
  * are laid out as [lb rows; ub rows] (nineq = (has_lb + has_ub) * nz). The inequality block of the KKT system is

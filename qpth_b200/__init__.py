@@ -1,5 +1,5 @@
 """qpth_b200 — H100-native batched differentiable QP layer (drop-in for qpth.qp.QPFunction)."""
-from .qp import QPFunction, QPSolvers   # noqa: F401
+from .qp import KKTSolvers, QPFunction, QPSolvers   # noqa: F401
 from .solution import QPSolutionFunction, cvxpy_forward   # noqa: F401
 from .box import BoxQPFunction   # noqa: F401
 

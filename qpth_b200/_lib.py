@@ -59,6 +59,11 @@ SIGNATURES = {
     "qpb200_pre_factor_kkt_reg": (_I, [ctypes.POINTER(Plan), _I, _P, _L, _P, _L, _P, _L, _D, _P, _P, _P, _P, _P, _P]),
     "qpb200_solve_kkt_reg": (_I, [ctypes.POINTER(Plan), _I, _P, _P, _P, _P, _P, _D, _P, _P, _P, _I,
                                   _P, _P, _P, _P, _P, _P]),
+    "qpb200_plan_init_reg": (_I, [_I, _I, _I, ctypes.POINTER(Plan)]),
+    "qpb200_forward_reg": (_I, [ctypes.POINTER(Plan), _I, _P, _L, _P, _L, _P, _L, _P, _P, _P, _I,
+                                _D, _D, _D, _I, _I, _D, _I, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
+    "qpb200_backward_reg": (_I, [ctypes.POINTER(Plan), _I, _P, _P, _P, _P, _P, _P, _P, _P, _I, _D, _I,
+                                 _P, _I, _P, _I, _P, _I, _P, _I, _P, _I, _P, _I, _P, _P, _P, _P, _P]),
     "qpb200_optnet_construct": (_I, [_I, _I, _P, _P, _P, _P, _D, _P, _P, _P]),
     "qpb200_optnet_chain": (_I, [_I, _I, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     "qpb200_dfma_probe": (_I, [_I, _I, _I, _P, _P]),
@@ -132,6 +137,20 @@ def plan_for(nz, nineq, neq, two=None):
             p.pf_two = 1 if (two and p.pf2_ok and not p.pf_three) else 0
         _plans[key] = p
     return _plans[key]
+
+
+_reg_plans = {}
+
+
+def plan_for_reg(nz, nineq, neq):
+    """Plan of the regularised mode (qpb200_plan_init_reg; cached). Raises QpthB200Error for shapes it does not take
+    (ms_pad > 256)."""
+    key = (nz, nineq, neq, os.environ.get("QPB200_PF"), os.environ.get("QPB200_SETUP_PF"))
+    if key not in _reg_plans:
+        p = Plan()
+        check(load().qpb200_plan_init_reg(nz, nineq, neq, ctypes.byref(p)))
+        _reg_plans[key] = p
+    return _reg_plans[key]
 
 
 _box_plans = {}

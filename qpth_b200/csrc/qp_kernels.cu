@@ -995,7 +995,8 @@ const char* qpb200_error_string(int code) {
 
 const char* qpb200_last_cuda_error(void) { return g_cuda_err; }
 
-int qpb200_plan_init(int nz, int nineq, int neq, qpb200_plan* plan) {
+// allow_tiny = false: the plan of the regularised mode, whose kernels exist in the product-form family only
+static int plan_init_impl(int nz, int nineq, int neq, qpb200_plan* plan, bool allow_tiny) {
     if (plan == nullptr || nz <= 0 || nineq < 0 || neq < 0) return QPB200_ERR_BAD_ARG;
     if (nineq == 0 && neq == 0) return QPB200_ERR_NO_CONSTRAINTS;
     if (nz > 4096 || nineq > 4096 || neq > 4096) return QPB200_ERR_TOO_LARGE;
@@ -1030,7 +1031,7 @@ int qpb200_plan_init(int nz, int nineq, int neq, qpb200_plan* plan) {
     const bool setup_fast_ok = fast_ok && nz <= 8 * kCholMaxTiles && (int64_t)SL.total * 8 <= kMaxSmem;
     // tiny problems (the sizes of the reference's own tests and prof scripts, test.py:99-187 nz = 10): a 256-thread
     // CTA per QP is 8 warps synchronising over a handful of rows; one warp per QP and 16 QPs per SM instead
-    const bool tiny = fits && nz <= kTinyMax && msp <= kTinyMax;
+    const bool tiny = allow_tiny && fits && nz <= kTinyMax && msp <= kTinyMax;
     plan->tiny = tiny ? 1 : 0;
     plan->pf = 0; plan->pf_global = 0; plan->pf_smem_bytes = 0; plan->pf2_ok = 0; plan->pf2_smem_bytes = 0; plan->pf_two = 0; plan->pf3_ok = 0; plan->pf3_smem_bytes = 0; plan->pf_three = 0; plan->pf_threads = 256; plan->setup_pf = 0; plan->setup_pf_smem_bytes = 0;
     if (tiny) {
@@ -1117,6 +1118,21 @@ int qpb200_plan_init(int nz, int nineq, int neq, qpb200_plan* plan) {
             if (plan->setup_pf) plan->setup_scratch_elems = 0;
         }
     }
+    return QPB200_OK;
+}
+
+int qpb200_plan_init(int nz, int nineq, int neq, qpb200_plan* plan) {
+    return plan_init_impl(nz, nineq, neq, plan, true);
+}
+
+int qpb200_plan_init_reg(int nz, int nineq, int neq, qpb200_plan* plan) {
+    const int rc = plan_init_impl(nz, nineq, neq, plan, false);
+    if (rc != QPB200_OK) return rc;
+    if (!plan->pf) return QPB200_ERR_TOO_LARGE;            // order ms_pad > 256, or no inequality rows
+    if (plan->pf_threads == 512) plan->pf_smem_bytes -= 512;
+    plan->pf_threads = 256;                                // one QP per SM, 256 threads: the only regularised build
+    plan->pf2_ok = 0; plan->pf_two = 0; plan->pf2_smem_bytes = 0;
+    plan->pf3_ok = 0; plan->pf_three = 0; plan->pf3_smem_bytes = 0;
     return QPB200_OK;
 }
 
@@ -1336,6 +1352,10 @@ static int solve_kkt_impl(const qpb200_plan* plan, int nbatch, const double* d, 
     return QPB200_OK;
 }
 
+static int launch_means(int nbatch, int n, int m, int e, const double* zhat, const double* lam, const double* nus,
+                        double* dQ, int mean_Q, double* dp, int mean_p, double* dG, int mean_G, double* dh, int mean_h,
+                        double* dA, int mean_A, double* db, int mean_b, const double* dxv, const double* dlamv,
+                        const double* dnuv, cudaStream_t st);
 int qpb200_backward(const qpb200_plan* plan, int nbatch, const double* dl_dzhat, const double* zhat,
                     const double* lam, const double* slacks, const double* nus, const double* Lfac,
                     const double* Wfac, const double* Kfac, int sF, double* dQ, int mean_Q, double* dp,
@@ -1410,6 +1430,15 @@ int qpb200_backward(const qpb200_plan* plan, int nbatch, const double* dl_dzhat,
     }
 #undef QPB_LAUNCH_BWD
     CK(cudaGetLastError());
+    return launch_means(nbatch, n, m, e, zhat, lam, nus, dQ, mean_Q, dp, mean_p, dG, mean_G, dh, mean_h, dA, mean_A, db,
+                        mean_b, dxv, dlamv, dnuv, st);
+}
+
+// Batch-mean gradients of the un-batched inputs (qp.py:159-177) from the per-QP dx, dlam, dnu of a backward kernel.
+static int launch_means(int nbatch, int n, int m, int e, const double* zhat, const double* lam, const double* nus,
+                        double* dQ, int mean_Q, double* dp, int mean_p, double* dG, int mean_G, double* dh, int mean_h,
+                        double* dA, int mean_A, double* db, int mean_b, const double* dxv, const double* dlamv,
+                        const double* dnuv, cudaStream_t st) {
     const int TB = 256;
     if (dQ && mean_Q)
         k_mean_outer<<<dim3((n + kMoC - 1) / kMoC, (n + kMoR - 1) / kMoR), 256, 0, st>>>(nbatch, n, n, dxv, zhat, zhat, dxv, 0.5, dQ);
@@ -1424,6 +1453,79 @@ int qpb200_backward(const qpb200_plan* plan, int nbatch, const double* dl_dzhat,
     }
     CK(cudaGetLastError());
     return QPB200_OK;
+}
+
+// ---- regularised mode (QPFunction kkt_solver=IR_UNOPT): the product-form solve kernels with kReg --------------------
+static int check_reg_plan(const qpb200_plan* plan, double reg_eps, int ir_steps) {
+    if (!(reg_eps >= 0.0) || ir_steps < 0 || ir_steps > 8) return QPB200_ERR_BAD_ARG;
+    if (plan->tiny || !plan->pf || plan->pf_two || plan->pf_three || plan->pf_threads != 256) return QPB200_ERR_TOO_LARGE;
+    return QPB200_OK;
+}
+
+int qpb200_forward_reg(const qpb200_plan* plan, int nbatch, const double* p, int64_t sp, const double* h,
+                       int64_t sh, const double* b, int64_t sb, const double* Lfac, const double* Wfac,
+                       const double* Kfac, int sF, double eps, double stall_tol, double best_tie,
+                       int notImprovedLim, int maxIter, double reg_eps, int ir_steps, double* zhat, double* lam,
+                       double* slacks, double* nus, int* iters, double* best_resid, double* trace, double* scratch,
+                       void* stream) {
+    (void)scratch;
+    if (!plan || nbatch <= 0 || !p || !h || !Lfac || !Wfac || !Kfac || !zhat || !lam || !slacks || !iters || !best_resid)
+        return QPB200_ERR_BAD_ARG;
+    if (plan->neq > 0 && (!b || !nus)) return QPB200_ERR_BAD_ARG;
+    int rc = check_reg_plan(plan, reg_eps, ir_steps);
+    if (rc) return rc;
+    cudaStream_t st = (cudaStream_t)stream;
+    KDims D = dims_of(plan);
+    D.reg = reg_eps;
+    const size_t sb_ = (size_t)plan->pf_smem_bytes;
+#define QPB_LAUNCH_REG(KG)                                                                                   \
+    do {                                                                                                     \
+        rc = set_smem(k_forward_fast<KG, true, 0, true>, sb_);                                               \
+        if (rc) return rc;                                                                                   \
+        k_forward_fast<KG, true, 0, true><<<nbatch, qpb::fast::kNT, sb_, st>>>(                              \
+            D, p, sp, h, sh, b, sb, Lfac, Wfac, Kfac, sF, eps, stall_tol, best_tie, notImprovedLim, maxIter, \
+            zhat, lam, slacks, nus, iters, best_resid, trace, ir_steps);                                     \
+    } while (0)
+    if (plan->pf_global) QPB_LAUNCH_REG(true);
+    else QPB_LAUNCH_REG(false);
+#undef QPB_LAUNCH_REG
+    CK(cudaGetLastError());
+    return QPB200_OK;
+}
+
+int qpb200_backward_reg(const qpb200_plan* plan, int nbatch, const double* dl_dzhat, const double* zhat,
+                        const double* lam, const double* slacks, const double* nus, const double* Lfac,
+                        const double* Wfac, const double* Kfac, int sF, double reg_eps, int ir_steps, double* dQ,
+                        int mean_Q, double* dp, int mean_p, double* dG, int mean_G, double* dh, int mean_h, double* dA,
+                        int mean_A, double* db, int mean_b, double* dxv, double* dlamv, double* dnuv, double* scratch,
+                        void* stream) {
+    (void)scratch;
+    if (!plan || nbatch <= 0 || !dl_dzhat || !zhat || !lam || !slacks || !Lfac || !Wfac || !Kfac || !dxv || !dlamv)
+        return QPB200_ERR_BAD_ARG;
+    if (plan->neq > 0 && (!nus || !dnuv)) return QPB200_ERR_BAD_ARG;
+    int rc = check_reg_plan(plan, reg_eps, ir_steps);
+    if (rc) return rc;
+    cudaStream_t st = (cudaStream_t)stream;
+    KDims D = dims_of(plan);
+    D.reg = reg_eps;
+    BwdOut O;
+    O.dQ = dQ; O.dp = dp; O.dG = dG; O.dh = dh; O.dA = dA; O.db = db;
+    O.mQ = mean_Q; O.mp = mean_p; O.mG = mean_G; O.mh = mean_h; O.mA = mean_A; O.mb = mean_b;
+    const size_t sb_ = (size_t)plan->pf_smem_bytes;
+#define QPB_LAUNCH_REG(KG)                                                                                   \
+    do {                                                                                                     \
+        rc = set_smem(k_kkt_fast<true, KG, true, 0, true>, sb_);                                             \
+        if (rc) return rc;                                                                                   \
+        k_kkt_fast<true, KG, true, 0, true><<<nbatch, qpb::fast::kNT, sb_, st>>>(                            \
+            D, nullptr, dl_dzhat, nullptr, nullptr, nullptr, zhat, lam, slacks, nus, Lfac, Wfac, Kfac, sF, dxv, \
+            nullptr, dlamv, dnuv, O, ir_steps);                                                              \
+    } while (0)
+    if (plan->pf_global) QPB_LAUNCH_REG(true);
+    else QPB_LAUNCH_REG(false);
+#undef QPB_LAUNCH_REG
+    CK(cudaGetLastError());
+    return launch_means(nbatch, plan->nz, plan->nineq, plan->neq, zhat, lam, nus, dQ, mean_Q, dp, mean_p, dG, mean_G, dh,
+                        mean_h, dA, mean_A, db, mean_b, dxv, dlamv, dnuv, st);
 }
 
 #ifdef QPB_TIMING

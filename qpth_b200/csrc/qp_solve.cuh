@@ -213,12 +213,16 @@ __device__ __forceinline__ void f_factor_and_solve(const KDims& D, FCtx& C) {
 }
 
 // The same with the product-form factor (qp_pf.cuh): F_AUG = -h_full, F_D = d  ->  F_W = -S^-1 h_full; F_T0 scratch.
+// kReg: F_D holds d + eps and the inequality diagonal gets 1 / (d + eps) + eps (the regularised system; the eps of the
+// equality rows is already in K, pre_factor_kkt_reg).
+template <bool kReg = false>
 __device__ __forceinline__ void f_factor_and_solve_pf(const KDims& D, FCtx& C) {
     QPB_SMEM;
     using namespace qpb::pf;
     const int tid = threadIdx.x;
     f_wait_K(C);
-    _Pragma("unroll 1") for (int i = D.ep + tid; i < D.ms; i += kNT) qsm[C.L.LS + pf_rowoff(i) + i] += 1.0 / qsm[FV(F_D) + i];
+    _Pragma("unroll 1") for (int i = D.ep + tid; i < D.ms; i += kNT)
+        qsm[C.L.LS + pf_rowoff(i) + i] += kReg ? 1.0 / qsm[FV(F_D) + i] + D.reg : 1.0 / qsm[FV(F_D) + i];
     __syncthreads();
     if (D.ep > 0) pf_fwd(C.L.LS, D.msp, 0, D.ep >> 3, FV(F_AUG));
     pf_chol(C.L.LS, D.msp >> 3, D.ep >> 3, FV(F_AUG), C.L.pan, C.L.tab);
@@ -230,6 +234,63 @@ __device__ __forceinline__ void f_factor_and_solve_pf(const KDims& D, FCtx& C) {
 
 __device__ __forceinline__ double f_step_fix(double v) { return (isinf(v) && v > 0.0) ? 1.0 : v; }
 
+// ---- regularised mode (kReg: QPFunction with kkt_solver=IR_UNOPT) ---------------------------------------------------
+// The factors are those of pre_factor_kkt_reg: L = chol(Q + eps I), K with eps on the equality rows. Every KKT solve
+// uses the regularised system [Q+eI 0 G' A'; 0 D+eI I 0; G I -eI 0; A 0 0 -eI], while the residuals are those of the
+// true problem, so the Newton loop converges to the exact KKT point of a Q that is only positive semidefinite.
+
+// r~x -= eps L^-1 L^-T x~: the whitened dual residual of the true problem (L^-1 (Qx + p + G'z + A'y)) from the one of
+// Q + eps I that the W pass produces. t0, t1: scratch. Ends with a block barrier.
+__device__ __forceinline__ void f_true_rx(const KDims& D, const FCtx& C, int xt, int rxt, int t0, int t1) {
+    QPB_SMEM;
+    const int tid = threadIdx.x;
+    _Pragma("unroll 1") for (int i = tid; i < D.n; i += kNT) qsm[t1 + i] = qsm[xt + i];
+    __syncthreads();
+    f_unwhiten_x(D, C, t1, t0);                              // t0 = x = L^-T x~
+    f_whiten_x(D, C, t0, t1);                                // t1 = L^-1 x
+    _Pragma("unroll 1") for (int i = tid; i < D.n; i += kNT) qsm[rxt + i] = fma(-D.reg, qsm[t1 + i], qsm[rxt + i]);
+    __syncthreads();
+}
+
+// One refinement step, with the factor still in the S workspace, of a solution of the regularised system: dv = [dy; dz],
+// ds, and dx~ = -base + ntx - W^T dv kept implicit. Against the true system that solution leaves the residual
+// (-eps dx, -eps ds, eps dz, eps dy); the correction solves the regularised system with it and is added in place
+// (ntx += eps L^-1 dx). F_D holds d + eps. a, b, c, e, f: scratch slots. Ends with a block barrier.
+template <bool kCoop>
+__device__ __forceinline__ void f_refine(const KDims& D, const FCtx& C, int base, int ntx, int dv, int ds, int a, int b,
+                                         int c, int e, int f) {
+    QPB_SMEM;
+    const int tid = threadIdx.x, dd = FV(F_D);
+    mv_cols<kCoop>(D, C, dv, e, f, a, base, -1.0, ntx, -1.0);  // a = dx~
+    f_unwhiten_x(D, C, a, b);                                // b = dx
+    f_whiten_x(D, C, b, c);                                  // c = L^-1 dx
+    _Pragma("unroll 1") for (int i = tid; i < D.n; i += kNT) {
+        const double r = D.reg * qsm[c + i];
+        qsm[c + i] = -r;                                     // whitened x residual  L^-1 (-eps dx)
+        qsm[ntx + i] += r;
+    }
+    __syncthreads();
+    mv_rows1<kCoop>(D, C, c, e);
+    __syncthreads();
+    // reduced right-hand side -(W t - [r_y; r_z] + [0; r_s / (d + eps)])  (the elimination of solve_kkt)
+    _Pragma("unroll 1") for (int i = tid; i < D.msp; i += kNT) {
+        double hf = 0.0;
+        if (i < D.ms) {
+            hf = fma(-D.reg, qsm[dv + i], qsm[e + i]);
+            if (i >= D.ep) hf -= D.reg * qsm[ds + i] / qsm[dd + i];
+        }
+        qsm[a + i] = -hf;
+    }
+    __syncthreads();
+    qpb::pf::pf_solve(C.L.LS, D.msp, a, b, f);              // f = correction of [dy; dz]
+    _Pragma("unroll 1") for (int i = tid; i < D.ms; i += kNT) {
+        const double wi = qsm[f + i];
+        if (i >= D.ep) qsm[ds + i] += (D.reg * qsm[ds + i] - wi) / qsm[dd + i];
+        qsm[dv + i] += wi;
+    }
+    __syncthreads();
+}
+
 }  // namespace fk
 
 // kCoop: co-resident mode (two CTAs per SM; W and L read from global memory, see qp_fast.cuh).
@@ -238,7 +299,9 @@ __device__ __forceinline__ double f_step_fix(double v) { return (isinf(v) && v >
 // kMinCtas (with kCoop && kPF): the same kernel compiled for 2 (256 threads, 128 registers) or 3 (192 threads, 112
 // registers: qp_alt.cu) CTAs per SM: <= 76.8 KB of shared memory per QP at C2, so the QPs of an SM fill each other's
 // pivot-chain bubbles.
-template <bool kCoop, bool kPF = false, int kMinCtas = 0>
+// kReg (with kPF, kMinCtas = 0): the regularised mode (fk::f_true_rx, fk::f_refine); D.reg = eps, ir_steps refinement
+// steps of the initial point and of each iteration's combined direction (a trailing parameter: KDims keeps its layout).
+template <bool kCoop, bool kPF = false, int kMinCtas = 0, bool kReg = false>
 __global__ void __launch_bounds__(qpb::fast::kNT, kMinCtas ? kMinCtas : ((kCoop && !kPF) ? 2 : 1))
 k_forward_fast(KDims D, const double* __restrict__ p, int64_t sp, const double* __restrict__ h, int64_t sh,
                const double* __restrict__ b, int64_t sb, const double* __restrict__ Lfac,
@@ -246,7 +309,7 @@ k_forward_fast(KDims D, const double* __restrict__ p, int64_t sp, const double* 
                double stall_tol, double best_tie, int notImprovedLim, int maxIter,
                double* __restrict__ zhat, double* __restrict__ lam, double* __restrict__ slacks,
                double* __restrict__ nus, int* __restrict__ iters_out, double* __restrict__ resid_out,
-               double* __restrict__ trace) {
+               double* __restrict__ trace, int ir_steps = 0) {
     using namespace fk;
     QPB_SMEM;
     const int tid = threadIdx.x;
@@ -275,7 +338,7 @@ k_forward_fast(KDims D, const double* __restrict__ p, int64_t sp, const double* 
         if (i < e) val = bg[i];
         else if (i >= ep && i < ms) val = hg[i - ep];
         qsm[hb + i] = val;
-        qsm[d + i] = 1.0;
+        qsm[d + i] = kReg ? 1.0 + D.reg : 1.0;
         qsm[s + i] = 0.0;
         qsm[v + i] = 0.0;
         qsm[aug + i] = 0.0;
@@ -295,17 +358,26 @@ k_forward_fast(KDims D, const double* __restrict__ p, int64_t sp, const double* 
     __syncthreads();
     _Pragma("unroll 1") for (int i = tid; i < ms; i += kNT) qsm[aug + i] = -(qsm[hW + i] + qsm[hb + i]);
     __syncthreads();
-    if (kPF) f_factor_and_solve_pf(D, C); else f_factor_and_solve(D, C);
+    if (kPF) f_factor_and_solve_pf<kReg>(D, C); else f_factor_and_solve(D, C);
+    const bool refine = kReg && ir_steps > 0;
+    if (kReg) {
+        // s = -w / (1 + eps); rv accumulates the x part of the refinement (x~ = -p~ + rv - W^T w)
+        _Pragma("unroll 1") for (int i = ep + tid; i < ms; i += kNT) qsm[s + i] = -qsm[w + i] / qsm[d + i];
+        _Pragma("unroll 1") for (int i = tid; i < n; i += kNT) qsm[rv + i] = 0.0;
+        __syncthreads();
+        _Pragma("unroll 1") for (int k = 0; k < ir_steps; ++k) f_refine<kCoop>(D, C, pt, rv, w, s, t1, t0, aug, hW, dsa);
+    }
     f_issue_K(D, C);
-    mv_cols<kCoop>(D, C, w, t0, t1, xt, pt, -1.0, -1, -1.0);   // x~ = -p~ - W^T w
+    mv_cols<kCoop>(D, C, w, t0, t1, xt, pt, -1.0, refine ? rv : -1, -1.0);   // x~ = -p~ - W^T w
     {
         double mn[2] = {INFINITY, INFINITY};
         _Pragma("unroll 1") for (int i = tid; i < ms; i += kNT) {
             const double wi = qsm[w + i];
             qsm[v + i] = wi;
             if (i >= ep) {
-                qsm[s + i] = -wi;
-                mn[0] = fmin(mn[0], -wi);
+                const double si = kReg ? qsm[s + i] : -wi;
+                qsm[s + i] = si;
+                mn[0] = fmin(mn[0], si);
                 mn[1] = fmin(mn[1], wi);
             }
         }
@@ -326,6 +398,7 @@ k_forward_fast(KDims D, const double* __restrict__ p, int64_t sp, const double* 
         QPB_TICK(3);
         // r~x = x~ + p~ + W^T [y;z]: here at the initial point; later iterations get it from the previous one's mv_cols2
         if (it == 0) mv_cols<kCoop>(D, C, v, t0, t1, rxt, xt, 1.0, pt, 1.0);
+        if (kReg) f_true_rx(D, C, xt, rxt, t0, t1);
         QPB_TICK(4);
         double acc[4] = {0.0, 0.0, 0.0, 0.0};                   // |ry|^2, |rz|^2, |L r~x|^2, s.z
         mv_rows2<kCoop>(D, C, xt, rxt, rv, hW);                      // W x~ , W r~x
@@ -361,7 +434,7 @@ k_forward_fast(KDims D, const double* __restrict__ p, int64_t sp, const double* 
         _Pragma("unroll 1") for (int i = tid; i < ms; i += kNT) {
             double hfull = qsm[hW + i] - qsm[rv + i];
             if (i >= ep) {
-                const double di = qsm[v + i] / qsm[s + i];
+                const double di = kReg ? qsm[v + i] / qsm[s + i] + D.reg : qsm[v + i] / qsm[s + i];
                 qsm[d + i] = di;
                 hfull += qsm[v + i] / di;
             }
@@ -369,7 +442,7 @@ k_forward_fast(KDims D, const double* __restrict__ p, int64_t sp, const double* 
         }
         __syncthreads();
         QPB_TICK(9);
-        if (kPF) f_factor_and_solve_pf(D, C); else f_factor_and_solve(D, C);   // w = [dy_aff; dz_aff]
+        if (kPF) f_factor_and_solve_pf<kReg>(D, C); else f_factor_and_solve(D, C);   // w = [dy_aff; dz_aff]
         QPB_TICK(10);
         // ---- affine step length and sigma (batch.py:160-168)
         double mn[2] = {INFINITY, INFINITY};
@@ -415,7 +488,7 @@ k_forward_fast(KDims D, const double* __restrict__ p, int64_t sp, const double* 
             f_trsv_bwd(C.L.LS, D.lds, msp, t0, t1);              // t1 = [dy_cor; dz_cor]
         }
         QPB_TICK(13);
-        f_issue_K(D, C);                                         // next factor_kkt's K copy overlaps the rest
+        if (!refine) f_issue_K(D, C);                            // next factor_kkt's K copy overlaps the rest
         // ---- combined direction, step length, update (batch.py:185-203)
         mn[0] = INFINITY; mn[1] = INFINITY;
         _Pragma("unroll 1") for (int i = tid; i < ms; i += kNT) {
@@ -429,6 +502,20 @@ k_forward_fast(KDims D, const double* __restrict__ p, int64_t sp, const double* 
                 mn[0] = fmin(mn[0], step_candidate(qsm[v + i], dv));
                 mn[1] = fmin(mn[1], step_candidate(qsm[s + i], dsi));
             }
+        }
+        if (refine) {
+            // The refinement is linear in the right-hand side, so refining the combined direction equals refining the
+            // affine and the corrector direction one by one; sigma above comes from the unrefined affine direction.
+            _Pragma("unroll 1") for (int i = tid; i < n; i += kNT) qsm[rv + i] = 0.0;
+            __syncthreads();
+            _Pragma("unroll 1") for (int k = 0; k < ir_steps; ++k) f_refine<kCoop>(D, C, rxt, rv, w, ds, t1, t0, aug, hW, dsa);
+            f_issue_K(D, C);
+            mn[0] = INFINITY; mn[1] = INFINITY;
+            _Pragma("unroll 1") for (int i = ep + tid; i < ms; i += kNT) {
+                mn[0] = fmin(mn[0], step_candidate(qsm[v + i], qsm[w + i]));
+                mn[1] = fmin(mn[1], step_candidate(qsm[s + i], qsm[ds + i]));
+            }
+            _Pragma("unroll 1") for (int i = tid; i < n; i += kNT) qsm[rxt + i] -= qsm[rv + i];   // dx~ = -(r~x - rv) - W^T dv
         }
         QPB_TICK(14);
         // the step length does not depend on dx~: v and s move first, then one pass over W gives dx~, x~ and the next
@@ -472,7 +559,10 @@ k_forward_fast(KDims D, const double* __restrict__ p, int64_t sp, const double* 
 #endif
 }
 
-template <bool kBackward, bool kCoop, bool kPF = false, int kMinCtas = 0>
+// kReg (with kBackward, kPF, kMinCtas = 0): the backward pass of the regularised mode, d + eps and ir_steps refinement
+// steps (fk::f_refine). chol(Q) is then read from global memory in the W/L-from-global build: the refinement needs it
+// while the factor occupies the S workspace.
+template <bool kBackward, bool kCoop, bool kPF = false, int kMinCtas = 0, bool kReg = false>
 __global__ void __launch_bounds__(qpb::fast::kNT, kMinCtas ? kMinCtas : ((kCoop && !kPF) ? 2 : 1))
 k_kkt_fast(KDims D, const double* __restrict__ d_in, const double* __restrict__ rx_in,
            const double* __restrict__ rs_in, const double* __restrict__ rz_in,
@@ -481,13 +571,13 @@ k_kkt_fast(KDims D, const double* __restrict__ d_in, const double* __restrict__ 
            const double* __restrict__ nus, const double* __restrict__ Lfac,
            const double* __restrict__ Wfac, const double* __restrict__ Kfac, int sF,
            double* __restrict__ dx_out, double* __restrict__ ds_out, double* __restrict__ dz_out,
-           double* __restrict__ dy_out, BwdOut O) {
+           double* __restrict__ dy_out, BwdOut O, int ir_steps = 0) {
     using namespace fk;
     QPB_SMEM;
     const int tid = threadIdx.x;
     const int qp = blockIdx.x;
     const int n = D.n, m = D.m, e = D.e, ep = D.ep, ms = D.ms, msp = D.msp;
-    FCtx C = f_make_ctx<kCoop, kPF, true>(D, qp, Lfac, Wfac, Kfac, sF);
+    FCtx C = f_make_ctx<kCoop, kPF, !kReg>(D, qp, Lfac, Wfac, Kfac, sF);
     const int t = FV(F_PT), d = FV(F_D), hW = FV(F_HW), aug = FV(F_AUG), w = FV(F_W), t0 = FV(F_T0),
               t1 = FV(F_T1), rsv = FV(F_S), c2 = FV(F_RV), dxt = FV(F_RXT), dxo = FV(F_XT);
     _Pragma("unroll 1") for (int i = tid; i < n; i += kNT) qsm[t1 + i] = rx_in[(int64_t)qp * n + i];
@@ -497,6 +587,7 @@ k_kkt_fast(KDims D, const double* __restrict__ d_in, const double* __restrict__ 
             const int j = i - ep;
             if (kBackward) {
                 di = fmax(lam[(int64_t)qp * m + j], 1e-8) / fmax(slacks[(int64_t)qp * m + j], 1e-8);   // qp.py:148
+                if (kReg) di += D.reg;
             } else {
                 // regularised variant (D.reg > 0, batch.py:244-310): d~ = d + eps in the complementarity row, and the slot
                 // holds 1 / (1/d~ + eps) because factor_kkt adds the RECIPROCAL of this slot to the diagonal of S
@@ -513,6 +604,9 @@ k_kkt_fast(KDims D, const double* __restrict__ d_in, const double* __restrict__ 
         qsm[hW + i] = extra;
         qsm[aug + i] = 0.0;
     }
+    if (kReg) {                                                  // x part of the refinement (dx~ = -t + it - W^T w)
+        _Pragma("unroll 1") for (int i = tid; i < n; i += kNT) qsm[FV(F_DSA) + i] = 0.0;
+    }
     __syncthreads();
     f_whiten_x(D, C, t1, t);                               // t = L^-1 rx
     if (kCoop && !C.lglobal) {
@@ -523,8 +617,14 @@ k_kkt_fast(KDims D, const double* __restrict__ d_in, const double* __restrict__ 
     __syncthreads();
     _Pragma("unroll 1") for (int i = tid; i < ms; i += kNT) qsm[aug + i] = -(qsm[c2 + i] + qsm[hW + i]);
     __syncthreads();
-    if (kPF) f_factor_and_solve_pf(D, C); else f_factor_and_solve(D, C);   // w = [dy; dz]
-    mv_cols<kCoop>(D, C, w, t0, t1, dxt, t, -1.0, -1, -1.0);
+    if (kPF) f_factor_and_solve_pf<kReg>(D, C); else f_factor_and_solve(D, C);   // w = [dy; dz]
+    const int ntx = FV(F_DSA), dsr = FV(F_DS);
+    if (kReg) {
+        _Pragma("unroll 1") for (int i = ep + tid; i < ms; i += kNT) qsm[dsr + i] = -qsm[w + i] / qsm[d + i];   // ds (rs = 0)
+        __syncthreads();
+        _Pragma("unroll 1") for (int k = 0; k < ir_steps; ++k) f_refine<kCoop>(D, C, t, ntx, w, dsr, aug, t0, t1, hW, c2);
+    }
+    mv_cols<kCoop>(D, C, w, t0, t1, dxt, t, -1.0, kReg ? ntx : -1, -1.0);
     if (kCoop && !C.lglobal) f_stage_L(D, C);                   // (mv_cols ended with a block barrier; no K copy in flight)
     f_unwhiten_x(D, C, dxt, dxo);                          // dx = L^-T dx~
     _Pragma("unroll 1") for (int i = tid; i < n; i += kNT) dx_out[(int64_t)qp * n + i] = qsm[dxo + i];

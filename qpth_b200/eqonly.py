@@ -16,6 +16,21 @@ from . import _lib, kkt
 from .util import bger, check_shapes, expandParam
 
 _factor = kkt._Factored          # (tests inject a CPU stand-in here)
+# Refinement steps of each solve in the regularised mode (kkt_solver=IR_UNOPT): with no Newton loop around it, the one
+# regularised solve is off by O(IR_EPS), and each step against the true system takes a factor of about IR_EPS off that.
+EQ_IR_STEPS = 2
+
+
+def _solve(F, Q, A, d, rx, rs, rz, ry, steps):
+    """F.solve, then `steps` refinement steps against the true system [Q 0 0 A'; 0 d 1 0; 0 1 0 0; A 0 0 0] (the dummy
+    inequality row has G = 0): K~ dd = -(K [dx ds dz dy] + r), one factorization for all of them."""
+    dx, ds, dz, dy = F.solve(d, rx, rs, rz, ry)
+    for _ in range(steps):
+        resx = torch.bmm(Q, dx.unsqueeze(2)).squeeze(2) + torch.bmm(A.transpose(1, 2), dy.unsqueeze(2)).squeeze(2) + rx
+        resy = torch.bmm(A, dx.unsqueeze(2)).squeeze(2) + ry
+        ex, es, ez, ey = F.solve(d, resx, d * ds + dz + rs, ds + rz, resy)
+        dx, ds, dz, dy = dx + ex, ds + es, dz + ez, dy + ey
+    return dx, ds, dz, dy
 
 
 def _target_device(Q_):
@@ -26,7 +41,7 @@ def _target_device(Q_):
 
 class QPEqualityFn(Function):
     @staticmethod
-    def forward(ctx, Q_, p_, A_, b_, check_Q_spd):
+    def forward(ctx, Q_, p_, A_, b_, check_Q_spd, reg=False):
         empty = Q_.new_empty(0)
         nBatch, nz, nineq, neq = check_shapes(Q_, p_, empty, empty, A_, b_)
         assert neq > 0 or nineq > 0                         # qp.py:89
@@ -39,12 +54,15 @@ class QPEqualityFn(Function):
             batched.append(Xe.contiguous())
             flags.append(was_unbatched)
         Q, p, A, b = batched
-        F = _factor(Q, torch.zeros(nBatch, 1, nz, **f64), A, 0.0)          # one dummy row: G = 0 (h = 1, d = 1 below)
+        # one dummy row: G = 0 (h = 1, d = 1 below); regularised mode: chol(Q + eps I), eps on the constraint blocks
+        F = _factor(Q, torch.zeros(nBatch, 1, nz, **f64), A, kkt.IR_EPS if reg else 0.0)
         if check_Q_spd and bool(F.spd.any()):
-            raise RuntimeError('Q is not SPD.')
+            raise RuntimeError('Q is not positive semidefinite.' if reg else 'Q is not SPD.')
         one, zero = torch.ones(nBatch, 1, **f64), torch.zeros(nBatch, 1, **f64)
-        zhat, _, _, nus = F.solve(one, p, zero, -one, -b)                   # K [x s z y] = -[p 0 -h -b]
+        steps = EQ_IR_STEPS if reg else 0
+        zhat, _, _, nus = _solve(F, Q, A, one, p, zero, -one, -b, steps)   # K [x s z y] = -[p 0 -h -b]
         ctx.F, ctx.flags, ctx.one, ctx.zero = F, flags, one, zero
+        ctx.QA, ctx.steps = (Q, A), steps
         ctx.zhat64, ctx.nus = zhat, nus
         ctx.meta = [(X.device, X.dtype) for X in (Q_, p_, A_, b_)]
         return zhat.to(device=Q_.device, dtype=Q_.dtype)
@@ -53,7 +71,7 @@ class QPEqualityFn(Function):
     def backward(ctx, dl_dzhat):
         z, nus = ctx.zhat64, ctx.nus
         dl = dl_dzhat.detach().to(device=z.device, dtype=torch.float64).contiguous().view_as(z)
-        dx, _, _, dnu = ctx.F.solve(ctx.one, dl, ctx.zero, ctx.zero, torch.zeros_like(nus))
+        dx, _, _, dnu = _solve(ctx.F, *ctx.QA, ctx.one, dl, ctx.zero, ctx.zero, torch.zeros_like(nus), ctx.steps)
         grads = [0.5 * (bger(dx, z) + bger(z, dx)),         # qp.py:175-177
                  dx,                                        # qp.py:150
                  bger(dnu, z) + bger(nus, dx),              # qp.py:166-167
@@ -64,9 +82,11 @@ class QPEqualityFn(Function):
                 out.append(None)
                 continue
             out.append((g.mean(0) if unb else g).to(device=dev, dtype=dt))
-        return tuple(out) + (None,)
+        return tuple(out) + (None, None)
 
 
-def solve_equality_qp(Q_, p_, A_, b_, check_Q_spd=True):
-    """z* of  argmin 1/2 z'Qz + p'z  s.t. Az = b  (differentiable in Q, p, A, b)."""
-    return QPEqualityFn.apply(Q_, p_, A_, b_, check_Q_spd)
+def solve_equality_qp(Q_, p_, A_, b_, check_Q_spd=True, reg=False):
+    """z* of  argmin 1/2 z'Qz + p'z  s.t. Az = b  (differentiable in Q, p, A, b). reg: the regularised mode of
+    QPFunction(kkt_solver=KKTSolvers.IR_UNOPT) for a Q that is only positive semidefinite on the null space of A, or
+    linearly dependent rows of A."""
+    return QPEqualityFn.apply(Q_, p_, A_, b_, check_Q_spd, reg)

@@ -16,6 +16,12 @@ import torch
 from . import _lib
 
 IR_EPS = 1e-7          # batch.py:247
+# Refinement steps per KKT solve of QPFunction(kkt_solver=KKTSolvers.IR_UNOPT). The Newton loop uses the residuals of
+# the true problem, so the forward pass reaches the exact KKT point with 0 as well (oracle/reg_model.py: residuals
+# <= 1e-12 either way); the backward pass is ONE solve, whose O(eps) error only refinement removes: on the rank-5 case
+# of oracle/psd_cases.py the gradients move from 1.8e-5 to 1e-6 of the dense implicit-differentiation ones. A step costs
+# a W pass pair, two chol(Q) sweeps and one reduced solve more per KKT solve.
+IR_STEPS = 1
 
 
 def _ptr(t):

@@ -23,7 +23,7 @@ from enum import Enum
 import torch
 from torch.autograd import Function
 
-from . import _lib
+from . import _lib, kkt
 from .util import check_shapes, expandParam, extract_nBatch
 
 INACC_ERR = """
@@ -92,12 +92,22 @@ def flush_checks(wait=True):
         if banner and inacc:
             print(INACC_ERR)
         if chk and bad_spd:
-            raise RuntimeError('Q is not SPD. (reported by a deferred check, qpth_b200.qp.LAZY_CHECKS)')
+            raise RuntimeError(chk + ' (reported by a deferred check, qpth_b200.qp.LAZY_CHECKS)')
 
 
 class QPSolvers(Enum):
     PDIPM_BATCHED = 1
     CVXPY = 2
+
+
+class KKTSolvers(Enum):
+    """The reference's KKT solver choice (batch.py:41-44). LU_PARTIAL: the default path (Q positive definite).
+    IR_UNOPT: the regularised mode, for Q only positive semidefinite (LPs, low-rank quadratic terms) or linearly dependent
+    equality rows: every KKT solve factors the system regularised with kkt.IR_EPS and the Newton loop uses the residuals
+    of the true problem. LU_FULL is not provided."""
+    LU_FULL = 1
+    LU_PARTIAL = 2
+    IR_UNOPT = 3
 
 
 def _ptr(t):
@@ -116,11 +126,11 @@ def _dev64(t, device):
 class _Solved:
     """State carried from forward to backward (the reference's ctx.Q_LU / S_LU / R / nus / lams / slacks)."""
     __slots__ = ("plan", "nBatch", "nsys", "L", "W", "K", "zhat", "lam", "slacks", "nus",
-                 "iters", "best_resid", "scratch", "device", "trace")
+                 "iters", "best_resid", "scratch", "device", "trace", "reg")
 
 
 def solve_forward(Q_, p_, G_, h_, A_, b_, eps=1e-12, verbose=0, notImprovedLim=3, maxIter=20,
-                  check_Q_spd=True):
+                  check_Q_spd=True, kkt_solver=KKTSolvers.LU_PARTIAL):
     """pre_factor_kkt + forward on the device. Inputs follow QPFunction's conventions. Returns _Solved."""
     # rank errors exactly as expandParam raises them (util.py:44-50), then every trailing dimension / batch size:
     # pure host logic, done before anything touches the device
@@ -141,8 +151,12 @@ def solve_forward(Q_, p_, G_, h_, A_, b_, eps=1e-12, verbose=0, notImprovedLim=3
         b = _dev64(b_, device) if neq > 0 else None
         # one QP per SM (W, chol(Q) and the factor all in shared memory) has the lower latency; two QPs per SM (W and
         # chol(Q) read from L2) the higher throughput once more QPs are in flight than the GPU has SMs (MODE above)
-        two = MODE == "throughput" or (MODE == "auto" and nBatch > _lib.sm_count(device.index or 0))
-        plan = _lib.plan_for(nz, nineq, neq, two=two)
+        reg = kkt_solver == KKTSolvers.IR_UNOPT
+        if reg:                      # one QP per SM, 256 threads: the only build of the regularised kernels (MODE ignored)
+            plan = _lib.plan_for_reg(nz, nineq, neq)
+        else:
+            two = MODE == "throughput" or (MODE == "auto" and nBatch > _lib.sm_count(device.index or 0))
+            plan = _lib.plan_for(nz, nineq, neq, two=two)
 
         def stride(t, nd, per):
             return per if (t is not None and t.dim() == nd) else 0
@@ -152,7 +166,7 @@ def solve_forward(Q_, p_, G_, h_, A_, b_, eps=1e-12, verbose=0, notImprovedLim=3
         sp, sh, sb = stride(p, 2, nz), stride(h, 2, nineq), stride(b, 2, neq)
         nsys = nBatch if (sQ or sG or sA) else 1
         st = _Solved()
-        st.plan, st.nBatch, st.nsys, st.device = plan, nBatch, nsys, device
+        st.plan, st.nBatch, st.nsys, st.device, st.reg = plan, nBatch, nsys, device, reg
         f64 = dict(dtype=torch.float64, device=device)
         st.L = torch.empty(nsys * plan.L_elems, **f64)
         st.W = torch.empty(nsys * plan.W_elems, **f64)
@@ -160,9 +174,14 @@ def solve_forward(Q_, p_, G_, h_, A_, b_, eps=1e-12, verbose=0, notImprovedLim=3
         spd = torch.zeros(nsys, dtype=torch.int32, device=device)
         nscr = max(nsys * plan.setup_scratch_elems, nBatch * plan.solve_scratch_elems)
         st.scratch = torch.empty(nscr, **f64) if nscr > 0 else None
-        _lib.check(lib.qpb200_pre_factor_kkt(
-            ctypes.byref(plan), nsys, _ptr(Q), sQ, _ptr(G), sG, _ptr(A), sA,
-            _ptr(st.L), _ptr(st.W), _ptr(st.K), _ptr(spd), _ptr(st.scratch), _stream()))
+        if reg:
+            _lib.check(lib.qpb200_pre_factor_kkt_reg(
+                ctypes.byref(plan), nsys, _ptr(Q), sQ, _ptr(G), sG, _ptr(A), sA, float(kkt.IR_EPS),
+                _ptr(st.L), _ptr(st.W), _ptr(st.K), _ptr(spd), _ptr(st.scratch), _stream()))
+        else:
+            _lib.check(lib.qpb200_pre_factor_kkt(
+                ctypes.byref(plan), nsys, _ptr(Q), sQ, _ptr(G), sG, _ptr(A), sA,
+                _ptr(st.L), _ptr(st.W), _ptr(st.K), _ptr(spd), _ptr(st.scratch), _stream()))
         st.zhat = torch.empty(nBatch, nz, **f64)
         st.lam = torch.empty(nBatch, nineq, **f64)
         st.slacks = torch.empty(nBatch, nineq, **f64)
@@ -170,17 +189,24 @@ def solve_forward(Q_, p_, G_, h_, A_, b_, eps=1e-12, verbose=0, notImprovedLim=3
         st.iters = torch.empty(nBatch, dtype=torch.int32, device=device)
         st.best_resid = torch.empty(nBatch, **f64)
         st.trace = torch.full((nBatch, int(maxIter), 4), float('nan'), **f64) if (verbose == 1 or TRACE) else None
-        _lib.check(lib.qpb200_forward(
+        common = (float(eps), float(STALL_TOL), float(BEST_TIE), int(notImprovedLim), int(maxIter))
+        if reg:
+            common += (float(kkt.IR_EPS), int(kkt.IR_STEPS))
+        _lib.check((lib.qpb200_forward_reg if reg else lib.qpb200_forward)(
             ctypes.byref(plan), nBatch, _ptr(p), sp, _ptr(h), sh, _ptr(b), sb,
-            _ptr(st.L), _ptr(st.W), _ptr(st.K), 1 if nsys > 1 else 0,
-            float(eps), float(STALL_TOL), float(BEST_TIE), int(notImprovedLim), int(maxIter),
+            _ptr(st.L), _ptr(st.W), _ptr(st.K), 1 if nsys > 1 else 0, *common,
             _ptr(st.zhat), _ptr(st.lam), _ptr(st.slacks), _ptr(st.nus),
             _ptr(st.iters), _ptr(st.best_resid), _ptr(st.trace), _ptr(st.scratch), _stream()))
-        diagnostics(spd, st, check_Q_spd, verbose)
+        diagnostics(spd, st, check_Q_spd, verbose, SPD_ERR_REG if reg else SPD_ERR)
     return st
 
 
-def diagnostics(spd, st, check_Q_spd, verbose):
+SPD_ERR = 'Q is not SPD.'
+# the regularised mode factors Q + IR_EPS I: a failed pivot means an eigenvalue of Q below -IR_EPS
+SPD_ERR_REG = 'Q is not positive semidefinite.'
+
+
+def diagnostics(spd, st, check_Q_spd, verbose, spd_err=SPD_ERR):
     """After a forward: 'Q is not SPD.' from the device flags `spd`, the inaccurate-solution banner from st.best_resid,
     and at verbose == 1 the per-iteration lines from st.trace / st.iters."""
     # One host read for both diagnostics (the reference syncs many times per iteration):
@@ -195,11 +221,11 @@ def diagnostics(spd, st, check_Q_spd, verbose):
             host.copy_(flags, non_blocking=True)
             ev = torch.cuda.Event()
             ev.record()
-            _pending.append((ev, host, bool(check_Q_spd), verbose >= 0))
+            _pending.append((ev, host, spd_err if check_Q_spd else None, verbose >= 0))
         else:
             bad_spd, inacc = flags.tolist()
             if check_Q_spd and bad_spd:
-                raise RuntimeError('Q is not SPD.')
+                raise RuntimeError(spd_err)
             if verbose >= 0 and inacc:
                 print(INACC_ERR)
     if verbose == 1:
@@ -239,16 +265,32 @@ def solve_backward(st, dl_dzhat, mean_flags, want):
         args = []
         for k in range(6):
             args += [_ptr(outs[k]), 1 if mean_flags[k] else 0]
-        _lib.check(lib.qpb200_backward(
+        reg = getattr(st, "reg", False)             # (solution.py builds _Solved without it: the default path)
+        _lib.check((lib.qpb200_backward_reg if reg else lib.qpb200_backward)(
             ctypes.byref(plan), B, _ptr(dl), _ptr(st.zhat), _ptr(st.lam), _ptr(st.slacks), _ptr(st.nus),
-            _ptr(st.L), _ptr(st.W), _ptr(st.K), 1 if st.nsys > 1 else 0,
+            _ptr(st.L), _ptr(st.W), _ptr(st.K), 1 if st.nsys > 1 else 0, *((float(kkt.IR_EPS), int(kkt.IR_STEPS)) if reg else ()),
             *args, _ptr(dxv), _ptr(dlamv), _ptr(dnuv), _ptr(st.scratch), _stream()))
     return outs
 
 
 def QPFunction(eps=1e-12, verbose=0, notImprovedLim=3, maxIter=20, solver=QPSolvers.PDIPM_BATCHED,
-               check_Q_spd=True):
-    """Factory with the reference's signature (`qpth/qp.py:18-20`); returns `Function.apply`."""
+               check_Q_spd=True, kkt_solver=KKTSolvers.LU_PARTIAL):
+    """Factory with the reference's signature (`qpth/qp.py:18-20`); returns `Function.apply`.
+
+    kkt_solver (an extension of the reference's signature): KKTSolvers.LU_PARTIAL, the default, needs Q positive definite.
+    KKTSolvers.IR_UNOPT also solves QPs whose Q is only positive semidefinite (LPs with Q = 0, low-rank quadratic terms)
+    and QPs whose equality rows are linearly dependent: every KKT solve factors the system regularised with kkt.IR_EPS
+    (chol(Q + eps I); eps on the constraint blocks) and refines it kkt.IR_STEPS times, while the residuals are those of
+    the true problem, so the returned point is the exact KKT point. check_Q_spd then checks that Q is positive
+    SEMIdefinite ('Q is not positive semidefinite.'). Shapes with ms_pad = 8 ceil(neq / 8) + nineq rounded up to 8
+    above 256 raise. With linearly dependent equality rows the equality duals, and so the gradients dA and db, are not
+    unique; z*, the inequality duals, the slacks and dQ, dp, dG, dh are. An unbounded or infeasible problem gives the
+    inaccurate-solution banner, as in the default mode."""
+    if kkt_solver == KKTSolvers.LU_FULL:
+        raise ValueError("qpth_b200: KKTSolvers.LU_FULL is not provided; use KKTSolvers.LU_PARTIAL (Q positive definite) "
+                         "or KKTSolvers.IR_UNOPT (Q positive semidefinite, linearly dependent equality rows)")
+    if kkt_solver not in (KKTSolvers.LU_PARTIAL, KKTSolvers.IR_UNOPT):
+        raise ValueError("qpth_b200: unknown kkt_solver %r" % (kkt_solver,))
     if solver == QPSolvers.CVXPY:
         # qp.py:97-120,142-143: per-sample CVXPY solve on the CPU, then pre_factor_kkt + the same backward.
         from .solution import QPSolutionFunction, cvxpy_forward
@@ -275,7 +317,7 @@ def QPFunction(eps=1e-12, verbose=0, notImprovedLim=3, maxIter=20, solver=QPSolv
             h (nBatch,nineq)|(nineq); A (nBatch,neq,nz)|(neq,nz)|empty; b (nBatch,neq)|(neq)|empty.
             Returns zhat (nBatch, nz).  (qp.py:23-125)
             """
-            st = solve_forward(Q_, p_, G_, h_, A_, b_, eps, verbose, notImprovedLim, maxIter, check_Q_spd)
+            st = solve_forward(Q_, p_, G_, h_, A_, b_, eps, verbose, notImprovedLim, maxIter, check_Q_spd, kkt_solver)
             ctx.st = st
             _last[0] = st
             ctx.neq, ctx.nineq, ctx.nz = st.plan.neq, st.plan.nineq, st.plan.nz
@@ -302,7 +344,7 @@ def QPFunction(eps=1e-12, verbose=0, notImprovedLim=3, maxIter=20, solver=QPSolv
         if G_.nelement() == 0 and h_.nelement() == 0 and A_.nelement() > 0:
             # equality-constrained QP: an extension (the reference cannot run nineq == 0); one KKT solve, eqonly.py
             from .eqonly import solve_equality_qp
-            return solve_equality_qp(Q_, p_, A_, b_, check_Q_spd)
+            return solve_equality_qp(Q_, p_, A_, b_, check_Q_spd, reg=kkt_solver == KKTSolvers.IR_UNOPT)
         return QPFunctionFn.apply(Q_, p_, G_, h_, A_, b_)
 
     # diagnostics the reference keeps on ctx (nus / lams / slacks) plus per-QP iteration counts
