@@ -175,11 +175,17 @@ int qpb200_solve_kkt_reg(const qpb200_plan* plan, int nbatch,
  * whose fixed point is the exact KKT point. In the forward pass the refinement is applied to each iteration's combined
  * direction (the same correction as refining the affine and corrector directions one by one: it is linear); sigma uses
  * the unrefined affine direction.
- * The plan comes from qpb200_plan_init_reg: the product-form kernels with 256 threads and one QP per SM (W and chol(Q)
- * in shared memory, or read from L2 when pf_global), on every shape they take, tiny ones included; it returns
- * QPB200_ERR_TOO_LARGE for ms_pad > 256 or nineq == 0. The factors come from qpb200_pre_factor_kkt_reg with that plan
- * and the same reg_eps; spd_flag is then 1 where a pivot of chol(Q + eps I) failed, i.e. Q has an eigenvalue below
- * -eps. With rank-deficient A the duals nus and the gradients dA, db are not unique. scratch is unused (may be NULL). */
+ * forward_reg and backward_reg take two kinds of plan:
+ *  - one from qpb200_plan_init_reg: the product-form kernels with 256 threads and one QP per SM (W and chol(Q) in
+ *    shared memory, or read from L2 when pf_global), on every shape they take, tiny ones included. plan_init_reg
+ *    returns QPB200_ERR_TOO_LARGE for ms_pad > 256 (in practice about 200: shared memory) or nineq == 0. scratch is
+ *    unused (may be NULL);
+ *  - one from qpb200_plan_init with tiny == 0, pf == 0 and smem_resident == 0: the generic global-scratch kernels, on
+ *    the larger shapes plan_init_reg refuses. scratch (nbatch * solve_scratch_elems doubles) is then required; NULL
+ *    returns QPB200_ERR_BAD_ARG.
+ * Every other plan returns QPB200_ERR_TOO_LARGE. The factors come from qpb200_pre_factor_kkt_reg with the same plan and
+ * reg_eps; spd_flag is then 1 where a pivot of chol(Q + eps I) failed, i.e. Q has an eigenvalue below -eps. With
+ * rank-deficient A the duals nus and the gradients dA, db are not unique. */
 int qpb200_plan_init_reg(int nz, int nineq, int neq, qpb200_plan* plan);
 int qpb200_forward_reg(const qpb200_plan* plan, int nbatch,
                        const double* p, int64_t sp, const double* h, int64_t sh,

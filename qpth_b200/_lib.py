@@ -153,6 +153,19 @@ def plan_for_reg(nz, nineq, neq):
     return _reg_plans[key]
 
 
+def plan_for_ir(nz, nineq, neq):
+    """Plan of QPFunction(kkt_solver=IR_UNOPT) for a shape: the product-form plan of plan_for_reg where it exists, else
+    the default latency plan when it uses the generic global-scratch kernels (tiny = pf = smem_resident = 0), which
+    qpb200_forward_reg / qpb200_backward_reg also run. Raises QpthB200Error for every other shape."""
+    try:
+        return plan_for_reg(nz, nineq, neq)
+    except QpthB200Error:
+        p = plan_for(nz, nineq, neq, two=False)
+        if p.tiny or p.pf or p.smem_resident:
+            raise
+        return p
+
+
 _box_plans = {}
 
 

@@ -258,11 +258,14 @@ __device__ __forceinline__ Ctx make_ctx(const KDims& D, double* smem, double* gs
 
 // factor_kkt + the forward half of solve_kkt: on entry V_AUG holds -h_full (length ms) and V_D holds d.
 // On exit V_W holds w = -S^-1 h_full. Destroys V_AUG, V_T0.
-template <bool kSmem>
+// kReg: V_D holds d + eps and the inequality diagonal gets 1 / (d + eps) + eps (the regularised system of the kReg
+// kernels; the eps of the equality rows is already in K, pre_factor_kkt_reg).
+template <bool kSmem, bool kReg = false>
 __device__ __forceinline__ void factor_and_solve(const KDims& D, Ctx& C, int tid, int nt) {
     double* aug = VEC(V_AUG);
     wait_K<kSmem>(D, C, tid, nt);
-    for (int i = D.ep + tid; i < D.ms; i += nt) C.LS[i * D.lds + i] += 1.0 / VEC(V_D)[i];
+    for (int i = D.ep + tid; i < D.ms; i += nt)
+        C.LS[i * D.lds + i] += kReg ? 1.0 / VEC(V_D)[i] + D.reg : 1.0 / VEC(V_D)[i];
     __syncthreads();
     const FullIdx at{D.lds};
     if (D.ep > 0) {
@@ -297,10 +300,73 @@ __device__ __forceinline__ void load_dinvs(const KDims& D, const Ctx& C, int tid
     for (int i = tid; i < D.ep; i += nt) VEC(V_DINV)[i] = C.Kg[(int64_t)i * D.lds + i];   // K stores 1/L_cc there
 }
 
+// ---- regularised mode (kReg: QPFunction with kkt_solver=IR_UNOPT) on the generic kernels ------------------------------
+// The arithmetic of fk::f_true_rx / fk::f_refine (qp_solve.cuh) with the generic building blocks: the factors are those
+// of pre_factor_kkt_reg (L = chol(Q + eps I), K with eps on the equality rows), every KKT solve uses the regularised
+// system [Q+eI 0 G' A'; 0 D+eI I 0; G I -eI 0; A 0 0 -eI], and the residuals are those of the true problem.
+
+// r~x -= eps L^-1 L^-T x~: the whitened dual residual of the true problem from the one of Q + eps I. Destroys V_T0,
+// V_T1. Ends with a block barrier.
+__device__ __forceinline__ void true_rx(const KDims& D, const Ctx& C, const double* xt, double* rxt, int tid, int nt) {
+    double* t0 = VEC(V_T0);
+    for (int i = tid; i < D.n; i += nt) t0[i] = xt[i];
+    __syncthreads();
+    unwhiten(D, C, t0, VEC(V_T1), tid, nt);                    // T1 = x = L^-T x~
+    whiten(D, C, t0, tid, nt);                                  // T0 = L^-1 x
+    for (int i = tid; i < D.n; i += nt) rxt[i] = fma(-D.reg, t0[i], rxt[i]);
+    __syncthreads();
+}
+
+// One refinement step, with the factor still in the S workspace, of a solution of the regularised system: dv = [dy; dz],
+// ds, and dx~ = -base + ntx - W^T dv kept implicit. Against the true system that solution leaves the residual
+// (-eps dx, -eps ds, eps dz, eps dy); the correction solves the regularised system with it and is added in place
+// (ntx += eps L^-1 dx). V_D holds d + eps. a, c, e, f: scratch slots; destroys V_T0, V_T1, V_PART. Ends with a block
+// barrier.
+__device__ __forceinline__ void refine(const KDims& D, const Ctx& C, const double* base, double* ntx, double* dv,
+                                       double* ds, double* a, double* c, double* e, double* f, int tid, int nt) {
+    const double* dd = VEC(V_D);
+    double* t1 = VEC(V_T1); double* part = VEC(V_PART);
+    const int G = matvec_cols_partial(C.W, D.ldw, D.ms, D.n, dv, part, D.vl, tid, nt);
+    __syncthreads();
+    for (int i = tid; i < D.n; i += nt) {
+        double s = 0.0;
+        for (int g = 0; g < G; ++g) s += part[g * D.vl + i];
+        a[i] = ntx[i] - base[i] - s;                            // dx~
+    }
+    __syncthreads();
+    unwhiten(D, C, a, t1, tid, nt);                             // T1 = dx
+    whiten(D, C, c, tid, nt);                                   // c = L^-1 dx
+    for (int i = tid; i < D.n; i += nt) {
+        const double r = D.reg * c[i];
+        c[i] = -r;                                              // whitened x residual  L^-1 (-eps dx)
+        ntx[i] += r;
+    }
+    __syncthreads();
+    matvec_rows<false>(C.W, D.ldw, D.ms, D.n, c, nullptr, e, nullptr, tid, nt);
+    __syncthreads();
+    // reduced right-hand side -(W t - [r_y; r_z] + [0; r_s / (d + eps)])  (the elimination of solve_kkt)
+    for (int i = tid; i < D.ms; i += nt) {
+        double hf = fma(-D.reg, dv[i], e[i]);
+        if (i >= D.ep) hf -= D.reg * ds[i] / dd[i];
+        t1[i] = -hf;
+    }
+    __syncthreads();
+    solve_with_factor(D, C, f, tid, nt);                        // f = correction of [dy; dz]
+    for (int i = tid; i < D.ms; i += nt) {
+        const double wi = f[i];
+        if (i >= D.ep) ds[i] += (D.reg * ds[i] - wi) / dd[i];
+        dv[i] += wi;
+    }
+    __syncthreads();
+}
+
 // ---------------------------------------------------------------------------------------------
 // k_forward: the PDIPM loop (batch.py:47-207), per-QP semantics.
 // ---------------------------------------------------------------------------------------------
-template <bool kSmem, bool kTiny = false>
+// kReg (with !kSmem, !kTiny: the global-scratch build): the regularised mode (true_rx, refine); D.reg = eps, ir_steps
+// refinement steps of the initial point and of each iteration's combined direction (a trailing parameter: KDims keeps
+// its layout).
+template <bool kSmem, bool kTiny = false, bool kReg = false>
 __global__ void __launch_bounds__(kTiny ? kTinyThreads : kThreads, kTiny ? kTinyCtasPerSm : 1)
 k_forward(KDims D, const double* __restrict__ p, int64_t sp, const double* __restrict__ h,
           int64_t sh, const double* __restrict__ b, int64_t sb, const double* __restrict__ Lfac,
@@ -308,7 +374,7 @@ k_forward(KDims D, const double* __restrict__ p, int64_t sp, const double* __res
           double stall_tol, double best_tie, int notImprovedLim, int maxIter, double* __restrict__ zhat, double* __restrict__ lam,
           double* __restrict__ slacks, double* __restrict__ nus, int* __restrict__ iters_out,
           double* __restrict__ resid_out, double* __restrict__ trace, double* __restrict__ gscratch,
-          int64_t scratch_per_qp) {
+          int64_t scratch_per_qp, int ir_steps = 0) {
     extern __shared__ __align__(16) double smem[];
     const int tid = threadIdx.x, nt = blockDim.x;
     const int qp = blockIdx.x;
@@ -331,7 +397,7 @@ k_forward(KDims D, const double* __restrict__ p, int64_t sp, const double* __res
         if (i < e) val = bg[i];
         else if (i >= ep) val = hg[i - ep];
         hb[i] = val;
-        d[i] = 1.0;
+        d[i] = kReg ? 1.0 + D.reg : 1.0;
         s[i] = 0.0;
     }
     load_dinvs(D, C, tid, nt);
@@ -343,15 +409,28 @@ k_forward(KDims D, const double* __restrict__ p, int64_t sp, const double* __res
     __syncthreads();
     for (int i = tid; i < ms; i += nt) aug[i] = -(hW[i] + hb[i]);
     __syncthreads();
-    factor_and_solve<kSmem>(D, C, tid, nt);
+    factor_and_solve<kSmem, kReg>(D, C, tid, nt);
+    const bool refine_on = kReg && ir_steps > 0;
+    if (kReg) {
+        // s = -w / (1 + eps); rv accumulates the x part of the refinement (x~ = -p~ + rv - W^T w)
+        for (int i = ep + tid; i < ms; i += nt) s[i] = -w[i] / d[i];
+        for (int i = tid; i < n; i += nt) rv[i] = 0.0;
+        __syncthreads();
+        for (int k = 0; k < ir_steps; ++k) refine(D, C, pt, rv, w, s, aug, hW, c2, dsa, tid, nt);
+        for (int i = tid; i < n; i += nt) hW[i] = pt[i] - rv[i];   // (read after finish_dxt's first barrier)
+    }
     issue_K<kSmem>(D, C, tid);
-    finish_dxt(C.W, D.ldw, ms, n, w, pt, xt, part, D.vl, tid, nt);   // x~ = -p~ - W^T w
+    finish_dxt(C.W, D.ldw, ms, n, w, kReg ? hW : pt, xt, part, D.vl, tid, nt);   // x~ = -p~ - W^T w
     {
         double mn[2] = {INFINITY, INFINITY};
         for (int i = ep + tid; i < ms; i += nt) {
             v[i] = w[i];
-            s[i] = -w[i];
-            mn[0] = fmin(mn[0], -w[i]);
+            if (kReg) {
+                mn[0] = fmin(mn[0], s[i]);
+            } else {
+                s[i] = -w[i];
+                mn[0] = fmin(mn[0], -w[i]);
+            }
             mn[1] = fmin(mn[1], w[i]);
         }
         for (int i = tid; i < ep; i += nt) v[i] = w[i];
@@ -380,6 +459,7 @@ k_forward(KDims D, const double* __restrict__ p, int64_t sp, const double* __res
             }
             __syncthreads();
         }
+        if (kReg) true_rx(D, C, xt, rxt, tid, nt);
         matvec_rows<true>(C.W, D.ldw, ms, n, xt, rxt, c2, hW, tid, nt);
         __syncthreads();
         double acc[4] = {0.0, 0.0, 0.0, 0.0};                   // |ry|^2, |rz|^2, |L r~x|^2, s.z
@@ -415,14 +495,14 @@ k_forward(KDims D, const double* __restrict__ p, int64_t sp, const double* __res
         for (int i = tid; i < ms; i += nt) {
             double hfull = hW[i] - rv[i];
             if (i >= ep) {
-                const double di = v[i] / s[i];
+                const double di = kReg ? v[i] / s[i] + D.reg : v[i] / s[i];
                 d[i] = di;
                 hfull += v[i] / di;                             // rs/d with rs = z
             }
             aug[i] = -hfull;
         }
         __syncthreads();
-        factor_and_solve<kSmem>(D, C, tid, nt);                      // w = [dy_aff; dz_aff]
+        factor_and_solve<kSmem, kReg>(D, C, tid, nt);                // w = [dy_aff; dz_aff]
         // ---- affine step length and sigma (batch.py:160-168)
         double mn[2] = {INFINITY, INFINITY};
         for (int i = ep + tid; i < ms; i += nt) {
@@ -458,7 +538,7 @@ k_forward(KDims D, const double* __restrict__ p, int64_t sp, const double* __res
             __syncthreads();
         }
         solve_with_factor(D, C, wc, tid, nt);                        // wc = [dy_cor; dz_cor]
-        issue_K<kSmem>(D, C, tid);                              // next factor_kkt's copy of K overlaps the rest
+        if (!refine_on) issue_K<kSmem>(D, C, tid);              // next factor_kkt's copy of K overlaps the rest
         // ---- combined direction, step length, update (batch.py:185-203)
         mn[0] = INFINITY; mn[1] = INFINITY;
         for (int i = tid; i < ms; i += nt) {
@@ -472,7 +552,20 @@ k_forward(KDims D, const double* __restrict__ p, int64_t sp, const double* __res
                 mn[1] = fmin(mn[1], step_candidate(s[i], dsi));
             }
         }
+        if (refine_on) for (int i = tid; i < n; i += nt) rv[i] = 0.0;
         __syncthreads();
+        if (refine_on) {
+            // The refinement is linear in the right-hand side, so refining the combined direction equals refining the
+            // affine and the corrector direction one by one; sigma above comes from the unrefined affine direction.
+            for (int k = 0; k < ir_steps; ++k) refine(D, C, rxt, rv, w, ds, aug, hW, c2, wc, tid, nt);
+            issue_K<kSmem>(D, C, tid);
+            mn[0] = INFINITY; mn[1] = INFINITY;
+            for (int i = ep + tid; i < ms; i += nt) {
+                mn[0] = fmin(mn[0], step_candidate(v[i], w[i]));
+                mn[1] = fmin(mn[1], step_candidate(s[i], ds[i]));
+            }
+            for (int i = tid; i < n; i += nt) rxt[i] -= rv[i];   // dx~ = -(r~x - rv) - W^T dv (read after a barrier)
+        }
         finish_dxt(C.W, D.ldw, ms, n, w, rxt, dxt, part, D.vl, tid, nt);   // dx~ = -r~x - W^T dv
         block_reduce<2, true>(mn, C.red, tid, nt);
         {
@@ -509,9 +602,11 @@ k_forward(KDims D, const double* __restrict__ p, int64_t sp, const double* __res
 // k_solve_kkt: factor_kkt + solve_kkt for caller-supplied d and right-hand sides.
 // kBackward: the backward pass of QPFunction (qp.py:128-182): d from clamped lam/slacks, rx = dl,
 // other right-hand sides zero, fused gradient outer products for batched inputs.
+// kReg (with kBackward, !kSmem, !kTiny: the global-scratch build): the backward pass of the regularised mode, d + eps and
+// ir_steps refinement steps (refine).
 // ---------------------------------------------------------------------------------------------
 
-template <bool kSmem, bool kBackward, bool kTiny = false>
+template <bool kSmem, bool kBackward, bool kTiny = false, bool kReg = false>
 __global__ void __launch_bounds__(kTiny ? kTinyThreads : kThreads, kTiny ? kTinyCtasPerSm : 1)
 k_solve_kkt(KDims D, const double* __restrict__ d_in, const double* __restrict__ rx_in,
             const double* __restrict__ rs_in, const double* __restrict__ rz_in,
@@ -521,7 +616,7 @@ k_solve_kkt(KDims D, const double* __restrict__ d_in, const double* __restrict__
             const double* __restrict__ Wfac, const double* __restrict__ Kfac, int sF,
             double* __restrict__ dx_out, double* __restrict__ ds_out, double* __restrict__ dz_out,
             double* __restrict__ dy_out, BwdOut O, double* __restrict__ gscratch,
-            int64_t scratch_per_qp) {
+            int64_t scratch_per_qp, int ir_steps = 0) {
     extern __shared__ __align__(16) double smem[];
     const int tid = threadIdx.x, nt = blockDim.x;
     const int qp = blockIdx.x;
@@ -538,6 +633,7 @@ k_solve_kkt(KDims D, const double* __restrict__ d_in, const double* __restrict__
             const int j = i - ep;
             if (kBackward) {
                 di = fmax(lam[(int64_t)qp * m + j], 1e-8) / fmax(slacks[(int64_t)qp * m + j], 1e-8);   // qp.py:148
+                if (kReg) di += D.reg;
             } else {
                 // regularised variant (D.reg > 0, batch.py:244-310): d~ = d + eps in the complementarity row, and the slot
                 // holds 1 / (1/d~ + eps) because factor_kkt adds the RECIPROCAL of this slot to the diagonal of S
@@ -560,7 +656,15 @@ k_solve_kkt(KDims D, const double* __restrict__ d_in, const double* __restrict__
     __syncthreads();
     for (int i = tid; i < ms; i += nt) aug[i] = -(VEC(V_C2)[i] + hW[i]);
     __syncthreads();
-    factor_and_solve<kSmem>(D, C, tid, nt);                          // w = [dy; dz]
+    factor_and_solve<kSmem, kReg>(D, C, tid, nt);                    // w = [dy; dz]
+    if (kReg) {
+        double* ntx = VEC(V_DSA); double* dsr = VEC(V_DS);     // x part of the refinement (dx~ = -t + ntx - W^T w), ds
+        for (int i = ep + tid; i < ms; i += nt) dsr[i] = -w[i] / d[i];   // (rs = 0)
+        for (int i = tid; i < n; i += nt) ntx[i] = 0.0;
+        __syncthreads();
+        for (int k = 0; k < ir_steps; ++k) refine(D, C, t, ntx, w, dsr, aug, hW, VEC(V_C2), VEC(V_WC), tid, nt);
+        for (int i = tid; i < n; i += nt) t[i] -= ntx[i];       // (read after finish_dxt's first barrier)
+    }
     finish_dxt(C.W, D.ldw, ms, n, w, t, dxt, part, D.vl, tid, nt);
     unwhiten(D, C, dxt, VEC(V_XT), tid, nt);                    // dx = L^-T dx~
     const double* dx = VEC(V_XT);
@@ -1455,9 +1559,14 @@ static int launch_means(int nbatch, int n, int m, int e, const double* zhat, con
     return QPB200_OK;
 }
 
-// ---- regularised mode (QPFunction kkt_solver=IR_UNOPT): the product-form solve kernels with kReg --------------------
-static int check_reg_plan(const qpb200_plan* plan, double reg_eps, int ir_steps) {
+// ---- regularised mode (QPFunction kkt_solver=IR_UNOPT): the solve kernels with kReg ---------------------------------
+// Two families: the product-form kernels (a plan from qpb200_plan_init_reg) and, for the larger shapes, the generic
+// global-scratch kernels (a plan from qpb200_plan_init with tiny = pf = smem_resident = 0), which need `scratch`.
+static bool reg_global_plan(const qpb200_plan* plan) { return !plan->tiny && !plan->pf && !plan->smem_resident; }
+
+static int check_reg_plan(const qpb200_plan* plan, double reg_eps, int ir_steps, const double* scratch) {
     if (!(reg_eps >= 0.0) || ir_steps < 0 || ir_steps > 8) return QPB200_ERR_BAD_ARG;
+    if (reg_global_plan(plan)) return scratch ? QPB200_OK : QPB200_ERR_BAD_ARG;
     if (plan->tiny || !plan->pf || plan->pf_two || plan->pf_three || plan->pf_threads != 256) return QPB200_ERR_TOO_LARGE;
     return QPB200_OK;
 }
@@ -1468,15 +1577,23 @@ int qpb200_forward_reg(const qpb200_plan* plan, int nbatch, const double* p, int
                        int notImprovedLim, int maxIter, double reg_eps, int ir_steps, double* zhat, double* lam,
                        double* slacks, double* nus, int* iters, double* best_resid, double* trace, double* scratch,
                        void* stream) {
-    (void)scratch;
     if (!plan || nbatch <= 0 || !p || !h || !Lfac || !Wfac || !Kfac || !zhat || !lam || !slacks || !iters || !best_resid)
         return QPB200_ERR_BAD_ARG;
     if (plan->neq > 0 && (!b || !nus)) return QPB200_ERR_BAD_ARG;
-    int rc = check_reg_plan(plan, reg_eps, ir_steps);
+    int rc = check_reg_plan(plan, reg_eps, ir_steps, scratch);
     if (rc) return rc;
     cudaStream_t st = (cudaStream_t)stream;
     KDims D = dims_of(plan);
     D.reg = reg_eps;
+    if (reg_global_plan(plan)) {
+        rc = set_smem(k_forward<false, false, true>, plan->solve_smem_bytes);
+        if (rc) return rc;
+        k_forward<false, false, true><<<nbatch, kThreads, plan->solve_smem_bytes, st>>>(
+            D, p, sp, h, sh, b, sb, Lfac, Wfac, Kfac, sF, eps, stall_tol, best_tie, notImprovedLim, maxIter, zhat, lam,
+            slacks, nus, iters, best_resid, trace, scratch, plan->solve_scratch_elems, ir_steps);
+        CK(cudaGetLastError());
+        return QPB200_OK;
+    }
     const size_t sb_ = (size_t)plan->pf_smem_bytes;
 #define QPB_LAUNCH_REG(KG)                                                                                   \
     do {                                                                                                     \
@@ -1499,11 +1616,10 @@ int qpb200_backward_reg(const qpb200_plan* plan, int nbatch, const double* dl_dz
                         int mean_Q, double* dp, int mean_p, double* dG, int mean_G, double* dh, int mean_h, double* dA,
                         int mean_A, double* db, int mean_b, double* dxv, double* dlamv, double* dnuv, double* scratch,
                         void* stream) {
-    (void)scratch;
     if (!plan || nbatch <= 0 || !dl_dzhat || !zhat || !lam || !slacks || !Lfac || !Wfac || !Kfac || !dxv || !dlamv)
         return QPB200_ERR_BAD_ARG;
     if (plan->neq > 0 && (!nus || !dnuv)) return QPB200_ERR_BAD_ARG;
-    int rc = check_reg_plan(plan, reg_eps, ir_steps);
+    int rc = check_reg_plan(plan, reg_eps, ir_steps, scratch);
     if (rc) return rc;
     cudaStream_t st = (cudaStream_t)stream;
     KDims D = dims_of(plan);
@@ -1511,6 +1627,16 @@ int qpb200_backward_reg(const qpb200_plan* plan, int nbatch, const double* dl_dz
     BwdOut O;
     O.dQ = dQ; O.dp = dp; O.dG = dG; O.dh = dh; O.dA = dA; O.db = db;
     O.mQ = mean_Q; O.mp = mean_p; O.mG = mean_G; O.mh = mean_h; O.mA = mean_A; O.mb = mean_b;
+    if (reg_global_plan(plan)) {
+        rc = set_smem(k_solve_kkt<false, true, false, true>, plan->solve_smem_bytes);
+        if (rc) return rc;
+        k_solve_kkt<false, true, false, true><<<nbatch, kThreads, plan->solve_smem_bytes, st>>>(
+            D, nullptr, dl_dzhat, nullptr, nullptr, nullptr, zhat, lam, slacks, nus, Lfac, Wfac, Kfac, sF, dxv, nullptr,
+            dlamv, dnuv, O, scratch, plan->solve_scratch_elems, ir_steps);
+        CK(cudaGetLastError());
+        return launch_means(nbatch, plan->nz, plan->nineq, plan->neq, zhat, lam, nus, dQ, mean_Q, dp, mean_p, dG, mean_G,
+                            dh, mean_h, dA, mean_A, db, mean_b, dxv, dlamv, dnuv, st);
+    }
     const size_t sb_ = (size_t)plan->pf_smem_bytes;
 #define QPB_LAUNCH_REG(KG)                                                                                   \
     do {                                                                                                     \

@@ -152,8 +152,8 @@ def solve_forward(Q_, p_, G_, h_, A_, b_, eps=1e-12, verbose=0, notImprovedLim=3
         # one QP per SM (W, chol(Q) and the factor all in shared memory) has the lower latency; two QPs per SM (W and
         # chol(Q) read from L2) the higher throughput once more QPs are in flight than the GPU has SMs (MODE above)
         reg = kkt_solver == KKTSolvers.IR_UNOPT
-        if reg:                      # one QP per SM, 256 threads: the only build of the regularised kernels (MODE ignored)
-            plan = _lib.plan_for_reg(nz, nineq, neq)
+        if reg:                      # one QP per SM, 256 threads: the only builds of the regularised kernels (MODE ignored)
+            plan = _lib.plan_for_ir(nz, nineq, neq)
         else:
             two = MODE == "throughput" or (MODE == "auto" and nBatch > _lib.sm_count(device.index or 0))
             plan = _lib.plan_for(nz, nineq, neq, two=two)
@@ -273,6 +273,14 @@ def solve_backward(st, dl_dzhat, mean_flags, want):
     return outs
 
 
+def check_kkt_solver(kkt_solver):
+    if kkt_solver == KKTSolvers.LU_FULL:
+        raise ValueError("qpth_b200: KKTSolvers.LU_FULL is not provided; use KKTSolvers.LU_PARTIAL (Q positive definite) "
+                         "or KKTSolvers.IR_UNOPT (Q positive semidefinite, linearly dependent equality rows)")
+    if kkt_solver not in (KKTSolvers.LU_PARTIAL, KKTSolvers.IR_UNOPT):
+        raise ValueError("qpth_b200: unknown kkt_solver %r" % (kkt_solver,))
+
+
 def QPFunction(eps=1e-12, verbose=0, notImprovedLim=3, maxIter=20, solver=QPSolvers.PDIPM_BATCHED,
                check_Q_spd=True, kkt_solver=KKTSolvers.LU_PARTIAL):
     """Factory with the reference's signature (`qpth/qp.py:18-20`); returns `Function.apply`.
@@ -282,15 +290,12 @@ def QPFunction(eps=1e-12, verbose=0, notImprovedLim=3, maxIter=20, solver=QPSolv
     and QPs whose equality rows are linearly dependent: every KKT solve factors the system regularised with kkt.IR_EPS
     (chol(Q + eps I); eps on the constraint blocks) and refines it kkt.IR_STEPS times, while the residuals are those of
     the true problem, so the returned point is the exact KKT point. check_Q_spd then checks that Q is positive
-    SEMIdefinite ('Q is not positive semidefinite.'). Shapes with ms_pad = 8 ceil(neq / 8) + nineq rounded up to 8
-    above 256 raise. With linearly dependent equality rows the equality duals, and so the gradients dA and db, are not
-    unique; z*, the inequality duals, the slacks and dQ, dp, dG, dh are. An unbounded or infeasible problem gives the
-    inaccurate-solution banner, as in the default mode."""
-    if kkt_solver == KKTSolvers.LU_FULL:
-        raise ValueError("qpth_b200: KKTSolvers.LU_FULL is not provided; use KKTSolvers.LU_PARTIAL (Q positive definite) "
-                         "or KKTSolvers.IR_UNOPT (Q positive semidefinite, linearly dependent equality rows)")
-    if kkt_solver not in (KKTSolvers.LU_PARTIAL, KKTSolvers.IR_UNOPT):
-        raise ValueError("qpth_b200: unknown kkt_solver %r" % (kkt_solver,))
+    SEMIdefinite ('Q is not positive semidefinite.'). IR_UNOPT takes every shape the default mode takes with
+    nineq >= 1: up to ms_pad = 8 ceil(neq / 8) + nineq rounded up to 8 of about 200 on the product-form kernels, beyond
+    that on the generic global-scratch kernels. With linearly dependent equality rows the equality duals, and so the
+    gradients dA and db, are not unique; z*, the inequality duals, the slacks and dQ, dp, dG, dh are. An unbounded or
+    infeasible problem gives the inaccurate-solution banner, as in the default mode."""
+    check_kkt_solver(kkt_solver)
     if solver == QPSolvers.CVXPY:
         # qp.py:97-120,142-143: per-sample CVXPY solve on the CPU, then pre_factor_kkt + the same backward.
         from .solution import QPSolutionFunction, cvxpy_forward
@@ -300,7 +305,7 @@ def QPFunction(eps=1e-12, verbose=0, notImprovedLim=3, maxIter=20, solver=QPSolv
             Q, p, G, h, A, b = (expandParam(X, nBatch, nd)[0]
                                 for X, nd in ((Q_, 3), (p_, 2), (G_, 3), (h_, 2), (A_, 3), (b_, 2)))
             zhats, nus, lams, slacks = cvxpy_forward(Q, p, G, h, A, b)
-            return QPSolutionFunction(check_Q_spd)(Q_, p_, G_, h_, A_, b_, zhats, lams, slacks, nus)
+            return QPSolutionFunction(check_Q_spd, kkt_solver)(Q_, p_, G_, h_, A_, b_, zhats, lams, slacks, nus)
 
         return apply_cvxpy
     if solver != QPSolvers.PDIPM_BATCHED:

@@ -25,12 +25,17 @@ import torch
 from torch.autograd import Function
 
 from . import _lib
+from .qp import KKTSolvers, check_kkt_solver
 from .util import expandParam, extract_nBatch
 
 
-def pre_factor_state(Q_, p_, G_, h_, A_, b_, zhat, lams, slacks, nus, check_Q_spd=True):
-    """`pre_factor_kkt` on the device + the given solution, packaged as the state `solve_backward` consumes."""
-    from .qp import _Solved, _dev64, _ptr, _stream
+def pre_factor_state(Q_, p_, G_, h_, A_, b_, zhat, lams, slacks, nus, check_Q_spd=True,
+                     kkt_solver=KKTSolvers.LU_PARTIAL):
+    """`pre_factor_kkt` on the device + the given solution, packaged as the state `solve_backward` consumes.
+    kkt_solver=KKTSolvers.IR_UNOPT: the regularised factors (`qpb200_pre_factor_kkt_reg`), so that the backward pass is
+    `qpb200_backward_reg` and Q need only be positive semidefinite."""
+    from . import kkt
+    from .qp import SPD_ERR, SPD_ERR_REG, _Solved, _dev64, _ptr, _stream
     from .util import check_shapes
     nBatch, nz, nineq, neq = check_shapes(Q_, p_, G_, h_, A_, b_)
     assert neq > 0 or nineq > 0                         # qp.py:89
@@ -43,13 +48,14 @@ def pre_factor_state(Q_, p_, G_, h_, A_, b_, zhat, lams, slacks, nus, check_Q_sp
     with torch.cuda.device(device):
         Q, G = _dev64(Q_, device), _dev64(G_, device)
         A = _dev64(A_, device) if neq > 0 else None
-        plan = _lib.plan_for(nz, nineq, neq)
+        reg = kkt_solver == KKTSolvers.IR_UNOPT
+        plan = _lib.plan_for_ir(nz, nineq, neq) if reg else _lib.plan_for(nz, nineq, neq)
         sQ = nz * nz if Q.dim() == 3 else 0
         sG = nineq * nz if G.dim() == 3 else 0
         sA = neq * nz if (A is not None and A.dim() == 3) else 0
         nsys = nBatch if (sQ or sG or sA) else 1
         st = _Solved()
-        st.plan, st.nBatch, st.nsys, st.device = plan, nBatch, nsys, device
+        st.plan, st.nBatch, st.nsys, st.device, st.reg = plan, nBatch, nsys, device, reg
         f64 = dict(dtype=torch.float64, device=device)
         st.L = torch.empty(nsys * plan.L_elems, **f64)
         st.W = torch.empty(nsys * plan.W_elems, **f64)
@@ -57,11 +63,16 @@ def pre_factor_state(Q_, p_, G_, h_, A_, b_, zhat, lams, slacks, nus, check_Q_sp
         spd = torch.zeros(nsys, dtype=torch.int32, device=device)
         nscr = max(nsys * plan.setup_scratch_elems, nBatch * plan.solve_scratch_elems)
         st.scratch = torch.empty(nscr, **f64) if nscr > 0 else None
-        _lib.check(lib.qpb200_pre_factor_kkt(
-            ctypes.byref(plan), nsys, _ptr(Q), sQ, _ptr(G), sG, _ptr(A), sA,
-            _ptr(st.L), _ptr(st.W), _ptr(st.K), _ptr(spd), _ptr(st.scratch), _stream()))
+        if reg:
+            _lib.check(lib.qpb200_pre_factor_kkt_reg(
+                ctypes.byref(plan), nsys, _ptr(Q), sQ, _ptr(G), sG, _ptr(A), sA, float(kkt.IR_EPS),
+                _ptr(st.L), _ptr(st.W), _ptr(st.K), _ptr(spd), _ptr(st.scratch), _stream()))
+        else:
+            _lib.check(lib.qpb200_pre_factor_kkt(
+                ctypes.byref(plan), nsys, _ptr(Q), sQ, _ptr(G), sG, _ptr(A), sA,
+                _ptr(st.L), _ptr(st.W), _ptr(st.K), _ptr(spd), _ptr(st.scratch), _stream()))
         if check_Q_spd and bool(spd.any()):
-            raise RuntimeError('Q is not SPD.')
+            raise RuntimeError(SPD_ERR_REG if reg else SPD_ERR)
 
         def sol(t, cols):
             t = t.detach().to(device=device, dtype=torch.float64)
@@ -82,13 +93,18 @@ def pre_factor_state(Q_, p_, G_, h_, A_, b_, zhat, lams, slacks, nus, check_Q_sp
     return st
 
 
-def QPSolutionFunction(check_Q_spd=True):
-    """Returns `f(Q, p, G, h, A, b, zhat, lams, slacks, nus) -> zhat`, differentiable in Q, p, G, h, A, b."""
+def QPSolutionFunction(check_Q_spd=True, kkt_solver=KKTSolvers.LU_PARTIAL):
+    """Returns `f(Q, p, G, h, A, b, zhat, lams, slacks, nus) -> zhat`, differentiable in Q, p, G, h, A, b.
+
+    kkt_solver: KKTSolvers.LU_PARTIAL (the default) needs Q positive definite. KKTSolvers.IR_UNOPT differentiates with
+    the regularised KKT solve of QPFunction(kkt_solver=IR_UNOPT), so an LP (Q = 0) or a low-rank Q solved by any solver
+    can be differentiated; check_Q_spd then checks that Q is positive semidefinite."""
+    check_kkt_solver(kkt_solver)
 
     class QPSolutionFn(Function):
         @staticmethod
         def forward(ctx, Q_, p_, G_, h_, A_, b_, zhat, lams, slacks, nus):
-            ctx.st = pre_factor_state(Q_, p_, G_, h_, A_, b_, zhat, lams, slacks, nus, check_Q_spd)
+            ctx.st = pre_factor_state(Q_, p_, G_, h_, A_, b_, zhat, lams, slacks, nus, check_Q_spd, kkt_solver)
             zhats = ctx.st.zhat.to(device=Q_.device, dtype=Q_.dtype)
             ctx.save_for_backward(zhats, Q_, p_, G_, h_, A_, b_)
             ctx.lams, ctx.slacks, ctx.nus = ctx.st.lam, ctx.st.slacks, ctx.st.nus
