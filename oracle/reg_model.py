@@ -27,12 +27,14 @@ def _solve(f, F, reg, Q, G, A, rx, rs, rz, ry, steps):
         return km._tri(f["L"], dxt, trans=True), ds, dz, dy
 
     dx, ds, dz, dy = one(rx, rs, rz, ry)
+    cx, cs, cz, cy = dx, ds, dz, dy                          # the last correction (the solve itself at first)
     for _ in range(steps):
-        # the true residual K d + r of a regularised solution is (-reg dx, -reg ds, reg dz, reg dy)
-        a, b, c, g = one(-reg * dx, -reg * ds, reg * dz, reg * dy if e > 0 else None)
-        dx, ds, dz = dx + a, ds + b, dz + c
+        # With K = K~ - Delta, the true residual K d + r of d = d0 + c1 + ... + ck is -Delta ck (K~ d0 = -r,
+        # K~ cj = Delta c(j-1)): (-reg cx, -reg cs, reg cz, reg cy) of the LAST correction, not of the running total
+        cx, cs, cz, cy = one(-reg * cx, -reg * cs, reg * cz, reg * cy if e > 0 else None)
+        dx, ds, dz = dx + cx, ds + cs, dz + cz
         if e > 0:
-            dy = dy + g
+            dy = dy + cy
     return dx, ds, dz, dy
 
 

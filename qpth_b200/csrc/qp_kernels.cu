@@ -318,20 +318,31 @@ __device__ __forceinline__ void true_rx(const KDims& D, const Ctx& C, const doub
 }
 
 // One refinement step, with the factor still in the S workspace, of a solution of the regularised system: dv = [dy; dz],
-// ds, and dx~ = -base + ntx - W^T dv kept implicit. Against the true system that solution leaves the residual
-// (-eps dx, -eps ds, eps dz, eps dy); the correction solves the regularised system with it and is added in place
-// (ntx += eps L^-1 dx). V_D holds d + eps. a, c, e, f: scratch slots; destroys V_T0, V_T1, V_PART. Ends with a block
-// barrier.
+// ds, and dx~ = -base + ntx - W^T dv kept implicit. With K = K~ - Delta, the true residual of d = d0 + c1 + .. + ck is
+// -Delta ck = (-eps dx, -eps ds, eps dz, eps dy) of the LAST correction ck (of the solution d0 itself in the first step);
+// the next correction solves the regularised system with it and is added in place (ntx += eps L^-1 dx).
+// Between the steps of one solve c, e, f carry that correction: c = -eps L^-1 dx, e = eps ds, f = [dy; dz]; the first
+// step (first = true) reads the solution instead. V_D holds d + eps. a: scratch slot; destroys V_T0, V_T1, V_PART.
+// Ends with a block barrier.
 __device__ __forceinline__ void refine(const KDims& D, const Ctx& C, const double* base, double* ntx, double* dv,
-                                       double* ds, double* a, double* c, double* e, double* f, int tid, int nt) {
+                                       double* ds, double* a, double* c, double* e, double* f, bool first, int tid,
+                                       int nt) {
     const double* dd = VEC(V_D);
     double* t1 = VEC(V_T1); double* part = VEC(V_PART);
-    const int G = matvec_cols_partial(C.W, D.ldw, D.ms, D.n, dv, part, D.vl, tid, nt);
+    const int G = matvec_cols_partial(C.W, D.ldw, D.ms, D.n, first ? dv : f, part, D.vl, tid, nt);
     __syncthreads();
-    for (int i = tid; i < D.n; i += nt) {
-        double s = 0.0;
-        for (int g = 0; g < G; ++g) s += part[g * D.vl + i];
-        a[i] = ntx[i] - base[i] - s;                            // dx~
+    if (first) {
+        for (int i = tid; i < D.n; i += nt) {
+            double s = 0.0;
+            for (int g = 0; g < G; ++g) s += part[g * D.vl + i];
+            a[i] = ntx[i] - base[i] - s;                        // dx~ of the solution
+        }
+    } else {
+        for (int i = tid; i < D.n; i += nt) {
+            double s = 0.0;
+            for (int g = 0; g < G; ++g) s += part[g * D.vl + i];
+            a[i] = -c[i] - s;                                   // dx~ of the correction: eps L^-1 dx - W^T f
+        }
     }
     __syncthreads();
     unwhiten(D, C, a, t1, tid, nt);                             // T1 = dx
@@ -342,20 +353,45 @@ __device__ __forceinline__ void refine(const KDims& D, const Ctx& C, const doubl
         ntx[i] += r;
     }
     __syncthreads();
-    matvec_rows<false>(C.W, D.ldw, D.ms, D.n, c, nullptr, e, nullptr, tid, nt);
+    double* wt = first ? e : a;                                 // W t (e holds eps ds of the correction after the first)
+    matvec_rows<false>(C.W, D.ldw, D.ms, D.n, c, nullptr, wt, nullptr, tid, nt);
     __syncthreads();
     // reduced right-hand side -(W t - [r_y; r_z] + [0; r_s / (d + eps)])  (the elimination of solve_kkt)
-    for (int i = tid; i < D.ms; i += nt) {
-        double hf = fma(-D.reg, dv[i], e[i]);
-        if (i >= D.ep) hf -= D.reg * ds[i] / dd[i];
-        t1[i] = -hf;
+    if (first) {
+        for (int i = tid; i < D.ms; i += nt) {
+            double hf = fma(-D.reg, dv[i], e[i]);
+            if (i >= D.ep) hf -= D.reg * ds[i] / dd[i];
+            t1[i] = -hf;
+        }
+    } else {
+        for (int i = tid; i < D.ms; i += nt) {
+            double hf = fma(-D.reg, f[i], a[i]);
+            if (i >= D.ep) hf -= e[i] / dd[i];
+            t1[i] = -hf;
+        }
     }
     __syncthreads();
     solve_with_factor(D, C, f, tid, nt);                        // f = correction of [dy; dz]
-    for (int i = tid; i < D.ms; i += nt) {
-        const double wi = f[i];
-        if (i >= D.ep) ds[i] += (D.reg * ds[i] - wi) / dd[i];
-        dv[i] += wi;
+    if (first) {
+        for (int i = tid; i < D.ms; i += nt) {
+            const double wi = f[i];
+            if (i >= D.ep) {
+                const double dsc = (D.reg * ds[i] - wi) / dd[i];
+                ds[i] += dsc;
+                e[i] = D.reg * dsc;
+            }
+            dv[i] += wi;
+        }
+    } else {
+        for (int i = tid; i < D.ms; i += nt) {
+            const double wi = f[i];
+            if (i >= D.ep) {
+                const double dsc = (e[i] - wi) / dd[i];
+                ds[i] += dsc;
+                e[i] = D.reg * dsc;
+            }
+            dv[i] += wi;
+        }
     }
     __syncthreads();
 }
@@ -416,7 +452,7 @@ k_forward(KDims D, const double* __restrict__ p, int64_t sp, const double* __res
         for (int i = ep + tid; i < ms; i += nt) s[i] = -w[i] / d[i];
         for (int i = tid; i < n; i += nt) rv[i] = 0.0;
         __syncthreads();
-        for (int k = 0; k < ir_steps; ++k) refine(D, C, pt, rv, w, s, aug, hW, c2, dsa, tid, nt);
+        for (int k = 0; k < ir_steps; ++k) refine(D, C, pt, rv, w, s, aug, hW, c2, dsa, k == 0, tid, nt);
         for (int i = tid; i < n; i += nt) hW[i] = pt[i] - rv[i];   // (read after finish_dxt's first barrier)
     }
     issue_K<kSmem>(D, C, tid);
@@ -557,7 +593,7 @@ k_forward(KDims D, const double* __restrict__ p, int64_t sp, const double* __res
         if (refine_on) {
             // The refinement is linear in the right-hand side, so refining the combined direction equals refining the
             // affine and the corrector direction one by one; sigma above comes from the unrefined affine direction.
-            for (int k = 0; k < ir_steps; ++k) refine(D, C, rxt, rv, w, ds, aug, hW, c2, wc, tid, nt);
+            for (int k = 0; k < ir_steps; ++k) refine(D, C, rxt, rv, w, ds, aug, hW, c2, wc, k == 0, tid, nt);
             issue_K<kSmem>(D, C, tid);
             mn[0] = INFINITY; mn[1] = INFINITY;
             for (int i = ep + tid; i < ms; i += nt) {
@@ -662,7 +698,7 @@ k_solve_kkt(KDims D, const double* __restrict__ d_in, const double* __restrict__
         for (int i = ep + tid; i < ms; i += nt) dsr[i] = -w[i] / d[i];   // (rs = 0)
         for (int i = tid; i < n; i += nt) ntx[i] = 0.0;
         __syncthreads();
-        for (int k = 0; k < ir_steps; ++k) refine(D, C, t, ntx, w, dsr, aug, hW, VEC(V_C2), VEC(V_WC), tid, nt);
+        for (int k = 0; k < ir_steps; ++k) refine(D, C, t, ntx, w, dsr, aug, hW, VEC(V_C2), VEC(V_WC), k == 0, tid, nt);
         for (int i = tid; i < n; i += nt) t[i] -= ntx[i];       // (read after finish_dxt's first barrier)
     }
     finish_dxt(C.W, D.ldw, ms, n, w, t, dxt, part, D.vl, tid, nt);

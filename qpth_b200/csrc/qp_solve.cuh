@@ -253,15 +253,18 @@ __device__ __forceinline__ void f_true_rx(const KDims& D, const FCtx& C, int xt,
 }
 
 // One refinement step, with the factor still in the S workspace, of a solution of the regularised system: dv = [dy; dz],
-// ds, and dx~ = -base + ntx - W^T dv kept implicit. Against the true system that solution leaves the residual
-// (-eps dx, -eps ds, eps dz, eps dy); the correction solves the regularised system with it and is added in place
-// (ntx += eps L^-1 dx). F_D holds d + eps. a, b, c, e, f: scratch slots. Ends with a block barrier.
+// ds, and dx~ = -base + ntx - W^T dv kept implicit. With K = K~ - Delta, the true residual of d = d0 + c1 + .. + ck is
+// -Delta ck = (-eps dx, -eps ds, eps dz, eps dy) of the LAST correction ck (of the solution d0 itself in the first step);
+// the next correction solves the regularised system with it and is added in place (ntx += eps L^-1 dx).
+// Between the steps of one solve c, e, f carry that correction: c = -eps L^-1 dx, e = eps ds, f = [dy; dz]; the first
+// step (first = true) reads the solution instead. F_D holds d + eps. a, b: scratch slots. Ends with a block barrier.
 template <bool kCoop>
 __device__ __forceinline__ void f_refine(const KDims& D, const FCtx& C, int base, int ntx, int dv, int ds, int a, int b,
-                                         int c, int e, int f) {
+                                         int c, int e, int f, bool first) {
     QPB_SMEM;
     const int tid = threadIdx.x, dd = FV(F_D);
-    mv_cols<kCoop>(D, C, dv, e, f, a, base, -1.0, ntx, -1.0);  // a = dx~
+    if (first) mv_cols<kCoop>(D, C, dv, e, f, a, base, -1.0, ntx, -1.0);   // a = dx~ of the solution
+    else mv_cols<kCoop>(D, C, f, a, b, a, c, -1.0, -1, -1.0);             // a = dx~ of the correction: eps L^-1 dx - W^T f
     f_unwhiten_x(D, C, a, b);                                // b = dx
     f_whiten_x(D, C, b, c);                                  // c = L^-1 dx
     _Pragma("unroll 1") for (int i = tid; i < D.n; i += kNT) {
@@ -270,23 +273,51 @@ __device__ __forceinline__ void f_refine(const KDims& D, const FCtx& C, int base
         qsm[ntx + i] += r;
     }
     __syncthreads();
-    mv_rows1<kCoop>(D, C, c, e);
+    const int wt = first ? e : b;                            // W t (e holds eps ds of the correction after the first)
+    mv_rows1<kCoop>(D, C, c, wt);
     __syncthreads();
     // reduced right-hand side -(W t - [r_y; r_z] + [0; r_s / (d + eps)])  (the elimination of solve_kkt)
-    _Pragma("unroll 1") for (int i = tid; i < D.msp; i += kNT) {
-        double hf = 0.0;
-        if (i < D.ms) {
-            hf = fma(-D.reg, qsm[dv + i], qsm[e + i]);
-            if (i >= D.ep) hf -= D.reg * qsm[ds + i] / qsm[dd + i];
+    if (first) {
+        _Pragma("unroll 1") for (int i = tid; i < D.msp; i += kNT) {
+            double hf = 0.0;
+            if (i < D.ms) {
+                hf = fma(-D.reg, qsm[dv + i], qsm[e + i]);
+                if (i >= D.ep) hf -= D.reg * qsm[ds + i] / qsm[dd + i];
+            }
+            qsm[a + i] = -hf;
         }
-        qsm[a + i] = -hf;
+    } else {
+        _Pragma("unroll 1") for (int i = tid; i < D.msp; i += kNT) {
+            double hf = 0.0;
+            if (i < D.ms) {
+                hf = fma(-D.reg, qsm[f + i], qsm[b + i]);
+                if (i >= D.ep) hf -= qsm[e + i] / qsm[dd + i];
+            }
+            qsm[a + i] = -hf;
+        }
     }
     __syncthreads();
     qpb::pf::pf_solve(C.L.LS, D.msp, a, b, f);              // f = correction of [dy; dz]
-    _Pragma("unroll 1") for (int i = tid; i < D.ms; i += kNT) {
-        const double wi = qsm[f + i];
-        if (i >= D.ep) qsm[ds + i] += (D.reg * qsm[ds + i] - wi) / qsm[dd + i];
-        qsm[dv + i] += wi;
+    if (first) {
+        _Pragma("unroll 1") for (int i = tid; i < D.ms; i += kNT) {
+            const double wi = qsm[f + i];
+            if (i >= D.ep) {
+                const double dsc = (D.reg * qsm[ds + i] - wi) / qsm[dd + i];
+                qsm[ds + i] += dsc;
+                qsm[e + i] = D.reg * dsc;
+            }
+            qsm[dv + i] += wi;
+        }
+    } else {
+        _Pragma("unroll 1") for (int i = tid; i < D.ms; i += kNT) {
+            const double wi = qsm[f + i];
+            if (i >= D.ep) {
+                const double dsc = (qsm[e + i] - wi) / qsm[dd + i];
+                qsm[ds + i] += dsc;
+                qsm[e + i] = D.reg * dsc;
+            }
+            qsm[dv + i] += wi;
+        }
     }
     __syncthreads();
 }
@@ -365,7 +396,7 @@ k_forward_fast(KDims D, const double* __restrict__ p, int64_t sp, const double* 
         _Pragma("unroll 1") for (int i = ep + tid; i < ms; i += kNT) qsm[s + i] = -qsm[w + i] / qsm[d + i];
         _Pragma("unroll 1") for (int i = tid; i < n; i += kNT) qsm[rv + i] = 0.0;
         __syncthreads();
-        _Pragma("unroll 1") for (int k = 0; k < ir_steps; ++k) f_refine<kCoop>(D, C, pt, rv, w, s, t1, t0, aug, hW, dsa);
+        _Pragma("unroll 1") for (int k = 0; k < ir_steps; ++k) f_refine<kCoop>(D, C, pt, rv, w, s, t1, t0, aug, hW, dsa, k == 0);
     }
     f_issue_K(D, C);
     mv_cols<kCoop>(D, C, w, t0, t1, xt, pt, -1.0, refine ? rv : -1, -1.0);   // x~ = -p~ - W^T w
@@ -508,7 +539,7 @@ k_forward_fast(KDims D, const double* __restrict__ p, int64_t sp, const double* 
             // affine and the corrector direction one by one; sigma above comes from the unrefined affine direction.
             _Pragma("unroll 1") for (int i = tid; i < n; i += kNT) qsm[rv + i] = 0.0;
             __syncthreads();
-            _Pragma("unroll 1") for (int k = 0; k < ir_steps; ++k) f_refine<kCoop>(D, C, rxt, rv, w, ds, t1, t0, aug, hW, dsa);
+            _Pragma("unroll 1") for (int k = 0; k < ir_steps; ++k) f_refine<kCoop>(D, C, rxt, rv, w, ds, t1, t0, aug, hW, dsa, k == 0);
             f_issue_K(D, C);
             mn[0] = INFINITY; mn[1] = INFINITY;
             _Pragma("unroll 1") for (int i = ep + tid; i < ms; i += kNT) {
@@ -622,7 +653,7 @@ k_kkt_fast(KDims D, const double* __restrict__ d_in, const double* __restrict__ 
     if (kReg) {
         _Pragma("unroll 1") for (int i = ep + tid; i < ms; i += kNT) qsm[dsr + i] = -qsm[w + i] / qsm[d + i];   // ds (rs = 0)
         __syncthreads();
-        _Pragma("unroll 1") for (int k = 0; k < ir_steps; ++k) f_refine<kCoop>(D, C, t, ntx, w, dsr, aug, t0, t1, hW, c2);
+        _Pragma("unroll 1") for (int k = 0; k < ir_steps; ++k) f_refine<kCoop>(D, C, t, ntx, w, dsr, aug, t0, t1, hW, c2, k == 0);
     }
     mv_cols<kCoop>(D, C, w, t0, t1, dxt, t, -1.0, kReg ? ntx : -1, -1.0);
     if (kCoop && !C.lglobal) f_stage_L(D, C);                   // (mv_cols ended with a block barrier; no K copy in flight)
