@@ -69,10 +69,29 @@ KKT_B = 3
 KKT_VARIANTS = [(shared, reg) for shared in (False, True) for reg in (0.0, 1e-7)]
 TRAJ_B = 2
 TRAJ_RUNS = [(it, eps) for eps in (1e-12, 1e-6) for it in (1, 2, 3, 5, 20)]
+# the edge entries (up to order 1056, where one model solve takes seconds): eps = 1e-12 only (the 1e-6 runs repeat its
+# first iterations) and no un-batched variant (the index arithmetic of a shared system is that of the mid-range shapes)
+TRAJ_RUNS_EDGE = [(it, 1e-12) for it in (1, 2, 3, 5, 20)]
+
+
+def traj_runs(fam):
+    from tests.kernel_families import FAMILIES
+    return TRAJ_RUNS_EDGE if "edge" in FAMILIES[fam] else TRAJ_RUNS
+
+
+def traj_unbatched(fam, shape):
+    """[False] plus, for the first shape of a family that is not an edge entry, True (Q, G, A, h, b shared)."""
+    from tests.kernel_families import FAMILIES
+    f = FAMILIES[fam]
+    return [False] + ([True] if shape == f["shapes"][0] and "edge" not in f else [])
 
 
 def kkt_job_name(fam, shape, shared, reg):
     return "kkt_%s_%dx%dx%d_%s_%s" % ((fam,) + tuple(shape) + ("shared" if shared else "batched", "reg" if reg else "plain"))
+
+
+def bwd_job_name(fam, shape):
+    return "bwd_%s_%dx%dx%d" % ((fam,) + tuple(shape))
 
 
 def traj_job_name(fam, shape, unbatched, it, eps):
@@ -86,13 +105,18 @@ def family_kkt_jobs():
             for fam, s in cases(child=True) for shared, reg in KKT_VARIANTS]
 
 
+def family_backward_jobs():
+    from tests.kernel_families import cases
+    return [(bwd_job_name(fam, s), "call", ("backward_on_gpu", dict(fam=fam, shape=s)), {}, None)
+            for fam, s in cases(child=True)]
+
+
 def family_trajectory_jobs():
-    from tests.kernel_families import FAMILIES, cases
+    from tests.kernel_families import cases
     out = []
     for fam, s in cases(child=True, forward=True):
-        unb = [False] + ([True] if s == FAMILIES[fam]["shapes"][0] else [])
-        for u in unb:
-            for it, eps in TRAJ_RUNS:
+        for u in traj_unbatched(fam, s):
+            for it, eps in traj_runs(fam):
                 out.append((traj_job_name(fam, s, u, it, eps), "call",
                             ("trajectory_on_gpu", dict(fam=fam, shape=s, B=TRAJ_B, unbatched=u, maxIter=it, eps=eps)),
                             {}, None))

@@ -9,25 +9,15 @@ relative with the outer-product formulas (qp.py:157-176) applied to dx, dlam, dn
 """
 import numpy as np
 import pytest
-import torch
 
 from oracle import dense_kkt as dk
-from tests.kernel_families import cases, family_env, family_plan, ids, seed_for
+from tests import gpu_child
+from tests.fallback_jobs import bwd_job_name
+from tests.kernel_families import (BWD_B, GRAD_NAMES as NAMES, backward_on_gpu, backward_point, cases, family_env,
+                                   family_plan, ids, seed_for, solution_backward)
 from tests.parity import rel_rows
 
 pytestmark = pytest.mark.gpu
-DEV = "cuda:0"
-NAMES = ("dQ", "dp", "dG", "dh", "dA", "db")
-
-
-def _point(shape, B, seed):
-    from qpth_b200.problems import random_qp_batch
-    nz, nineq, neq = shape
-    pr = random_qp_batch(B, nz, nineq, neq, seed=seed)
-    rs = np.random.RandomState(seed + 1)
-    pr.update(z=rs.randn(B, nz), nu=rs.randn(B, neq), lam=rs.uniform(0.1, 10, (B, nineq)),
-              s=rs.uniform(0.1, 10, (B, nineq)))
-    return pr
 
 
 def _per_qp_reference(pr, i):
@@ -44,47 +34,39 @@ def _per_qp_reference(pr, i):
     return g
 
 
-def _backward(pr, batched, plan=None, monkeypatch=None):
-    """QPSolutionFunction + backward(dl). batched: {name: bool} for Q, p, G, h, A, b (un-batched inputs take QP 0's
-    value). plan: force this plan (a several-QPs-per-SM one) on pre_factor_kkt and the backward."""
-    from qpth_b200 import _lib
-    from qpth_b200.solution import QPSolutionFunction
-    if plan is not None:
-        monkeypatch.setattr(_lib, "plan_for", lambda *a, **k: plan)
-    neq = pr["A"].shape[1]
-    t = {}
-    for k in ("Q", "p", "G", "h", "A", "b"):
-        v = pr[k] if batched[k] else pr[k][0]
-        t[k] = torch.tensor(v, dtype=torch.float64, device=DEV, requires_grad=True) if (neq or k not in "Ab") \
-            else torch.Tensor().to(DEV).double()
-    sol = [torch.tensor(pr[k], dtype=torch.float64, device=DEV) for k in ("z", "lam", "s")]
-    nu = torch.tensor(pr["nu"], dtype=torch.float64, device=DEV) if neq else torch.Tensor().to(DEV).double()
-    z = QPSolutionFunction()(t["Q"], t["p"], t["G"], t["h"], t["A"], t["b"], sol[0], sol[1], sol[2], nu)
-    z.backward(torch.tensor(pr["dl"], dtype=torch.float64, device=DEV))
-    return {n: (t[k].grad.cpu().numpy() if t[k].grad is not None else None) for n, k in zip(NAMES, "QpGhAb")}
-
-
-ALL_BATCHED = dict(Q=True, p=True, G=True, h=True, A=True, b=True)
-
-
-@pytest.mark.parametrize("fam,shape", cases(), ids=ids(cases()))
-def test_backward_matches_dense_solve(fam, shape, monkeypatch):
+def check_backward(fam, shape, got):
     from tests.test_gpu_parity import _report
-    B = 4
-    pr = _point(shape, B, seed_for(fam, shape, 4))
-    with family_env(fam):
-        plan = family_plan(fam, shape)
-        got = _backward(pr, ALL_BATCHED, plan, monkeypatch)
-    refs = [_per_qp_reference(pr, i) for i in range(B)]
+    pr = backward_point(shape, BWD_B, seed_for(fam, shape, 4), fam)
+    refs = [_per_qp_reference(pr, i) for i in range(BWD_B)]
     worst = {}
     for n in NAMES:
         if n not in refs[0]:
-            assert got[n] is None, n
+            assert got.get(n) is None, n
             continue
         e = rel_rows(got[n], np.stack([r[n] for r in refs])).max()
         worst[n] = e
         assert e <= 1e-10, (n, e)
     _report("bwd[%s %s]" % (fam, shape), worst)
+
+
+@pytest.mark.parametrize("fam,shape", cases(child=False), ids=ids(cases(child=False)))
+def test_backward_matches_dense_solve(fam, shape):
+    check_backward(fam, shape, backward_on_gpu(fam, shape))
+
+
+@pytest.fixture(scope="module")
+def child_results(tmp_path_factory):
+    out_dir = str(tmp_path_factory.mktemp("backward_families"))
+    return out_dir, gpu_child.run(out_dir, "family_backward_jobs")
+
+
+@pytest.mark.parametrize("fam,shape", cases(child=True), ids=ids(cases(child=True)))
+def test_backward_matches_dense_solve_new_dispatch(fam, shape, child_results):
+    """The families whose dispatch branches had never run before these tests, and the edge entries: solved in the child
+    process."""
+    with family_env(fam):
+        family_plan(fam, shape)
+    check_backward(fam, shape, gpu_child.load(*child_results, bwd_job_name(fam, shape)))
 
 
 MEAN_SHARING = {
@@ -103,11 +85,11 @@ def test_batch_mean_of_unbatched_gradients(sharing):
     from tests.test_gpu_parity import _report
     B, shape = 37, (100, 100, 8)
     bat = MEAN_SHARING[sharing]
-    pr = _point(shape, B, 900)
+    pr = backward_point(shape, B, 900)
     for k, v in bat.items():             # un-batched inputs: every QP sees QP 0's value
         if not v:
             pr[k] = np.broadcast_to(pr[k][:1], pr[k].shape).copy()
-    got = _backward(pr, bat)
+    got = solution_backward(pr, bat)
     refs = [_per_qp_reference(pr, i) for i in range(B)]
     worst = {}
     for n, k in zip(NAMES, "QpGhAb"):

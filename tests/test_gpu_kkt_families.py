@@ -13,6 +13,11 @@ formulation and differ from the model only in FMA use and summation order, so th
 the same size, which varies ~10x from system to system. Each block is held to max(bound, 10 x the model's largest
 error on the batch's systems (for ds and for the other blocks separately): that leaves every well-conditioned shape at
 1e-10 / 1e-8.
+
+The normwise backward error is held to 1e-14, except on three edge entries of kernel_families.py (MODEL_BERR). They
+have fewer than 10 inequality rows next to hundreds of columns. With d over 16 decades, the formulation itself leaves a
+larger backward error there: the model's (measured) is 1.0e-10 at 213/8/0, 9.4e-13 at 880/1/128 and 3.7e-14 at
+740/1/0. On those three the bound is max(1e-14, 10 x the model's largest backward error on the batch's systems).
 """
 import numpy as np
 import pytest
@@ -26,6 +31,8 @@ from tests.kernel_families import cases, family_env, family_plan, ids, kkt_input
 pytestmark = pytest.mark.gpu
 
 BERR, XTOL, STOL = 1e-14, 1e-10, 1e-8
+# edge entries whose backward error is held to max(BERR, 10 x the model's) (module docstring); every other family to BERR
+MODEL_BERR = ("edge_gs_pf_res", "edge_512_wide", "edge_two_wide")
 
 
 def _report(name, errs):
@@ -37,20 +44,24 @@ def check_kkt(fam, shape, shared, reg, out):
     neq = shape[2]
     x = kkt_inputs(fam, shape, KKT_B, shared)
     assert int(np.asarray(out["spd"]).sum()) == 0
-    refs, merr = [], dict(x=0.0, s=0.0)          # the model's largest error: dx, dz, dy / ds
+    refs, merr = [], dict(x=0.0, s=0.0, b=0.0)   # the model's largest error: dx, dz, dy / ds / backward error
     for i in range(KKT_B):
         j = 0 if shared else i
         args = (x["Q"][j], x["G"][j], x["A"][j], x["d"][i], x["rx"][i], x["rs"][i], x["rz"][i], x["ry"][i] if neq else None)
         refs.append(dk.solve(*args, reg=reg))
-        for k, (a, b) in enumerate(zip(km.kkt_solve(*args, reg=reg), refs[-1][:4])):
+        m = km.kkt_solve(*args, reg=reg)
+        for k, (a, b) in enumerate(zip(m, refs[-1][:4])):
             if b is not None:
                 merr["s" if k == 1 else "x"] = max(merr["s" if k == 1 else "x"], dk.rel(a, b))
-    worst = dict(berr=0.0, dx=0.0, ds=0.0, dz=0.0, dy=0.0, model_x=merr["x"], model_s=merr["s"])
+        mu = np.concatenate([m[0], m[1], m[2]] + ([m[3]] if neq else []))
+        merr["b"] = max(merr["b"], dk.backward_error(refs[-1][4], mu, refs[-1][5]))
+    worst = dict(berr=0.0, dx=0.0, ds=0.0, dz=0.0, dy=0.0, model_x=merr["x"], model_s=merr["s"], model_berr=merr["b"])
     for i, ref in enumerate(refs):
         u = np.concatenate([out["dx"][i], out["ds"][i], out["dz"][i]] + ([out["dy"][i]] if neq else []))
         berr = dk.backward_error(ref[4], u, ref[5])
         worst["berr"] = max(worst["berr"], berr)
-        assert berr <= BERR, (i, berr)
+        tol_b = max(BERR, 10 * merr["b"]) if fam in MODEL_BERR else BERR
+        assert berr <= tol_b, (i, berr, tol_b)
         for k, name in enumerate(("dx", "ds", "dz", "dy")):
             if ref[k] is None:
                 continue

@@ -12,8 +12,12 @@ are inactive), IR_STEPS in {0, 1, 2, 3}:
 The model's own error (max over the four gradients, relative to their max-norm) at k = 0 / >= 1 is about 2e-7 / 1e-14
 on the SPD cases and 1e-7 / 1e-8 .. 2e-7 on the low-rank and LP cases: only the SPD cases can tell a refinement error at
 rounding level; on the others (chol(Q + eps I) ~ sqrt(eps) I on Q's null space) it must exceed the floor of ~1e-7.
+On the SPD cases of the four families the error from k = 1 on is held to 1e-12. On the SPD cases of the edge entries
+it is held to max(1e-12, 10 x the model's error at that k): some of them have many equality rows or a small A Q^-1 A'
+(for example 64 rows at nz = 97, or 129 rows at nz = 208). One step contracts less there, and the model's own error at k = 1 is up to 1.1e-11 (measured:
+9.6e-12 at 39/144/17, 7.8e-12 at 97/9/64, 3.8e-12 at 208/57/129, 1.1e-11 at 4/193/0). From k = 2 on it is below 1e-13.
 
-Forward trajectories: maxIter in {1, 2, 3, 5, 20}, eps in {1e-12, 1e-6}, IR_STEPS in {0, 1, 2}, qp.TRACE on:
+Forward trajectories (every family but the backward_only one of tests/reg_families.py): maxIter in {1, 2, 3, 5, 20}, eps in {1e-12, 1e-6}, IR_STEPS in {0, 1, 2}, qp.TRACE on:
   * each trace row [pri, dual, mu, resid] against reg_model.solve_one_reg(trace=...), row-relative l2 error within
     ROW_TOL[case] while the model's resid >= 1e-3, ROW_TOL[case] x 1e-3 / resid for 1e-6 <= resid < 1e-3, and
     unchecked below (the iterates sit at the rounding floor there);
@@ -48,6 +52,15 @@ MODEL_SPREAD = {
     ("global_scratch", "spd"): (9.7e-11, 4.5e-10),
     ("global_scratch", "lowrank"): (5.7e-7, 7.6e-7),
     ("global_scratch", "lp"): (7.2e-7, 5.1e-7),
+    ("edge_pf_res_full", "spd"): (2.8e-13, 3.0e-12),
+    ("edge_pf_res_full", "lp"): (8.3e-6, 1.3e-5),
+    ("edge_pf_res_order", "spd"): (9.9e-12, 6.1e-12),
+    ("edge_pf_res_order", "lp"): (7.9e-5, 3.8e-5),
+    ("edge_gs_pf_res", "spd"): (1.3e-12, 2.8e-12),
+    ("edge_sf_pf_res", "spd"): (3.5e-12, 4.2e-12),
+    ("edge_l2_full", "spd"): (2.0e-12, 4.1e-12),
+    ("edge_l2_order", "spd"): (2.5e-12, 4.0e-12),
+    ("edge_l2_wide", "spd"): (2.1e-12, 9.7e-12),
 }
 
 
@@ -117,32 +130,41 @@ def test_backward_at_chosen_point(case, monkeypatch):
     neq = cases[0][4].shape[0]
     pts = [_point(c, i) for i, c in enumerate(cases)]
     dense = [_dense_grads(c, pt[0], pt[1], pt[2], pt[3], pt[4]) for c, pt in zip(cases, pts)]
-    errs = []
+    errs, model_errs, worst = [], [], dict(model=0.0)
     for steps in range(4):
         monkeypatch.setattr(kkt, "IR_STEPS", steps)
         g = _backward_on_gpu(cases, pts, shared=False)
         assert set(g) == {"dQ", "dp", "dG", "dh"} | ({"dA", "db"} if neq else set())
-        err = 0.0
+        err = merr = 0.0
         for i, (c, pt) in enumerate(zip(cases, pts)):
             gm = _model_grads(c, *pt, steps, kkt.IR_EPS)
             model_err = max(_rel(gm[k], dense[i][k]) for k in dense[i])
+            merr = max(merr, model_err)
             tol = max(1e-12, 10 * model_err)
             for k in g:
                 assert _rel(g[k][i], gm[k]) <= tol, (steps, i, k, _rel(g[k][i], gm[k]), tol)
             for k in dense[i]:
                 assert _rel(g[k][i], dense[i][k]) <= tol, (steps, i, k, _rel(g[k][i], dense[i][k]), tol)
             err = max(err, max(_rel(g[k][i], dense[i][k]) for k in dense[i]))
+            worst["model"] = max(worst["model"], max(_rel(g[k][i], gm[k]) for k in g))
         errs.append(err)
+        model_errs.append(merr)
+    _report("reg_bwd[%s %s]" % case, dict(worst, **{"dense_k%d" % k: e for k, e in enumerate(errs)}))
     for k in range(3):
         assert errs[k + 1] <= 2 * errs[k] + 1e-13, errs
-    if kind == "spd":
+    if kind == "spd" and "pair" not in FAMILIES[fam]:
         assert max(errs[1:]) <= 1e-12 < errs[0], errs
+    elif kind == "spd":                    # edge entries: the bound the model's own error allows (module docstring)
+        assert errs[0] > 1e-12, errs
+        for k in range(1, 4):
+            assert errs[k] <= max(1e-12, 10 * model_errs[k]), (k, errs, model_errs)
 
 
 @pytest.mark.parametrize("fam", list(FAMILIES))
 def test_backward_shared_inputs_mean(fam, monkeypatch):
     """Q, G, h, A, b shared and p batched (B = 3), IR_STEPS = 2: the shared inputs get the batch mean of the per-QP
-    gradients of the model."""
+    gradients of the model, within 1e-12. Edge entries: within max(1e-12, 10 x the model's error against the dense solve),
+    the bound of test_backward_at_chosen_point (at order 1056 the refinement contracts slowly, reg_families.py)."""
     _, _, _, kkt, _ = _qpth()
     monkeypatch.setattr(kkt, "IR_STEPS", 2)
     base = problem(fam, "spd", 0)
@@ -152,9 +174,14 @@ def test_backward_shared_inputs_mean(fam, monkeypatch):
     pts = [_point(base, i) for i in range(3)]
     g = _backward_on_gpu(cases, pts, shared=True)
     per = [_model_grads(c, *pt, 2, kkt.IR_EPS) for c, pt in zip(cases, pts)]
+    tol = 1e-12
+    if "pair" in FAMILIES[fam]:
+        for c, pt, gm in zip(cases, pts, per):
+            dense = _dense_grads(c, *pt)
+            tol = max(tol, 10 * max(_rel(gm[k], dense[k]) for k in dense))
     for k in g:
         want = np.stack([q[k] for q in per]) if k == "dp" else np.mean([q[k] for q in per], 0)
-        assert _rel(g[k], want) <= 1e-12, (k, _rel(g[k], want))
+        assert _rel(g[k], want) <= tol, (k, _rel(g[k], want), tol)
 
 
 def _forward_on_gpu(cases, shared, **opts):
@@ -173,8 +200,14 @@ def _forward_on_gpu(cases, shared, **opts):
             st.iters.cpu().numpy(), st.best_resid.cpu().numpy(), st.trace.cpu().numpy())
 
 
-def _check_forward(case, cases, out, maxIter, eps, steps, reg):
+def _report(name, errs):
+    from tests.test_gpu_parity import _report as rep
+    rep(name, errs)
+
+
+def _check_forward(case, cases, out, maxIter, eps, steps, reg, worst=None):
     from qpth_b200.qp import BEST_TIE, STALL_TOL
+    worst = {} if worst is None else worst
     z, lam, s, nu, iters, best, trace = out
     for i, (Q, p, G, h, A, b) in enumerate(cases):
         tr = []
@@ -185,12 +218,15 @@ def _check_forward(case, cases, out, maxIter, eps, steps, reg):
         for it in range(k):
             tol = _row_tol(case, tr[it, 3])
             err = np.linalg.norm(trace[i, it] - tr[it]) / np.linalg.norm(tr[it])
+            if tr[it, 3] >= 1e-3:
+                worst["trace"] = max(worst.get("trace", 0.0), err)
             assert err <= tol, (i, it, err, tol, trace[i, it], tr[it])
         assert best[i] == np.nanmin(trace[i, :int(iters[i]), 3])
         if maxIter < 20:
             assert int(iters[i]) == m["iters"], (i, int(iters[i]), m["iters"])
             tol = _row_tol(case, tr[m["best_iter"], 3])
             if np.isfinite(tol):
+                worst["iterate"] = max(worst.get("iterate", 0.0), _rel(z[i], m["x"]))
                 assert _rel(z[i], m["x"]) <= tol
                 assert _rel(lam[i], m["lam"]) <= tol
                 assert _rel(s[i], m["s"]) <= tol
@@ -201,22 +237,28 @@ def _check_forward(case, cases, out, maxIter, eps, steps, reg):
             assert best[i] <= max(1e-9, 10 * m["best_resid"]), (i, best[i], m["best_resid"])
 
 
-@pytest.mark.parametrize("case", CASES, ids=ids(CASES))
+FWD_CASES = [c for c in CASES if not FAMILIES[c[0]].get("backward_only")]
+FWD_FAMILIES = [f for f in FAMILIES if not FAMILIES[f].get("backward_only")]
+
+
+@pytest.mark.parametrize("case", FWD_CASES, ids=ids(FWD_CASES))
 def test_forward_trajectory(case, monkeypatch):
     _, _, _, kkt, qp = _qpth()
     fam, kind = case
     monkeypatch.setattr(qp, "TRACE", True)
     cases = [problem(fam, kind, s) for s in range(B)]
     family_plan(fam, cases[0])
+    worst = {}
     for steps in (0, 1, 2):
         monkeypatch.setattr(kkt, "IR_STEPS", steps)
         for eps in (1e-12, 1e-6):
             for maxIter in (1, 2, 3, 5, 20):
                 out = _forward_on_gpu(cases, False, eps=eps, maxIter=maxIter)
-                _check_forward(case, cases, out, maxIter, eps, steps, kkt.IR_EPS)
+                _check_forward(case, cases, out, maxIter, eps, steps, kkt.IR_EPS, worst)
+    _report("reg_traj[%s %s]" % case, worst)
 
 
-@pytest.mark.parametrize("fam", list(FAMILIES))
+@pytest.mark.parametrize("fam", FWD_FAMILIES)
 def test_forward_trajectory_shared_inputs(fam, monkeypatch):
     """Q, G, h, A, b shared (one system for the batch), p batched, IR_STEPS = 2, truncated at 3 iterations."""
     _, _, _, kkt, qp = _qpth()

@@ -3,7 +3,7 @@ checked against the dense KKT solve and the reference in tests/test_oracle.py).
 
 A converged z* hides a wrong step: the iteration corrects itself and only takes longer. Below convergence it cannot.
 For maxIter in {1, 2, 3, 5, 20} and eps in {1e-12, 1e-6}, on well-conditioned random_qp_batch shapes, and once per family
-with Q, G, A, h, b shared by the batch:
+with Q, G, A, h, b shared by the batch (the edge entries: wellcond_qp_batch, eps = 1e-12 only, batched only):
   * every trace row [||rz|| + ||ry||, ||L r~x||, mu, resid] against the model's, row-relative l2 error <= 1e-9 while the
     model's resid >= 1e-3. Below that the iterates sit close to the rounding floor: a 1e-15 relative perturbation of p
     and h moves the model's own rows by up to 1.5e-8 at resid ~1e-6 and 1e-3 at resid ~1e-9 (measured at these
@@ -17,20 +17,15 @@ import pytest
 
 from oracle import kernel_model as km
 from tests import gpu_child
-from tests.fallback_jobs import TRAJ_B, TRAJ_RUNS, traj_job_name
-from tests.kernel_families import FAMILIES, cases, family_env, family_plan, trajectory_on_gpu, trajectory_problem
+from tests.fallback_jobs import TRAJ_B, traj_job_name, traj_runs, traj_unbatched
+from tests.kernel_families import cases, family_env, family_plan, trajectory_on_gpu, trajectory_problem
 from tests.parity import rel_rows
 
 pytestmark = pytest.mark.gpu
 
 
 def _variants(child):
-    out = []
-    for fam, s in cases(child=child, forward=True):
-        out.append((fam, s, False))
-        if s == FAMILIES[fam]["shapes"][0]:
-            out.append((fam, s, True))
-    return out
+    return [(fam, s, u) for fam, s in cases(child=child, forward=True) for u in traj_unbatched(fam, s)]
 
 
 def _ids(vs):
@@ -89,7 +84,7 @@ def check_run(fam, shape, unbatched, maxIter, eps, out, worst):
 def _check_all(fam, shape, unbatched, get):
     from tests.test_gpu_parity import _report
     worst = dict(trace=0.0, iterate=0.0)
-    for maxIter, eps in TRAJ_RUNS:
+    for maxIter, eps in traj_runs(fam):
         check_run(fam, shape, unbatched, maxIter, eps, get(maxIter, eps), worst)
     _report("traj[%s %s%s]" % (fam, shape, " unbatched" if unbatched else ""), worst)
 

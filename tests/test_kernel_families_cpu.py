@@ -19,8 +19,9 @@ def test_family_shapes_plan_to_their_family(fam, shape, lib):
         family_plan(fam, shape)
 
 
-@pytest.mark.parametrize("fam", sorted(FAMILIES))
+@pytest.mark.parametrize("fam", sorted(f for f in FAMILIES if "edge" not in FAMILIES[f]))
 def test_family_shapes_cover_padding_edges(fam):
+    """(The edge entries are single shapes chosen by the planner's limits; tests/test_plan_edges_cpu.py checks them.)"""
     shapes = FAMILIES[fam]["shapes"]
     assert len(shapes) >= 2
     assert any(nz % 2 for nz, _, _ in shapes)
