@@ -10,8 +10,10 @@
 //
 // Three layouts run this solver, all with 128-thread CTAs:
 //   one CTA per QP (family OneCta): A (neq x nz, row stride nz | 1), the factor of M and every vector live in shared
-//            memory. neq_pad <= 128 (the substitutions own one row per thread) and a footprint within the 227 KB an
-//            H100 CTA may use (qpb200_box_plan.ok).
+//            memory, within the 227 KB an H100 CTA may use, and neq_pad <= 128: the substitutions own one row per
+//            thread (qpb200_box_plan.ok needs both). For neq <= nz (A of full row rank) shared memory binds first: the
+//            most such a CTA holds is neq_pad 120 ((121, 117, both), 128 B left). For neq > nz the 128-row term is the
+//            one that decides: (8, 136, lb) fits in 114 KB and is rejected by it alone.
 //   a cluster per QP (family Cluster): past that, a thread block cluster of 2, 4 or 8 CTAs (qpb200_box_plan.cl_ctas),
 //            each CTA holding a slice of the variables; M is summed and factored redundantly in every CTA.
 //   distributed M (k_box_*_dm): past neq_pad = 128, M is distributed over the cluster as well and A is read from
