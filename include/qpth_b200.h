@@ -136,6 +136,23 @@ int qpb200_backward(const qpb200_plan* plan, int nbatch,
                     double* dxv, double* dlamv, double* dnuv,
                     double* scratch, void* stream);
 
+/* qpb200_backward for a loss that also depends on the returned duals (an extension: the reference returns only zhat).
+ * dl_dlam (B,nineq) and dl_dnu (B,neq) are the gradients of the loss with respect to lam and nus; either may be NULL
+ * (zero), and dl_dnu must be NULL when neq == 0. They enter the right-hand side of the backward solve,
+ *   [Q 0 G' A'; 0 D I 0; G I 0 0; A 0 0 0] [dx ds dlam dnu] = -[dl_dzhat; 0; dl_dlam; dl_dnu],   D = lam / s (clamped),
+ * the row-scaled implicit derivative of Qz + p + G'lam + A'nu = 0, diag(lam)(Gz - h) = 0, Az = b at the returned
+ * point. The gradients are the outer products of qpb200_backward applied to this dx, dlam, dnu. qpb200_backward is
+ * this call with both NULL. */
+int qpb200_backward_duals(const qpb200_plan* plan, int nbatch,
+                          const double* dl_dzhat, const double* dl_dlam, const double* dl_dnu,
+                          const double* zhat, const double* lam, const double* slacks, const double* nus,
+                          const double* Lfac, const double* Wfac, const double* Kfac, int sF,
+                          double* dQ, int mean_Q, double* dp, int mean_p,
+                          double* dG, int mean_G, double* dh, int mean_h,
+                          double* dA, int mean_A, double* db, int mean_b,
+                          double* dxv, double* dlamv, double* dnuv,
+                          double* scratch, void* stream);
+
 /* factor_kkt + solve_kkt (batch.py:435-470, 349-372) for caller-supplied d and
  * right-hand sides: one call = LU/Cholesky of R + D^-1 and one reduced KKT solve.
  * Used by the parity tests of rows a8/a9; not needed by QPFunction itself.
@@ -205,6 +222,19 @@ int qpb200_backward_reg(const qpb200_plan* plan, int nbatch,
                         double* dA, int mean_A, double* db, int mean_b,
                         double* dxv, double* dlamv, double* dnuv,
                         double* scratch, void* stream);
+/* qpb200_backward_reg with the adjoints of the duals, as qpb200_backward_duals (the refinement steps are unchanged: each
+ * works from the residual of the last correction, whatever the right-hand side). With linearly dependent equality rows
+ * nus is not unique, and the gradient through it belongs to the nus returned. */
+int qpb200_backward_reg_duals(const qpb200_plan* plan, int nbatch,
+                              const double* dl_dzhat, const double* dl_dlam, const double* dl_dnu,
+                              const double* zhat, const double* lam, const double* slacks, const double* nus,
+                              const double* Lfac, const double* Wfac, const double* Kfac, int sF,
+                              double reg_eps, int ir_steps,
+                              double* dQ, int mean_Q, double* dp, int mean_p,
+                              double* dG, int mean_G, double* dh, int mean_h,
+                              double* dA, int mean_A, double* db, int mean_b,
+                              double* dxv, double* dlamv, double* dnuv,
+                              double* scratch, void* stream);
 
 /* ---- Box QPs (qpth_b200/box.py BoxQPFunction): min 1/2 z' diag(q) z + p'z  s.t.  A z = b,  lb <= z <= ub -------------
  * The dense equivalent is Q = diag(q), G = [-I; I] (only the sides given: lb rows first), h = [-lb; ub]; lam and slacks
@@ -249,6 +279,14 @@ int qpb200_box_backward(const qpb200_box_plan* plan, int nbatch, const double* q
                         const double* nus, double* dq, int mean_q, double* dp, int mean_p, double* dlb, int mean_lb,
                         double* dub, int mean_ub, double* dA, int mean_A, double* db, int mean_b, double* dxv,
                         double* dlamv, double* dnuv, void* stream);
+/* qpb200_box_backward with the adjoints of the duals, as qpb200_backward_duals: dl_dlam (B,nineq) in the [lb rows; ub
+ * rows] layout of lam, dl_dnu (B,neq); either may be NULL (zero), dl_dnu must be NULL when neq == 0. */
+int qpb200_box_backward_duals(const qpb200_box_plan* plan, int nbatch, const double* q, int64_t sq, const double* A,
+                              int64_t sA, const double* dl_dzhat, const double* dl_dlam, const double* dl_dnu,
+                              const double* zhat, const double* lam, const double* slacks, const double* nus, double* dq,
+                              int mean_q, double* dp, int mean_p, double* dlb, int mean_lb, double* dub, int mean_ub,
+                              double* dA, int mean_A, double* db, int mean_b, double* dxv, double* dlamv, double* dnuv,
+                              void* stream);
 
 /* The structured factor and solve for caller-supplied d (B,nineq) and right-hand sides (the counterpart of
  * qpb200_solve_kkt):  [diag(q) 0 G' A'; 0 D I 0; G I 0 0; A 0 0 0] [dx ds dz dy] = -[rx rs rz ry].

@@ -54,6 +54,8 @@ SIGNATURES = {
                             _D, _D, _D, _I, _I, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     "qpb200_backward": (_I, [ctypes.POINTER(Plan), _I, _P, _P, _P, _P, _P, _P, _P, _P, _I,
                              _P, _I, _P, _I, _P, _I, _P, _I, _P, _I, _P, _I, _P, _P, _P, _P, _P]),
+    "qpb200_backward_duals": (_I, [ctypes.POINTER(Plan), _I, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _I,
+                                   _P, _I, _P, _I, _P, _I, _P, _I, _P, _I, _P, _I, _P, _P, _P, _P, _P]),
     "qpb200_solve_kkt": (_I, [ctypes.POINTER(Plan), _I, _P, _P, _P, _P, _P, _P, _P, _P, _I,
                               _P, _P, _P, _P, _P, _P]),
     "qpb200_pre_factor_kkt_reg": (_I, [ctypes.POINTER(Plan), _I, _P, _L, _P, _L, _P, _L, _D, _P, _P, _P, _P, _P, _P]),
@@ -64,6 +66,8 @@ SIGNATURES = {
                                 _D, _D, _D, _I, _I, _D, _I, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     "qpb200_backward_reg": (_I, [ctypes.POINTER(Plan), _I, _P, _P, _P, _P, _P, _P, _P, _P, _I, _D, _I,
                                  _P, _I, _P, _I, _P, _I, _P, _I, _P, _I, _P, _I, _P, _P, _P, _P, _P]),
+    "qpb200_backward_reg_duals": (_I, [ctypes.POINTER(Plan), _I, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _I, _D, _I,
+                                       _P, _I, _P, _I, _P, _I, _P, _I, _P, _I, _P, _I, _P, _P, _P, _P, _P]),
     "qpb200_optnet_construct": (_I, [_I, _I, _P, _P, _P, _P, _D, _P, _P, _P]),
     "qpb200_optnet_chain": (_I, [_I, _I, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     "qpb200_dfma_probe": (_I, [_I, _I, _I, _P, _P]),
@@ -75,6 +79,8 @@ SIGNATURES = {
                                 _D, _D, _D, _I, _I, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     "qpb200_box_backward": (_I, [ctypes.POINTER(BoxPlan), _I, _P, _L, _P, _L, _P, _P, _P, _P, _P,
                                  _P, _I, _P, _I, _P, _I, _P, _I, _P, _I, _P, _I, _P, _P, _P, _P]),
+    "qpb200_box_backward_duals": (_I, [ctypes.POINTER(BoxPlan), _I, _P, _L, _P, _L, _P, _P, _P, _P, _P, _P, _P,
+                                       _P, _I, _P, _I, _P, _I, _P, _I, _P, _I, _P, _I, _P, _P, _P, _P]),
     "qpb200_box_solve_kkt": (_I, [ctypes.POINTER(BoxPlan), _I, _P, _L, _P, _L, _P, _P, _P, _P, _P,
                                   _P, _P, _P, _P, _P]),
 }

@@ -114,8 +114,9 @@ def solve_box_forward(q_, p_, A_, b_, lb_, ub_, eps=1e-12, verbose=0, notImprove
     return st
 
 
-def solve_box_backward(st, dl_dzhat, mean_flags, want):
-    """Gradients (dq, dp, dA, db, dlb, dub) on the device; mean_flags / want: 6-tuples in that order."""
+def solve_box_backward(st, dl_dzhat, mean_flags, want, dl_dlam=None, dl_dnu=None):
+    """Gradients (dq, dp, dA, db, dlb, dub) on the device; mean_flags / want: 6-tuples in that order. dl_dlam ([lb rows;
+    ub rows]) / dl_dnu: the gradients with respect to the returned duals (None: zero); dl_dzhat None: zero."""
     if _qp._pending:
         _qp.flush_checks(wait=False)
     lib = _lib.load()
@@ -123,7 +124,8 @@ def solve_box_backward(st, dl_dzhat, mean_flags, want):
     nz, neq, m = plan.nz, plan.neq, plan.nineq
     f64 = dict(dtype=torch.float64, device=device)
     with torch.cuda.device(device):
-        dl = dl_dzhat.detach().to(device=device, dtype=torch.float64).contiguous().view(B, nz)
+        dl = _qp._adjoint(dl_dzhat, B, nz, device) if dl_dzhat is not None else torch.zeros(B, nz, **f64)
+        glam, gnu = _qp._adjoint(dl_dlam, B, m, device), _qp._adjoint(dl_dnu, B, neq, device)
         shapes = [(nz,), (nz,), (neq, nz), (neq,), (nz,), (nz,)]
         outs = []
         for k in range(6):
@@ -137,8 +139,12 @@ def solve_box_backward(st, dl_dzhat, mean_flags, want):
         dnuv = torch.empty(B, neq, **f64) if neq > 0 else None
         dq, dp, dA, db, dlb, dub = outs
         mq, mp, mA, mb, mlb, mub = (1 if f else 0 for f in mean_flags)
-        _lib.check(lib.qpb200_box_backward(
-            ctypes.byref(plan), B, _ptr(st.q), st.sq, _ptr(st.A), st.sA, _ptr(dl), _ptr(st.zhat), _ptr(st.lam),
+        if glam is None and gnu is None:            # no dual was used: the entry point of a zhat-only loss
+            fn, adj = lib.qpb200_box_backward, ()
+        else:
+            fn, adj = lib.qpb200_box_backward_duals, (_ptr(glam), _ptr(gnu))
+        _lib.check(fn(
+            ctypes.byref(plan), B, _ptr(st.q), st.sq, _ptr(st.A), st.sA, _ptr(dl), *adj, _ptr(st.zhat), _ptr(st.lam),
             _ptr(st.slacks), _ptr(st.nus), _ptr(dq), mq, _ptr(dp), mp, _ptr(dlb), mlb, _ptr(dub), mub,
             _ptr(dA), mA, _ptr(db), mb, _ptr(dxv), _ptr(dlamv), _ptr(dnuv), _stream()))
     return outs
@@ -176,11 +182,12 @@ def solve_dense_forward(q_, p_, A_, b_, lb_, ub_, eps, verbose, notImprovedLim, 
     return st
 
 
-def dense_backward(st, dl, mean_flags, want, nlb, has_ub):
+def dense_backward(st, dl, mean_flags, want, nlb, has_ub, dl_dlam=None, dl_dnu=None):
     dst, h_shared = st.dense
     mq, mp, mA, mb, mlb, mub = mean_flags
+    # the dense equivalent's rows are lam's [lb rows; ub rows]: the dual adjoints pass through as they are
     outs = _qp.solve_backward(dst, dl, (mq, mp, True, h_shared, mA, mb),
-                              (want[0], want[1], False, want[4] or want[5], want[2], want[3]))
+                              (want[0], want[1], False, want[4] or want[5], want[2], want[3]), dl_dlam, dl_dnu)
     dQ, dp, _, dh, dA, db = outs
     dq = None if dQ is None else torch.diagonal(dQ, dim1=-2, dim2=-1).contiguous()
     dlb = dub = None
@@ -194,12 +201,15 @@ def dense_backward(st, dl, mean_flags, want, nlb, has_ub):
     return [dq, dp, dA, db, dlb, dub]
 
 
-def BoxQPFunction(eps=1e-12, verbose=0, notImprovedLim=3, maxIter=20, check_Q_spd=True):
+def BoxQPFunction(eps=1e-12, verbose=0, notImprovedLim=3, maxIter=20, check_Q_spd=True, duals=False):
     """Factory with QPFunction's options; returns f(q, p, A, b, lb, ub) -> z (nBatch, nz).
 
     q, p, lb, ub: (nBatch, nz) or (nz); A: (nBatch, neq, nz), (neq, nz) or an empty tensor; b follows A. lb or ub may
     be None (no bound on that side), not both. f.last_solve() returns the state of the last forward: lam, slacks
-    ([lb rows; ub rows]), nus, iters, best_resid."""
+    ([lb rows; ub rows]), nus, iters, best_resid.
+
+    duals=True: f returns (z, lam, nu) as QPFunction(duals=True) does: lam (nBatch, nineq) in the [lb rows; ub rows]
+    layout of last_solve(), nu (nBatch, neq) or (nBatch, 0), and a loss may use all three."""
     _last = [None]
 
     class BoxQPFunctionFn(Function):
@@ -213,10 +223,13 @@ def BoxQPFunction(eps=1e-12, verbose=0, notImprovedLim=3, maxIter=20, check_Q_sp
             zhats = st.zhat.to(device=q_.device, dtype=q_.dtype)
             ctx.save_for_backward(zhats, q_, p_, A_, b_, lb_, ub_)
             ctx.lams, ctx.slacks, ctx.nus = st.lam, st.slacks, st.nus
-            return zhats
+            if not duals:
+                return zhats
+            ctx.set_materialize_grads(False)
+            return (zhats,) + _qp.dual_outputs(st, q_)
 
         @staticmethod
-        def backward(ctx, dl_dzhat):
+        def backward(ctx, dl_dzhat, dl_dlam=None, dl_dnu=None):
             zhats, q, p, A, b, lb, ub = ctx.saved_tensors
             st = ctx.st
             ins = (q, p, A, b, lb, ub)
@@ -224,9 +237,10 @@ def BoxQPFunction(eps=1e-12, verbose=0, notImprovedLim=3, maxIter=20, check_Q_sp
             flags = [X is not None and X.nelement() > 0 and X.dim() == r - 1 for X, r in zip(ins, ranks)]
             want = list(ctx.needs_input_grad)
             if st.dense is None:
-                outs = solve_box_backward(st, dl_dzhat, flags, want)
+                outs = solve_box_backward(st, dl_dzhat, flags, want, dl_dlam, dl_dnu)
             else:
-                outs = dense_backward(st, dl_dzhat, flags, want, q.size(-1) if lb is not None else 0, ub is not None)
+                outs = dense_backward(st, dl_dzhat, flags, want, q.size(-1) if lb is not None else 0, ub is not None,
+                                      dl_dlam, dl_dnu)
             return tuple(None if (g is None or X is None or not w) else g.to(device=X.device, dtype=X.dtype)
                          for X, g, w in zip(ins, outs, want))
 

@@ -137,8 +137,10 @@ int QPB_ALT_NAME(_setup)(const qpb200_plan* plan, size_t smem, int nsys, const d
 }
 #endif
 
-// (the batch-mean reductions of qpb200_backward stay in qp_kernels.cu: this is only the per-QP kernel)
-int QPB_ALT_NAME(_backward)(const qpb200_plan* plan, size_t smem, int nbatch, const double* dl_dzhat, const double* zhat,
+// (the batch-mean reductions of qpb200_backward stay in qp_kernels.cu: this is only the per-QP kernel). dl_dlam, dl_dnu:
+// the adjoints of the duals (NULL: zero), as in qpb200_backward_duals
+int QPB_ALT_NAME(_backward)(const qpb200_plan* plan, size_t smem, int nbatch, const double* dl_dzhat,
+                            const double* dl_dlam, const double* dl_dnu, const double* zhat,
                             const double* lam, const double* slacks, const double* nus, const double* Lfac,
                             const double* Wfac, const double* Kfac, int sF, double* dQ, int mean_Q, double* dp, int mean_p,
                             double* dG, int mean_G, double* dh, int mean_h, double* dA, int mean_A, double* db, int mean_b,
@@ -151,7 +153,7 @@ int QPB_ALT_NAME(_backward)(const qpb200_plan* plan, size_t smem, int nbatch, co
     int rc = alt_set_smem(k_kkt_fast<true, true, true, kMin>, smem, g_bwd);
     if (rc) return rc;
     k_kkt_fast<true, true, true, kMin><<<nbatch, qpb::fast::kNT, smem, st>>>(
-        D, nullptr, dl_dzhat, nullptr, nullptr, nullptr, zhat, lam, slacks, nus, Lfac, Wfac, Kfac, sF, dxv, nullptr,
+        D, nullptr, dl_dzhat, nullptr, dl_dlam, dl_dnu, zhat, lam, slacks, nus, Lfac, Wfac, Kfac, sF, dxv, nullptr,
         dlamv, dnuv, O);
     return alt_check_launch();
 }

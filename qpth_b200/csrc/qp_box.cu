@@ -655,7 +655,8 @@ k_box_forward(typename F::Dims P, const double* __restrict__ q, int64_t sq, cons
 // QPFunctionFn.backward (qp.py:128-182) for the box QP: d from the clamped duals (qp.py:148), one factor of M and one
 // solve per QP, then dq = dx o z, dp = dx, dlb = dlam_lb, dub = -dlam_ub, dA = dnu z' + nu dx', db = -dnu. dxv, dlamv
 // and dnuv always receive dx, dlam, dnu (the batch means read them); a gradient whose mean flag is set is skipped here.
-// Every CTA writes its slice of dx, dlam, dq, dp, dlb, dub and its columns of dA; the leader dnu and db.
+// Every CTA writes its slice of dx, dlam, dq, dp, dlb, dub and its columns of dA; the leader dnu and db. dl_dlam and dl_dnu
+// (NULL: zero) are the adjoints of the returned duals: they are the rz and ry of the solve, which rz / ry are not otherwise.
 struct BoxGrads {
     double *dq, *dp, *dlb, *dub, *dA, *db;
     int mq, mp, mlb, mub, mA, mb;
@@ -664,7 +665,8 @@ struct BoxGrads {
 template <class F>
 __global__ void __launch_bounds__(kBoxNT, F::kMinBwd)
 k_box_backward(typename F::Dims P, const double* __restrict__ q, int64_t sq, const double* __restrict__ A, int64_t sA,
-               const double* __restrict__ dl, const double* __restrict__ zhat, const double* __restrict__ lam,
+               const double* __restrict__ dl, const double* __restrict__ dl_dlam, const double* __restrict__ dl_dnu,
+               const double* __restrict__ zhat, const double* __restrict__ lam,
                const double* __restrict__ slacks, const double* __restrict__ nus, BoxGrads O,
                double* __restrict__ dxv, double* __restrict__ dlamv, double* __restrict__ dnuv) {
     QPB_SMEM;
@@ -677,10 +679,14 @@ k_box_backward(typename F::Dims P, const double* __restrict__ q, int64_t sq, con
     for (int i = tid; i < m; i += kBoxNT) {
         const int64_t g = (int64_t)qp * f.mg() + f.grow(i);
         qsm[D.d + i] = fmax(lam[g], 1e-8) / fmax(slacks[g], 1e-8);
+        if (dl_dlam != nullptr) qsm[D.rz + i] = dl_dlam[g];
     }
+    // every CTA loads all of dl_dnu: the right-hand side of M stays bit-identical across the cluster (see k_box_forward)
+    if (dl_dnu != nullptr)
+        for (int i = tid; i < e; i += kBoxNT) qsm[D.ry + i] = dl_dnu[(int64_t)qp * e + i];
     __syncthreads();
     f.form();
-    box_solve(f, true, D.rx, -1, -1, -1, D.dx, D.ds, D.dz, D.dy);
+    box_solve(f, true, D.rx, -1, dl_dlam != nullptr ? D.rz : -1, dl_dnu != nullptr ? D.ry : -1, D.dx, D.ds, D.dz, D.dy);
     for (int j = tid; j < n; j += kBoxNT) {
         const int64_t g = (int64_t)qp * N + j0 + j;
         const double dx = qsm[D.dx + j], z = zhat[g];
@@ -1282,7 +1288,8 @@ k_box_forward_dm(DmDims Y, const double* __restrict__ q, int64_t sq, const doubl
 // k_box_backward<Cluster> with M distributed
 __global__ void __launch_bounds__(kBoxNT, 1)
 k_box_backward_dm(DmDims Y, const double* __restrict__ q, int64_t sq, const double* __restrict__ A, int64_t sA,
-                  const double* __restrict__ dl, const double* __restrict__ zhat, const double* __restrict__ lam,
+                  const double* __restrict__ dl, const double* __restrict__ dl_dlam,
+                  const double* __restrict__ dl_dnu, const double* __restrict__ zhat, const double* __restrict__ lam,
                   const double* __restrict__ slacks, const double* __restrict__ nus, BoxGrads O,
                   double* __restrict__ dxv, double* __restrict__ dlamv, double* __restrict__ dnuv) {
     QPB_SMEM;
@@ -1298,10 +1305,14 @@ k_box_backward_dm(DmDims Y, const double* __restrict__ q, int64_t sq, const doub
     for (int i = tid; i < m; i += kBoxNT) {
         const int64_t g = (int64_t)qp * X.mg + cl_grow(X, D, j0, i);
         qsm[D.d + i] = fmax(lam[g], 1e-8) / fmax(slacks[g], 1e-8);
+        if (dl_dlam != nullptr) qsm[D.rz + i] = dl_dlam[g];
     }
+    if (dl_dnu != nullptr)                                       // all of it in every CTA, as in k_box_backward
+        for (int i = tid; i < e; i += kBoxNT) qsm[D.ry + i] = dl_dnu[(int64_t)qp * e + i];
     __syncthreads();
     dm_form(Y, D, rank, Ag);
-    dm_solve(Y, D, rank, Ag, j0, ph, true, D.rx, -1, -1, -1, D.dx, D.ds, D.dz, D.dy);
+    dm_solve(Y, D, rank, Ag, j0, ph, true, D.rx, -1, dl_dlam != nullptr ? D.rz : -1, dl_dnu != nullptr ? D.ry : -1,
+             D.dx, D.ds, D.dz, D.dy);
     for (int j = tid; j < n; j += kBoxNT) {
         const int64_t g = (int64_t)qp * N + j0 + j;
         const double dx = qsm[D.dx + j], z = zhat[g];
@@ -1573,17 +1584,30 @@ int qpb200_box_backward(const qpb200_box_plan* plan, int nbatch, const double* q
                         const double* nus, double* dq, int mean_q, double* dp, int mean_p, double* dlb, int mean_lb,
                         double* dub, int mean_ub, double* dA, int mean_A, double* db, int mean_b, double* dxv,
                         double* dlamv, double* dnuv, void* stream) {
+    return qpb200_box_backward_duals(plan, nbatch, q, sq, A, sA, dl_dzhat, nullptr, nullptr, zhat, lam, slacks, nus, dq,
+                                     mean_q, dp, mean_p, dlb, mean_lb, dub, mean_ub, dA, mean_A, db, mean_b, dxv, dlamv,
+                                     dnuv, stream);
+}
+
+int qpb200_box_backward_duals(const qpb200_box_plan* plan, int nbatch, const double* q, int64_t sq, const double* A,
+                              int64_t sA, const double* dl_dzhat, const double* dl_dlam, const double* dl_dnu,
+                              const double* zhat, const double* lam, const double* slacks, const double* nus, double* dq,
+                              int mean_q, double* dp, int mean_p, double* dlb, int mean_lb, double* dub, int mean_ub,
+                              double* dA, int mean_A, double* db, int mean_b, double* dxv, double* dlamv, double* dnuv,
+                              void* stream) {
     int rc = box_plan_check(plan);
     if (rc) return rc;
     if (nbatch <= 0 || !q || !dl_dzhat || !zhat || !lam || !slacks || !dxv || !dlamv) return QPB200_ERR_BAD_ARG;
     if (plan->neq > 0 && (!A || !nus || !dnuv)) return QPB200_ERR_BAD_ARG;
+    if (dl_dnu && plan->neq == 0) return QPB200_ERR_BAD_ARG;
     if ((dlb && !plan->has_lb) || (dub && !plan->has_ub)) return QPB200_ERR_BAD_ARG;
     const int n = plan->nz, m = plan->nineq, e = plan->neq, nlb = plan->has_lb ? n : 0;
     BoxGrads O;
     O.dq = dq; O.dp = dp; O.dlb = dlb; O.dub = dub; O.dA = e > 0 ? dA : nullptr; O.db = e > 0 ? db : nullptr;
     O.mq = mean_q; O.mp = mean_p; O.mlb = mean_lb; O.mub = mean_ub; O.mA = mean_A; O.mb = mean_b;
     rc = box_launch("k_box_backward", plan, nbatch, stream, k_box_backward<OneCta>, k_box_backward<Cluster>,
-                    k_box_backward_dm, q, sq, A, sA, dl_dzhat, zhat, lam, slacks, nus, O, dxv, dlamv, dnuv);
+                    k_box_backward_dm, q, sq, A, sA, dl_dzhat, dl_dlam, dl_dnu, zhat, lam, slacks, nus, O, dxv, dlamv,
+                    dnuv);
     if (rc) return rc;
     cudaStream_t st = (cudaStream_t)stream;
     const int TB = 128;

@@ -670,6 +670,7 @@ k_solve_kkt(KDims D, const double* __restrict__ d_in, const double* __restrict__
             if (kBackward) {
                 di = fmax(lam[(int64_t)qp * m + j], 1e-8) / fmax(slacks[(int64_t)qp * m + j], 1e-8);   // qp.py:148
                 if (kReg) di += D.reg;
+                if (rz_in != nullptr) extra = -rz_in[(int64_t)qp * m + j];   // dl/dlam (rs = 0)
             } else {
                 // regularised variant (D.reg > 0, batch.py:244-310): d~ = d + eps in the complementarity row, and the slot
                 // holds 1 / (1/d~ + eps) because factor_kkt adds the RECIPROCAL of this slot to the diagonal of S
@@ -678,7 +679,7 @@ k_solve_kkt(KDims D, const double* __restrict__ d_in, const double* __restrict__
                 rsi = rs_in[(int64_t)qp * m + j];
                 extra = rsi / dt - rz_in[(int64_t)qp * m + j];
             }
-        } else if (!kBackward && i < e) {
+        } else if (i < e && (!kBackward || ry_in != nullptr)) {     // (backward: dl/dnu)
             extra = -ry_in[(int64_t)qp * e + i];
         }
         d[i] = di;
@@ -1104,9 +1105,9 @@ extern "C" {
                                    const double*, const double*, const double*, const double*, const double*, int,         \
                                    double*, double*, double*, double*, void*);                                             \
     int qpb200_alt##NT##_backward(const qpb200_plan*, size_t, int, const double*, const double*, const double*,            \
-                                  const double*, const double*, const double*, const double*, const double*, int, double*, \
-                                  int, double*, int, double*, int, double*, int, double*, int, double*, int, double*,      \
-                                  double*, double*, void*);
+                                  const double*, const double*, const double*, const double*, const double*,              \
+                                  const double*, const double*, int, double*, int, double*, int, double*, int, double*,    \
+                                  int, double*, int, double*, int, double*, double*, double*, void*);
 QPB_ALT_DECL(192)
 QPB_ALT_DECL(512)
 int qpb200_alt192_setup(const qpb200_plan*, size_t, int, const double*, int64_t, const double*, int64_t, const double*,
@@ -1502,10 +1503,28 @@ int qpb200_backward(const qpb200_plan* plan, int nbatch, const double* dl_dzhat,
                     int mean_p, double* dG, int mean_G, double* dh, int mean_h, double* dA, int mean_A,
                     double* db, int mean_b, double* dxv, double* dlamv, double* dnuv, double* scratch,
                     void* stream) {
+    return qpb200_backward_duals(plan, nbatch, dl_dzhat, nullptr, nullptr, zhat, lam, slacks, nus, Lfac, Wfac, Kfac, sF,
+                                 dQ, mean_Q, dp, mean_p, dG, mean_G, dh, mean_h, dA, mean_A, db, mean_b, dxv, dlamv, dnuv,
+                                 scratch, stream);
+}
+
+// dl_dlam / dl_dnu (either may be NULL: zero) go into the rz / ry slots of the backward solve:
+//   [Q 0 G' A'; 0 D I 0; G I 0 0; A 0 0 0] [dx ds dlam dnu] = -[dl_dzhat; 0; dl_dlam; dl_dnu]
+static int check_dual_adjoints(const qpb200_plan* plan, const double* dl_dnu) {
+    return (dl_dnu != nullptr && plan->neq == 0) ? QPB200_ERR_BAD_ARG : QPB200_OK;
+}
+
+int qpb200_backward_duals(const qpb200_plan* plan, int nbatch, const double* dl_dzhat, const double* dl_dlam,
+                          const double* dl_dnu, const double* zhat, const double* lam, const double* slacks,
+                          const double* nus, const double* Lfac, const double* Wfac, const double* Kfac, int sF,
+                          double* dQ, int mean_Q, double* dp, int mean_p, double* dG, int mean_G, double* dh, int mean_h,
+                          double* dA, int mean_A, double* db, int mean_b, double* dxv, double* dlamv, double* dnuv,
+                          double* scratch, void* stream) {
     if (!plan || nbatch <= 0 || !dl_dzhat || !zhat || !lam || !slacks || !Lfac || !Wfac || !Kfac ||
         !dxv || !dlamv)
         return QPB200_ERR_BAD_ARG;
     if (plan->neq > 0 && (!nus || !dnuv)) return QPB200_ERR_BAD_ARG;
+    if (check_dual_adjoints(plan, dl_dnu)) return QPB200_ERR_BAD_ARG;
     cudaStream_t st = (cudaStream_t)stream;
     KDims D = dims_of(plan);
     const int n = plan->nz, m = plan->nineq, e = plan->neq;
@@ -1517,14 +1536,14 @@ int qpb200_backward(const qpb200_plan* plan, int nbatch, const double* dl_dzhat,
         int rc = set_smem(k_solve_kkt<KS, true>, plan->solve_smem_bytes);                               \
         if (rc) return rc;                                                                              \
         k_solve_kkt<KS, true><<<nbatch, kThreads, plan->solve_smem_bytes, st>>>(                        \
-            D, nullptr, dl_dzhat, nullptr, nullptr, nullptr, zhat, lam, slacks, nus, Lfac, Wfac, Kfac,  \
+            D, nullptr, dl_dzhat, nullptr, dl_dlam, dl_dnu, zhat, lam, slacks, nus, Lfac, Wfac, Kfac,  \
             sF, dxv, nullptr, dlamv, dnuv, O, SCR, SCRN);                                               \
     } while (0)
     if (plan->tiny) {
         int rc = set_smem(k_solve_kkt<true, true, true>, plan->solve_smem_bytes);
         if (rc) return rc;
         k_solve_kkt<true, true, true><<<nbatch, kTinyThreads, plan->solve_smem_bytes, st>>>(
-            D, nullptr, dl_dzhat, nullptr, nullptr, nullptr, zhat, lam, slacks, nus, Lfac, Wfac, Kfac, sF, dxv, nullptr,
+            D, nullptr, dl_dzhat, nullptr, dl_dlam, dl_dnu, zhat, lam, slacks, nus, Lfac, Wfac, Kfac, sF, dxv, nullptr,
             dlamv, dnuv, O, nullptr, 0);
     } else if (plan->pf) {
 #define QPB_LAUNCH_PF(KG, K2)                                                                           \
@@ -1533,19 +1552,19 @@ int qpb200_backward(const qpb200_plan* plan, int nbatch, const double* dl_dzhat,
             int rc = set_smem(k_kkt_fast<true, KG, true, K2>, sb_);                                     \
             if (rc) return rc;                                                                          \
             k_kkt_fast<true, KG, true, K2><<<nbatch, qpb::fast::kNT, sb_, st>>>(                              \
-                D, nullptr, dl_dzhat, nullptr, nullptr, nullptr, zhat, lam, slacks, nus, Lfac, Wfac, Kfac, sF, dxv, \
+                D, nullptr, dl_dzhat, nullptr, dl_dlam, dl_dnu, zhat, lam, slacks, nus, Lfac, Wfac, Kfac, sF, dxv, \
                 nullptr, dlamv, dnuv, O);                                                               \
         } while (0)
         if (plan->pf_three && plan->pf3_ok) {
-            int rc = qpb200_alt192_backward(plan, (size_t)plan->pf3_smem_bytes, nbatch, dl_dzhat, zhat, lam, slacks, nus, Lfac, Wfac,
-                                            Kfac, sF, dQ, mean_Q, dp, mean_p, dG, mean_G, dh, mean_h, dA, mean_A, db, mean_b, dxv,
-                                            dlamv, dnuv, stream);
+            int rc = qpb200_alt192_backward(plan, (size_t)plan->pf3_smem_bytes, nbatch, dl_dzhat, dl_dlam, dl_dnu, zhat, lam,
+                                            slacks, nus, Lfac, Wfac, Kfac, sF, dQ, mean_Q, dp, mean_p, dG, mean_G, dh,
+                                            mean_h, dA, mean_A, db, mean_b, dxv, dlamv, dnuv, stream);
             if (rc) return rc;
         } else if (plan->pf_two && plan->pf2_ok) QPB_LAUNCH_PF(true, 2);
         else if (plan->pf_global && plan->pf_threads == 512) {
-            int rc = qpb200_alt512_backward(plan, (size_t)plan->pf_smem_bytes, nbatch, dl_dzhat, zhat, lam, slacks, nus, Lfac, Wfac,
-                                            Kfac, sF, dQ, mean_Q, dp, mean_p, dG, mean_G, dh, mean_h, dA, mean_A, db, mean_b, dxv,
-                                            dlamv, dnuv, stream);
+            int rc = qpb200_alt512_backward(plan, (size_t)plan->pf_smem_bytes, nbatch, dl_dzhat, dl_dlam, dl_dnu, zhat, lam,
+                                            slacks, nus, Lfac, Wfac, Kfac, sF, dQ, mean_Q, dp, mean_p, dG, mean_G, dh,
+                                            mean_h, dA, mean_A, db, mean_b, dxv, dlamv, dnuv, stream);
             if (rc) return rc;
         } else if (plan->pf_global) QPB_LAUNCH_PF(true, 0);
         else QPB_LAUNCH_PF(false, 0);
@@ -1554,13 +1573,13 @@ int qpb200_backward(const qpb200_plan* plan, int nbatch, const double* dl_dzhat,
         int rc = set_smem(k_kkt_fast<true, true>, plan->coop_smem_bytes);
         if (rc) return rc;
         k_kkt_fast<true, true><<<nbatch, kThreads, plan->coop_smem_bytes, st>>>(
-            D, nullptr, dl_dzhat, nullptr, nullptr, nullptr, zhat, lam, slacks, nus, Lfac, Wfac, Kfac, sF, dxv,
+            D, nullptr, dl_dzhat, nullptr, dl_dlam, dl_dnu, zhat, lam, slacks, nus, Lfac, Wfac, Kfac, sF, dxv,
             nullptr, dlamv, dnuv, O);
     } else if (plan->fast) {
         int rc = set_smem(k_kkt_fast<true, false>, plan->solve_smem_bytes);
         if (rc) return rc;
         k_kkt_fast<true, false><<<nbatch, kThreads, plan->solve_smem_bytes, st>>>(
-            D, nullptr, dl_dzhat, nullptr, nullptr, nullptr, zhat, lam, slacks, nus, Lfac, Wfac, Kfac, sF, dxv,
+            D, nullptr, dl_dzhat, nullptr, dl_dlam, dl_dnu, zhat, lam, slacks, nus, Lfac, Wfac, Kfac, sF, dxv,
             nullptr, dlamv, dnuv, O);
     } else if (plan->smem_resident) {
         QPB_LAUNCH_BWD(true, nullptr, 0);
@@ -1652,9 +1671,21 @@ int qpb200_backward_reg(const qpb200_plan* plan, int nbatch, const double* dl_dz
                         int mean_Q, double* dp, int mean_p, double* dG, int mean_G, double* dh, int mean_h, double* dA,
                         int mean_A, double* db, int mean_b, double* dxv, double* dlamv, double* dnuv, double* scratch,
                         void* stream) {
+    return qpb200_backward_reg_duals(plan, nbatch, dl_dzhat, nullptr, nullptr, zhat, lam, slacks, nus, Lfac, Wfac, Kfac,
+                                     sF, reg_eps, ir_steps, dQ, mean_Q, dp, mean_p, dG, mean_G, dh, mean_h, dA, mean_A, db,
+                                     mean_b, dxv, dlamv, dnuv, scratch, stream);
+}
+
+int qpb200_backward_reg_duals(const qpb200_plan* plan, int nbatch, const double* dl_dzhat, const double* dl_dlam,
+                              const double* dl_dnu, const double* zhat, const double* lam, const double* slacks,
+                              const double* nus, const double* Lfac, const double* Wfac, const double* Kfac, int sF,
+                              double reg_eps, int ir_steps, double* dQ, int mean_Q, double* dp, int mean_p, double* dG,
+                              int mean_G, double* dh, int mean_h, double* dA, int mean_A, double* db, int mean_b,
+                              double* dxv, double* dlamv, double* dnuv, double* scratch, void* stream) {
     if (!plan || nbatch <= 0 || !dl_dzhat || !zhat || !lam || !slacks || !Lfac || !Wfac || !Kfac || !dxv || !dlamv)
         return QPB200_ERR_BAD_ARG;
     if (plan->neq > 0 && (!nus || !dnuv)) return QPB200_ERR_BAD_ARG;
+    if (check_dual_adjoints(plan, dl_dnu)) return QPB200_ERR_BAD_ARG;
     int rc = check_reg_plan(plan, reg_eps, ir_steps, scratch);
     if (rc) return rc;
     cudaStream_t st = (cudaStream_t)stream;
@@ -1667,7 +1698,7 @@ int qpb200_backward_reg(const qpb200_plan* plan, int nbatch, const double* dl_dz
         rc = set_smem(k_solve_kkt<false, true, false, true>, plan->solve_smem_bytes);
         if (rc) return rc;
         k_solve_kkt<false, true, false, true><<<nbatch, kThreads, plan->solve_smem_bytes, st>>>(
-            D, nullptr, dl_dzhat, nullptr, nullptr, nullptr, zhat, lam, slacks, nus, Lfac, Wfac, Kfac, sF, dxv, nullptr,
+            D, nullptr, dl_dzhat, nullptr, dl_dlam, dl_dnu, zhat, lam, slacks, nus, Lfac, Wfac, Kfac, sF, dxv, nullptr,
             dlamv, dnuv, O, scratch, plan->solve_scratch_elems, ir_steps);
         CK(cudaGetLastError());
         return launch_means(nbatch, plan->nz, plan->nineq, plan->neq, zhat, lam, nus, dQ, mean_Q, dp, mean_p, dG, mean_G,
@@ -1679,7 +1710,7 @@ int qpb200_backward_reg(const qpb200_plan* plan, int nbatch, const double* dl_dz
         rc = set_smem(k_kkt_fast<true, KG, true, 0, true>, sb_);                                             \
         if (rc) return rc;                                                                                   \
         k_kkt_fast<true, KG, true, 0, true><<<nbatch, qpb::fast::kNT, sb_, st>>>(                            \
-            D, nullptr, dl_dzhat, nullptr, nullptr, nullptr, zhat, lam, slacks, nus, Lfac, Wfac, Kfac, sF, dxv, \
+            D, nullptr, dl_dzhat, nullptr, dl_dlam, dl_dnu, zhat, lam, slacks, nus, Lfac, Wfac, Kfac, sF, dxv, \
             nullptr, dlamv, dnuv, O, ir_steps);                                                              \
     } while (0)
     if (plan->pf_global) QPB_LAUNCH_REG(true);

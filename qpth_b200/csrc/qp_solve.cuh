@@ -635,6 +635,17 @@ k_kkt_fast(KDims D, const double* __restrict__ d_in, const double* __restrict__ 
         qsm[hW + i] = extra;
         qsm[aug + i] = 0.0;
     }
+    // backward: the adjoints of the duals (either may be NULL) are rz = dl/dlam and ry = dl/dnu, with rs = 0. A loop of
+    // its own, over each thread's own rows: inside the one above the load cost the 256-thread coop build spills.
+    if (kBackward && (rz_in != nullptr || ry_in != nullptr)) {
+        _Pragma("unroll 1") for (int i = tid; i < ms; i += kNT) {
+            if (i >= ep) {
+                if (rz_in != nullptr) qsm[hW + i] = -rz_in[(int64_t)qp * m + i - ep];
+            } else if (i < e && ry_in != nullptr) {
+                qsm[hW + i] = -ry_in[(int64_t)qp * e + i];
+            }
+        }
+    }
     if (kReg) {                                                  // x part of the refinement (dx~ = -t + it - W^T w)
         _Pragma("unroll 1") for (int i = tid; i < n; i += kNT) qsm[FV(F_DSA) + i] = 0.0;
     }

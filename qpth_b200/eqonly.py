@@ -41,7 +41,7 @@ def _target_device(Q_):
 
 class QPEqualityFn(Function):
     @staticmethod
-    def forward(ctx, Q_, p_, A_, b_, check_Q_spd, reg=False):
+    def forward(ctx, Q_, p_, A_, b_, check_Q_spd, reg=False, duals=False):
         empty = Q_.new_empty(0)
         nBatch, nz, nineq, neq = check_shapes(Q_, p_, empty, empty, A_, b_)
         assert neq > 0 or nineq > 0                         # qp.py:89
@@ -65,13 +65,22 @@ class QPEqualityFn(Function):
         ctx.QA, ctx.steps = (Q, A), steps
         ctx.zhat64, ctx.nus = zhat, nus
         ctx.meta = [(X.device, X.dtype) for X in (Q_, p_, A_, b_)]
-        return zhat.to(device=Q_.device, dtype=Q_.dtype)
+        zhat_out = zhat.to(device=Q_.device, dtype=Q_.dtype)
+        if not duals:
+            return zhat_out
+        # duals: no inequality rows (lam is (nBatch, 0)); nu is the dy of the solve
+        ctx.set_materialize_grads(False)
+        return zhat_out, Q_.new_zeros(nBatch, 0), nus.to(device=Q_.device, dtype=Q_.dtype)
 
     @staticmethod
-    def backward(ctx, dl_dzhat):
+    def backward(ctx, dl_dzhat, dl_dlam=None, dl_dnu=None):
         z, nus = ctx.zhat64, ctx.nus
-        dl = dl_dzhat.detach().to(device=z.device, dtype=torch.float64).contiguous().view_as(z)
-        dx, _, _, dnu = _solve(ctx.F, *ctx.QA, ctx.one, dl, ctx.zero, ctx.zero, torch.zeros_like(nus), ctx.steps)
+        dl = (torch.zeros_like(z) if dl_dzhat is None
+              else dl_dzhat.detach().to(device=z.device, dtype=torch.float64).contiguous().view_as(z))
+        # dl/dnu is the ry of the solve: K [dx ds dz dnu] = -[dl 0 0 dl/dnu]
+        ry = (torch.zeros_like(nus) if dl_dnu is None
+              else dl_dnu.detach().to(device=z.device, dtype=torch.float64).contiguous().view_as(nus))
+        dx, _, _, dnu = _solve(ctx.F, *ctx.QA, ctx.one, dl, ctx.zero, ctx.zero, ry, ctx.steps)
         grads = [0.5 * (bger(dx, z) + bger(z, dx)),         # qp.py:175-177
                  dx,                                        # qp.py:150
                  bger(dnu, z) + bger(nus, dx),              # qp.py:166-167
@@ -82,11 +91,11 @@ class QPEqualityFn(Function):
                 out.append(None)
                 continue
             out.append((g.mean(0) if unb else g).to(device=dev, dtype=dt))
-        return tuple(out) + (None, None)
+        return tuple(out) + (None, None, None)
 
 
-def solve_equality_qp(Q_, p_, A_, b_, check_Q_spd=True, reg=False):
+def solve_equality_qp(Q_, p_, A_, b_, check_Q_spd=True, reg=False, duals=False):
     """z* of  argmin 1/2 z'Qz + p'z  s.t. Az = b  (differentiable in Q, p, A, b). reg: the regularised mode of
     QPFunction(kkt_solver=KKTSolvers.IR_UNOPT) for a Q that is only positive semidefinite on the null space of A, or
-    linearly dependent rows of A."""
-    return QPEqualityFn.apply(Q_, p_, A_, b_, check_Q_spd, reg)
+    linearly dependent rows of A. duals: return (z*, lam, nu) as QPFunction(duals=True) does, lam (nBatch, 0)."""
+    return QPEqualityFn.apply(Q_, p_, A_, b_, check_Q_spd, reg, duals)

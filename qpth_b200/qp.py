@@ -241,8 +241,24 @@ def diagnostics(spd, st, check_Q_spd, verbose, spd_err=SPD_ERR):
                 i, row[:, 0].mean(), row[:, 1].mean(), row[:, 2].mean()))
 
 
-def solve_backward(st, dl_dzhat, mean_flags, want):
-    """QPFunctionFn.backward on the device. mean_flags / want: 6-tuples for (Q,p,G,h,A,b)."""
+def _adjoint(g, B, n, device):
+    """An incoming gradient as a (B, n) fp64 device tensor; None (no gradient reached this output) stays None."""
+    if g is None or n == 0:
+        return None
+    return g.detach().to(device=device, dtype=torch.float64).contiguous().view(B, n)
+
+
+def dual_outputs(st, like):
+    """(lam, nu) of the returned iterate with the dtype and device of `like`; nu is (nBatch, 0) without equality rows."""
+    lam = st.lam.to(device=like.device, dtype=like.dtype)
+    nu = (st.nus.to(device=like.device, dtype=like.dtype) if st.nus is not None
+          else torch.zeros(st.nBatch, 0, device=like.device, dtype=like.dtype))
+    return lam, nu
+
+
+def solve_backward(st, dl_dzhat, mean_flags, want, dl_dlam=None, dl_dnu=None):
+    """QPFunctionFn.backward on the device. mean_flags / want: 6-tuples for (Q,p,G,h,A,b). dl_dlam / dl_dnu: the
+    gradients of the loss with respect to the returned duals (None: zero); dl_dzhat None: zero."""
     if _pending:
         flush_checks(wait=False)
     lib = _lib.load()
@@ -250,7 +266,8 @@ def solve_backward(st, dl_dzhat, mean_flags, want):
     nz, nineq, neq = plan.nz, plan.nineq, plan.neq
     f64 = dict(dtype=torch.float64, device=device)
     with torch.cuda.device(device):
-        dl = dl_dzhat.detach().to(device=device, dtype=torch.float64).contiguous().view(B, nz)
+        dl = _adjoint(dl_dzhat, B, nz, device) if dl_dzhat is not None else torch.zeros(B, nz, **f64)
+        glam, gnu = _adjoint(dl_dlam, B, nineq, device), _adjoint(dl_dnu, B, neq, device)
         shapes = [(nz, nz), (nz,), (nineq, nz), (nineq,), (neq, nz), (neq,)]
         outs = []
         for k in range(6):
@@ -266,8 +283,12 @@ def solve_backward(st, dl_dzhat, mean_flags, want):
         for k in range(6):
             args += [_ptr(outs[k]), 1 if mean_flags[k] else 0]
         reg = getattr(st, "reg", False)             # (solution.py builds _Solved without it: the default path)
-        _lib.check((lib.qpb200_backward_reg if reg else lib.qpb200_backward)(
-            ctypes.byref(plan), B, _ptr(dl), _ptr(st.zhat), _ptr(st.lam), _ptr(st.slacks), _ptr(st.nus),
+        if glam is None and gnu is None:            # no dual was used: the entry point of a zhat-only loss
+            fn, adj = (lib.qpb200_backward_reg if reg else lib.qpb200_backward), ()
+        else:
+            fn, adj = (lib.qpb200_backward_reg_duals if reg else lib.qpb200_backward_duals), (_ptr(glam), _ptr(gnu))
+        _lib.check(fn(
+            ctypes.byref(plan), B, _ptr(dl), *adj, _ptr(st.zhat), _ptr(st.lam), _ptr(st.slacks), _ptr(st.nus),
             _ptr(st.L), _ptr(st.W), _ptr(st.K), 1 if st.nsys > 1 else 0, *((float(kkt.IR_EPS), int(kkt.IR_STEPS)) if reg else ()),
             *args, _ptr(dxv), _ptr(dlamv), _ptr(dnuv), _ptr(st.scratch), _stream()))
     return outs
@@ -282,8 +303,16 @@ def check_kkt_solver(kkt_solver):
 
 
 def QPFunction(eps=1e-12, verbose=0, notImprovedLim=3, maxIter=20, solver=QPSolvers.PDIPM_BATCHED,
-               check_Q_spd=True, kkt_solver=KKTSolvers.LU_PARTIAL):
+               check_Q_spd=True, kkt_solver=KKTSolvers.LU_PARTIAL, duals=False):
     """Factory with the reference's signature (`qpth/qp.py:18-20`); returns `Function.apply`.
+
+    duals (an extension): False returns zhat (nBatch, nz), as the reference does. True returns (zhat, lam, nu): the
+    inequality duals (nBatch, nineq) and the equality duals (nBatch, neq), or (nBatch, 0) without equality rows, of the
+    returned iterate (the values of last_solve(), with zhat's dtype and device), and a loss may use all three: the
+    backward pass puts the gradients of lam and nu into the right-hand side of its KKT solve,
+    [Q 0 G' A'; 0 D I 0; G I 0 0; A 0 0 0] [dx ds dlam dnu] = -[dl/dz; 0; dl/dlam; dl/dnu], and the gradient formulas
+    are unchanged. With linearly dependent equality rows (IR_UNOPT) nu is not unique, and the gradient through nu is
+    that of the nu returned. Slacks are not an output: s = h - Gz.
 
     kkt_solver (an extension of the reference's signature): KKTSolvers.LU_PARTIAL, the default, needs Q positive definite.
     KKTSolvers.IR_UNOPT also solves QPs whose Q is only positive semidefinite (LPs with Q = 0, low-rank quadratic terms)
@@ -305,7 +334,9 @@ def QPFunction(eps=1e-12, verbose=0, notImprovedLim=3, maxIter=20, solver=QPSolv
             Q, p, G, h, A, b = (expandParam(X, nBatch, nd)[0]
                                 for X, nd in ((Q_, 3), (p_, 2), (G_, 3), (h_, 2), (A_, 3), (b_, 2)))
             zhats, nus, lams, slacks = cvxpy_forward(Q, p, G, h, A, b)
-            return QPSolutionFunction(check_Q_spd, kkt_solver)(Q_, p_, G_, h_, A_, b_, zhats, lams, slacks, nus)
+            f = QPSolutionFunction(check_Q_spd, kkt_solver, duals=True) if duals else QPSolutionFunction(check_Q_spd,
+                                                                                                          kkt_solver)
+            return f(Q_, p_, G_, h_, A_, b_, zhats, lams, slacks, nus)
 
         return apply_cvxpy
     if solver != QPSolvers.PDIPM_BATCHED:
@@ -330,16 +361,19 @@ def QPFunction(eps=1e-12, verbose=0, notImprovedLim=3, maxIter=20, solver=QPSolv
             ctx.save_for_backward(zhats, Q_, p_, G_, h_, A_, b_)
             # parity with the reference's ctx attributes (device fp64 views)
             ctx.lams, ctx.slacks, ctx.nus = st.lam, st.slacks, st.nus
-            return zhats
+            if not duals:
+                return zhats
+            ctx.set_materialize_grads(False)       # an unused output's gradient arrives as None: no adjoint is read
+            return (zhats,) + dual_outputs(st, Q_)
 
         @staticmethod
-        def backward(ctx, dl_dzhat):
+        def backward(ctx, dl_dzhat, dl_dlam=None, dl_dnu=None):
             zhats, Q, p, G, h, A, b = ctx.saved_tensors
             nBatch = extract_nBatch(Q, p, G, h, A, b)
             flags = [expandParam(X, nBatch, nd)[1]
                      for X, nd in ((Q, 3), (p, 2), (G, 3), (h, 2), (A, 3), (b, 2))]   # qp.py:131-136
             want = list(ctx.needs_input_grad)
-            outs = solve_backward(ctx.st, dl_dzhat, flags, want)
+            outs = solve_backward(ctx.st, dl_dzhat, flags, want, dl_dlam, dl_dnu)
             grads = []
             for X, g in zip((Q, p, G, h, A, b), outs):
                 grads.append(None if g is None else g.to(device=X.device, dtype=X.dtype))
@@ -349,7 +383,7 @@ def QPFunction(eps=1e-12, verbose=0, notImprovedLim=3, maxIter=20, solver=QPSolv
         if G_.nelement() == 0 and h_.nelement() == 0 and A_.nelement() > 0:
             # equality-constrained QP: an extension (the reference cannot run nineq == 0); one KKT solve, eqonly.py
             from .eqonly import solve_equality_qp
-            return solve_equality_qp(Q_, p_, A_, b_, check_Q_spd, reg=kkt_solver == KKTSolvers.IR_UNOPT)
+            return solve_equality_qp(Q_, p_, A_, b_, check_Q_spd, reg=kkt_solver == KKTSolvers.IR_UNOPT, duals=duals)
         return QPFunctionFn.apply(Q_, p_, G_, h_, A_, b_)
 
     # diagnostics the reference keeps on ctx (nus / lams / slacks) plus per-QP iteration counts

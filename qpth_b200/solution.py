@@ -93,8 +93,11 @@ def pre_factor_state(Q_, p_, G_, h_, A_, b_, zhat, lams, slacks, nus, check_Q_sp
     return st
 
 
-def QPSolutionFunction(check_Q_spd=True, kkt_solver=KKTSolvers.LU_PARTIAL):
+def QPSolutionFunction(check_Q_spd=True, kkt_solver=KKTSolvers.LU_PARTIAL, duals=False):
     """Returns `f(Q, p, G, h, A, b, zhat, lams, slacks, nus) -> zhat`, differentiable in Q, p, G, h, A, b.
+
+    duals=True: f returns (zhat, lam, nu), the given solution's duals as functions of Q, p, G, h, A, b (nu is (nBatch, 0)
+    without equality rows), as QPFunction(duals=True) does; a loss may use all three.
 
     kkt_solver: KKTSolvers.LU_PARTIAL (the default) needs Q positive definite. KKTSolvers.IR_UNOPT differentiates with
     the regularised KKT solve of QPFunction(kkt_solver=IR_UNOPT), so an LP (Q = 0) or a low-rank Q solved by any solver
@@ -108,17 +111,21 @@ def QPSolutionFunction(check_Q_spd=True, kkt_solver=KKTSolvers.LU_PARTIAL):
             zhats = ctx.st.zhat.to(device=Q_.device, dtype=Q_.dtype)
             ctx.save_for_backward(zhats, Q_, p_, G_, h_, A_, b_)
             ctx.lams, ctx.slacks, ctx.nus = ctx.st.lam, ctx.st.slacks, ctx.st.nus
-            return zhats
+            if not duals:
+                return zhats
+            from .qp import dual_outputs
+            ctx.set_materialize_grads(False)
+            return (zhats,) + dual_outputs(ctx.st, Q_)
 
         @staticmethod
-        def backward(ctx, dl_dzhat):
+        def backward(ctx, dl_dzhat, dl_dlam=None, dl_dnu=None):
             from .qp import solve_backward
             zhats, Q, p, G, h, A, b = ctx.saved_tensors
             nBatch = extract_nBatch(Q, p, G, h, A, b)
             flags = [expandParam(X, nBatch, nd)[1]
                      for X, nd in ((Q, 3), (p, 2), (G, 3), (h, 2), (A, 3), (b, 2))]   # qp.py:131-136
             want = list(ctx.needs_input_grad[:6])
-            outs = solve_backward(ctx.st, dl_dzhat, flags, want)
+            outs = solve_backward(ctx.st, dl_dzhat, flags, want, dl_dlam, dl_dnu)
             grads = [None if g is None else g.to(device=X.device, dtype=X.dtype)
                      for X, g in zip((Q, p, G, h, A, b), outs)]
             return tuple(grads) + (None, None, None, None)
