@@ -236,6 +236,37 @@ int qpb200_backward_reg_duals(const qpb200_plan* plan, int nbatch,
                               double* dxv, double* dlamv, double* dnuv,
                               double* scratch, void* stream);
 
+/* Forward mode (JVP) at the returned point, for input tangents dQ, dp, dG, dh, dA, db. Each tangent is a pointer with
+ * its own batch stride in elements (0: one tangent for every QP, as for an un-batched input) and may be NULL (zero: it is
+ * never read); dG, dh must be NULL when nineq == 0, and dA, db, dnu when neq == 0. The call forms
+ *   rx = sym(dQ) z + dp + dG' lam + dA' nu,   rz = dG z - dh,   ry = dA z - db,     sym(dQ) = (dQ + dQ') / 2
+ * in `rhs` (B (nz + nineq + neq) doubles: rx (B,nz), then rz (B,nineq), then ry (B,neq)) and solves the backward's
+ * system with it, qpb200_backward_duals(dl_dzhat = rx, dl_dlam = rz, dl_dnu = ry) with every gradient NULL:
+ *   [Q 0 G' A'; 0 D I 0; G I 0 0; A 0 0 0] [dz ds dlam dnu] = -[rx; 0; rz; ry],   D = lam / s (clamped at 1e-8).
+ * dz (B,nz), dlam (B,nineq), dnu (B,neq) receive the tangents of zhat, lam and nus. This is the exact transpose of
+ * qpb200_backward_duals: sum_b <(g_z, g_lam, g_nu), (dz, dlam, dnu)> = sum_X <grad_X, dX> for batched inputs. For an
+ * un-batched input the JVP is the true derivative, while the backward returns the batch mean, so there the identity
+ * carries a factor nbatch. Arguments are checked as qpb200_backward_duals checks them, before anything is launched. */
+int qpb200_jvp(const qpb200_plan* plan, int nbatch,
+               const double* dQ, int64_t sdQ, const double* dp, int64_t sdp,
+               const double* dG, int64_t sdG, const double* dh, int64_t sdh,
+               const double* dA, int64_t sdA, const double* db, int64_t sdb,
+               const double* zhat, const double* lam, const double* slacks, const double* nus,
+               const double* Lfac, const double* Wfac, const double* Kfac, int sF,
+               double* rhs, double* dz, double* dlam, double* dnu,
+               double* scratch, void* stream);
+/* qpb200_jvp for the regularised mode: the solve is qpb200_backward_reg_duals with its ir_steps refinement steps (plan,
+ * reg_eps and ir_steps as there). With linearly dependent equality rows dnu is not unique; dz and dlam are. */
+int qpb200_jvp_reg(const qpb200_plan* plan, int nbatch,
+                   const double* dQ, int64_t sdQ, const double* dp, int64_t sdp,
+                   const double* dG, int64_t sdG, const double* dh, int64_t sdh,
+                   const double* dA, int64_t sdA, const double* db, int64_t sdb,
+                   const double* zhat, const double* lam, const double* slacks, const double* nus,
+                   const double* Lfac, const double* Wfac, const double* Kfac, int sF,
+                   double reg_eps, int ir_steps,
+                   double* rhs, double* dz, double* dlam, double* dnu,
+                   double* scratch, void* stream);
+
 /* ---- Box QPs (qpth_b200/box.py BoxQPFunction): min 1/2 z' diag(q) z + p'z  s.t.  A z = b,  lb <= z <= ub -------------
  * The dense equivalent is Q = diag(q), G = [-I; I] (only the sides given: lb rows first), h = [-lb; ub]; lam and slacks
  * are laid out as [lb rows; ub rows] (nineq = (has_lb + has_ub) * nz). The inequality block of the KKT system is
@@ -287,6 +318,16 @@ int qpb200_box_backward_duals(const qpb200_box_plan* plan, int nbatch, const dou
                               int mean_q, double* dp, int mean_p, double* dlb, int mean_lb, double* dub, int mean_ub,
                               double* dA, int mean_A, double* db, int mean_b, double* dxv, double* dlamv, double* dnuv,
                               void* stream);
+/* Forward mode (JVP), as qpb200_jvp: tangents dq, dp, dA, db, dlb, dub, each with a batch stride (0: shared) and NULL
+ * allowed (dA, db, dnu must be NULL when neq == 0; dlb / dub when that side is absent). rhs (B (nz + nineq + neq)
+ * doubles) receives rx = dq o z + dp + dA' nu (B,nz), rz = [dlb; -dub] (B,nineq, lam's [lb rows; ub rows] layout) and
+ * ry = dA z - db (B,neq); the solve is qpb200_box_backward_duals with them and every gradient NULL, on the layout the plan
+ * selects. dz, dlam, dnu receive the tangents of zhat, lam and nus. */
+int qpb200_box_jvp(const qpb200_box_plan* plan, int nbatch, const double* q, int64_t sq, const double* A, int64_t sA,
+                   const double* dq, int64_t sdq, const double* dp, int64_t sdp, const double* dA, int64_t sdA,
+                   const double* db, int64_t sdb, const double* dlb, int64_t sdlb, const double* dub, int64_t sdub,
+                   const double* zhat, const double* lam, const double* slacks, const double* nus, double* rhs,
+                   double* dz, double* dlam, double* dnu, void* stream);
 
 /* The structured factor and solve for caller-supplied d (B,nineq) and right-hand sides (the counterpart of
  * qpb200_solve_kkt):  [diag(q) 0 G' A'; 0 D I 0; G I 0 0; A 0 0 0] [dx ds dz dy] = -[rx rs rz ry].

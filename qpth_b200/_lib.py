@@ -68,6 +68,10 @@ SIGNATURES = {
                                  _P, _I, _P, _I, _P, _I, _P, _I, _P, _I, _P, _I, _P, _P, _P, _P, _P]),
     "qpb200_backward_reg_duals": (_I, [ctypes.POINTER(Plan), _I, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _I, _D, _I,
                                        _P, _I, _P, _I, _P, _I, _P, _I, _P, _I, _P, _I, _P, _P, _P, _P, _P]),
+    "qpb200_jvp": (_I, [ctypes.POINTER(Plan), _I, _P, _L, _P, _L, _P, _L, _P, _L, _P, _L, _P, _L,
+                        _P, _P, _P, _P, _P, _P, _P, _I, _P, _P, _P, _P, _P, _P]),
+    "qpb200_jvp_reg": (_I, [ctypes.POINTER(Plan), _I, _P, _L, _P, _L, _P, _L, _P, _L, _P, _L, _P, _L,
+                            _P, _P, _P, _P, _P, _P, _P, _I, _D, _I, _P, _P, _P, _P, _P, _P]),
     "qpb200_optnet_construct": (_I, [_I, _I, _P, _P, _P, _P, _D, _P, _P, _P]),
     "qpb200_optnet_chain": (_I, [_I, _I, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     "qpb200_dfma_probe": (_I, [_I, _I, _I, _P, _P]),
@@ -81,6 +85,8 @@ SIGNATURES = {
                                  _P, _I, _P, _I, _P, _I, _P, _I, _P, _I, _P, _I, _P, _P, _P, _P]),
     "qpb200_box_backward_duals": (_I, [ctypes.POINTER(BoxPlan), _I, _P, _L, _P, _L, _P, _P, _P, _P, _P, _P, _P,
                                        _P, _I, _P, _I, _P, _I, _P, _I, _P, _I, _P, _I, _P, _P, _P, _P]),
+    "qpb200_box_jvp": (_I, [ctypes.POINTER(BoxPlan), _I, _P, _L, _P, _L, _P, _L, _P, _L, _P, _L, _P, _L, _P, _L,
+                            _P, _L, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     "qpb200_box_solve_kkt": (_I, [ctypes.POINTER(BoxPlan), _I, _P, _L, _P, _L, _P, _P, _P, _P, _P,
                                   _P, _P, _P, _P, _P]),
 }

@@ -150,6 +150,32 @@ def solve_box_backward(st, dl_dzhat, mean_flags, want, dl_dlam=None, dl_dnu=None
     return outs
 
 
+def solve_box_jvp(st, tangents):
+    """The JVP of (zhat, lam, nu) at the returned point on the device. tangents: (dq, dp, dA, db, dlb, dub), each None
+    (zero), batched or un-batched as its input. Returns fp64 (dz (B,nz), dlam (B,nineq) in the [lb rows; ub rows]
+    layout, dnu (B,neq) or None); one qpb200_box_jvp call: the right-hand side kernel and the backward's solve."""
+    if _qp._pending:
+        _qp.flush_checks(wait=False)
+    lib = _lib.load()
+    plan, B, device = st.plan, st.nBatch, st.device
+    nz, neq, m = plan.nz, plan.neq, plan.nineq
+    f64 = dict(dtype=torch.float64, device=device)
+    with torch.cuda.device(device):
+        per = (nz, nz, neq * nz, neq, nz if plan.has_lb else 0, nz if plan.has_ub else 0)
+        tans = _qp.tangent_args(tangents, (2, 2, 3, 2, 2, 2), per, device)
+        rhs = torch.empty(B * (nz + m + neq), **f64)
+        dz = torch.empty(B, nz, **f64)
+        dlam = torch.empty(B, m, **f64)
+        dnu = torch.empty(B, neq, **f64) if neq > 0 else None
+        args = []
+        for t, s in tans:
+            args += [_ptr(t), s]
+        _lib.check(lib.qpb200_box_jvp(
+            ctypes.byref(plan), B, _ptr(st.q), st.sq, _ptr(st.A), st.sA, *args, _ptr(st.zhat), _ptr(st.lam),
+            _ptr(st.slacks), _ptr(st.nus), _ptr(rhs), _ptr(dz), _ptr(dlam), _ptr(dnu), _stream()))
+    return dz, dlam, dnu
+
+
 # ---- shapes beyond the box kernels: the dense kernels on the dense equivalent ---------------------------------------
 def dense_equivalent(q, lb, ub):
     """(Q, G, h) of QPFunction for a box QP: Q = diag(q), G = [-I; I] (sides given), h = [-lb; ub]. Batched where
@@ -201,6 +227,23 @@ def dense_backward(st, dl, mean_flags, want, nlb, has_ub, dl_dlam=None, dl_dnu=N
     return [dq, dp, dA, db, dlb, dub]
 
 
+def dense_jvp(st, tangents, nlb, has_ub):
+    """solve_box_jvp on the dense equivalent: dQ = diag(dq), no dG, dh = [-dlb; dub] (a missing side's tangent is 0)."""
+    dst, _ = st.dense
+    dq, dp, dA, db, dlb, dub = tangents
+    dQ = None if dq is None else torch.diag_embed(dq)
+    dh = None
+    if dlb is not None or dub is not None:
+        sides = ([None if dlb is None else -dlb] if nlb else []) + ([dub] if has_ub else [])
+        like = next(s for s in sides if s is not None)
+        sides = [torch.zeros_like(like) if s is None else s for s in sides]
+        if any(s.dim() == 2 for s in sides):
+            B = next(s.size(0) for s in sides if s.dim() == 2)
+            sides = [s if s.dim() == 2 else s.unsqueeze(0).expand(B, s.size(-1)) for s in sides]
+        dh = torch.cat(sides, -1)
+    return _qp.solve_jvp(dst, (dQ, dp, None, dh, dA, db))
+
+
 def BoxQPFunction(eps=1e-12, verbose=0, notImprovedLim=3, maxIter=20, check_Q_spd=True, duals=False):
     """Factory with QPFunction's options; returns f(q, p, A, b, lb, ub) -> z (nBatch, nz).
 
@@ -209,7 +252,11 @@ def BoxQPFunction(eps=1e-12, verbose=0, notImprovedLim=3, maxIter=20, check_Q_sp
     ([lb rows; ub rows]), nus, iters, best_resid.
 
     duals=True: f returns (z, lam, nu) as QPFunction(duals=True) does: lam (nBatch, nineq) in the [lb rows; ub rows]
-    layout of last_solve(), nu (nBatch, neq) or (nBatch, 0), and a loss may use all three."""
+    layout of last_solve(), nu (nBatch, neq) or (nBatch, 0), and a loss may use all three.
+
+    Forward mode (torch.autograd.forward_ad) is supported as for QPFunction: rx = dq o z + dp + dA' nu, rz = [dlb; -dub],
+    ry = dA z - db on the right-hand side of the backward's solve (qpb200_box_jvp; the dense fallback maps the tangents
+    to its dense equivalent, dQ = diag(dq), dh = [-dlb; dub])."""
     _last = [None]
 
     class BoxQPFunctionFn(Function):
@@ -223,10 +270,19 @@ def BoxQPFunction(eps=1e-12, verbose=0, notImprovedLim=3, maxIter=20, check_Q_sp
             zhats = st.zhat.to(device=q_.device, dtype=q_.dtype)
             ctx.save_for_backward(zhats, q_, p_, A_, b_, lb_, ub_)
             ctx.lams, ctx.slacks, ctx.nus = st.lam, st.slacks, st.nus
+            ctx.out = (q_.device, q_.dtype)
+            ctx.sides = (q_.size(-1) if lb_ is not None else 0, ub_ is not None)
+            ctx.set_materialize_grads(False)
             if not duals:
                 return zhats
-            ctx.set_materialize_grads(False)
             return (zhats,) + _qp.dual_outputs(st, q_)
+
+        @staticmethod
+        def jvp(ctx, dq, dp, dA, db, dlb, dub):
+            tangents = (dq, dp, dA, db, dlb, dub)
+            st = ctx.st
+            out = solve_box_jvp(st, tangents) if st.dense is None else dense_jvp(st, tangents, *ctx.sides)
+            return _qp.jvp_outputs(*out, ctx.out, duals)
 
         @staticmethod
         def backward(ctx, dl_dzhat, dl_dlam=None, dl_dnu=None):

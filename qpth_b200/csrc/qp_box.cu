@@ -40,6 +40,7 @@
 // the device functions of the headers have external linkage (host stubs): give this build its own namespace
 #define qpb qpb_box
 #include "qp_pf.cuh"
+#include "qp_jvp.cuh"
 
 extern "C" void qpb200_internal_cuda_error(int err, const char* what);   // (qp_kernels.cu) records the message, per thread
 
@@ -1403,6 +1404,52 @@ __global__ void k_box_mean_outer(int B, int rows, int cols, const double* __rest
     out[(int64_t)r * cols + c] = s / (double)B;
 }
 
+// Forward mode (qpb200_box_jvp): the right-hand side of the JVP solve for one QP per CTA, whatever layout solves it,
+//   rx = dq o z + dp + dA' nu,   rz = [dlb; -dub] (lam's [lb rows; ub rows] layout),   ry = dA z - db,
+// written to rx (B,n), rz (B,m), ry (B,e). Each tangent has its own batch stride (0: shared) and may be NULL (zero:
+// never read). z, nu and the ry accumulator are staged in shared memory (n + 2 e doubles plus the column partials:
+// 200 KB at the plan's limits n = 16384, e = 4096); rx is written straight from the column pass of dA.
+// Algorithmic bytes per QP: 8 e n of dA (read once: 1.45 MB at the 9x9 sudoku shape, n = 729, e = 249), 8 (4 n + e) of
+// tangent vectors (dq, dp, dlb, dub, db), 8 (n + e) of z and nu, and 8 (n + m + e) written.
+constexpr int kJvpNT = 256;
+inline size_t box_jvp_smem_bytes(int n, int e) { return (size_t)(r8(n) + 2 * r8(e) + qpb::jvp::part_doubles(kJvpNT)) * 8; }
+__global__ void __launch_bounds__(kJvpNT)
+k_box_jvp_rhs(int n, int e, int nlb, int m, const double* __restrict__ dq, int64_t sdq, const double* __restrict__ dp,
+              int64_t sdp, const double* __restrict__ dA, int64_t sdA, const double* __restrict__ db, int64_t sdb,
+              const double* __restrict__ dlb, int64_t sdlb, const double* __restrict__ dub, int64_t sdub,
+              const double* __restrict__ zhat, const double* __restrict__ nus, double* __restrict__ rx,
+              double* __restrict__ rz, double* __restrict__ ry) {
+    QPB_SMEM;
+    const int64_t qp = blockIdx.x;
+    const int tid = threadIdx.x;
+    double* z = qsm;
+    double* nu = z + r8(n);
+    double* ay = nu + r8(e);
+    double* part = ay + r8(e);
+    for (int i = tid; i < n; i += kJvpNT) z[i] = zhat[qp * n + i];
+    for (int i = tid; i < e; i += kJvpNT) {
+        nu[i] = nus[qp * e + i];
+        ay[i] = db ? -db[qp * sdb + i] : 0.0;
+    }
+    __syncthreads();
+    auto x_part = [&](int c) {                   // dq o z + dp
+        double v = dp ? dp[qp * sdp + c] : 0.0;
+        return dq ? fma(dq[qp * sdq + c], z[c], v) : v;
+    };
+    if (dA && e > 0) {
+        qpb::jvp::contract<kJvpNT>(dA + qp * sdA, e, n, z, nu, part, [&](int r, double s) { ay[r] += s; },
+                                   [&](int c, double s) { rx[qp * n + c] = x_part(c) + s; });
+    } else {
+        for (int c = tid; c < n; c += kJvpNT) rx[qp * n + c] = x_part(c);
+        __syncthreads();
+    }
+    for (int i = tid; i < n; i += kJvpNT) {
+        if (nlb) rz[qp * m + i] = dlb ? dlb[qp * sdlb + i] : 0.0;
+        if (m > nlb) rz[qp * m + nlb + i] = dub ? -dub[qp * sdub + i] : 0.0;
+    }
+    for (int i = tid; i < e; i += kJvpNT) ry[qp * e + i] = ay[i];
+}
+
 std::mutex g_mu;
 // cudaFuncAttributeMaxDynamicSharedMemorySize already set, per (kernel, device): its high-water mark
 std::map<std::pair<const void*, int>, size_t> g_smem;
@@ -1621,6 +1668,36 @@ int qpb200_box_backward_duals(const qpb200_box_plan* plan, int nbatch, const dou
         if (db && mean_b) k_box_mean_vec<<<(e + TB - 1) / TB, TB, 0, st>>>(nbatch, e, dnuv, e, nullptr, -1.0, db);
     }
     return box_check_launch("k_box_mean");
+}
+
+int qpb200_box_jvp(const qpb200_box_plan* plan, int nbatch, const double* q, int64_t sq, const double* A, int64_t sA,
+                   const double* dq, int64_t sdq, const double* dp, int64_t sdp, const double* dA, int64_t sdA,
+                   const double* db, int64_t sdb, const double* dlb, int64_t sdlb, const double* dub, int64_t sdub,
+                   const double* zhat, const double* lam, const double* slacks, const double* nus, double* rhs,
+                   double* dz, double* dlam, double* dnu, void* stream) {
+    // every check of qpb200_box_backward_duals, before k_box_jvp_rhs is launched
+    int rc = box_plan_check(plan);
+    if (rc) return rc;
+    if (nbatch <= 0 || !q || !zhat || !lam || !slacks || !rhs || !dz || !dlam) return QPB200_ERR_BAD_ARG;
+    if (sdq < 0 || sdp < 0 || sdA < 0 || sdb < 0 || sdlb < 0 || sdub < 0) return QPB200_ERR_BAD_ARG;
+    if (plan->neq > 0 && (!A || !nus || !dnu)) return QPB200_ERR_BAD_ARG;
+    if (plan->neq == 0 && (dA || db || dnu)) return QPB200_ERR_BAD_ARG;
+    if ((dlb && !plan->has_lb) || (dub && !plan->has_ub)) return QPB200_ERR_BAD_ARG;
+    const int n = plan->nz, m = plan->nineq, e = plan->neq, nlb = plan->has_lb ? n : 0;
+    const size_t bytes = box_jvp_smem_bytes(n, e);
+    rc = box_set_smem(k_box_jvp_rhs, bytes);
+    if (rc) return rc;
+    const int64_t B = nbatch;
+    double* rx = rhs;
+    double* rz = rx + B * n;
+    double* ry = rz + B * m;
+    k_box_jvp_rhs<<<nbatch, kJvpNT, bytes, (cudaStream_t)stream>>>(n, e, nlb, m, dq, sdq, dp, sdp, dA, sdA, db, sdb, dlb,
+                                                                   sdlb, dub, sdub, zhat, nus, rx, rz, ry);
+    rc = box_check_launch("k_box_jvp_rhs");
+    if (rc) return rc;
+    return qpb200_box_backward_duals(plan, nbatch, q, sq, A, sA, rx, (dlb || dub) ? rz : nullptr, (dA || db) ? ry : nullptr,
+                                     zhat, lam, slacks, nus, nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0,
+                                     nullptr, 0, dz, dlam, dnu, stream);
 }
 
 int qpb200_box_solve_kkt(const qpb200_box_plan* plan, int nbatch, const double* q, int64_t sq, const double* A,

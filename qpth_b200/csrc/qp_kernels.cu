@@ -28,6 +28,7 @@
 #include "qp_device.cuh"
 #include "qp_fast.cuh"
 #include "qp_pf.cuh"
+#include "qp_jvp.cuh"
 
 using namespace qpb;
 
@@ -800,6 +801,61 @@ __global__ void k_mean_vec(int B, int len, const double* __restrict__ u, double 
     double s = 0.0;
     for (int bidx = 0; bidx < B; ++bidx) s += u[(int64_t)bidx * len + idx];
     out[idx] = s * scale / (double)B;
+}
+
+// Forward mode (qpb200_jvp): the right-hand side of the JVP solve for one QP per CTA (qp_jvp.cuh),
+//   rx = sym(dQ) z + dp + dG' lam + dA' nu,   rz = dG z - dh,   ry = dA z - db,
+// written to rx (B,n), rz (B,m), ry (B,e). Each tangent has its own batch stride (0: one tangent for every QP) and may
+// be NULL (zero: never read). z, lam, nu and the three accumulators are staged in shared memory, 2 (n + m + e) doubles
+// plus the column partials: 200 KB at n = m = e = 4096, the largest shape qpb200_plan_init accepts.
+// Algorithmic bytes per QP: 8 (n^2 + m n + e n) of tangent matrices (each element read once), 8 (n + m + e) of tangent
+// vectors and of z, lam, nu, and 8 (n + m + e) written.
+__host__ __device__ inline int jvp_r8(int v) { return (v + 7) & ~7; }
+inline size_t jvp_smem_bytes(int n, int m, int e) {
+    return (size_t)(2 * (jvp_r8(n) + jvp_r8(m) + jvp_r8(e)) + jvp::part_doubles(kThreads)) * 8;
+}
+__global__ void __launch_bounds__(kThreads)
+k_jvp_rhs(int n, int m, int e, const double* __restrict__ dQ, int64_t sdQ, const double* __restrict__ dp, int64_t sdp,
+          const double* __restrict__ dG, int64_t sdG, const double* __restrict__ dh, int64_t sdh,
+          const double* __restrict__ dA, int64_t sdA, const double* __restrict__ db, int64_t sdb,
+          const double* __restrict__ zhat, const double* __restrict__ lam, const double* __restrict__ nus,
+          double* __restrict__ rx, double* __restrict__ rz, double* __restrict__ ry) {
+    QPB_SMEM;
+    const int64_t qp = blockIdx.x;
+    const int tid = threadIdx.x;
+    double* z = qsm;
+    double* l = z + jvp_r8(n);
+    double* nu = l + jvp_r8(m);
+    double* ax = nu + jvp_r8(e);
+    double* az = ax + jvp_r8(n);
+    double* ay = az + jvp_r8(m);
+    double* part = ay + jvp_r8(e);
+    for (int i = tid; i < n; i += kThreads) {
+        z[i] = zhat[qp * n + i];
+        ax[i] = dp ? dp[qp * sdp + i] : 0.0;
+    }
+    for (int i = tid; i < m; i += kThreads) {
+        l[i] = lam[qp * m + i];
+        az[i] = dh ? -dh[qp * sdh + i] : 0.0;
+    }
+    for (int i = tid; i < e; i += kThreads) {
+        nu[i] = nus[qp * e + i];
+        ay[i] = db ? -db[qp * sdb + i] : 0.0;
+    }
+    __syncthreads();
+    if (dQ)
+        jvp::contract<kThreads>(dQ + qp * sdQ, n, n, z, z, part, [&](int r, double s) { ax[r] += 0.5 * s; },
+                                [&](int c, double s) { ax[c] += 0.5 * s; });
+    if (dG && m > 0)
+        jvp::contract<kThreads>(dG + qp * sdG, m, n, z, l, part, [&](int r, double s) { az[r] += s; },
+                                [&](int c, double s) { ax[c] += s; });
+    if (dA && e > 0)
+        jvp::contract<kThreads>(dA + qp * sdA, e, n, z, nu, part, [&](int r, double s) { ay[r] += s; },
+                                [&](int c, double s) { ax[c] += s; });
+    __syncthreads();
+    for (int i = tid; i < n; i += kThreads) rx[qp * n + i] = ax[i];
+    for (int i = tid; i < m; i += kThreads) rz[qp * m + i] = az[i];
+    for (int i = tid; i < e; i += kThreads) ry[qp * e + i] = ay[i];
 }
 
 
@@ -1719,6 +1775,83 @@ int qpb200_backward_reg_duals(const qpb200_plan* plan, int nbatch, const double*
     CK(cudaGetLastError());
     return launch_means(nbatch, plan->nz, plan->nineq, plan->neq, zhat, lam, nus, dQ, mean_Q, dp, mean_p, dG, mean_G, dh,
                         mean_h, dA, mean_A, db, mean_b, dxv, dlamv, dnuv, st);
+}
+
+// ---- forward mode: k_jvp_rhs, then the backward-with-duals solve with the right-hand side it wrote -------------------
+// Every argument check of the solve runs here too, before k_jvp_rhs is launched.
+static int check_jvp_args(const qpb200_plan* plan, int nbatch, int64_t sdQ, int64_t sdp, int64_t sdG, int64_t sdh,
+                          int64_t sdA, int64_t sdb, const double* dG, const double* dh, const double* dA,
+                          const double* db, const double* zhat, const double* lam, const double* slacks,
+                          const double* nus, const double* Lfac, const double* Wfac, const double* Kfac,
+                          const double* rhs, const double* dz, const double* dlam, const double* dnu,
+                          const double* scratch) {
+    if (!plan || nbatch <= 0 || !zhat || !lam || !slacks || !Lfac || !Wfac || !Kfac || !rhs || !dz || !dlam)
+        return QPB200_ERR_BAD_ARG;
+    if (sdQ < 0 || sdp < 0 || sdG < 0 || sdh < 0 || sdA < 0 || sdb < 0) return QPB200_ERR_BAD_ARG;
+    if (plan->neq > 0 && (!nus || !dnu)) return QPB200_ERR_BAD_ARG;
+    if (plan->neq == 0 && (dA || db || dnu)) return QPB200_ERR_BAD_ARG;
+    if (plan->nineq == 0 && (dG || dh)) return QPB200_ERR_BAD_ARG;
+    // the generic global-scratch kernels (the only plan neither tiny, product form, fast nor resident) need scratch
+    if (!plan->tiny && !plan->pf && !plan->fast && !plan->smem_resident && !scratch) return QPB200_ERR_BAD_ARG;
+    return QPB200_OK;
+}
+
+static int launch_jvp_rhs(const qpb200_plan* plan, int nbatch, const double* dQ, int64_t sdQ, const double* dp,
+                          int64_t sdp, const double* dG, int64_t sdG, const double* dh, int64_t sdh, const double* dA,
+                          int64_t sdA, const double* db, int64_t sdb, const double* zhat, const double* lam,
+                          const double* nus, double* rhs, cudaStream_t st) {
+    const int n = plan->nz, m = plan->nineq, e = plan->neq;
+    const size_t bytes = jvp_smem_bytes(n, m, e);
+    int rc = set_smem(k_jvp_rhs, bytes);
+    if (rc) return rc;
+    double* rx = rhs;
+    double* rz = rx + (int64_t)nbatch * n;
+    double* ry = rz + (int64_t)nbatch * m;
+    k_jvp_rhs<<<nbatch, kThreads, bytes, st>>>(n, m, e, dQ, sdQ, dp, sdp, dG, sdG, dh, sdh, dA, sdA, db, sdb, zhat, lam,
+                                               nus, rx, rz, ry);
+    CK(cudaGetLastError());
+    return QPB200_OK;
+}
+
+int qpb200_jvp(const qpb200_plan* plan, int nbatch, const double* dQ, int64_t sdQ, const double* dp, int64_t sdp,
+               const double* dG, int64_t sdG, const double* dh, int64_t sdh, const double* dA, int64_t sdA,
+               const double* db, int64_t sdb, const double* zhat, const double* lam, const double* slacks,
+               const double* nus, const double* Lfac, const double* Wfac, const double* Kfac, int sF, double* rhs,
+               double* dz, double* dlam, double* dnu, double* scratch, void* stream) {
+    int rc = check_jvp_args(plan, nbatch, sdQ, sdp, sdG, sdh, sdA, sdb, dG, dh, dA, db, zhat, lam, slacks, nus, Lfac,
+                            Wfac, Kfac, rhs, dz, dlam, dnu, scratch);
+    if (rc) return rc;
+    rc = launch_jvp_rhs(plan, nbatch, dQ, sdQ, dp, sdp, dG, sdG, dh, sdh, dA, sdA, db, sdb, zhat, lam, nus, rhs,
+                        (cudaStream_t)stream);
+    if (rc) return rc;
+    const int64_t B = nbatch;
+    const double* rz = (dG || dh) ? rhs + B * plan->nz : nullptr;                    // NULL: the solve reads no zeros
+    const double* ry = (dA || db) ? rhs + B * (plan->nz + plan->nineq) : nullptr;
+    return qpb200_backward_duals(plan, nbatch, rhs, rz, ry, zhat, lam, slacks, nus, Lfac, Wfac, Kfac, sF, nullptr, 0,
+                                 nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0, dz, dlam, dnu, scratch,
+                                 stream);
+}
+
+int qpb200_jvp_reg(const qpb200_plan* plan, int nbatch, const double* dQ, int64_t sdQ, const double* dp, int64_t sdp,
+                   const double* dG, int64_t sdG, const double* dh, int64_t sdh, const double* dA, int64_t sdA,
+                   const double* db, int64_t sdb, const double* zhat, const double* lam, const double* slacks,
+                   const double* nus, const double* Lfac, const double* Wfac, const double* Kfac, int sF,
+                   double reg_eps, int ir_steps, double* rhs, double* dz, double* dlam, double* dnu, double* scratch,
+                   void* stream) {
+    int rc = check_jvp_args(plan, nbatch, sdQ, sdp, sdG, sdh, sdA, sdb, dG, dh, dA, db, zhat, lam, slacks, nus, Lfac,
+                            Wfac, Kfac, rhs, dz, dlam, dnu, scratch);
+    if (rc) return rc;
+    rc = check_reg_plan(plan, reg_eps, ir_steps, scratch);
+    if (rc) return rc;
+    rc = launch_jvp_rhs(plan, nbatch, dQ, sdQ, dp, sdp, dG, sdG, dh, sdh, dA, sdA, db, sdb, zhat, lam, nus, rhs,
+                        (cudaStream_t)stream);
+    if (rc) return rc;
+    const int64_t B = nbatch;
+    const double* rz = (dG || dh) ? rhs + B * plan->nz : nullptr;
+    const double* ry = (dA || db) ? rhs + B * (plan->nz + plan->nineq) : nullptr;
+    return qpb200_backward_reg_duals(plan, nbatch, rhs, rz, ry, zhat, lam, slacks, nus, Lfac, Wfac, Kfac, sF, reg_eps,
+                                     ir_steps, nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0,
+                                     dz, dlam, dnu, scratch, stream);
 }
 
 #ifdef QPB_TIMING

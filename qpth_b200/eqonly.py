@@ -65,12 +65,37 @@ class QPEqualityFn(Function):
         ctx.QA, ctx.steps = (Q, A), steps
         ctx.zhat64, ctx.nus = zhat, nus
         ctx.meta = [(X.device, X.dtype) for X in (Q_, p_, A_, b_)]
+        ctx.duals = duals
+        ctx.set_materialize_grads(False)
         zhat_out = zhat.to(device=Q_.device, dtype=Q_.dtype)
         if not duals:
             return zhat_out
         # duals: no inequality rows (lam is (nBatch, 0)); nu is the dy of the solve
-        ctx.set_materialize_grads(False)
         return zhat_out, Q_.new_zeros(nBatch, 0), nus.to(device=Q_.device, dtype=Q_.dtype)
+
+    @staticmethod
+    def jvp(ctx, dQ, dp, dA, db, *_):
+        # the backward's solve with rx = sym(dQ) z + dp + dA' nu and ry = dA z - db (the dummy row's rz is 0)
+        z, nus = ctx.zhat64, ctx.nus
+        T = lambda t: None if t is None else t.detach().to(device=z.device, dtype=torch.float64)
+        dQ, dp, dA, db = T(dQ), T(dp), T(dA), T(db)
+        rx, ry = torch.zeros_like(z), torch.zeros_like(nus)
+        if dQ is not None:
+            zc = z.unsqueeze(2)
+            rx = rx + 0.5 * (torch.matmul(dQ, zc) + torch.matmul(dQ.transpose(-1, -2), zc)).squeeze(2)
+        if dp is not None:
+            rx = rx + dp
+        if dA is not None:
+            rx = rx + torch.matmul(dA.transpose(-1, -2), nus.unsqueeze(2)).squeeze(2)
+            ry = ry + torch.matmul(dA, z.unsqueeze(2)).squeeze(2)
+        if db is not None:
+            ry = ry - db
+        dx, _, _, dnu = _solve(ctx.F, *ctx.QA, ctx.one, rx.contiguous(), ctx.zero, ctx.zero, ry.contiguous(), ctx.steps)
+        dev, dt = ctx.meta[0]
+        dz = dx.to(device=dev, dtype=dt)
+        if not ctx.duals:
+            return dz
+        return dz, torch.zeros(dz.shape[0], 0, device=dev, dtype=dt), dnu.to(device=dev, dtype=dt)
 
     @staticmethod
     def backward(ctx, dl_dzhat, dl_dlam=None, dl_dnu=None):

@@ -294,6 +294,60 @@ def solve_backward(st, dl_dzhat, mean_flags, want, dl_dlam=None, dl_dnu=None):
     return outs
 
 
+def tangent_args(tangents, ranks, per, device):
+    """Forward-mode input tangents as (fp64 device tensor, batch stride) pairs for the C ABI: None (no tangent) stays
+    None with stride 0, an un-batched tangent (rank - 1 dimensions) gets stride 0, a batched one `per` elements."""
+    out = []
+    for t, r, n in zip(tangents, ranks, per):
+        if t is None or t.numel() == 0 or n == 0:
+            out.append((None, 0))
+        else:
+            out.append((_dev64(t, device), n if t.dim() == r else 0))
+    return out
+
+
+def solve_jvp(st, tangents):
+    """The JVP of (zhat, lam, nu) at the returned point on the device. tangents: (dQ, dp, dG, dh, dA, db), each None
+    (zero), batched or un-batched as its input. Returns fp64 (dz (B,nz), dlam (B,nineq), dnu (B,neq) or None); one
+    qpb200_jvp(_reg) call: the right-hand side kernel and the backward's KKT solve."""
+    if _pending:
+        flush_checks(wait=False)
+    lib = _lib.load()
+    plan, B, device = st.plan, st.nBatch, st.device
+    nz, nineq, neq = plan.nz, plan.nineq, plan.neq
+    f64 = dict(dtype=torch.float64, device=device)
+    with torch.cuda.device(device):
+        tans = tangent_args(tangents, (3, 2, 3, 2, 3, 2),
+                            (nz * nz, nz, nineq * nz, nineq, neq * nz, neq), device)
+        rhs = torch.empty(B * (nz + nineq + neq), **f64)
+        dz = torch.empty(B, nz, **f64)
+        dlam = torch.empty(B, nineq, **f64)
+        dnu = torch.empty(B, neq, **f64) if neq > 0 else None
+        args = []
+        for t, s in tans:
+            args += [_ptr(t), s]
+        reg = getattr(st, "reg", False)             # (solution.py builds _Solved without it: the default path)
+        _lib.check((lib.qpb200_jvp_reg if reg else lib.qpb200_jvp)(
+            ctypes.byref(plan), B, *args, _ptr(st.zhat), _ptr(st.lam), _ptr(st.slacks), _ptr(st.nus),
+            _ptr(st.L), _ptr(st.W), _ptr(st.K), 1 if st.nsys > 1 else 0,
+            *((float(kkt.IR_EPS), int(kkt.IR_STEPS)) if reg else ()),
+            _ptr(rhs), _ptr(dz), _ptr(dlam), _ptr(dnu), _ptr(st.scratch), _stream()))
+    return dz, dlam, dnu
+
+
+def jvp_outputs(dz, dlam, dnu, out, duals):
+    """The output tangents of a Function whose outputs have out = (device, dtype): dz, or (dz, dlam, dnu) with duals
+    (dnu (B, 0) without equality rows). Every output gets a tensor: forward AD does not take None for an output of
+    these Functions."""
+    device, dtype = out
+    z = dz.to(device=device, dtype=dtype)
+    if not duals:
+        return z
+    nu = (dnu.to(device=device, dtype=dtype) if dnu is not None
+          else torch.zeros(dz.shape[0], 0, device=device, dtype=dtype))
+    return z, dlam.to(device=device, dtype=dtype), nu
+
+
 def check_kkt_solver(kkt_solver):
     if kkt_solver == KKTSolvers.LU_FULL:
         raise ValueError("qpth_b200: KKTSolvers.LU_FULL is not provided; use KKTSolvers.LU_PARTIAL (Q positive definite) "
@@ -313,6 +367,11 @@ def QPFunction(eps=1e-12, verbose=0, notImprovedLim=3, maxIter=20, solver=QPSolv
     [Q 0 G' A'; 0 D I 0; G I 0 0; A 0 0 0] [dx ds dlam dnu] = -[dl/dz; 0; dl/dlam; dl/dnu], and the gradient formulas
     are unchanged. With linearly dependent equality rows (IR_UNOPT) nu is not unique, and the gradient through nu is
     that of the nu returned. Slacks are not an output: s = h - Gz.
+
+    Forward mode (torch.autograd.forward_ad, gradcheck's check_forward_ad) is supported: the tangents of the outputs are
+    one solve of the backward's system with -[rx; 0; rz; ry], rx = sym(dQ) z + dp + dG' lam + dA' nu, rz = dG z - dh,
+    ry = dA z - db (qpb200_jvp), the exact transpose of the backward pass. The tangent of an un-batched input applies
+    to every QP and gives the true derivative, where the backward returns the batch mean.
 
     kkt_solver (an extension of the reference's signature): KKTSolvers.LU_PARTIAL, the default, needs Q positive definite.
     KKTSolvers.IR_UNOPT also solves QPs whose Q is only positive semidefinite (LPs with Q = 0, low-rank quadratic terms)
@@ -361,10 +420,16 @@ def QPFunction(eps=1e-12, verbose=0, notImprovedLim=3, maxIter=20, solver=QPSolv
             ctx.save_for_backward(zhats, Q_, p_, G_, h_, A_, b_)
             # parity with the reference's ctx attributes (device fp64 views)
             ctx.lams, ctx.slacks, ctx.nus = st.lam, st.slacks, st.nus
+            ctx.out = (Q_.device, Q_.dtype)
+            # an unused output's gradient, and an input without a tangent, arrive as None: nothing zero-filled is read
+            ctx.set_materialize_grads(False)
             if not duals:
                 return zhats
-            ctx.set_materialize_grads(False)       # an unused output's gradient arrives as None: no adjoint is read
             return (zhats,) + dual_outputs(st, Q_)
+
+        @staticmethod
+        def jvp(ctx, dQ, dp, dG, dh, dA, db):
+            return jvp_outputs(*solve_jvp(ctx.st, (dQ, dp, dG, dh, dA, db)), ctx.out, duals)
 
         @staticmethod
         def backward(ctx, dl_dzhat, dl_dlam=None, dl_dnu=None):

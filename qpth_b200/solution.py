@@ -99,6 +99,9 @@ def QPSolutionFunction(check_Q_spd=True, kkt_solver=KKTSolvers.LU_PARTIAL, duals
     duals=True: f returns (zhat, lam, nu), the given solution's duals as functions of Q, p, G, h, A, b (nu is (nBatch, 0)
     without equality rows), as QPFunction(duals=True) does; a loss may use all three.
 
+    Forward mode (torch.autograd.forward_ad) is supported as for QPFunction; the tangents of the four solution tensors
+    are ignored.
+
     kkt_solver: KKTSolvers.LU_PARTIAL (the default) needs Q positive definite. KKTSolvers.IR_UNOPT differentiates with
     the regularised KKT solve of QPFunction(kkt_solver=IR_UNOPT), so an LP (Q = 0) or a low-rank Q solved by any solver
     can be differentiated; check_Q_spd then checks that Q is positive semidefinite."""
@@ -111,11 +114,18 @@ def QPSolutionFunction(check_Q_spd=True, kkt_solver=KKTSolvers.LU_PARTIAL, duals
             zhats = ctx.st.zhat.to(device=Q_.device, dtype=Q_.dtype)
             ctx.save_for_backward(zhats, Q_, p_, G_, h_, A_, b_)
             ctx.lams, ctx.slacks, ctx.nus = ctx.st.lam, ctx.st.slacks, ctx.st.nus
+            ctx.out = (Q_.device, Q_.dtype)
+            ctx.set_materialize_grads(False)
             if not duals:
                 return zhats
             from .qp import dual_outputs
-            ctx.set_materialize_grads(False)
             return (zhats,) + dual_outputs(ctx.st, Q_)
+
+        @staticmethod
+        def jvp(ctx, dQ, dp, dG, dh, dA, db, *solution_tangents):
+            # the solution tensors are constants of this node: their tangents are ignored
+            from .qp import jvp_outputs, solve_jvp
+            return jvp_outputs(*solve_jvp(ctx.st, (dQ, dp, dG, dh, dA, db)), ctx.out, duals)
 
         @staticmethod
         def backward(ctx, dl_dzhat, dl_dlam=None, dl_dnu=None):
