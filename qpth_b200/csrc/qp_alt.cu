@@ -158,4 +158,26 @@ int QPB_ALT_NAME(_backward)(const qpb200_plan* plan, size_t smem, int nbatch, co
     return alt_check_launch();
 }
 
+#ifdef QPB_TIMING
+// the cycle accounting of this build's k_forward_fast (its own g_tim / g_cta: the namespace differs from qp_kernels.cu's)
+int QPB_ALT_NAME(_debug_timing)(long long* host64, int reset) {
+    cudaError_t e;
+    if (reset) {
+        long long z[128] = {0};
+        const int target = reset >= 2 ? reset - 2 : 0;
+        e = cudaMemcpyToSymbol(qpb::fast::g_tim, z, sizeof(z));
+        if (e == cudaSuccess) e = cudaMemcpyToSymbol(qpb::fast::g_tim_target, &target, sizeof(int));
+    } else {
+        e = cudaMemcpyFromSymbol(host64, qpb::fast::g_tim, 128 * sizeof(long long));
+    }
+    if (e != cudaSuccess) { qpb200_internal_cuda_error((int)e, "debug_timing (qp_alt.cu)"); return QPB200_ERR_CUDA; }
+    return QPB200_OK;
+}
+int QPB_ALT_NAME(_debug_cta)(long long* host64, int nqp) {
+    const cudaError_t e = cudaMemcpyFromSymbol(host64, qpb::fast::g_cta, (size_t)4 * nqp * sizeof(long long));
+    if (e != cudaSuccess) { qpb200_internal_cuda_error((int)e, "debug_cta (qp_alt.cu)"); return QPB200_ERR_CUDA; }
+    return QPB200_OK;
+}
+#endif
+
 }  // extern "C"

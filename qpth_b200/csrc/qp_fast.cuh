@@ -26,22 +26,24 @@ __device__ int g_tim_target = 0;          // which QP's phase slots are exported
 __device__ __forceinline__ long long gtimer() { long long t; asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t)); return t; }
 __device__ __forceinline__ int smid() { int r; asm volatile("mov.u32 %0, %smid;" : "=r"(r)); return r; }
 __device__ long long g_tim[128];
-// accumulators live in (static) shared memory so that a tick costs ~40 cycles, not a global round trip
-__shared__ long long s_tim[129];
+// accumulators live in (static) shared memory so that a tick costs ~40 cycles, not a global round trip. 32-bit
+// (differences of the low clock word; one QP's slot stays far below 2^32 cycles): 520 B instead of 1,040 B of static
+// shared memory, so a timing build of the three-per-SM forward (76.2 KB dynamic at C2) still fits three CTAs per SM.
+__shared__ unsigned s_tim[129];
 #define QPB_TICK(i)                                                         \
     do {                                                                    \
         if (threadIdx.x == 0) {                                             \
-            const long long _t = clock64();                                 \
+            const unsigned _t = (unsigned)clock64();                        \
             s_tim[i] += _t - s_tim[128];                                    \
             s_tim[128] = _t;                                                \
         }                                                                   \
     } while (0)
 // second clock on thread 32 (warp 1, an update warp): slots 40.., own time base in s_tim2
-__shared__ long long s_tim2;
+__shared__ unsigned s_tim2;
 #define QPB_TICK1(i)                                                        \
     do {                                                                    \
         if (threadIdx.x == 32) {                                            \
-            const long long _t = clock64();                                 \
+            const unsigned _t = (unsigned)clock64();                        \
             s_tim[i] += _t - s_tim2;                                        \
             s_tim2 = _t;                                                    \
         }                                                                   \
@@ -55,6 +57,14 @@ __shared__ long long s_tim2;
 #define QPB_NT 256       // CTA size of the solve kernels; qp_alt.cu builds the product-form ones at 192 and 512 threads as well
 #endif
 constexpr int kNT = QPB_NT;
+// threadIdx.x read at the point of use. A value kept in a register across the __noinline__ calls of a long kernel body
+// is, under register pressure, spilled and reloaded from local memory (ptxas does not re-read the special register
+// itself); the volatile read cannot be hoisted, so every use costs one S2R instead.
+__device__ __forceinline__ int tid_x() {
+    int t;
+    asm volatile("mov.u32 %0, %%tid.x;" : "=r"(t));
+    return t;
+}
 
 // ---- 8x8 diagonal block helpers (always full blocks here) -------------------------------------------
 // Storage convention of a factored diagonal block: strictly-lower part = L, DIAGONAL = 1 / L_cc.
@@ -818,17 +828,32 @@ __device__ __noinline__ double g_tri_norm2(const double* __restrict__ Lg, int n,
 }
 
 constexpr int kFastStride = (kNT / 32 <= 8) ? 8 : 16;       // per-value stride of the fast kernels' reduction scratch
-__device__ __noinline__ void f_reduce_sum4(double (&v)[4], int red) {
+// The shared reductions take and return their values in registers: an array passed by reference to a __noinline__
+// function has to live in local memory.
+__device__ __noinline__ double4 f_reduce_sum4_r(double a, double b, double c, double d, int red) {
     QPB_SMEM;
+    double v[4] = {a, b, c, d};
     block_reduce<4, false, kFastStride>(v, qsm + red, (int)threadIdx.x, kNT);
+    return make_double4(v[0], v[1], v[2], v[3]);
 }
-__device__ __noinline__ void f_reduce_sum2(double (&v)[2], int red) {
+template <bool kMin>
+__device__ __noinline__ double2 f_reduce2_r(double a, double b, int red) {
     QPB_SMEM;
-    block_reduce<2, false, kFastStride>(v, qsm + red, (int)threadIdx.x, kNT);
+    double v[2] = {a, b};
+    block_reduce<2, kMin, kFastStride>(v, qsm + red, (int)threadIdx.x, kNT);
+    return make_double2(v[0], v[1]);
 }
-__device__ __noinline__ void f_reduce_min2(double (&v)[2], int red) {
-    QPB_SMEM;
-    block_reduce<2, true, kFastStride>(v, qsm + red, (int)threadIdx.x, kNT);
+__device__ __forceinline__ void f_reduce_sum4(double (&v)[4], int red) {
+    const double4 r = f_reduce_sum4_r(v[0], v[1], v[2], v[3], red);
+    v[0] = r.x; v[1] = r.y; v[2] = r.z; v[3] = r.w;
+}
+__device__ __forceinline__ void f_reduce_sum2(double (&v)[2], int red) {
+    const double2 r = f_reduce2_r<false>(v[0], v[1], red);
+    v[0] = r.x; v[1] = r.y;
+}
+__device__ __forceinline__ void f_reduce_min2(double (&v)[2], int red) {
+    const double2 r = f_reduce2_r<true>(v[0], v[1], red);
+    v[0] = r.x; v[1] = r.y;
 }
 
 }  // namespace fast

@@ -328,6 +328,10 @@ __device__ __forceinline__ void pf_chol_setup(int S, int nts, int kb0, int kend,
 // a named barrier, and one warp running the whole sweep (four rows per lane, __syncwarp between steps) at about 1.8x
 // the cycles per sweep in the latency-mode kernel; prefetching that warp's next P rows into registers spilled in the
 // three-per-SM build and was slower still.
+// kPrefetch: each thread loads its P row of the next step before the step barrier. Without it (the forward kernels of
+// two and three QPs per SM) the row is loaded after the barrier: there the eight doubles carried across the barrier did
+// not fit the registers ptxas leaves this subroutine and went to local memory on every step. Same loads, same arithmetic.
+template <bool kPrefetch = true>
 __device__ __noinline__ void pf_fwd(int S, int n, int kb, int ke, int b) {
     QPB_SMEM;
     const int tid = threadIdx.x;
@@ -337,12 +341,13 @@ __device__ __noinline__ void pf_fwd(int S, int n, int kb, int ke, int b) {
         const int ro = pf_rowoff(mine ? tid : 0);
         double acc = mine ? qsm[b + tid] : 0.0;
         double row[8];
-        if (mine && tid >= 8 * kb + 8 && kb < ke) f_ld8(M + ro + 8 * kb, row);
+        if (kPrefetch && mine && tid >= 8 * kb + 8 && kb < ke) f_ld8(M + ro + 8 * kb, row);
 #pragma unroll 1
         for (int k = kb; k < ke; ++k) {
             const int k0 = 8 * k;
             if (mine && tid >= k0 + 8) {
                 double y[8];
+                if (!kPrefetch) f_ld8(M + ro + k0, row);
                 f_ld8(qsm + b + k0, y);
                 double s1 = row[1] * y[1];
                 acc = fma(-row[0], y[0], acc); s1 = fma(row[3], y[3], s1);
@@ -351,7 +356,7 @@ __device__ __noinline__ void pf_fwd(int S, int n, int kb, int ke, int b) {
                 acc = fma(-row[6], y[6], acc);
                 acc -= s1;
                 if (tid < k0 + 16) qsm[b + tid] = acc;           // block k+1 becomes final
-                else if (k + 1 < ke) f_ld8(M + ro + k0 + 8, row);  // next step's P row (static data: no hazard)
+                else if (kPrefetch && k + 1 < ke) f_ld8(M + ro + k0 + 8, row);   // next step's P row (static data: no hazard)
             }
             __syncthreads();
         }
@@ -396,7 +401,9 @@ __device__ __noinline__ void pf_diag(int S, int n, int b, int y, int c) {
     __syncthreads();
 }
 
-// w_k = c_k - sum_{i > k} P_ik^T w_i. c is only read. c != w. Ends with a block barrier.
+// w_k = c_k - sum_{i > k} P_ik^T w_i. c is only read. c != w. Ends with a block barrier. kPrefetch as in pf_fwd (the
+// P column of the next step).
+template <bool kPrefetch = true>
 __device__ __noinline__ void pf_bwd(int S, int n, int c, int w) {
     QPB_SMEM;
     const int tid = threadIdx.x;
@@ -406,7 +413,7 @@ __device__ __noinline__ void pf_bwd(int S, int n, int c, int w) {
         double acc = (tid < n) ? qsm[c + tid] : 0.0;
         if (tid >= n - 8 && tid < n) qsm[w + tid] = acc;
         double col[8];
-        {
+        if (kPrefetch) {
             const int i = nts - 1, ldi = 8 * i + 12;
             const double* Pc = M + (32 * i + 64) * i + tid;
             if (tid < 8 * i) {
@@ -420,6 +427,12 @@ __device__ __noinline__ void pf_bwd(int S, int n, int c, int w) {
             const int i0 = 8 * i;
             if (tid < i0) {
                 double y[8];
+                if (!kPrefetch) {
+                    const int ldi = 8 * i + 12;
+                    const double* Pc = M + (32 * i + 64) * i + tid;
+#pragma unroll
+                    for (int r = 0; r < 8; ++r) col[r] = Pc[r * ldi];
+                }
                 f_ld8(qsm + w + i0, y);
                 double s1 = col[1] * y[1];
                 acc = fma(-col[0], y[0], acc); s1 = fma(col[3], y[3], s1);
@@ -428,7 +441,7 @@ __device__ __noinline__ void pf_bwd(int S, int n, int c, int w) {
                 acc = fma(-col[6], y[6], acc);
                 acc -= s1;
                 if (tid >= i0 - 8) qsm[w + tid] = acc;           // block i-1 becomes final
-                else {
+                else if (kPrefetch) {
                     const int im = i - 1, ldm = 8 * im + 12;
                     const double* Pc = M + (32 * im + 64) * im + tid;
 #pragma unroll
@@ -442,10 +455,11 @@ __device__ __noinline__ void pf_bwd(int S, int n, int c, int w) {
 }
 
 // Full solve with a product-form factor: rhs (destroyed) -> out. y: scratch. rhs, y, out distinct.
+template <bool kPrefetch = true>
 __device__ __forceinline__ void pf_solve(int S, int n, int rhs, int y, int out) {
-    pf_fwd(S, n, 0, (n >> 3) - 1, rhs);
+    pf_fwd<kPrefetch>(S, n, 0, (n >> 3) - 1, rhs);
     pf_diag(S, n, rhs, y, rhs);
-    pf_bwd(S, n, rhs, out);
+    pf_bwd<kPrefetch>(S, n, rhs, out);
 }
 
 // ---- pre_factor_kkt side: equality columns of the K template into product form, K into the staircase ----------------

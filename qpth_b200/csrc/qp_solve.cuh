@@ -214,21 +214,20 @@ __device__ __forceinline__ void f_factor_and_solve(const KDims& D, FCtx& C) {
 
 // The same with the product-form factor (qp_pf.cuh): F_AUG = -h_full, F_D = d  ->  F_W = -S^-1 h_full; F_T0 scratch.
 // kReg: F_D holds d + eps and the inequality diagonal gets 1 / (d + eps) + eps (the regularised system; the eps of the
-// equality rows is already in K, pre_factor_kkt_reg).
-template <bool kReg = false>
+// equality rows is already in K, pre_factor_kkt_reg). kPrefetch: of the substitutions (pf_fwd, pf_bwd).
+template <bool kReg = false, bool kPrefetch = true>
 __device__ __forceinline__ void f_factor_and_solve_pf(const KDims& D, FCtx& C) {
     QPB_SMEM;
     using namespace qpb::pf;
-    const int tid = threadIdx.x;
     f_wait_K(C);
-    _Pragma("unroll 1") for (int i = D.ep + tid; i < D.ms; i += kNT)
+    _Pragma("unroll 1") for (int i = D.ep + tid_x(); i < D.ms; i += kNT)
         qsm[C.L.LS + pf_rowoff(i) + i] += kReg ? 1.0 / qsm[FV(F_D) + i] + D.reg : 1.0 / qsm[FV(F_D) + i];
     __syncthreads();
-    if (D.ep > 0) pf_fwd(C.L.LS, D.msp, 0, D.ep >> 3, FV(F_AUG));
+    if (D.ep > 0) pf_fwd<kPrefetch>(C.L.LS, D.msp, 0, D.ep >> 3, FV(F_AUG));
     pf_chol(C.L.LS, D.msp >> 3, D.ep >> 3, FV(F_AUG), C.L.pan, C.L.tab);
     QPB_TICK(32);
     pf_diag(C.L.LS, D.msp, FV(F_AUG), FV(F_T0), FV(F_AUG));
-    pf_bwd(C.L.LS, D.msp, FV(F_AUG), FV(F_W));
+    pf_bwd<kPrefetch>(C.L.LS, D.msp, FV(F_AUG), FV(F_W));
     QPB_TICK(33);
 }
 
@@ -343,7 +342,8 @@ k_forward_fast(KDims D, const double* __restrict__ p, int64_t sp, const double* 
                double* __restrict__ trace, int ir_steps = 0) {
     using namespace fk;
     QPB_SMEM;
-    const int tid = threadIdx.x;
+    // the co-resident builds (two or three QPs per SM) load the substitutions' P rows after each step barrier
+    constexpr bool kPrefetchP = kMinCtas == 0;
     const int qp = blockIdx.x;
     const int n = D.n, m = D.m, e = D.e, ep = D.ep, ms = D.ms, msp = D.msp;
 #ifdef QPB_TIMING
@@ -363,8 +363,8 @@ k_forward_fast(KDims D, const double* __restrict__ p, int64_t sp, const double* 
     const double* pg = p + (int64_t)qp * sp;
     const double* hg = h + (int64_t)qp * sh;
     const double* bg = (e > 0) ? (b + (int64_t)qp * sb) : nullptr;
-    _Pragma("unroll 1") for (int i = tid; i < n; i += kNT) qsm[t1 + i] = pg[i];
-    _Pragma("unroll 1") for (int i = tid; i < msp; i += kNT) {
+    _Pragma("unroll 1") for (int i = tid_x(); i < n; i += kNT) qsm[t1 + i] = pg[i];
+    _Pragma("unroll 1") for (int i = tid_x(); i < msp; i += kNT) {
         double val = 0.0;
         if (i < e) val = bg[i];
         else if (i >= ep && i < ms) val = hg[i - ep];
@@ -387,14 +387,14 @@ k_forward_fast(KDims D, const double* __restrict__ p, int64_t sp, const double* 
     // ---- initial point: solve_kkt(p, 0, -h, -b) with d = 1   (batch.py:61-67)
     mv_rows1<kCoop>(D, C, pt, hW);
     __syncthreads();
-    _Pragma("unroll 1") for (int i = tid; i < ms; i += kNT) qsm[aug + i] = -(qsm[hW + i] + qsm[hb + i]);
+    _Pragma("unroll 1") for (int i = tid_x(); i < ms; i += kNT) qsm[aug + i] = -(qsm[hW + i] + qsm[hb + i]);
     __syncthreads();
-    if (kPF) f_factor_and_solve_pf<kReg>(D, C); else f_factor_and_solve(D, C);
+    if (kPF) f_factor_and_solve_pf<kReg, kPrefetchP>(D, C); else f_factor_and_solve(D, C);
     const bool refine = kReg && ir_steps > 0;
     if (kReg) {
         // s = -w / (1 + eps); rv accumulates the x part of the refinement (x~ = -p~ + rv - W^T w)
-        _Pragma("unroll 1") for (int i = ep + tid; i < ms; i += kNT) qsm[s + i] = -qsm[w + i] / qsm[d + i];
-        _Pragma("unroll 1") for (int i = tid; i < n; i += kNT) qsm[rv + i] = 0.0;
+        _Pragma("unroll 1") for (int i = ep + tid_x(); i < ms; i += kNT) qsm[s + i] = -qsm[w + i] / qsm[d + i];
+        _Pragma("unroll 1") for (int i = tid_x(); i < n; i += kNT) qsm[rv + i] = 0.0;
         __syncthreads();
         _Pragma("unroll 1") for (int k = 0; k < ir_steps; ++k) f_refine<kCoop>(D, C, pt, rv, w, s, t1, t0, aug, hW, dsa, k == 0);
     }
@@ -402,7 +402,7 @@ k_forward_fast(KDims D, const double* __restrict__ p, int64_t sp, const double* 
     mv_cols<kCoop>(D, C, w, t0, t1, xt, pt, -1.0, refine ? rv : -1, -1.0);   // x~ = -p~ - W^T w
     {
         double mn[2] = {INFINITY, INFINITY};
-        _Pragma("unroll 1") for (int i = tid; i < ms; i += kNT) {
+        _Pragma("unroll 1") for (int i = tid_x(); i < ms; i += kNT) {
             const double wi = qsm[w + i];
             qsm[v + i] = wi;
             if (i >= ep) {
@@ -413,7 +413,7 @@ k_forward_fast(KDims D, const double* __restrict__ p, int64_t sp, const double* 
             }
         }
         f_reduce_min2(mn, C.L.red);
-        _Pragma("unroll 1") for (int i = ep + tid; i < ms; i += kNT) {               // slacks and duals >= 1 (batch.py:77-87)
+        _Pragma("unroll 1") for (int i = ep + tid_x(); i < ms; i += kNT) {               // slacks and duals >= 1 (batch.py:77-87)
             if (mn[0] < 0.0) qsm[s + i] -= mn[0] - 1.0;
             if (mn[1] < 0.0) qsm[v + i] -= mn[1] - 1.0;
         }
@@ -437,7 +437,7 @@ k_forward_fast(KDims D, const double* __restrict__ p, int64_t sp, const double* 
         acc[2] = kCoop ? g_tri_norm2(C.Lg, n, rxt) : f_tri_norm2(C.L.Lp, n, rxt);
         __syncthreads();
         QPB_TICK(5);
-        _Pragma("unroll 1") for (int i = tid; i < ms; i += kNT) {
+        _Pragma("unroll 1") for (int i = tid_x(); i < ms; i += kNT) {
             const double r = qsm[rv + i] - qsm[hb + i] + ((i >= ep) ? qsm[s + i] : 0.0);
             qsm[rv + i] = r;
             if (i < ep) acc[0] = fma(r, r, acc[0]);
@@ -448,7 +448,7 @@ k_forward_fast(KDims D, const double* __restrict__ p, int64_t sp, const double* 
         QPB_TICK(8);
         const double mu = fabs(acc[3] / dm);
         const double resid = sqrt(acc[1]) + sqrt(acc[0]) + sqrt(acc[2]) + dm * mu;
-        if (trace != nullptr && tid == 0) {                     // what verbose=1 prints (batch.py:115-117)
+        if (trace != nullptr && tid_x() == 0) {                     // what verbose=1 prints (batch.py:115-117)
             double* tr = trace + ((int64_t)qp * maxIter + it) * 4;
             tr[0] = sqrt(acc[1]) + sqrt(acc[0]); tr[1] = sqrt(acc[2]); tr[2] = mu; tr[3] = resid;
         }
@@ -456,13 +456,13 @@ k_forward_fast(KDims D, const double* __restrict__ p, int64_t sp, const double* 
         const bool improved = (it == 0) || (resid < best);
         if (improved) { best = resid; nNot = 0; } else { ++nNot; }
         if (improved || resid < best_tie * best) {
-            _Pragma("unroll 1") for (int i = tid; i < n; i += kNT) qsm[FV(F_BXT) + i] = qsm[xt + i];
-            _Pragma("unroll 1") for (int i = tid; i < ms; i += kNT) { qsm[FV(F_BS) + i] = qsm[s + i]; qsm[FV(F_BV) + i] = qsm[v + i]; }
+            _Pragma("unroll 1") for (int i = tid_x(); i < n; i += kNT) qsm[FV(F_BXT) + i] = qsm[xt + i];
+            _Pragma("unroll 1") for (int i = tid_x(); i < ms; i += kNT) { qsm[FV(F_BS) + i] = qsm[s + i]; qsm[FV(F_BV) + i] = qsm[v + i]; }
         }
         if ((nNot == notImprovedLim && best < stall_tol) || best < eps || mu > 1e32) break;
         if (!(resid == resid) || isinf(resid)) break;
         // ---- factor_kkt with d = z/s and the affine right-hand side (batch.py:109-113,150)
-        _Pragma("unroll 1") for (int i = tid; i < ms; i += kNT) {
+        _Pragma("unroll 1") for (int i = tid_x(); i < ms; i += kNT) {
             double hfull = qsm[hW + i] - qsm[rv + i];
             if (i >= ep) {
                 const double di = kReg ? qsm[v + i] / qsm[s + i] + D.reg : qsm[v + i] / qsm[s + i];
@@ -473,11 +473,11 @@ k_forward_fast(KDims D, const double* __restrict__ p, int64_t sp, const double* 
         }
         __syncthreads();
         QPB_TICK(9);
-        if (kPF) f_factor_and_solve_pf<kReg>(D, C); else f_factor_and_solve(D, C);   // w = [dy_aff; dz_aff]
+        if (kPF) f_factor_and_solve_pf<kReg, kPrefetchP>(D, C); else f_factor_and_solve(D, C);   // w = [dy_aff; dz_aff]
         QPB_TICK(10);
         // ---- affine step length and sigma (batch.py:160-168)
         double mn[2] = {INFINITY, INFINITY};
-        _Pragma("unroll 1") for (int i = ep + tid; i < ms; i += kNT) {
+        _Pragma("unroll 1") for (int i = ep + tid_x(); i < ms; i += kNT) {
             const double dz = qsm[w + i];
             const double dsi = (-qsm[v + i] - dz) / qsm[d + i];
             qsm[dsa + i] = dsi;
@@ -488,7 +488,7 @@ k_forward_fast(KDims D, const double* __restrict__ p, int64_t sp, const double* 
         {
             const double alpha = fmin(fmin(f_step_fix(mn[0]), f_step_fix(mn[1])), 1.0);
             double sm[2] = {0.0, 0.0};
-            _Pragma("unroll 1") for (int i = ep + tid; i < ms; i += kNT) {
+            _Pragma("unroll 1") for (int i = ep + tid_x(); i < ms; i += kNT) {
                 sm[0] = fma(qsm[s + i] + alpha * qsm[dsa + i], qsm[v + i] + alpha * qsm[w + i], sm[0]);
                 sm[1] = fma(qsm[s + i], qsm[v + i], sm[1]);
             }
@@ -496,7 +496,7 @@ k_forward_fast(KDims D, const double* __restrict__ p, int64_t sp, const double* 
             const double sr = sm[0] / sm[1];
             const double sig = sr * sr * sr;
             // ---- corrector right-hand side (batch.py:170-181)
-            _Pragma("unroll 1") for (int i = tid; i < msp; i += kNT) {
+            _Pragma("unroll 1") for (int i = tid_x(); i < msp; i += kNT) {
                 double rhs = 0.0;
                 if (i >= ep && i < ms) {
                     const double rsc = (-mu * sig + qsm[dsa + i] * qsm[w + i]) / qsm[s + i];
@@ -510,7 +510,7 @@ k_forward_fast(KDims D, const double* __restrict__ p, int64_t sp, const double* 
         QPB_TICK(11);
         int wc = t1;                                             // where [dy_cor; dz_cor] lands
         if (kPF) {
-            qpb::pf::pf_solve(C.L.LS, msp, t1, t0, hW);         // (hW is dead until the combined direction below)
+            qpb::pf::pf_solve<kPrefetchP>(C.L.LS, msp, t1, t0, hW);   // (hW is dead until the combined direction below)
             wc = hW;
             QPB_TICK(12);
         } else {
@@ -522,7 +522,7 @@ k_forward_fast(KDims D, const double* __restrict__ p, int64_t sp, const double* 
         if (!refine) f_issue_K(D, C);                            // next factor_kkt's K copy overlaps the rest
         // ---- combined direction, step length, update (batch.py:185-203)
         mn[0] = INFINITY; mn[1] = INFINITY;
-        _Pragma("unroll 1") for (int i = tid; i < ms; i += kNT) {
+        _Pragma("unroll 1") for (int i = tid_x(); i < ms; i += kNT) {
             const double wci = qsm[wc + i];
             const double dv = qsm[w + i] + wci;
             qsm[w + i] = dv;
@@ -537,23 +537,23 @@ k_forward_fast(KDims D, const double* __restrict__ p, int64_t sp, const double* 
         if (refine) {
             // The refinement is linear in the right-hand side, so refining the combined direction equals refining the
             // affine and the corrector direction one by one; sigma above comes from the unrefined affine direction.
-            _Pragma("unroll 1") for (int i = tid; i < n; i += kNT) qsm[rv + i] = 0.0;
+            _Pragma("unroll 1") for (int i = tid_x(); i < n; i += kNT) qsm[rv + i] = 0.0;
             __syncthreads();
             _Pragma("unroll 1") for (int k = 0; k < ir_steps; ++k) f_refine<kCoop>(D, C, rxt, rv, w, ds, t1, t0, aug, hW, dsa, k == 0);
             f_issue_K(D, C);
             mn[0] = INFINITY; mn[1] = INFINITY;
-            _Pragma("unroll 1") for (int i = ep + tid; i < ms; i += kNT) {
+            _Pragma("unroll 1") for (int i = ep + tid_x(); i < ms; i += kNT) {
                 mn[0] = fmin(mn[0], step_candidate(qsm[v + i], qsm[w + i]));
                 mn[1] = fmin(mn[1], step_candidate(qsm[s + i], qsm[ds + i]));
             }
-            _Pragma("unroll 1") for (int i = tid; i < n; i += kNT) qsm[rxt + i] -= qsm[rv + i];   // dx~ = -(r~x - rv) - W^T dv
+            _Pragma("unroll 1") for (int i = tid_x(); i < n; i += kNT) qsm[rxt + i] -= qsm[rv + i];   // dx~ = -(r~x - rv) - W^T dv
         }
         QPB_TICK(14);
         // the step length does not depend on dx~: v and s move first, then one pass over W gives dx~, x~ and the next
         // iteration's r~x (none after the last iteration: nothing reads x~ then)
         f_reduce_min2(mn, C.L.red);
         const double alpha = fmin(0.999 * fmin(f_step_fix(mn[0]), f_step_fix(mn[1])), 1.0);
-        _Pragma("unroll 1") for (int i = tid; i < ms; i += kNT) {
+        _Pragma("unroll 1") for (int i = tid_x(); i < ms; i += kNT) {
             qsm[v + i] = fma(alpha, qsm[w + i], qsm[v + i]);
             if (i >= ep) qsm[s + i] = fma(alpha, qsm[ds + i], qsm[s + i]);
         }
@@ -572,21 +572,21 @@ k_forward_fast(KDims D, const double* __restrict__ p, int64_t sp, const double* 
     }
     f_unwhiten_x(D, C, FV(F_BXT), t0);
     if (C.kpending) f_wait_K(C);                                 // drain the in-flight copy before exit
-    _Pragma("unroll 1") for (int i = tid; i < n; i += kNT) zhat[(int64_t)qp * n + i] = qsm[t0 + i];
-    _Pragma("unroll 1") for (int i = tid; i < m; i += kNT) {
+    _Pragma("unroll 1") for (int i = tid_x(); i < n; i += kNT) zhat[(int64_t)qp * n + i] = qsm[t0 + i];
+    _Pragma("unroll 1") for (int i = tid_x(); i < m; i += kNT) {
         lam[(int64_t)qp * m + i] = qsm[FV(F_BV) + ep + i];
         slacks[(int64_t)qp * m + i] = qsm[FV(F_BS) + ep + i];
     }
     if (e > 0 && nus != nullptr)
-        _Pragma("unroll 1") for (int i = tid; i < e; i += kNT) nus[(int64_t)qp * e + i] = qsm[FV(F_BV) + i];
-    if (tid == 0) {
+        _Pragma("unroll 1") for (int i = tid_x(); i < e; i += kNT) nus[(int64_t)qp * e + i] = qsm[FV(F_BV) + i];
+    if (tid_x() == 0) {
         iters_out[qp] = iters_run;
         resid_out[qp] = best;          // the minimum over the iterations, as the reference reports (batch.py:126-142)
     }
 #ifdef QPB_TIMING
     QPB_TICK(16);
-    if (tid == 0 && qp == g_tim_target) for (int i = 0; i < 128; ++i) g_tim[i] = s_tim[i];
-    if (tid == 0 && qp < 8192) { g_cta[4 * qp + 1] = gtimer(); g_cta[4 * qp + 2] = iters_run; }
+    if (tid_x() == 0 && qp == g_tim_target) for (int i = 0; i < 128; ++i) g_tim[i] = s_tim[i];
+    if (tid_x() == 0 && qp < 8192) { g_cta[4 * qp + 1] = gtimer(); g_cta[4 * qp + 2] = iters_run; }
 #endif
 }
 
