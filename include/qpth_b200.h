@@ -59,8 +59,8 @@ typedef struct qpb200_plan {
     int64_t coop_smem_bytes;       /* dynamic shared memory of the co-resident solve kernels */
     int coop_ok;            /* 1: the co-resident kernels exist for this shape (two QPs per SM: W and chol(Q) are read
                              *    from L2 instead of being staged in shared memory)                                  */
-    int coop;               /* 1: use them (plan_init's default when coop_ok; the caller may clear it to get the
-                             *    one-QP-per-SM kernels, which have the lower latency for a batch smaller than the GPU) */
+    int coop;               /* 1: use them. plan_init sets 0 (they lost to the one-QP-per-SM kernels in A/B runs); the caller
+                             *    may set it where coop_ok. Only the round-1 kernels (pf == 0) have this variant.        */
     int tiny;               /* 1: nz, ms_pad <= 32: one WARP per QP (32-thread CTAs, up to 16 QPs per SM) with the generic
                              *    shared-memory kernels; `threads` is then 32                                        */
     int pf;                 /* 1: product-form kernels: factor_kkt produces T_k = L_kk^-1 and P_ik = L_ik T_k directly (fp64
@@ -90,6 +90,40 @@ const char* qpb200_last_cuda_error(void);
 
 /* Fill `plan` for a problem shape. No device work. */
 int qpb200_plan_init(int nz, int nineq, int neq, qpb200_plan* plan);
+
+/* Entry points of qpb200_plan_kernels */
+enum {
+    QPB200_ENTRY_SETUP = 0,     /* qpb200_pre_factor_kkt, qpb200_pre_factor_kkt_reg */
+    QPB200_ENTRY_FORWARD,       /* qpb200_forward */
+    QPB200_ENTRY_KKT,           /* qpb200_backward, qpb200_backward_duals, qpb200_solve_kkt, qpb200_jvp */
+    QPB200_ENTRY_REG,           /* qpb200_forward_reg, qpb200_backward_reg, qpb200_backward_reg_duals, qpb200_jvp_reg */
+    QPB200_ENTRY_KKT_REG,       /* qpb200_solve_kkt_reg */
+    QPB200_ENTRY_COUNT
+};
+/* Kernels of qpb200_plan_kernels */
+enum {
+    QPB200_K_NONE = 0,          /* none: the entry point returns QPB200_ERR_TOO_LARGE for this plan */
+    QPB200_K_SETUP_TINY,        /* pre_factor_kkt, one warp per system */
+    QPB200_K_SETUP_PF192,       /* product-form setup, 192 threads (three per SM, next to the pf_three solve kernels) */
+    QPB200_K_SETUP_PF,          /* product-form setup, 256 threads */
+    QPB200_K_SETUP_FAST,        /* the compact shared-memory setup (setup_fast) */
+    QPB200_K_SETUP_SMEM,        /* the generic setup, shared memory */
+    QPB200_K_SETUP_GLOBAL,      /* the generic setup, global scratch (needs `scratch`) */
+    QPB200_K_TINY,              /* solve kernels, one warp per QP */
+    QPB200_K_PF192,             /* product form, three QPs per SM (pf_three), 192 threads */
+    QPB200_K_PF_TWO,            /* product form, two QPs per SM (pf_two) */
+    QPB200_K_PF_GLOBAL512,      /* product form, W and chol(Q) from global memory (pf_global), 512 threads */
+    QPB200_K_PF_GLOBAL256,      /* the same at 256 threads */
+    QPB200_K_PF_RES512,         /* product form, W and chol(Q) in shared memory, 512 threads (a forward only) */
+    QPB200_K_PF_RES,            /* the same at 256 threads */
+    QPB200_K_COOP,              /* the round-1 co-resident kernels (coop) */
+    QPB200_K_FAST,              /* the round-1 compact shared-memory kernels (fast) */
+    QPB200_K_GENERIC_SMEM,      /* the generic kernels, shared memory */
+    QPB200_K_GENERIC_GLOBAL     /* the generic kernels, global scratch (needs `scratch`) */
+};
+/* The kernel each entry point launches for `plan` as it stands (with the caller's pf_two, pf_three and coop):
+ * out[entry] = {QPB200_K_* kernel, CTA size, dynamic shared-memory bytes}. No device work. */
+int qpb200_plan_kernels(const qpb200_plan* plan, int64_t out[QPB200_ENTRY_COUNT][3]);
 
 /* pre_factor_kkt (batch.py:375-429) + the SPD check of qp.py:81-85.
  * nsys systems (1 if Q, G, A are all shared, else nBatch); sQ/sG/sA strides as above.

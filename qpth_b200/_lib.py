@@ -49,6 +49,7 @@ SIGNATURES = {
     "qpb200_error_string": (ctypes.c_char_p, [_I]),
     "qpb200_last_cuda_error": (ctypes.c_char_p, []),
     "qpb200_plan_init": (_I, [_I, _I, _I, ctypes.POINTER(Plan)]),
+    "qpb200_plan_kernels": (_I, [ctypes.POINTER(Plan), _P]),
     "qpb200_pre_factor_kkt": (_I, [ctypes.POINTER(Plan), _I, _P, _L, _P, _L, _P, _L, _P, _P, _P, _P, _P, _P]),
     "qpb200_forward": (_I, [ctypes.POINTER(Plan), _I, _P, _L, _P, _L, _P, _L, _P, _P, _P, _I,
                             _D, _D, _D, _I, _I, _P, _P, _P, _P, _P, _P, _P, _P, _P]),

@@ -43,6 +43,7 @@
 #include "qp_jvp.cuh"
 
 extern "C" void qpb200_internal_cuda_error(int err, const char* what);   // (qp_kernels.cu) records the message, per thread
+extern "C" int qpb200_internal_set_smem(const void* kernel, size_t bytes);   // (qp_kernels.cu) the kernels' smem limits
 
 namespace {
 
@@ -1450,23 +1451,6 @@ k_box_jvp_rhs(int n, int e, int nlb, int m, const double* __restrict__ dq, int64
     for (int i = tid; i < e; i += kJvpNT) ry[qp * e + i] = ay[i];
 }
 
-std::mutex g_mu;
-// cudaFuncAttributeMaxDynamicSharedMemorySize already set, per (kernel, device): its high-water mark
-std::map<std::pair<const void*, int>, size_t> g_smem;
-
-template <typename K>
-int box_set_smem(K kernel, size_t bytes) {
-    int dev = 0;
-    cudaError_t err = cudaGetDevice(&dev);
-    if (err != cudaSuccess) { qpb200_internal_cuda_error((int)err, "cudaGetDevice"); return QPB200_ERR_CUDA; }
-    std::lock_guard<std::mutex> lock(g_mu);
-    size_t& cur = g_smem[{(const void*)kernel, dev}];
-    if (cur >= bytes) return QPB200_OK;
-    err = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
-    if (err != cudaSuccess) { qpb200_internal_cuda_error((int)err, "cudaFuncSetAttribute"); return QPB200_ERR_CUDA; }
-    cur = bytes;
-    return QPB200_OK;
-}
 int box_check_launch(const char* what) {
     cudaError_t err = cudaGetLastError();
     if (err != cudaSuccess) { qpb200_internal_cuda_error((int)err, what); return QPB200_ERR_CUDA; }
@@ -1492,10 +1476,11 @@ struct ClKey {
     }
 };
 std::map<ClKey, bool> g_cl_ok;
+std::mutex g_mu;
 
 template <typename K>
 int cl_prepare(K kernel, int C, size_t bytes) {
-    int rc = box_set_smem(kernel, bytes);
+    int rc = qpb200_internal_set_smem((const void*)kernel, bytes);
     if (rc) return rc;
     int dev = 0;
     cudaError_t err = cudaGetDevice(&dev);
@@ -1544,7 +1529,7 @@ int box_launch(const char* what, const qpb200_box_plan* plan, int nbatch, void* 
     auto run = [&](auto kernel, const auto& P) {
         const size_t bytes = (size_t)P.total * 8;
         if (!plan->cl_ctas) {
-            const int rc = box_set_smem(kernel, bytes);
+            const int rc = qpb200_internal_set_smem((const void*)kernel, bytes);
             if (rc) return rc;
             kernel<<<nbatch, kBoxNT, bytes, st>>>(P, args...);
             return box_check_launch(what);
@@ -1685,7 +1670,7 @@ int qpb200_box_jvp(const qpb200_box_plan* plan, int nbatch, const double* q, int
     if ((dlb && !plan->has_lb) || (dub && !plan->has_ub)) return QPB200_ERR_BAD_ARG;
     const int n = plan->nz, m = plan->nineq, e = plan->neq, nlb = plan->has_lb ? n : 0;
     const size_t bytes = box_jvp_smem_bytes(n, e);
-    rc = box_set_smem(k_box_jvp_rhs, bytes);
+    rc = qpb200_internal_set_smem((const void*)k_box_jvp_rhs, bytes);
     if (rc) return rc;
     const int64_t B = nbatch;
     double* rx = rhs;

@@ -22,7 +22,9 @@
 #include <stdlib.h>
 #include <string.h>
 
+#include <map>
 #include <mutex>
+#include <utility>
 
 #include "../../include/qpth_b200.h"
 #include "qp_device.cuh"
@@ -1113,69 +1115,106 @@ int cuda_fail(cudaError_t err, const char* what) {
         if (_e != cudaSuccess) return cuda_fail(_e, #call); \
     } while (0)
 
-KDims dims_of(const qpb200_plan* p) {
-    KDims D;
-    D.n = p->nz; D.m = p->nineq; D.e = p->neq; D.ep = p->neq_pad; D.ms = p->ms; D.msp = p->ms_pad;
-    D.ldw = p->ldw; D.lds = p->lds; D.rows_s = p->rows_s; D.vl = p->vl;
-    D.lp = (int)p->L_elems;
-    D.reg = 0.0;
-    return D;
+}  // namespace
+#include "qp_launch.cuh"
+
+// ---- the 192- and 512-thread builds of the product-form kernels (qp_alt.cu) -----------------------------------------
+extern "C" {
+int qpb200_alt192_setup(const QpbSetupArgs* a, size_t smem);
+int qpb200_alt192_forward(const QpbFwdArgs* a, size_t smem);
+int qpb200_alt512_forward(const QpbFwdArgs* a, size_t smem);
+int qpb200_alt512_forward_res(const QpbFwdArgs* a, size_t smem);
+int qpb200_alt192_kkt(const QpbKktArgs* a, size_t smem, int backward);
+int qpb200_alt512_kkt(const QpbKktArgs* a, size_t smem, int backward);
 }
 
-// cudaFuncSetAttribute is not free (and may serialise with the driver): raise the dynamic shared-memory
-// limit of a kernel only when it has to grow. Keyed by (device, kernel).
+namespace {
+
+// cudaFuncSetAttribute is not free (and may serialise with the driver): raise the dynamic shared-memory limit of a kernel
+// only when it has to grow. Keyed by (kernel, device), for every unit of the library (qpb200_internal_set_smem).
 // The table is shared by every host thread that calls into the library (ctypes releases the GIL: the autograd engine
 // thread runs backward while user threads run forward, one thread per GPU in multi-device processes), hence the lock.
-struct SmemSet { const void* fn; int dev; size_t bytes; };
-SmemSet g_smem_set[64];
-int g_smem_n = 0;
+std::map<std::pair<const void*, int>, size_t> g_smem_set;
 std::mutex g_smem_mu;
 
-template <typename K>
-int set_smem(K kernel, size_t bytes) {
-    int dev = 0;
-    CK(cudaGetDevice(&dev));
-    const void* fn = reinterpret_cast<const void*>(kernel);
-    std::lock_guard<std::mutex> lock(g_smem_mu);
-    for (int i = 0; i < g_smem_n; ++i)
-        if (g_smem_set[i].fn == fn && g_smem_set[i].dev == dev) {
-            if (g_smem_set[i].bytes >= bytes) return QPB200_OK;
-            CK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
-            g_smem_set[i].bytes = bytes;
-            return QPB200_OK;
-        }
-    CK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
-    if (g_smem_n < 64) g_smem_set[g_smem_n++] = SmemSet{fn, dev, bytes};
-    return QPB200_OK;
+// What an entry point launches for a plan: a QPB200_K_* kernel id, the CTA size, the dynamic shared-memory bytes
+struct Kern { int id; int threads; size_t smem; };
+
+// The one table of the dispatch: the kernel that `entry` (QPB200_ENTRY_*) launches for `p`. It reads the plan as it
+// stands, since callers set pf_two, pf_three and coop after plan_init; a flag whose *_ok is clear falls through to the
+// next rule. Every entry point switches on its result; qpb200_plan_kernels exports it.
+Kern choose_kernel(const qpb200_plan* p, int entry) {
+    if (entry == QPB200_ENTRY_KKT_REG) {     // the rules of solve_kkt, restricted to the 256-thread builds (with D.reg)
+        qpb200_plan p256 = *p;
+        p256.pf_three = 0;
+        p256.pf_threads = 256;
+        return choose_kernel(&p256, QPB200_ENTRY_KKT);
+    }
+    if (entry == QPB200_ENTRY_REG) {         // the kReg kernels: generic global scratch, or product form at one QP per SM
+        if (!p->tiny && !p->pf && !p->smem_resident) return {QPB200_K_GENERIC_GLOBAL, kThreads, (size_t)p->solve_smem_bytes};
+        if (p->tiny || !p->pf || p->pf_two || p->pf_three || p->pf_threads != 256) return {QPB200_K_NONE, 0, 0};
+        return {p->pf_global ? QPB200_K_PF_GLOBAL256 : QPB200_K_PF_RES, kThreads, (size_t)p->pf_smem_bytes};
+    }
+    const bool setup = entry == QPB200_ENTRY_SETUP;
+    if (p->tiny)
+        return {setup ? QPB200_K_SETUP_TINY : QPB200_K_TINY, kTinyThreads,
+                (size_t)(setup ? p->setup_smem_bytes : p->solve_smem_bytes)};
+    if (setup) {
+        // throughput mode: the setup CTA fits a three-per-SM slot like the forward / backward CTAs around it
+        if (p->pf && p->pf_three && p->pf3_ok && p->setup_pf_smem_bytes <= p->pf3_smem_bytes)
+            return {QPB200_K_SETUP_PF192, 192, (size_t)p->setup_pf_smem_bytes};
+        if (p->pf && p->setup_pf) return {QPB200_K_SETUP_PF, kThreads, (size_t)p->setup_pf_smem_bytes};
+        const int id = p->setup_fast ? QPB200_K_SETUP_FAST : p->smem_resident ? QPB200_K_SETUP_SMEM : QPB200_K_SETUP_GLOBAL;
+        return {id, kThreads, (size_t)p->setup_smem_bytes};
+    }
+    if (p->pf) {
+        if (p->pf_three && p->pf3_ok) return {QPB200_K_PF192, 192, (size_t)p->pf3_smem_bytes};
+        if (p->pf_two && p->pf2_ok) return {QPB200_K_PF_TWO, kThreads, (size_t)p->pf2_smem_bytes};
+        // the resident 512-thread build is a forward only: the backward and solve_kkt of such a plan run at 256 threads
+        const bool nt512 = p->pf_threads == 512 && (p->pf_global || entry == QPB200_ENTRY_FORWARD);
+        const int id = p->pf_global ? (nt512 ? QPB200_K_PF_GLOBAL512 : QPB200_K_PF_GLOBAL256)
+                                    : (nt512 ? QPB200_K_PF_RES512 : QPB200_K_PF_RES);
+        return {id, nt512 ? 512 : kThreads, (size_t)p->pf_smem_bytes};
+    }
+    if (p->fast && p->coop && p->coop_ok) return {QPB200_K_COOP, kThreads, (size_t)p->coop_smem_bytes};
+    const int id = p->fast ? QPB200_K_FAST : p->smem_resident ? QPB200_K_GENERIC_SMEM : QPB200_K_GENERIC_GLOBAL;
+    return {id, kThreads, (size_t)p->solve_smem_bytes};
 }
 
+// The solve_kkt (kBackward = false) or backward kernel `k` of the KKT entry points on `a`
+template <bool kBackward>
+int launch_kkt_kernel(const Kern& k, const QpbKktArgs& a, double* scratch) {
+    switch (k.id) {
+        case QPB200_K_TINY: return launch_kkt(k_solve_kkt<true, kBackward, true>, k.threads, k.smem, a, nullptr, 0);
+        case QPB200_K_PF192: return qpb200_alt192_kkt(&a, k.smem, kBackward);
+        case QPB200_K_PF_TWO: return launch_kkt(k_kkt_fast<kBackward, true, true, 2>, k.threads, k.smem, a);
+        case QPB200_K_PF_GLOBAL512: return qpb200_alt512_kkt(&a, k.smem, kBackward);
+        case QPB200_K_PF_GLOBAL256: return launch_kkt(k_kkt_fast<kBackward, true, true, 0>, k.threads, k.smem, a);
+        case QPB200_K_PF_RES: return launch_kkt(k_kkt_fast<kBackward, false, true, 0>, k.threads, k.smem, a);
+        case QPB200_K_COOP: return launch_kkt(k_kkt_fast<kBackward, true>, k.threads, k.smem, a);
+        case QPB200_K_FAST: return launch_kkt(k_kkt_fast<kBackward, false>, k.threads, k.smem, a);
+        case QPB200_K_GENERIC_SMEM: return launch_kkt(k_solve_kkt<true, kBackward>, k.threads, k.smem, a, nullptr, 0);
+        case QPB200_K_GENERIC_GLOBAL:
+            return launch_kkt(k_solve_kkt<false, kBackward>, k.threads, k.smem, a, scratch, a.plan->solve_scratch_elems);
+    }
+    return QPB200_ERR_BAD_ARG;
+}
 }  // namespace
 
-// ---- the 192- and 512-thread builds of the product-form solve kernels (qp_alt.cu) ----------------------------------
 extern "C" {
-#define QPB_ALT_DECL(NT)                                                                                                  \
-    int qpb200_alt##NT##_forward(const qpb200_plan*, size_t, int, const double*, int64_t, const double*, int64_t,          \
-                                 const double*, int64_t, const double*, const double*, const double*, int, double, double, \
-                                 double, int, int, double*, double*, double*, double*, int*, double*, double*, void*);     \
-    int qpb200_alt##NT##_solve_kkt(const qpb200_plan*, size_t, int, const double*, const double*, const double*,           \
-                                   const double*, const double*, const double*, const double*, const double*, int,         \
-                                   double*, double*, double*, double*, void*);                                             \
-    int qpb200_alt##NT##_backward(const qpb200_plan*, size_t, int, const double*, const double*, const double*,            \
-                                  const double*, const double*, const double*, const double*, const double*,              \
-                                  const double*, const double*, int, double*, int, double*, int, double*, int, double*,    \
-                                  int, double*, int, double*, int, double*, double*, double*, void*);
-QPB_ALT_DECL(192)
-QPB_ALT_DECL(512)
-int qpb200_alt192_setup(const qpb200_plan*, size_t, int, const double*, int64_t, const double*, int64_t, const double*,
-                        int64_t, double, double*, double*, double*, int*, void*);
-int qpb200_alt512_forward_res(const qpb200_plan*, size_t, int, const double*, int64_t, const double*, int64_t,
-                              const double*, int64_t, const double*, const double*, const double*, int, double, double,
-                              double, int, int, double*, double*, double*, double*, int*, double*, double*, void*);
-#undef QPB_ALT_DECL
-void qpb200_internal_cuda_error(int err, const char* what) { cuda_fail((cudaError_t)err, what); }
-}
 
-extern "C" {
+void qpb200_internal_cuda_error(int err, const char* what) { cuda_fail((cudaError_t)err, what); }
+
+int qpb200_internal_set_smem(const void* kernel, size_t bytes) {
+    int dev = 0;
+    CK(cudaGetDevice(&dev));
+    std::lock_guard<std::mutex> lock(g_smem_mu);
+    size_t& cur = g_smem_set[{kernel, dev}];
+    if (cur >= bytes) return QPB200_OK;
+    CK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
+    cur = bytes;
+    return QPB200_OK;
+}
 
 int qpb200_version(void) { return 100; }
 
@@ -1218,7 +1257,7 @@ static int plan_init_impl(int nz, int nineq, int neq, qpb200_plan* plan, bool al
     const int64_t solve_mat_s = (int64_t)ms * plan->ldw + (int64_t)plan->rows_s * plan->lds + plan->L_elems;
     const int64_t solve_mat = (int64_t)plan->rows_s * plan->lds;     // global mode: only the S workspace
     const int64_t solve_vec = (int64_t)solve_vec_doubles(plan->vl);
-    KDims D = dims_of(plan);
+    KDims D = dims_of(plan, 0.0);
     const int64_t fast_doubles = (int64_t)fk::fast_smem_doubles(D, false);
     const int64_t coop_doubles = (int64_t)fk::fast_smem_doubles(D, true);
     const bool setup_fits = (setup_mat + setup_vec) * 8 <= kMaxSmem;
@@ -1300,7 +1339,7 @@ static int plan_init_impl(int nz, int nineq, int neq, qpb200_plan* plan, bool al
             plan->K_elems = (int64_t)qpb::pf::pf_elems(msp >> 3);
             plan->solve_scratch_elems = 0;                   // the factor lives in shared memory: no per-QP global workspace
             // pre_factor_kkt on the same machinery (k_setup_pf) whenever its shared memory fits. In throughput mode
-            // (pf_three) pre_factor_impl runs its 192-thread build wherever it fits the three-per-SM slot; the choice
+            // (pf_three) qpb200_pre_factor_kkt runs its 192-thread build wherever it fits the three-per-SM slot; the choice
             // below is the latency-mode one: the 256-thread build is faster than the global-scratch setup at
             // nz = nineq = 200, but a lone CTA of it is slower than k_setup_fast at C2 - so it is the default only where
             // there is no fast setup or the problem is small (nz <= 64: it wins at C3)
@@ -1333,6 +1372,15 @@ int qpb200_plan_init_reg(int nz, int nineq, int neq, qpb200_plan* plan) {
     return QPB200_OK;
 }
 
+int qpb200_plan_kernels(const qpb200_plan* plan, int64_t out[QPB200_ENTRY_COUNT][3]) {
+    if (!plan || !out) return QPB200_ERR_BAD_ARG;
+    for (int entry = 0; entry < QPB200_ENTRY_COUNT; ++entry) {
+        const Kern k = choose_kernel(plan, entry);
+        out[entry][0] = k.id; out[entry][1] = k.threads; out[entry][2] = (int64_t)k.smem;
+    }
+    return QPB200_OK;
+}
+
 static int pre_factor_impl(const qpb200_plan* plan, int nsys, const double* Q, int64_t sQ,
                            const double* G, int64_t sG, const double* A, int64_t sA, double* Lfac,
                            double* Wfac, double* Kfac, int* spd_flag, double* scratch, void* stream, double reg);
@@ -1353,40 +1401,20 @@ static int pre_factor_impl(const qpb200_plan* plan, int nsys, const double* Q, i
     if (!plan || nsys <= 0 || !Q || !Lfac || !Wfac || !Kfac || !spd_flag) return QPB200_ERR_BAD_ARG;
     if (plan->nineq > 0 && !G) return QPB200_ERR_BAD_ARG;
     if (plan->neq > 0 && !A) return QPB200_ERR_BAD_ARG;
-    cudaStream_t st = (cudaStream_t)stream;
-    KDims D = dims_of(plan);
-    D.reg = reg;
-    if (plan->tiny) {
-        int rc = set_smem(k_setup<true, true>, plan->setup_smem_bytes);
-        if (rc) return rc;
-        k_setup<true, true><<<nsys, kTinyThreads, plan->setup_smem_bytes, st>>>(D, Q, sQ, G, sG, A, sA, Lfac, Wfac, Kfac,
-                                                                                 spd_flag, nullptr, 0, 0);
-    } else if (plan->pf && plan->pf_three && plan->pf3_ok && plan->setup_pf_smem_bytes <= plan->pf3_smem_bytes) {
-        // throughput mode: the setup CTA fits a three-per-SM slot like the forward / backward CTAs around it
-        return qpb200_alt192_setup(plan, (size_t)plan->setup_pf_smem_bytes, nsys, Q, sQ, G, sG, A, sA, reg, Lfac, Wfac, Kfac,
-                                   spd_flag, stream);
-    } else if (plan->pf && plan->setup_pf) {
-        int rc = set_smem(k_setup_pf<2>, plan->setup_pf_smem_bytes);
-        if (rc) return rc;
-        k_setup_pf<2><<<nsys, kThreads, plan->setup_pf_smem_bytes, st>>>(D, Q, sQ, G, sG, A, sA, Lfac, Wfac, Kfac, spd_flag);
-    } else if (plan->setup_fast) {
-        int rc = set_smem(k_setup_fast, plan->setup_smem_bytes);
-        if (rc) return rc;
-        k_setup_fast<<<nsys, kThreads, plan->setup_smem_bytes, st>>>(D, Q, sQ, G, sG, A, sA, Lfac, Wfac, Kfac, spd_flag, plan->pf);
-    } else if (plan->smem_resident) {
-        int rc = set_smem(k_setup<true>, plan->setup_smem_bytes);
-        if (rc) return rc;
-        k_setup<true><<<nsys, kThreads, plan->setup_smem_bytes, st>>>(D, Q, sQ, G, sG, A, sA, Lfac, Wfac,
-                                                                    Kfac, spd_flag, nullptr, 0, plan->pf);
-    } else {
-        if (!scratch) return QPB200_ERR_BAD_ARG;
-        int rc = set_smem(k_setup<false>, plan->setup_smem_bytes);
-        if (rc) return rc;
-        k_setup<false><<<nsys, kThreads, plan->setup_smem_bytes, st>>>(
-            D, Q, sQ, G, sG, A, sA, Lfac, Wfac, Kfac, spd_flag, scratch, plan->setup_scratch_elems, plan->pf);
+    const Kern k = choose_kernel(plan, QPB200_ENTRY_SETUP);
+    if (k.id == QPB200_K_SETUP_GLOBAL && !scratch) return QPB200_ERR_BAD_ARG;
+    const QpbSetupArgs a{plan, reg, nsys, (cudaStream_t)stream, Q, sQ, G, sG, A, sA, Lfac, Wfac, Kfac, spd_flag};
+    const int pf = plan->pf;
+    switch (k.id) {
+        case QPB200_K_SETUP_TINY: return launch_setup(k_setup<true, true>, k.threads, k.smem, a, nullptr, 0, 0);
+        case QPB200_K_SETUP_PF192: return qpb200_alt192_setup(&a, k.smem);
+        case QPB200_K_SETUP_PF: return launch_setup(k_setup_pf<2>, k.threads, k.smem, a);
+        case QPB200_K_SETUP_FAST: return launch_setup(k_setup_fast, k.threads, k.smem, a, pf);
+        case QPB200_K_SETUP_SMEM: return launch_setup(k_setup<true>, k.threads, k.smem, a, nullptr, 0, pf);
+        case QPB200_K_SETUP_GLOBAL:
+            return launch_setup(k_setup<false>, k.threads, k.smem, a, scratch, plan->setup_scratch_elems, pf);
     }
-    CK(cudaGetLastError());
-    return QPB200_OK;
+    return QPB200_ERR_BAD_ARG;
 }
 
 int qpb200_forward(const qpb200_plan* plan, int nbatch, const double* p, int64_t sp, const double* h,
@@ -1399,154 +1427,56 @@ int qpb200_forward(const qpb200_plan* plan, int nbatch, const double* p, int64_t
         return QPB200_ERR_BAD_ARG;
     if (plan->nineq > 0 && !h) return QPB200_ERR_BAD_ARG;
     if (plan->neq > 0 && (!b || !nus)) return QPB200_ERR_BAD_ARG;
-    cudaStream_t st = (cudaStream_t)stream;
-    KDims D = dims_of(plan);
-#define QPB_LAUNCH_FWD(KS, SCR, SCRN)                                                                   \
-    do {                                                                                                \
-        int rc = set_smem(k_forward<KS>, plan->solve_smem_bytes);                                       \
-        if (rc) return rc;                                                                              \
-        k_forward<KS><<<nbatch, kThreads, plan->solve_smem_bytes, st>>>(                                \
-            D, p, sp, h, sh, b, sb, Lfac, Wfac, Kfac, sF, eps, stall_tol, best_tie, notImprovedLim,     \
-            maxIter, zhat, lam, slacks, nus, iters, best_resid, trace, SCR, SCRN);                      \
-    } while (0)
-    if (plan->tiny) {
-        int rc = set_smem(k_forward<true, true>, plan->solve_smem_bytes);
-        if (rc) return rc;
-        k_forward<true, true><<<nbatch, kTinyThreads, plan->solve_smem_bytes, st>>>(
-            D, p, sp, h, sh, b, sb, Lfac, Wfac, Kfac, sF, eps, stall_tol, best_tie, notImprovedLim, maxIter, zhat, lam,
-            slacks, nus, iters, best_resid, trace, nullptr, 0);
-    } else if (plan->pf) {
-#define QPB_LAUNCH_PF(KG, K2)                                                                           \
-        do {                                                                                            \
-            const size_t sb_ = K2 ? plan->pf2_smem_bytes : plan->pf_smem_bytes;                         \
-            int rc = set_smem(k_forward_fast<KG, true, K2>, sb_);                                       \
-            if (rc) return rc;                                                                          \
-            k_forward_fast<KG, true, K2><<<nbatch, qpb::fast::kNT, sb_, st>>>(                                \
-                D, p, sp, h, sh, b, sb, Lfac, Wfac, Kfac, sF, eps, stall_tol, best_tie, notImprovedLim, \
-                maxIter, zhat, lam, slacks, nus, iters, best_resid, trace);                             \
-        } while (0)
-        if (plan->pf_three && plan->pf3_ok)
-            return qpb200_alt192_forward(plan, (size_t)plan->pf3_smem_bytes, nbatch, p, sp, h, sh, b, sb, Lfac, Wfac, Kfac, sF, eps,
-                                         stall_tol, best_tie, notImprovedLim, maxIter, zhat, lam, slacks, nus, iters, best_resid,
-                                         trace, stream);
-        else if (plan->pf_two && plan->pf2_ok) QPB_LAUNCH_PF(true, 2);
-        else if (plan->pf_global && plan->pf_threads == 512)
-            return qpb200_alt512_forward(plan, (size_t)plan->pf_smem_bytes, nbatch, p, sp, h, sh, b, sb, Lfac, Wfac, Kfac, sF, eps,
-                                         stall_tol, best_tie, notImprovedLim, maxIter, zhat, lam, slacks, nus, iters, best_resid,
-                                         trace, stream);
-        else if (plan->pf_global) QPB_LAUNCH_PF(true, 0);
-        else if (plan->pf_threads == 512)                    // resident (latency) kernel at 512 threads: 15 update warps
-            return qpb200_alt512_forward_res(plan, (size_t)plan->pf_smem_bytes, nbatch, p, sp, h, sh, b, sb, Lfac, Wfac, Kfac, sF,
-                                             eps, stall_tol, best_tie, notImprovedLim, maxIter, zhat, lam, slacks, nus, iters,
-                                             best_resid, trace, stream);
-        else QPB_LAUNCH_PF(false, 0);
-#undef QPB_LAUNCH_PF
-    } else if (plan->fast && plan->coop && plan->coop_ok) {
-        int rc = set_smem(k_forward_fast<true>, plan->coop_smem_bytes);
-        if (rc) return rc;
-        k_forward_fast<true><<<nbatch, kThreads, plan->coop_smem_bytes, st>>>(
-            D, p, sp, h, sh, b, sb, Lfac, Wfac, Kfac, sF, eps, stall_tol, best_tie, notImprovedLim, maxIter,
-            zhat, lam, slacks, nus, iters, best_resid, trace);
-    } else if (plan->fast) {
-        int rc = set_smem(k_forward_fast<false>, plan->solve_smem_bytes);
-        if (rc) return rc;
-        k_forward_fast<false><<<nbatch, kThreads, plan->solve_smem_bytes, st>>>(
-            D, p, sp, h, sh, b, sb, Lfac, Wfac, Kfac, sF, eps, stall_tol, best_tie, notImprovedLim, maxIter,
-            zhat, lam, slacks, nus, iters, best_resid, trace);
-    } else if (plan->smem_resident) {
-        QPB_LAUNCH_FWD(true, nullptr, 0);
-    } else {
-        if (!scratch) return QPB200_ERR_BAD_ARG;
-        QPB_LAUNCH_FWD(false, scratch, plan->solve_scratch_elems);
+    const Kern k = choose_kernel(plan, QPB200_ENTRY_FORWARD);
+    if (k.id == QPB200_K_GENERIC_GLOBAL && !scratch) return QPB200_ERR_BAD_ARG;
+    const QpbFwdArgs a{plan, 0.0, nbatch, (cudaStream_t)stream, p, sp, h, sh, b, sb, Lfac, Wfac, Kfac, sF, eps, stall_tol,
+                       best_tie, notImprovedLim, maxIter, zhat, lam, slacks, nus, iters, best_resid, trace, 0};
+    switch (k.id) {
+        case QPB200_K_TINY: return launch_forward(k_forward<true, true>, k.threads, k.smem, a, nullptr, 0);
+        case QPB200_K_PF192: return qpb200_alt192_forward(&a, k.smem);
+        case QPB200_K_PF_TWO: return launch_forward(k_forward_fast<true, true, 2>, k.threads, k.smem, a);
+        case QPB200_K_PF_GLOBAL512: return qpb200_alt512_forward(&a, k.smem);
+        case QPB200_K_PF_GLOBAL256: return launch_forward(k_forward_fast<true, true, 0>, k.threads, k.smem, a);
+        case QPB200_K_PF_RES512: return qpb200_alt512_forward_res(&a, k.smem);
+        case QPB200_K_PF_RES: return launch_forward(k_forward_fast<false, true, 0>, k.threads, k.smem, a);
+        case QPB200_K_COOP: return launch_forward(k_forward_fast<true>, k.threads, k.smem, a);
+        case QPB200_K_FAST: return launch_forward(k_forward_fast<false>, k.threads, k.smem, a);
+        case QPB200_K_GENERIC_SMEM: return launch_forward(k_forward<true>, k.threads, k.smem, a, nullptr, 0);
+        case QPB200_K_GENERIC_GLOBAL:
+            return launch_forward(k_forward<false>, k.threads, k.smem, a, scratch, plan->solve_scratch_elems);
     }
-#undef QPB_LAUNCH_FWD
-    CK(cudaGetLastError());
-    return QPB200_OK;
+    return QPB200_ERR_BAD_ARG;
 }
 
+// entry: QPB200_ENTRY_KKT, or QPB200_ENTRY_KKT_REG for the regularised solve (reg = its eps)
 static int solve_kkt_impl(const qpb200_plan* plan, int nbatch, const double* d, const double* rx,
                           const double* rs, const double* rz, const double* ry, const double* Lfac,
                           const double* Wfac, const double* Kfac, int sF, double* dx, double* ds,
-                          double* dz, double* dy, double* scratch, void* stream, double reg);
+                          double* dz, double* dy, double* scratch, void* stream, double reg, int entry) {
+    if (!plan || nbatch <= 0 || !d || !rx || !rs || !rz || !Lfac || !Wfac || !Kfac || !dx || !ds || !dz)
+        return QPB200_ERR_BAD_ARG;
+    if (plan->neq > 0 && (!ry || !dy)) return QPB200_ERR_BAD_ARG;
+    const Kern k = choose_kernel(plan, entry);
+    if (k.id == QPB200_K_GENERIC_GLOBAL && !scratch) return QPB200_ERR_BAD_ARG;
+    const QpbKktArgs a{plan, reg, nbatch, (cudaStream_t)stream, d, rx, rs, rz, ry, nullptr, nullptr, nullptr, nullptr,
+                       Lfac, Wfac, Kfac, sF, dx, ds, dz, dy, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr,
+                       0, 0, 0, 0, 0, 0, 0};
+    return launch_kkt_kernel<false>(k, a, scratch);
+}
 int qpb200_solve_kkt(const qpb200_plan* plan, int nbatch, const double* d, const double* rx,
                      const double* rs, const double* rz, const double* ry, const double* Lfac,
                      const double* Wfac, const double* Kfac, int sF, double* dx, double* ds,
                      double* dz, double* dy, double* scratch, void* stream) {
-    return solve_kkt_impl(plan, nbatch, d, rx, rs, rz, ry, Lfac, Wfac, Kfac, sF, dx, ds, dz, dy, scratch, stream, 0.0);
+    return solve_kkt_impl(plan, nbatch, d, rx, rs, rz, ry, Lfac, Wfac, Kfac, sF, dx, ds, dz, dy, scratch, stream, 0.0,
+                          QPB200_ENTRY_KKT);
 }
 int qpb200_solve_kkt_reg(const qpb200_plan* plan, int nbatch, const double* d, const double* rx,
                          const double* rs, const double* rz, const double* ry, double reg_eps, const double* Lfac,
                          const double* Wfac, const double* Kfac, int sF, double* dx, double* ds,
                          double* dz, double* dy, double* scratch, void* stream) {
     if (!plan || !(reg_eps >= 0.0)) return QPB200_ERR_BAD_ARG;
-    qpb200_plan p256 = *plan;            // the regularised variant exists in the 256-thread builds only
-    p256.pf_three = 0;
-    p256.pf_threads = 256;
-    return solve_kkt_impl(&p256, nbatch, d, rx, rs, rz, ry, Lfac, Wfac, Kfac, sF, dx, ds, dz, dy, scratch, stream, reg_eps);
-}
-static int solve_kkt_impl(const qpb200_plan* plan, int nbatch, const double* d, const double* rx,
-                          const double* rs, const double* rz, const double* ry, const double* Lfac,
-                          const double* Wfac, const double* Kfac, int sF, double* dx, double* ds,
-                          double* dz, double* dy, double* scratch, void* stream, double reg) {
-    if (!plan || nbatch <= 0 || !d || !rx || !rs || !rz || !Lfac || !Wfac || !Kfac || !dx || !ds || !dz)
-        return QPB200_ERR_BAD_ARG;
-    if (plan->neq > 0 && (!ry || !dy)) return QPB200_ERR_BAD_ARG;
-    cudaStream_t st = (cudaStream_t)stream;
-    KDims D = dims_of(plan);
-    D.reg = reg;
-    BwdOut O;
-    memset(&O, 0, sizeof(O));
-#define QPB_LAUNCH_KKT(KS, SCR, SCRN)                                                                   \
-    do {                                                                                                \
-        int rc = set_smem(k_solve_kkt<KS, false>, plan->solve_smem_bytes);                              \
-        if (rc) return rc;                                                                              \
-        k_solve_kkt<KS, false><<<nbatch, kThreads, plan->solve_smem_bytes, st>>>(                       \
-            D, d, rx, rs, rz, ry, nullptr, nullptr, nullptr, nullptr, Lfac, Wfac, Kfac, sF, dx, ds, dz, \
-            dy, O, SCR, SCRN);                                                                          \
-    } while (0)
-    if (plan->tiny) {
-        int rc = set_smem(k_solve_kkt<true, false, true>, plan->solve_smem_bytes);
-        if (rc) return rc;
-        k_solve_kkt<true, false, true><<<nbatch, kTinyThreads, plan->solve_smem_bytes, st>>>(
-            D, d, rx, rs, rz, ry, nullptr, nullptr, nullptr, nullptr, Lfac, Wfac, Kfac, sF, dx, ds, dz, dy, O, nullptr, 0);
-    } else if (plan->pf) {
-#define QPB_LAUNCH_PF(KG, K2)                                                                           \
-        do {                                                                                            \
-            const size_t sb_ = K2 ? plan->pf2_smem_bytes : plan->pf_smem_bytes;                         \
-            int rc = set_smem(k_kkt_fast<false, KG, true, K2>, sb_);                                    \
-            if (rc) return rc;                                                                          \
-            k_kkt_fast<false, KG, true, K2><<<nbatch, qpb::fast::kNT, sb_, st>>>(                             \
-                D, d, rx, rs, rz, ry, nullptr, nullptr, nullptr, nullptr, Lfac, Wfac, Kfac, sF, dx, ds, dz, dy, O); \
-        } while (0)
-        if (plan->pf_three && plan->pf3_ok)
-            return qpb200_alt192_solve_kkt(plan, (size_t)plan->pf3_smem_bytes, nbatch, d, rx, rs, rz, ry, Lfac, Wfac, Kfac, sF, dx, ds,
-                                           dz, dy, stream);
-        else if (plan->pf_two && plan->pf2_ok) QPB_LAUNCH_PF(true, 2);
-        else if (plan->pf_global && plan->pf_threads == 512)
-            return qpb200_alt512_solve_kkt(plan, (size_t)plan->pf_smem_bytes, nbatch, d, rx, rs, rz, ry, Lfac, Wfac, Kfac, sF, dx, ds,
-                                           dz, dy, stream);
-        else if (plan->pf_global) QPB_LAUNCH_PF(true, 0);
-        else QPB_LAUNCH_PF(false, 0);
-#undef QPB_LAUNCH_PF
-    } else if (plan->fast && plan->coop && plan->coop_ok) {
-        int rc = set_smem(k_kkt_fast<false, true>, plan->coop_smem_bytes);
-        if (rc) return rc;
-        k_kkt_fast<false, true><<<nbatch, kThreads, plan->coop_smem_bytes, st>>>(
-            D, d, rx, rs, rz, ry, nullptr, nullptr, nullptr, nullptr, Lfac, Wfac, Kfac, sF, dx, ds, dz, dy, O);
-    } else if (plan->fast) {
-        int rc = set_smem(k_kkt_fast<false, false>, plan->solve_smem_bytes);
-        if (rc) return rc;
-        k_kkt_fast<false, false><<<nbatch, kThreads, plan->solve_smem_bytes, st>>>(
-            D, d, rx, rs, rz, ry, nullptr, nullptr, nullptr, nullptr, Lfac, Wfac, Kfac, sF, dx, ds, dz, dy, O);
-    } else if (plan->smem_resident) {
-        QPB_LAUNCH_KKT(true, nullptr, 0);
-    } else {
-        if (!scratch) return QPB200_ERR_BAD_ARG;
-        QPB_LAUNCH_KKT(false, scratch, plan->solve_scratch_elems);
-    }
-#undef QPB_LAUNCH_KKT
-    CK(cudaGetLastError());
-    return QPB200_OK;
+    return solve_kkt_impl(plan, nbatch, d, rx, rs, rz, ry, Lfac, Wfac, Kfac, sF, dx, ds, dz, dy, scratch, stream, reg_eps,
+                          QPB200_ENTRY_KKT_REG);
 }
 
 static int launch_means(int nbatch, int n, int m, int e, const double* zhat, const double* lam, const double* nus,
@@ -1581,72 +1511,15 @@ int qpb200_backward_duals(const qpb200_plan* plan, int nbatch, const double* dl_
         return QPB200_ERR_BAD_ARG;
     if (plan->neq > 0 && (!nus || !dnuv)) return QPB200_ERR_BAD_ARG;
     if (check_dual_adjoints(plan, dl_dnu)) return QPB200_ERR_BAD_ARG;
-    cudaStream_t st = (cudaStream_t)stream;
-    KDims D = dims_of(plan);
-    const int n = plan->nz, m = plan->nineq, e = plan->neq;
-    BwdOut O;
-    O.dQ = dQ; O.dp = dp; O.dG = dG; O.dh = dh; O.dA = dA; O.db = db;
-    O.mQ = mean_Q; O.mp = mean_p; O.mG = mean_G; O.mh = mean_h; O.mA = mean_A; O.mb = mean_b;
-#define QPB_LAUNCH_BWD(KS, SCR, SCRN)                                                                   \
-    do {                                                                                                \
-        int rc = set_smem(k_solve_kkt<KS, true>, plan->solve_smem_bytes);                               \
-        if (rc) return rc;                                                                              \
-        k_solve_kkt<KS, true><<<nbatch, kThreads, plan->solve_smem_bytes, st>>>(                        \
-            D, nullptr, dl_dzhat, nullptr, dl_dlam, dl_dnu, zhat, lam, slacks, nus, Lfac, Wfac, Kfac,  \
-            sF, dxv, nullptr, dlamv, dnuv, O, SCR, SCRN);                                               \
-    } while (0)
-    if (plan->tiny) {
-        int rc = set_smem(k_solve_kkt<true, true, true>, plan->solve_smem_bytes);
-        if (rc) return rc;
-        k_solve_kkt<true, true, true><<<nbatch, kTinyThreads, plan->solve_smem_bytes, st>>>(
-            D, nullptr, dl_dzhat, nullptr, dl_dlam, dl_dnu, zhat, lam, slacks, nus, Lfac, Wfac, Kfac, sF, dxv, nullptr,
-            dlamv, dnuv, O, nullptr, 0);
-    } else if (plan->pf) {
-#define QPB_LAUNCH_PF(KG, K2)                                                                           \
-        do {                                                                                            \
-            const size_t sb_ = K2 ? plan->pf2_smem_bytes : plan->pf_smem_bytes;                         \
-            int rc = set_smem(k_kkt_fast<true, KG, true, K2>, sb_);                                     \
-            if (rc) return rc;                                                                          \
-            k_kkt_fast<true, KG, true, K2><<<nbatch, qpb::fast::kNT, sb_, st>>>(                              \
-                D, nullptr, dl_dzhat, nullptr, dl_dlam, dl_dnu, zhat, lam, slacks, nus, Lfac, Wfac, Kfac, sF, dxv, \
-                nullptr, dlamv, dnuv, O);                                                               \
-        } while (0)
-        if (plan->pf_three && plan->pf3_ok) {
-            int rc = qpb200_alt192_backward(plan, (size_t)plan->pf3_smem_bytes, nbatch, dl_dzhat, dl_dlam, dl_dnu, zhat, lam,
-                                            slacks, nus, Lfac, Wfac, Kfac, sF, dQ, mean_Q, dp, mean_p, dG, mean_G, dh,
-                                            mean_h, dA, mean_A, db, mean_b, dxv, dlamv, dnuv, stream);
-            if (rc) return rc;
-        } else if (plan->pf_two && plan->pf2_ok) QPB_LAUNCH_PF(true, 2);
-        else if (plan->pf_global && plan->pf_threads == 512) {
-            int rc = qpb200_alt512_backward(plan, (size_t)plan->pf_smem_bytes, nbatch, dl_dzhat, dl_dlam, dl_dnu, zhat, lam,
-                                            slacks, nus, Lfac, Wfac, Kfac, sF, dQ, mean_Q, dp, mean_p, dG, mean_G, dh,
-                                            mean_h, dA, mean_A, db, mean_b, dxv, dlamv, dnuv, stream);
-            if (rc) return rc;
-        } else if (plan->pf_global) QPB_LAUNCH_PF(true, 0);
-        else QPB_LAUNCH_PF(false, 0);
-#undef QPB_LAUNCH_PF
-    } else if (plan->fast && plan->coop && plan->coop_ok) {
-        int rc = set_smem(k_kkt_fast<true, true>, plan->coop_smem_bytes);
-        if (rc) return rc;
-        k_kkt_fast<true, true><<<nbatch, kThreads, plan->coop_smem_bytes, st>>>(
-            D, nullptr, dl_dzhat, nullptr, dl_dlam, dl_dnu, zhat, lam, slacks, nus, Lfac, Wfac, Kfac, sF, dxv,
-            nullptr, dlamv, dnuv, O);
-    } else if (plan->fast) {
-        int rc = set_smem(k_kkt_fast<true, false>, plan->solve_smem_bytes);
-        if (rc) return rc;
-        k_kkt_fast<true, false><<<nbatch, kThreads, plan->solve_smem_bytes, st>>>(
-            D, nullptr, dl_dzhat, nullptr, dl_dlam, dl_dnu, zhat, lam, slacks, nus, Lfac, Wfac, Kfac, sF, dxv,
-            nullptr, dlamv, dnuv, O);
-    } else if (plan->smem_resident) {
-        QPB_LAUNCH_BWD(true, nullptr, 0);
-    } else {
-        if (!scratch) return QPB200_ERR_BAD_ARG;
-        QPB_LAUNCH_BWD(false, scratch, plan->solve_scratch_elems);
-    }
-#undef QPB_LAUNCH_BWD
-    CK(cudaGetLastError());
-    return launch_means(nbatch, n, m, e, zhat, lam, nus, dQ, mean_Q, dp, mean_p, dG, mean_G, dh, mean_h, dA, mean_A, db,
-                        mean_b, dxv, dlamv, dnuv, st);
+    const Kern k = choose_kernel(plan, QPB200_ENTRY_KKT);
+    if (k.id == QPB200_K_GENERIC_GLOBAL && !scratch) return QPB200_ERR_BAD_ARG;
+    const QpbKktArgs a{plan, 0.0, nbatch, (cudaStream_t)stream, nullptr, dl_dzhat, nullptr, dl_dlam, dl_dnu, zhat, lam,
+                       slacks, nus, Lfac, Wfac, Kfac, sF, dxv, nullptr, dlamv, dnuv, dQ, dp, dG, dh, dA, db,
+                       mean_Q, mean_p, mean_G, mean_h, mean_A, mean_b, 0};
+    const int rc = launch_kkt_kernel<true>(k, a, scratch);
+    if (rc) return rc;
+    return launch_means(nbatch, plan->nz, plan->nineq, plan->neq, zhat, lam, nus, dQ, mean_Q, dp, mean_p, dG, mean_G, dh,
+                        mean_h, dA, mean_A, db, mean_b, dxv, dlamv, dnuv, a.st);
 }
 
 // Batch-mean gradients of the un-batched inputs (qp.py:159-177) from the per-QP dx, dlam, dnu of a backward kernel.
@@ -1673,13 +1546,13 @@ static int launch_means(int nbatch, int n, int m, int e, const double* zhat, con
 // ---- regularised mode (QPFunction kkt_solver=IR_UNOPT): the solve kernels with kReg ---------------------------------
 // Two families: the product-form kernels (a plan from qpb200_plan_init_reg) and, for the larger shapes, the generic
 // global-scratch kernels (a plan from qpb200_plan_init with tiny = pf = smem_resident = 0), which need `scratch`.
-static bool reg_global_plan(const qpb200_plan* plan) { return !plan->tiny && !plan->pf && !plan->smem_resident; }
-
 static int check_reg_plan(const qpb200_plan* plan, double reg_eps, int ir_steps, const double* scratch) {
     if (!(reg_eps >= 0.0) || ir_steps < 0 || ir_steps > 8) return QPB200_ERR_BAD_ARG;
-    if (reg_global_plan(plan)) return scratch ? QPB200_OK : QPB200_ERR_BAD_ARG;
-    if (plan->tiny || !plan->pf || plan->pf_two || plan->pf_three || plan->pf_threads != 256) return QPB200_ERR_TOO_LARGE;
-    return QPB200_OK;
+    switch (choose_kernel(plan, QPB200_ENTRY_REG).id) {
+        case QPB200_K_NONE: return QPB200_ERR_TOO_LARGE;
+        case QPB200_K_GENERIC_GLOBAL: return scratch ? QPB200_OK : QPB200_ERR_BAD_ARG;
+        default: return QPB200_OK;
+    }
 }
 
 int qpb200_forward_reg(const qpb200_plan* plan, int nbatch, const double* p, int64_t sp, const double* h,
@@ -1691,34 +1564,19 @@ int qpb200_forward_reg(const qpb200_plan* plan, int nbatch, const double* p, int
     if (!plan || nbatch <= 0 || !p || !h || !Lfac || !Wfac || !Kfac || !zhat || !lam || !slacks || !iters || !best_resid)
         return QPB200_ERR_BAD_ARG;
     if (plan->neq > 0 && (!b || !nus)) return QPB200_ERR_BAD_ARG;
-    int rc = check_reg_plan(plan, reg_eps, ir_steps, scratch);
+    const int rc = check_reg_plan(plan, reg_eps, ir_steps, scratch);
     if (rc) return rc;
-    cudaStream_t st = (cudaStream_t)stream;
-    KDims D = dims_of(plan);
-    D.reg = reg_eps;
-    if (reg_global_plan(plan)) {
-        rc = set_smem(k_forward<false, false, true>, plan->solve_smem_bytes);
-        if (rc) return rc;
-        k_forward<false, false, true><<<nbatch, kThreads, plan->solve_smem_bytes, st>>>(
-            D, p, sp, h, sh, b, sb, Lfac, Wfac, Kfac, sF, eps, stall_tol, best_tie, notImprovedLim, maxIter, zhat, lam,
-            slacks, nus, iters, best_resid, trace, scratch, plan->solve_scratch_elems, ir_steps);
-        CK(cudaGetLastError());
-        return QPB200_OK;
+    const Kern k = choose_kernel(plan, QPB200_ENTRY_REG);
+    const QpbFwdArgs a{plan, reg_eps, nbatch, (cudaStream_t)stream, p, sp, h, sh, b, sb, Lfac, Wfac, Kfac, sF, eps,
+                       stall_tol, best_tie, notImprovedLim, maxIter, zhat, lam, slacks, nus, iters, best_resid, trace,
+                       ir_steps};
+    switch (k.id) {
+        case QPB200_K_GENERIC_GLOBAL:
+            return launch_forward(k_forward<false, false, true>, k.threads, k.smem, a, scratch, plan->solve_scratch_elems);
+        case QPB200_K_PF_GLOBAL256: return launch_forward(k_forward_fast<true, true, 0, true>, k.threads, k.smem, a);
+        case QPB200_K_PF_RES: return launch_forward(k_forward_fast<false, true, 0, true>, k.threads, k.smem, a);
     }
-    const size_t sb_ = (size_t)plan->pf_smem_bytes;
-#define QPB_LAUNCH_REG(KG)                                                                                   \
-    do {                                                                                                     \
-        rc = set_smem(k_forward_fast<KG, true, 0, true>, sb_);                                               \
-        if (rc) return rc;                                                                                   \
-        k_forward_fast<KG, true, 0, true><<<nbatch, qpb::fast::kNT, sb_, st>>>(                              \
-            D, p, sp, h, sh, b, sb, Lfac, Wfac, Kfac, sF, eps, stall_tol, best_tie, notImprovedLim, maxIter, \
-            zhat, lam, slacks, nus, iters, best_resid, trace, ir_steps);                                     \
-    } while (0)
-    if (plan->pf_global) QPB_LAUNCH_REG(true);
-    else QPB_LAUNCH_REG(false);
-#undef QPB_LAUNCH_REG
-    CK(cudaGetLastError());
-    return QPB200_OK;
+    return QPB200_ERR_TOO_LARGE;
 }
 
 int qpb200_backward_reg(const qpb200_plan* plan, int nbatch, const double* dl_dzhat, const double* zhat,
@@ -1744,37 +1602,21 @@ int qpb200_backward_reg_duals(const qpb200_plan* plan, int nbatch, const double*
     if (check_dual_adjoints(plan, dl_dnu)) return QPB200_ERR_BAD_ARG;
     int rc = check_reg_plan(plan, reg_eps, ir_steps, scratch);
     if (rc) return rc;
-    cudaStream_t st = (cudaStream_t)stream;
-    KDims D = dims_of(plan);
-    D.reg = reg_eps;
-    BwdOut O;
-    O.dQ = dQ; O.dp = dp; O.dG = dG; O.dh = dh; O.dA = dA; O.db = db;
-    O.mQ = mean_Q; O.mp = mean_p; O.mG = mean_G; O.mh = mean_h; O.mA = mean_A; O.mb = mean_b;
-    if (reg_global_plan(plan)) {
-        rc = set_smem(k_solve_kkt<false, true, false, true>, plan->solve_smem_bytes);
-        if (rc) return rc;
-        k_solve_kkt<false, true, false, true><<<nbatch, kThreads, plan->solve_smem_bytes, st>>>(
-            D, nullptr, dl_dzhat, nullptr, dl_dlam, dl_dnu, zhat, lam, slacks, nus, Lfac, Wfac, Kfac, sF, dxv, nullptr,
-            dlamv, dnuv, O, scratch, plan->solve_scratch_elems, ir_steps);
-        CK(cudaGetLastError());
-        return launch_means(nbatch, plan->nz, plan->nineq, plan->neq, zhat, lam, nus, dQ, mean_Q, dp, mean_p, dG, mean_G,
-                            dh, mean_h, dA, mean_A, db, mean_b, dxv, dlamv, dnuv, st);
+    const Kern k = choose_kernel(plan, QPB200_ENTRY_REG);
+    const QpbKktArgs a{plan, reg_eps, nbatch, (cudaStream_t)stream, nullptr, dl_dzhat, nullptr, dl_dlam, dl_dnu, zhat,
+                       lam, slacks, nus, Lfac, Wfac, Kfac, sF, dxv, nullptr, dlamv, dnuv, dQ, dp, dG, dh, dA, db,
+                       mean_Q, mean_p, mean_G, mean_h, mean_A, mean_b, ir_steps};
+    switch (k.id) {
+        case QPB200_K_GENERIC_GLOBAL:
+            rc = launch_kkt(k_solve_kkt<false, true, false, true>, k.threads, k.smem, a, scratch, plan->solve_scratch_elems);
+            break;
+        case QPB200_K_PF_GLOBAL256: rc = launch_kkt(k_kkt_fast<true, true, true, 0, true>, k.threads, k.smem, a); break;
+        case QPB200_K_PF_RES: rc = launch_kkt(k_kkt_fast<true, false, true, 0, true>, k.threads, k.smem, a); break;
+        default: return QPB200_ERR_TOO_LARGE;
     }
-    const size_t sb_ = (size_t)plan->pf_smem_bytes;
-#define QPB_LAUNCH_REG(KG)                                                                                   \
-    do {                                                                                                     \
-        rc = set_smem(k_kkt_fast<true, KG, true, 0, true>, sb_);                                             \
-        if (rc) return rc;                                                                                   \
-        k_kkt_fast<true, KG, true, 0, true><<<nbatch, qpb::fast::kNT, sb_, st>>>(                            \
-            D, nullptr, dl_dzhat, nullptr, dl_dlam, dl_dnu, zhat, lam, slacks, nus, Lfac, Wfac, Kfac, sF, dxv, \
-            nullptr, dlamv, dnuv, O, ir_steps);                                                              \
-    } while (0)
-    if (plan->pf_global) QPB_LAUNCH_REG(true);
-    else QPB_LAUNCH_REG(false);
-#undef QPB_LAUNCH_REG
-    CK(cudaGetLastError());
+    if (rc) return rc;
     return launch_means(nbatch, plan->nz, plan->nineq, plan->neq, zhat, lam, nus, dQ, mean_Q, dp, mean_p, dG, mean_G, dh,
-                        mean_h, dA, mean_A, db, mean_b, dxv, dlamv, dnuv, st);
+                        mean_h, dA, mean_A, db, mean_b, dxv, dlamv, dnuv, a.st);
 }
 
 // ---- forward mode: k_jvp_rhs, then the backward-with-duals solve with the right-hand side it wrote -------------------
@@ -1791,9 +1633,10 @@ static int check_jvp_args(const qpb200_plan* plan, int nbatch, int64_t sdQ, int6
     if (plan->neq > 0 && (!nus || !dnu)) return QPB200_ERR_BAD_ARG;
     if (plan->neq == 0 && (dA || db || dnu)) return QPB200_ERR_BAD_ARG;
     if (plan->nineq == 0 && (dG || dh)) return QPB200_ERR_BAD_ARG;
-    // the generic global-scratch kernels (the only plan neither tiny, product form, fast nor resident) need scratch
-    if (!plan->tiny && !plan->pf && !plan->fast && !plan->smem_resident && !scratch) return QPB200_ERR_BAD_ARG;
-    return QPB200_OK;
+    switch (choose_kernel(plan, QPB200_ENTRY_KKT).id) {
+        case QPB200_K_GENERIC_GLOBAL: return scratch ? QPB200_OK : QPB200_ERR_BAD_ARG;
+        default: return QPB200_OK;
+    }
 }
 
 static int launch_jvp_rhs(const qpb200_plan* plan, int nbatch, const double* dQ, int64_t sdQ, const double* dp,
@@ -1801,16 +1644,11 @@ static int launch_jvp_rhs(const qpb200_plan* plan, int nbatch, const double* dQ,
                           int64_t sdA, const double* db, int64_t sdb, const double* zhat, const double* lam,
                           const double* nus, double* rhs, cudaStream_t st) {
     const int n = plan->nz, m = plan->nineq, e = plan->neq;
-    const size_t bytes = jvp_smem_bytes(n, m, e);
-    int rc = set_smem(k_jvp_rhs, bytes);
-    if (rc) return rc;
     double* rx = rhs;
     double* rz = rx + (int64_t)nbatch * n;
     double* ry = rz + (int64_t)nbatch * m;
-    k_jvp_rhs<<<nbatch, kThreads, bytes, st>>>(n, m, e, dQ, sdQ, dp, sdp, dG, sdG, dh, sdh, dA, sdA, db, sdb, zhat, lam,
-                                               nus, rx, rz, ry);
-    CK(cudaGetLastError());
-    return QPB200_OK;
+    return launch(k_jvp_rhs, nbatch, kThreads, jvp_smem_bytes(n, m, e), st, n, m, e, dQ, sdQ, dp, sdp, dG, sdG, dh, sdh,
+                  dA, sdA, db, sdb, zhat, lam, nus, rx, rz, ry);
 }
 
 int qpb200_jvp(const qpb200_plan* plan, int nbatch, const double* dQ, int64_t sdQ, const double* dp, int64_t sdp,

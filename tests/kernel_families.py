@@ -113,10 +113,10 @@ PER_CTA = {2: SM_SMEM // 2 - 1024, 3: SM_SMEM // 3 - 1024}     # the planner's l
 
 
 def dispatch(plan):
-    """(setup kernel, solve kernel) that `plan` runs: a restatement of the branches of pre_factor_impl (setup) and of
-    qpb200_forward, qpb200_backward and solve_kkt_impl (solve) in qpth_b200/csrc/qp_kernels.cu. The three solve entry
-    points take the same branch, except that a resident product-form plan at 512 threads ("pf_res512") runs only the
-    forward at 512 threads and the backward / solve_kkt at 256 ("pf_res").
+    """(setup kernel, solve kernel) that `plan` runs: a restatement of the setup and forward rules of choose_kernel in
+    qpth_b200/csrc/qp_kernels.cu (qpb200_plan_kernels), written independently of it. The three solve entry points take
+    the same branch, except that a resident product-form plan at 512 threads ("pf_res512") runs only the forward at 512
+    threads and the backward / solve_kkt at 256 ("pf_res").
 
     setup: "tiny" k_setup<true, true>, "setup_pf192" the 192-thread k_setup_pf (qpb200_alt192_setup), "setup_pf"
     k_setup_pf<2>, "setup_fast" k_setup_fast, "setup_smem" k_setup<true>, "setup_global" k_setup<false>.
@@ -152,6 +152,18 @@ def dispatch(plan):
     else:
         solve = "generic_smem" if p.smem_resident else "generic_global"
     return setup, solve
+
+
+def reg_dispatch(plan):
+    """The solve kernel of the regularised forward / backward (qpb200_forward_reg, qpb200_backward_reg_duals,
+    qpb200_jvp_reg), or None where they return QPB200_ERR_TOO_LARGE: the generic global-scratch kernels for a plan that
+    is neither tiny, product form nor resident, else the one-QP-per-SM, 256-thread product-form kernels only."""
+    p = plan
+    if not p.tiny and not p.pf and not p.smem_resident:
+        return "generic_global"
+    if p.tiny or not p.pf or p.pf_two or p.pf_three or p.pf_threads != 256:
+        return None
+    return "pf_global256" if p.pf_global else "pf_res"
 
 
 def slack(plan):
