@@ -370,6 +370,48 @@ int qpb200_box_solve_kkt(const qpb200_box_plan* plan, int nbatch, const double* 
                          int64_t sA, const double* d, const double* rx, const double* rs, const double* rz,
                          const double* ry, double* dx, double* ds, double* dz, double* dy, void* stream);
 
+/* ---- Box QPs with a dense Q (BoxQPFunction(dense_Q=True)): min 1/2 z'Qz + p'z  s.t.  A z = b,  lb <= z <= ub --------
+ * Only the lower triangle of Q (nz x nz, batch stride sQ, 0 = shared) is read. The dense equivalent, the [lb rows; ub
+ * rows] layout of lam / slacks and every stride convention are those of the qpb200_box_* entry points above. The
+ * inequality block is eliminated as there, and each Newton iteration factors the bordered matrix [Q + G'DG  A'; A  0] of
+ * order nz_pad + neq_pad once, as L diag(I, -I) L' (csrc/qp_boxq.cu), one CTA of `threads` threads per QP. */
+typedef struct qpb200_boxq_plan {
+    int nz, neq, neq_pad, nineq;
+    int has_lb, has_ub;
+    int order;              /* nz_pad + neq_pad: the order of the factored matrix (at most threads) */
+    int threads;            /* CTA size (one CTA per QP) */
+    int64_t smem_bytes;     /* dynamic shared memory per CTA: the factor, A and every vector */
+    int ok;                 /* 1: the kernels cover this shape (order <= threads, smem_bytes <= 227 KB); 0: the entry points
+                             *    below return QPB200_ERR_TOO_LARGE and the dense path on the dense equivalent is the
+                             *    one to use */
+} qpb200_boxq_plan;
+
+int qpb200_boxq_plan_init(int nz, int neq, int has_lb, int has_ub, qpb200_boxq_plan* plan);
+/* As qpb200_box_forward; spd_flag[B] (may be NULL): 1 where chol(Q) breaks down ('Q is not SPD.'). */
+int qpb200_boxq_forward(const qpb200_boxq_plan* plan, int nbatch, const double* Q, int64_t sQ, const double* p,
+                        int64_t sp, const double* A, int64_t sA, const double* b, int64_t sb, const double* lb,
+                        int64_t slb, const double* ub, int64_t sub, double eps, double stall_tol, double best_tie,
+                        int notImprovedLim, int maxIter, double* zhat, double* lam, double* slacks, double* nus,
+                        int* iters, double* best_resid, double* trace, int* spd_flag, void* stream);
+/* As qpb200_box_backward_duals (NULL dl_dlam and dl_dnu: the loss of zhat alone), with dQ = 1/2 (dx z' + z dx')
+ * (B,nz,nz), or its batch mean (nz,nz) with mean_Q = 1, in place of dq. */
+int qpb200_boxq_backward_duals(const qpb200_boxq_plan* plan, int nbatch, const double* Q, int64_t sQ, const double* A,
+                               int64_t sA, const double* dl_dzhat, const double* dl_dlam, const double* dl_dnu,
+                               const double* zhat, const double* lam, const double* slacks, const double* nus,
+                               double* dQ, int mean_Q, double* dp, int mean_p, double* dlb, int mean_lb, double* dub,
+                               int mean_ub, double* dA, int mean_A, double* db, int mean_b, double* dxv,
+                               double* dlamv, double* dnuv, void* stream);
+/* As qpb200_box_jvp, with the tangent dQ (nz x nz, stride sdQ) in place of dq: rx = sym(dQ) z + dp + dA' nu. */
+int qpb200_boxq_jvp(const qpb200_boxq_plan* plan, int nbatch, const double* Q, int64_t sQ, const double* A, int64_t sA,
+                    const double* dQ, int64_t sdQ, const double* dp, int64_t sdp, const double* dA, int64_t sdA,
+                    const double* db, int64_t sdb, const double* dlb, int64_t sdlb, const double* dub, int64_t sdub,
+                    const double* zhat, const double* lam, const double* slacks, const double* nus, double* rhs,
+                    double* dz, double* dlam, double* dnu, void* stream);
+/* As qpb200_box_solve_kkt: [Q 0 G' A'; 0 D I 0; G I 0 0; A 0 0 0] [dx ds dz dy] = -[rx rs rz ry]. */
+int qpb200_boxq_solve_kkt(const qpb200_boxq_plan* plan, int nbatch, const double* Q, int64_t sQ, const double* A,
+                          int64_t sA, const double* d, const double* rx, const double* rs, const double* rz,
+                          const double* ry, double* dx, double* ds, double* dz, double* dy, void* stream);
+
 /* Measurement aid: launches blocks x threads threads each issuing 8*iters dependent-chain-free fp64 FMAs
  * (2*8*iters*blocks*threads flops); out needs blocks*threads doubles. bench.py times it with CUDA
  * events to obtain the fp64 roofline denominator on the box it runs on. */

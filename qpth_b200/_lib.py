@@ -42,6 +42,15 @@ class BoxPlan(ctypes.Structure):
     ]
 
 
+class BoxQPlan(ctypes.Structure):
+    """Mirror of `qpb200_boxq_plan` (include/qpth_b200.h)."""
+    _fields_ = [
+        ("nz", ctypes.c_int), ("neq", ctypes.c_int), ("neq_pad", ctypes.c_int), ("nineq", ctypes.c_int),
+        ("has_lb", ctypes.c_int), ("has_ub", ctypes.c_int), ("order", ctypes.c_int), ("threads", ctypes.c_int),
+        ("smem_bytes", ctypes.c_int64), ("ok", ctypes.c_int),
+    ]
+
+
 # symbol -> (restype, argtypes); also the list tests use to check every declared export exists
 _I, _L, _D, _P = ctypes.c_int, ctypes.c_int64, ctypes.c_double, ctypes.c_void_p
 SIGNATURES = {
@@ -90,6 +99,15 @@ SIGNATURES = {
                             _P, _L, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     "qpb200_box_solve_kkt": (_I, [ctypes.POINTER(BoxPlan), _I, _P, _L, _P, _L, _P, _P, _P, _P, _P,
                                   _P, _P, _P, _P, _P]),
+    "qpb200_boxq_plan_init": (_I, [_I, _I, _I, _I, ctypes.POINTER(BoxQPlan)]),
+    "qpb200_boxq_forward": (_I, [ctypes.POINTER(BoxQPlan), _I, _P, _L, _P, _L, _P, _L, _P, _L, _P, _L, _P, _L,
+                                 _D, _D, _D, _I, _I, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
+    "qpb200_boxq_backward_duals": (_I, [ctypes.POINTER(BoxQPlan), _I, _P, _L, _P, _L, _P, _P, _P, _P, _P, _P, _P,
+                                        _P, _I, _P, _I, _P, _I, _P, _I, _P, _I, _P, _I, _P, _P, _P, _P]),
+    "qpb200_boxq_jvp": (_I, [ctypes.POINTER(BoxQPlan), _I, _P, _L, _P, _L, _P, _L, _P, _L, _P, _L, _P, _L, _P, _L,
+                             _P, _L, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
+    "qpb200_boxq_solve_kkt": (_I, [ctypes.POINTER(BoxQPlan), _I, _P, _L, _P, _L, _P, _P, _P, _P, _P,
+                                   _P, _P, _P, _P, _P]),
 }
 
 _lib = None
@@ -192,6 +210,19 @@ def box_plan_for(nz, neq, has_lb, has_ub):
         check(load().qpb200_box_plan_init(nz, neq, int(bool(has_lb)), int(bool(has_ub)), ctypes.byref(p)))
         _box_plans[key] = p
     return _box_plans[key]
+
+
+_boxq_plans = {}
+
+
+def boxq_plan_for(nz, neq, has_lb, has_ub):
+    """Plan of the dense-Q box kernels for a shape (cached; no device work). plan.ok: they cover it."""
+    key = (nz, neq, bool(has_lb), bool(has_ub))
+    if key not in _boxq_plans:
+        p = BoxQPlan()
+        check(load().qpb200_boxq_plan_init(nz, neq, int(bool(has_lb)), int(bool(has_ub)), ctypes.byref(p)))
+        _boxq_plans[key] = p
+    return _boxq_plans[key]
 
 
 _sm_count = {}

@@ -16,6 +16,11 @@ covers run the dense kernels on the dense equivalent instead.
 
 The OptNet sudoku layer (Q = 0.1 I, G = -I, h = 0, a learned A) is one such problem; a differentiable projection
 min 1/2 ||z - v||^2 s.t. Az = b, lb <= z <= ub is another (q = 1, p = -v).
+
+BoxQPFunction(dense_Q=True) takes a dense Q instead (long-only portfolios, condensed MPC with input bounds, metric
+projections onto a box): the bounds are eliminated the same way, and each Newton iteration factors the bordered matrix
+[Q + G'DG  A'; A  0] of order nz + neq once (csrc/qp_boxq.cu, qpb200_boxq_plan.ok) instead of the dense equivalent's
+order 2 nz + neq. Shapes past one CTA run the dense kernels on the dense equivalent.
 """
 import ctypes
 
@@ -27,12 +32,14 @@ from . import qp as _qp
 from .qp import _dev64, _ptr, _stream
 
 
-def check_box_shapes(q, p, A, b, lb, ub):
+def check_box_shapes(q, p, A, b, lb, ub, dense_Q=False):
     """Validate ranks, trailing dimensions and batch sizes before anything touches the device.
-    Returns (nBatch, nz, neq). q, p, lb, ub: (B, nz) | (nz); A: (B, neq, nz) | (neq, nz) | empty; b follows A."""
+    Returns (nBatch, nz, neq). q, p, lb, ub: (B, nz) | (nz); A: (B, neq, nz) | (neq, nz) | empty; b follows A.
+    dense_Q: q is a dense Q, (B, nz, nz) | (nz, nz)."""
     if lb is None and ub is None:
         raise ValueError("BoxQPFunction: at least one of lb, ub must be given")
-    ins = (("q", q, 2), ("p", p, 2), ("A", A, 3), ("b", b, 2), ("lb", lb, 2), ("ub", ub, 2))
+    ins = (("Q" if dense_Q else "q", q, 3 if dense_Q else 2), ("p", p, 2), ("A", A, 3), ("b", b, 2), ("lb", lb, 2),
+           ("ub", ub, 2))
     nBatch = next((int(X.size(0)) for _, X, r in ins if X is not None and X.nelement() > 0 and X.dim() == r), 1)
     for _, X, r in ins:
         if X is not None and X.nelement() > 0 and X.dim() not in (r, r - 1):
@@ -42,8 +49,10 @@ def check_box_shapes(q, p, A, b, lb, ub):
         raise RuntimeError("qpth_b200: inconsistent shapes: " + msg)
 
     if q.nelement() == 0:
-        fail("q is empty")
+        fail("%s is empty" % ins[0][0])
     nz = int(q.size(-1))
+    if dense_Q and int(q.size(-2)) != nz:
+        fail("Q has shape %s, expected trailing dimensions (nz, nz)" % (tuple(q.shape),))
     neq = int(A.size(-2)) if (A is not None and A.nelement() > 0 and A.dim() >= 2) else 0
     for name, X, trail, needed in (("p", p, (nz,), True), ("lb", lb, (nz,), lb is not None),
                                    ("ub", ub, (nz,), ub is not None), ("A", A, (neq, nz), neq > 0),
@@ -150,6 +159,110 @@ def solve_box_backward(st, dl_dzhat, mean_flags, want, dl_dlam=None, dl_dnu=None
     return outs
 
 
+def solve_boxq_forward(Q_, p_, A_, b_, lb_, ub_, eps=1e-12, verbose=0, notImprovedLim=3, maxIter=20,
+                       check_Q_spd=True):
+    """The dense-Q box kernels on the device (one CTA per QP). Returns _BoxSolved (dense = None; q / sq hold Q and its
+    batch stride), or None when they do not cover the shape."""
+    nBatch, nz, neq = check_box_shapes(Q_, p_, A_, b_, lb_, ub_, dense_Q=True)
+    if _qp._pending:
+        _qp.flush_checks(wait=False)
+    assert maxIter >= 1
+    lib = _lib.load()
+    if not torch.cuda.is_available():
+        raise _lib.QpthB200Error("qpth_b200: no CUDA device available (there is no CPU fallback).")
+    plan = _lib.boxq_plan_for(nz, neq, lb_ is not None, ub_ is not None)
+    if not plan.ok:
+        return None
+    device = Q_.device if Q_.is_cuda else torch.device("cuda", torch.cuda.current_device())
+    with torch.cuda.device(device):
+        Q, p = _dev64(Q_, device), _dev64(p_, device)
+        lb = _dev64(lb_, device) if lb_ is not None else None
+        ub = _dev64(ub_, device) if ub_ is not None else None
+        A = _dev64(A_, device) if neq > 0 else None
+        b = _dev64(b_, device) if neq > 0 else None
+
+        def stride(t, nd, per):
+            return per if (t is not None and t.dim() == nd) else 0
+
+        m = plan.nineq
+        st = _BoxSolved()
+        st.plan, st.nBatch, st.device, st.dense = plan, nBatch, device, None
+        st.q, st.sq, st.A, st.sA = Q, stride(Q, 3, nz * nz), A, stride(A, 3, neq * nz)
+        f64 = dict(dtype=torch.float64, device=device)
+        st.zhat = torch.empty(nBatch, nz, **f64)
+        st.lam = torch.empty(nBatch, m, **f64)
+        st.slacks = torch.empty(nBatch, m, **f64)
+        st.nus = torch.empty(nBatch, neq, **f64) if neq > 0 else None
+        st.iters = torch.empty(nBatch, dtype=torch.int32, device=device)
+        st.best_resid = torch.empty(nBatch, **f64)
+        st.trace = torch.full((nBatch, int(maxIter), 4), float('nan'), **f64) if (verbose == 1 or _qp.TRACE) else None
+        spd = torch.zeros(nBatch, dtype=torch.int32, device=device)
+        _lib.check(lib.qpb200_boxq_forward(
+            ctypes.byref(plan), nBatch, _ptr(Q), st.sq, _ptr(p), stride(p, 2, nz), _ptr(A), st.sA,
+            _ptr(b), stride(b, 2, neq), _ptr(lb), stride(lb, 2, nz), _ptr(ub), stride(ub, 2, nz),
+            float(eps), float(_qp.STALL_TOL), float(_qp.BEST_TIE), int(notImprovedLim), int(maxIter),
+            _ptr(st.zhat), _ptr(st.lam), _ptr(st.slacks), _ptr(st.nus), _ptr(st.iters), _ptr(st.best_resid),
+            _ptr(st.trace), _ptr(spd), _stream()))
+        _qp.diagnostics(spd, st, check_Q_spd, verbose)
+    return st
+
+
+def solve_boxq_backward(st, dl_dzhat, mean_flags, want, dl_dlam=None, dl_dnu=None):
+    """Gradients (dQ, dp, dA, db, dlb, dub) of a solve_boxq_forward state, as solve_box_backward (dQ (B, nz, nz), or
+    (nz, nz) with its mean flag)."""
+    if _qp._pending:
+        _qp.flush_checks(wait=False)
+    lib = _lib.load()
+    plan, B, device = st.plan, st.nBatch, st.device
+    nz, neq, m = plan.nz, plan.neq, plan.nineq
+    f64 = dict(dtype=torch.float64, device=device)
+    with torch.cuda.device(device):
+        dl = _qp._adjoint(dl_dzhat, B, nz, device) if dl_dzhat is not None else torch.zeros(B, nz, **f64)
+        glam, gnu = _qp._adjoint(dl_dlam, B, m, device), _qp._adjoint(dl_dnu, B, neq, device)
+        shapes = [(nz, nz), (nz,), (neq, nz), (neq,), (nz,), (nz,)]
+        outs = []
+        for k in range(6):
+            absent = (k in (2, 3) and neq == 0) or (k == 4 and not plan.has_lb) or (k == 5 and not plan.has_ub)
+            if not want[k] or absent:
+                outs.append(None)
+            else:
+                outs.append(torch.empty(*(shapes[k] if mean_flags[k] else (B,) + shapes[k]), **f64))
+        dxv = torch.empty(B, nz, **f64)
+        dlamv = torch.empty(B, m, **f64)
+        dnuv = torch.empty(B, neq, **f64) if neq > 0 else None
+        dQ, dp, dA, db, dlb, dub = outs
+        mQ, mp, mA, mb, mlb, mub = (1 if f else 0 for f in mean_flags)
+        _lib.check(lib.qpb200_boxq_backward_duals(
+            ctypes.byref(plan), B, _ptr(st.q), st.sq, _ptr(st.A), st.sA, _ptr(dl), _ptr(glam), _ptr(gnu),
+            _ptr(st.zhat), _ptr(st.lam), _ptr(st.slacks), _ptr(st.nus), _ptr(dQ), mQ, _ptr(dp), mp, _ptr(dlb), mlb,
+            _ptr(dub), mub, _ptr(dA), mA, _ptr(db), mb, _ptr(dxv), _ptr(dlamv), _ptr(dnuv), _stream()))
+    return outs
+
+
+def solve_boxq_jvp(st, tangents):
+    """solve_box_jvp for a solve_boxq_forward state: tangents (dQ, dp, dA, db, dlb, dub); one qpb200_boxq_jvp call."""
+    if _qp._pending:
+        _qp.flush_checks(wait=False)
+    lib = _lib.load()
+    plan, B, device = st.plan, st.nBatch, st.device
+    nz, neq, m = plan.nz, plan.neq, plan.nineq
+    f64 = dict(dtype=torch.float64, device=device)
+    with torch.cuda.device(device):
+        per = (nz * nz, nz, neq * nz, neq, nz if plan.has_lb else 0, nz if plan.has_ub else 0)
+        tans = _qp.tangent_args(tangents, (3, 2, 3, 2, 2, 2), per, device)
+        rhs = torch.empty(B * (nz + m + neq), **f64)
+        dz = torch.empty(B, nz, **f64)
+        dlam = torch.empty(B, m, **f64)
+        dnu = torch.empty(B, neq, **f64) if neq > 0 else None
+        args = []
+        for t, s in tans:
+            args += [_ptr(t), s]
+        _lib.check(lib.qpb200_boxq_jvp(
+            ctypes.byref(plan), B, _ptr(st.q), st.sq, _ptr(st.A), st.sA, *args, _ptr(st.zhat), _ptr(st.lam),
+            _ptr(st.slacks), _ptr(st.nus), _ptr(rhs), _ptr(dz), _ptr(dlam), _ptr(dnu), _stream()))
+    return dz, dlam, dnu
+
+
 def solve_box_jvp(st, tangents):
     """The JVP of (zhat, lam, nu) at the returned point on the device. tangents: (dq, dp, dA, db, dlb, dub), each None
     (zero), batched or un-batched as its input. Returns fp64 (dz (B,nz), dlam (B,nineq) in the [lb rows; ub rows]
@@ -177,11 +290,11 @@ def solve_box_jvp(st, tangents):
 
 
 # ---- shapes beyond the box kernels: the dense kernels on the dense equivalent ---------------------------------------
-def dense_equivalent(q, lb, ub):
-    """(Q, G, h) of QPFunction for a box QP: Q = diag(q), G = [-I; I] (sides given), h = [-lb; ub]. Batched where
-    q (for Q) or either bound (for h) is batched."""
+def dense_equivalent(q, lb, ub, dense_Q=False):
+    """(Q, G, h) of QPFunction for a box QP: Q = diag(q) (dense_Q: q itself), G = [-I; I] (sides given),
+    h = [-lb; ub]. Batched where q (for Q) or either bound (for h) is batched."""
     nz = q.size(-1)
-    Q = torch.diag_embed(q)
+    Q = q if dense_Q else torch.diag_embed(q)
     eye = torch.eye(nz, dtype=q.dtype, device=q.device)
     G = torch.cat(([-eye] if lb is not None else []) + ([eye] if ub is not None else []), 0)
     sides = [(-lb) if lb is not None else None, ub]
@@ -193,10 +306,11 @@ def dense_equivalent(q, lb, ub):
     return Q, G, h
 
 
-def solve_dense_forward(q_, p_, A_, b_, lb_, ub_, eps, verbose, notImprovedLim, maxIter, check_Q_spd):
+def solve_dense_forward(q_, p_, A_, b_, lb_, ub_, eps, verbose, notImprovedLim, maxIter, check_Q_spd, dense_Q=False):
     A_ = A_ if A_ is not None else torch.empty(0, dtype=q_.dtype, device=q_.device)
     b_ = b_ if b_ is not None else torch.empty(0, dtype=q_.dtype, device=q_.device)
-    Q, G, h = dense_equivalent(q_.detach(), None if lb_ is None else lb_.detach(), None if ub_ is None else ub_.detach())
+    Q, G, h = dense_equivalent(q_.detach(), None if lb_ is None else lb_.detach(), None if ub_ is None else ub_.detach(),
+                               dense_Q)
     dst = _qp.solve_forward(Q, p_.detach(), G, h, A_.detach(), b_.detach(), eps, verbose, notImprovedLim, maxIter,
                             check_Q_spd)
     st = _BoxSolved()
@@ -208,14 +322,14 @@ def solve_dense_forward(q_, p_, A_, b_, lb_, ub_, eps, verbose, notImprovedLim, 
     return st
 
 
-def dense_backward(st, dl, mean_flags, want, nlb, has_ub, dl_dlam=None, dl_dnu=None):
+def dense_backward(st, dl, mean_flags, want, nlb, has_ub, dl_dlam=None, dl_dnu=None, dense_Q=False):
     dst, h_shared = st.dense
     mq, mp, mA, mb, mlb, mub = mean_flags
     # the dense equivalent's rows are lam's [lb rows; ub rows]: the dual adjoints pass through as they are
     outs = _qp.solve_backward(dst, dl, (mq, mp, True, h_shared, mA, mb),
                               (want[0], want[1], False, want[4] or want[5], want[2], want[3]), dl_dlam, dl_dnu)
     dQ, dp, _, dh, dA, db = outs
-    dq = None if dQ is None else torch.diagonal(dQ, dim1=-2, dim2=-1).contiguous()
+    dq = dQ if (dQ is None or dense_Q) else torch.diagonal(dQ, dim1=-2, dim2=-1).contiguous()
     dlb = dub = None
     if dh is not None:
         if want[4] and nlb:
@@ -227,11 +341,12 @@ def dense_backward(st, dl, mean_flags, want, nlb, has_ub, dl_dlam=None, dl_dnu=N
     return [dq, dp, dA, db, dlb, dub]
 
 
-def dense_jvp(st, tangents, nlb, has_ub):
-    """solve_box_jvp on the dense equivalent: dQ = diag(dq), no dG, dh = [-dlb; dub] (a missing side's tangent is 0)."""
+def dense_jvp(st, tangents, nlb, has_ub, dense_Q=False):
+    """solve_box_jvp on the dense equivalent: dQ = diag(dq) (dense_Q: dq is dQ), no dG, dh = [-dlb; dub] (a missing
+    side's tangent is 0)."""
     dst, _ = st.dense
     dq, dp, dA, db, dlb, dub = tangents
-    dQ = None if dq is None else torch.diag_embed(dq)
+    dQ = dq if (dq is None or dense_Q) else torch.diag_embed(dq)
     dh = None
     if dlb is not None or dub is not None:
         sides = ([None if dlb is None else -dlb] if nlb else []) + ([dub] if has_ub else [])
@@ -244,7 +359,7 @@ def dense_jvp(st, tangents, nlb, has_ub):
     return _qp.solve_jvp(dst, (dQ, dp, None, dh, dA, db))
 
 
-def BoxQPFunction(eps=1e-12, verbose=0, notImprovedLim=3, maxIter=20, check_Q_spd=True, duals=False):
+def BoxQPFunction(eps=1e-12, verbose=0, notImprovedLim=3, maxIter=20, check_Q_spd=True, duals=False, dense_Q=False):
     """Factory with QPFunction's options; returns f(q, p, A, b, lb, ub) -> z (nBatch, nz).
 
     q, p, lb, ub: (nBatch, nz) or (nz); A: (nBatch, neq, nz), (neq, nz) or an empty tensor; b follows A. lb or ub may
@@ -256,15 +371,25 @@ def BoxQPFunction(eps=1e-12, verbose=0, notImprovedLim=3, maxIter=20, check_Q_sp
 
     Forward mode (torch.autograd.forward_ad) is supported as for QPFunction: rx = dq o z + dp + dA' nu, rz = [dlb; -dub],
     ry = dA z - db on the right-hand side of the backward's solve (qpb200_box_jvp; the dense fallback maps the tangents
-    to its dense equivalent, dQ = diag(dq), dh = [-dlb; dub])."""
+    to its dense equivalent, dQ = diag(dq), dh = [-dlb; dub]).
+
+    dense_Q=True: the first argument is a dense Q, (nBatch, nz, nz) or (nz, nz) (a 2-D Q is un-batched), of which only
+    the lower triangle is read, as in QPFunction's kernels. Everything else is as above, with QPFunction's semantics on
+    the dense equivalent (Q, G = [-I; I], h = [-lb; ub]): 'Q is not SPD.' where chol(Q) breaks down, the gradient
+    dQ = 1/2 (dx z' + z dx') (the batch mean for an un-batched Q), and the tangent dQ enters forward mode as
+    sym(dQ) z. Shapes past the dense-Q kernels (qpb200_boxq_plan.ok) run the dense kernels on the dense equivalent."""
     _last = [None]
 
     class BoxQPFunctionFn(Function):
         @staticmethod
         def forward(ctx, q_, p_, A_, b_, lb_, ub_):
-            st = solve_box_forward(q_, p_, A_, b_, lb_, ub_, eps, verbose, notImprovedLim, maxIter, check_Q_spd)
+            if dense_Q:
+                st = solve_boxq_forward(q_, p_, A_, b_, lb_, ub_, eps, verbose, notImprovedLim, maxIter, check_Q_spd)
+            else:
+                st = solve_box_forward(q_, p_, A_, b_, lb_, ub_, eps, verbose, notImprovedLim, maxIter, check_Q_spd)
             if st is None:
-                st = solve_dense_forward(q_, p_, A_, b_, lb_, ub_, eps, verbose, notImprovedLim, maxIter, check_Q_spd)
+                st = solve_dense_forward(q_, p_, A_, b_, lb_, ub_, eps, verbose, notImprovedLim, maxIter, check_Q_spd,
+                                         dense_Q)
             ctx.st = st
             _last[0] = st
             zhats = st.zhat.to(device=q_.device, dtype=q_.dtype)
@@ -281,7 +406,10 @@ def BoxQPFunction(eps=1e-12, verbose=0, notImprovedLim=3, maxIter=20, check_Q_sp
         def jvp(ctx, dq, dp, dA, db, dlb, dub):
             tangents = (dq, dp, dA, db, dlb, dub)
             st = ctx.st
-            out = solve_box_jvp(st, tangents) if st.dense is None else dense_jvp(st, tangents, *ctx.sides)
+            if st.dense is not None:
+                out = dense_jvp(st, tangents, *ctx.sides, dense_Q=dense_Q)
+            else:
+                out = (solve_boxq_jvp if dense_Q else solve_box_jvp)(st, tangents)
             return _qp.jvp_outputs(*out, ctx.out, duals)
 
         @staticmethod
@@ -289,14 +417,15 @@ def BoxQPFunction(eps=1e-12, verbose=0, notImprovedLim=3, maxIter=20, check_Q_sp
             zhats, q, p, A, b, lb, ub = ctx.saved_tensors
             st = ctx.st
             ins = (q, p, A, b, lb, ub)
-            ranks = (2, 2, 3, 2, 2, 2)
+            ranks = (3 if dense_Q else 2, 2, 3, 2, 2, 2)
             flags = [X is not None and X.nelement() > 0 and X.dim() == r - 1 for X, r in zip(ins, ranks)]
             want = list(ctx.needs_input_grad)
             if st.dense is None:
-                outs = solve_box_backward(st, dl_dzhat, flags, want, dl_dlam, dl_dnu)
+                outs = (solve_boxq_backward if dense_Q else solve_box_backward)(st, dl_dzhat, flags, want, dl_dlam,
+                                                                                dl_dnu)
             else:
                 outs = dense_backward(st, dl_dzhat, flags, want, q.size(-1) if lb is not None else 0, ub is not None,
-                                      dl_dlam, dl_dnu)
+                                      dl_dlam, dl_dnu, dense_Q)
             return tuple(None if (g is None or X is None or not w) else g.to(device=X.device, dtype=X.dtype)
                          for X, g, w in zip(ins, outs, want))
 

@@ -1548,6 +1548,11 @@ int box_launch(const char* what, const qpb200_box_plan* plan, int nbatch, void* 
 
 extern "C" {
 
+int qpb200_internal_box_means(int nbatch, int n, int m, int e, int nlb, const double* dxv, const double* dlamv,
+                              const double* dnuv, const double* zhat, const double* nus, double* dp, int mean_p,
+                              double* dlb, int mean_lb, double* dub, int mean_ub, double* dA, int mean_A, double* db,
+                              int mean_b, void* stream);
+
 int qpb200_box_plan_init(int nz, int neq, int has_lb, int has_ub, qpb200_box_plan* plan) {
     if (plan == nullptr || nz <= 0 || neq < 0) return QPB200_ERR_BAD_ARG;
     if (!has_lb && !has_ub) return QPB200_ERR_NO_CONSTRAINTS;
@@ -1641,9 +1646,19 @@ int qpb200_box_backward_duals(const qpb200_box_plan* plan, int nbatch, const dou
                     k_box_backward_dm, q, sq, A, sA, dl_dzhat, dl_dlam, dl_dnu, zhat, lam, slacks, nus, O, dxv, dlamv,
                     dnuv);
     if (rc) return rc;
+    if (dq && mean_q)
+        k_box_mean_vec<<<(n + 127) / 128, 128, 0, (cudaStream_t)stream>>>(nbatch, n, dxv, n, zhat, 1.0, dq);
+    return qpb200_internal_box_means(nbatch, n, m, e, nlb, dxv, dlamv, dnuv, zhat, nus, dp, mean_p, dlb, mean_lb, dub,
+                                     mean_ub, dA, mean_A, db, mean_b, stream);
+}
+
+// the batch means of dp, dlb, dub, dA, db from dx, dlam, dnu (here and in qpb200_boxq_backward_duals, qp_boxq.cu)
+int qpb200_internal_box_means(int nbatch, int n, int m, int e, int nlb, const double* dxv, const double* dlamv,
+                              const double* dnuv, const double* zhat, const double* nus, double* dp, int mean_p,
+                              double* dlb, int mean_lb, double* dub, int mean_ub, double* dA, int mean_A, double* db,
+                              int mean_b, void* stream) {
     cudaStream_t st = (cudaStream_t)stream;
     const int TB = 128;
-    if (dq && mean_q) k_box_mean_vec<<<(n + TB - 1) / TB, TB, 0, st>>>(nbatch, n, dxv, n, zhat, 1.0, dq);
     if (dp && mean_p) k_box_mean_vec<<<(n + TB - 1) / TB, TB, 0, st>>>(nbatch, n, dxv, n, nullptr, 1.0, dp);
     if (dlb && mean_lb) k_box_mean_vec<<<(n + TB - 1) / TB, TB, 0, st>>>(nbatch, n, dlamv, m, nullptr, 1.0, dlb);
     if (dub && mean_ub)

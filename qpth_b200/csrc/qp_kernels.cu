@@ -1216,6 +1216,15 @@ int qpb200_internal_set_smem(const void* kernel, size_t bytes) {
     return QPB200_OK;
 }
 
+// (qp_boxq.cu) the batch mean of dQ for an un-batched Q: out = scale / B (U^T X + Y^T V) by k_mean_outer
+int qpb200_internal_mean_outer(int B, int rows, int cols, const double* u, const double* x, const double* y,
+                               const double* v, double scale, double* out, void* stream) {
+    k_mean_outer<<<dim3((cols + kMoC - 1) / kMoC, (rows + kMoR - 1) / kMoR), 256, 0, (cudaStream_t)stream>>>(
+        B, rows, cols, u, x, y, v, scale, out);
+    CK(cudaGetLastError());
+    return QPB200_OK;
+}
+
 int qpb200_version(void) { return 100; }
 
 const char* qpb200_error_string(int code) {
