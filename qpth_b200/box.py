@@ -71,24 +71,31 @@ def check_box_shapes(q, p, A, b, lb, ub, dense_Q=False):
 
 
 class _BoxSolved:
-    """State carried from forward to backward; lam / slacks are laid out as [lb rows; ub rows]."""
+    """State carried from forward to backward; lam / slacks are laid out as [lb rows; ub rows]. dense_Q: q / sq hold a
+    dense Q and its batch stride, and plan is a qpb200_boxq_plan."""
     __slots__ = ("plan", "nBatch", "device", "q", "sq", "A", "sA", "zhat", "lam", "slacks", "nus", "iters",
-                 "best_resid", "trace", "dense")
+                 "best_resid", "trace", "dense", "dense_Q")
 
 
-def solve_box_forward(q_, p_, A_, b_, lb_, ub_, eps=1e-12, verbose=0, notImprovedLim=3, maxIter=20, check_Q_spd=True):
-    """The box kernels on the device (one CTA per QP, or a cluster of plan.cl_ctas CTAs per QP). Returns _BoxSolved
-    (dense = None), or None when neither covers the shape."""
-    nBatch, nz, neq = check_box_shapes(q_, p_, A_, b_, lb_, ub_)
+def solve_box_forward(q_, p_, A_, b_, lb_, ub_, eps=1e-12, verbose=0, notImprovedLim=3, maxIter=20, check_Q_spd=True,
+                      dense_Q=False):
+    """The box kernels on the device: one CTA per QP, or a cluster of plan.cl_ctas CTAs per QP; dense_Q: the dense-Q
+    kernels, one CTA per QP. Returns _BoxSolved (dense = None), or None when they do not cover the shape."""
+    nBatch, nz, neq = check_box_shapes(q_, p_, A_, b_, lb_, ub_, dense_Q)
     if _qp._pending:
         _qp.flush_checks(wait=False)
     assert maxIter >= 1
     lib = _lib.load()
     if not torch.cuda.is_available():
         raise _lib.QpthB200Error("qpth_b200: no CUDA device available (there is no CPU fallback).")
-    plan = _lib.box_plan_for(nz, neq, lb_ is not None, ub_ is not None)
-    if not (plan.ok or plan.cl_ctas):
-        return None
+    if dense_Q:
+        plan = _lib.boxq_plan_for(nz, neq, lb_ is not None, ub_ is not None)
+        if not plan.ok:
+            return None
+    else:
+        plan = _lib.box_plan_for(nz, neq, lb_ is not None, ub_ is not None)
+        if not (plan.ok or plan.cl_ctas):
+            return None
     device = q_.device if q_.is_cuda else torch.device("cuda", torch.cuda.current_device())
     with torch.cuda.device(device):
         q, p = _dev64(q_, device), _dev64(p_, device)
@@ -102,8 +109,9 @@ def solve_box_forward(q_, p_, A_, b_, lb_, ub_, eps=1e-12, verbose=0, notImprove
 
         m = plan.nineq
         st = _BoxSolved()
-        st.plan, st.nBatch, st.device, st.dense = plan, nBatch, device, None
-        st.q, st.sq, st.A, st.sA = q, stride(q, 2, nz), A, stride(A, 3, neq * nz)
+        st.plan, st.nBatch, st.device, st.dense, st.dense_Q = plan, nBatch, device, None, dense_Q
+        st.q, st.sq = q, (stride(q, 3, nz * nz) if dense_Q else stride(q, 2, nz))
+        st.A, st.sA = A, stride(A, 3, neq * nz)
         f64 = dict(dtype=torch.float64, device=device)
         st.zhat = torch.empty(nBatch, nz, **f64)
         st.lam = torch.empty(nBatch, m, **f64)
@@ -113,7 +121,8 @@ def solve_box_forward(q_, p_, A_, b_, lb_, ub_, eps=1e-12, verbose=0, notImprove
         st.best_resid = torch.empty(nBatch, **f64)
         st.trace = torch.full((nBatch, int(maxIter), 4), float('nan'), **f64) if (verbose == 1 or _qp.TRACE) else None
         spd = torch.zeros(nBatch, dtype=torch.int32, device=device)
-        _lib.check(lib.qpb200_box_forward(
+        fn = lib.qpb200_boxq_forward if dense_Q else lib.qpb200_box_forward
+        _lib.check(fn(
             ctypes.byref(plan), nBatch, _ptr(q), st.sq, _ptr(p), stride(p, 2, nz), _ptr(A), st.sA,
             _ptr(b), stride(b, 2, neq), _ptr(lb), stride(lb, 2, nz), _ptr(ub), stride(ub, 2, nz),
             float(eps), float(_qp.STALL_TOL), float(_qp.BEST_TIE), int(notImprovedLim), int(maxIter),
@@ -125,7 +134,8 @@ def solve_box_forward(q_, p_, A_, b_, lb_, ub_, eps=1e-12, verbose=0, notImprove
 
 def solve_box_backward(st, dl_dzhat, mean_flags, want, dl_dlam=None, dl_dnu=None):
     """Gradients (dq, dp, dA, db, dlb, dub) on the device; mean_flags / want: 6-tuples in that order. dl_dlam ([lb rows;
-    ub rows]) / dl_dnu: the gradients with respect to the returned duals (None: zero); dl_dzhat None: zero."""
+    ub rows]) / dl_dnu: the gradients with respect to the returned duals (None: zero); dl_dzhat None: zero. With a
+    dense Q the first is dQ, (B, nz, nz) or (nz, nz) with its mean flag."""
     if _qp._pending:
         _qp.flush_checks(wait=False)
     lib = _lib.load()
@@ -135,7 +145,7 @@ def solve_box_backward(st, dl_dzhat, mean_flags, want, dl_dlam=None, dl_dnu=None
     with torch.cuda.device(device):
         dl = _qp._adjoint(dl_dzhat, B, nz, device) if dl_dzhat is not None else torch.zeros(B, nz, **f64)
         glam, gnu = _qp._adjoint(dl_dlam, B, m, device), _qp._adjoint(dl_dnu, B, neq, device)
-        shapes = [(nz,), (nz,), (neq, nz), (neq,), (nz,), (nz,)]
+        shapes = [(nz, nz) if st.dense_Q else (nz,), (nz,), (neq, nz), (neq,), (nz,), (nz,)]
         outs = []
         for k in range(6):
             absent = (k in (2, 3) and neq == 0) or (k == 4 and not plan.has_lb) or (k == 5 and not plan.has_ub)
@@ -148,7 +158,9 @@ def solve_box_backward(st, dl_dzhat, mean_flags, want, dl_dlam=None, dl_dnu=None
         dnuv = torch.empty(B, neq, **f64) if neq > 0 else None
         dq, dp, dA, db, dlb, dub = outs
         mq, mp, mA, mb, mlb, mub = (1 if f else 0 for f in mean_flags)
-        if glam is None and gnu is None:            # no dual was used: the entry point of a zhat-only loss
+        if st.dense_Q:
+            fn, adj = lib.qpb200_boxq_backward_duals, (_ptr(glam), _ptr(gnu))
+        elif glam is None and gnu is None:          # no dual was used: the entry point of a zhat-only loss
             fn, adj = lib.qpb200_box_backward, ()
         else:
             fn, adj = lib.qpb200_box_backward_duals, (_ptr(glam), _ptr(gnu))
@@ -159,114 +171,11 @@ def solve_box_backward(st, dl_dzhat, mean_flags, want, dl_dlam=None, dl_dnu=None
     return outs
 
 
-def solve_boxq_forward(Q_, p_, A_, b_, lb_, ub_, eps=1e-12, verbose=0, notImprovedLim=3, maxIter=20,
-                       check_Q_spd=True):
-    """The dense-Q box kernels on the device (one CTA per QP). Returns _BoxSolved (dense = None; q / sq hold Q and its
-    batch stride), or None when they do not cover the shape."""
-    nBatch, nz, neq = check_box_shapes(Q_, p_, A_, b_, lb_, ub_, dense_Q=True)
-    if _qp._pending:
-        _qp.flush_checks(wait=False)
-    assert maxIter >= 1
-    lib = _lib.load()
-    if not torch.cuda.is_available():
-        raise _lib.QpthB200Error("qpth_b200: no CUDA device available (there is no CPU fallback).")
-    plan = _lib.boxq_plan_for(nz, neq, lb_ is not None, ub_ is not None)
-    if not plan.ok:
-        return None
-    device = Q_.device if Q_.is_cuda else torch.device("cuda", torch.cuda.current_device())
-    with torch.cuda.device(device):
-        Q, p = _dev64(Q_, device), _dev64(p_, device)
-        lb = _dev64(lb_, device) if lb_ is not None else None
-        ub = _dev64(ub_, device) if ub_ is not None else None
-        A = _dev64(A_, device) if neq > 0 else None
-        b = _dev64(b_, device) if neq > 0 else None
-
-        def stride(t, nd, per):
-            return per if (t is not None and t.dim() == nd) else 0
-
-        m = plan.nineq
-        st = _BoxSolved()
-        st.plan, st.nBatch, st.device, st.dense = plan, nBatch, device, None
-        st.q, st.sq, st.A, st.sA = Q, stride(Q, 3, nz * nz), A, stride(A, 3, neq * nz)
-        f64 = dict(dtype=torch.float64, device=device)
-        st.zhat = torch.empty(nBatch, nz, **f64)
-        st.lam = torch.empty(nBatch, m, **f64)
-        st.slacks = torch.empty(nBatch, m, **f64)
-        st.nus = torch.empty(nBatch, neq, **f64) if neq > 0 else None
-        st.iters = torch.empty(nBatch, dtype=torch.int32, device=device)
-        st.best_resid = torch.empty(nBatch, **f64)
-        st.trace = torch.full((nBatch, int(maxIter), 4), float('nan'), **f64) if (verbose == 1 or _qp.TRACE) else None
-        spd = torch.zeros(nBatch, dtype=torch.int32, device=device)
-        _lib.check(lib.qpb200_boxq_forward(
-            ctypes.byref(plan), nBatch, _ptr(Q), st.sq, _ptr(p), stride(p, 2, nz), _ptr(A), st.sA,
-            _ptr(b), stride(b, 2, neq), _ptr(lb), stride(lb, 2, nz), _ptr(ub), stride(ub, 2, nz),
-            float(eps), float(_qp.STALL_TOL), float(_qp.BEST_TIE), int(notImprovedLim), int(maxIter),
-            _ptr(st.zhat), _ptr(st.lam), _ptr(st.slacks), _ptr(st.nus), _ptr(st.iters), _ptr(st.best_resid),
-            _ptr(st.trace), _ptr(spd), _stream()))
-        _qp.diagnostics(spd, st, check_Q_spd, verbose)
-    return st
-
-
-def solve_boxq_backward(st, dl_dzhat, mean_flags, want, dl_dlam=None, dl_dnu=None):
-    """Gradients (dQ, dp, dA, db, dlb, dub) of a solve_boxq_forward state, as solve_box_backward (dQ (B, nz, nz), or
-    (nz, nz) with its mean flag)."""
-    if _qp._pending:
-        _qp.flush_checks(wait=False)
-    lib = _lib.load()
-    plan, B, device = st.plan, st.nBatch, st.device
-    nz, neq, m = plan.nz, plan.neq, plan.nineq
-    f64 = dict(dtype=torch.float64, device=device)
-    with torch.cuda.device(device):
-        dl = _qp._adjoint(dl_dzhat, B, nz, device) if dl_dzhat is not None else torch.zeros(B, nz, **f64)
-        glam, gnu = _qp._adjoint(dl_dlam, B, m, device), _qp._adjoint(dl_dnu, B, neq, device)
-        shapes = [(nz, nz), (nz,), (neq, nz), (neq,), (nz,), (nz,)]
-        outs = []
-        for k in range(6):
-            absent = (k in (2, 3) and neq == 0) or (k == 4 and not plan.has_lb) or (k == 5 and not plan.has_ub)
-            if not want[k] or absent:
-                outs.append(None)
-            else:
-                outs.append(torch.empty(*(shapes[k] if mean_flags[k] else (B,) + shapes[k]), **f64))
-        dxv = torch.empty(B, nz, **f64)
-        dlamv = torch.empty(B, m, **f64)
-        dnuv = torch.empty(B, neq, **f64) if neq > 0 else None
-        dQ, dp, dA, db, dlb, dub = outs
-        mQ, mp, mA, mb, mlb, mub = (1 if f else 0 for f in mean_flags)
-        _lib.check(lib.qpb200_boxq_backward_duals(
-            ctypes.byref(plan), B, _ptr(st.q), st.sq, _ptr(st.A), st.sA, _ptr(dl), _ptr(glam), _ptr(gnu),
-            _ptr(st.zhat), _ptr(st.lam), _ptr(st.slacks), _ptr(st.nus), _ptr(dQ), mQ, _ptr(dp), mp, _ptr(dlb), mlb,
-            _ptr(dub), mub, _ptr(dA), mA, _ptr(db), mb, _ptr(dxv), _ptr(dlamv), _ptr(dnuv), _stream()))
-    return outs
-
-
-def solve_boxq_jvp(st, tangents):
-    """solve_box_jvp for a solve_boxq_forward state: tangents (dQ, dp, dA, db, dlb, dub); one qpb200_boxq_jvp call."""
-    if _qp._pending:
-        _qp.flush_checks(wait=False)
-    lib = _lib.load()
-    plan, B, device = st.plan, st.nBatch, st.device
-    nz, neq, m = plan.nz, plan.neq, plan.nineq
-    f64 = dict(dtype=torch.float64, device=device)
-    with torch.cuda.device(device):
-        per = (nz * nz, nz, neq * nz, neq, nz if plan.has_lb else 0, nz if plan.has_ub else 0)
-        tans = _qp.tangent_args(tangents, (3, 2, 3, 2, 2, 2), per, device)
-        rhs = torch.empty(B * (nz + m + neq), **f64)
-        dz = torch.empty(B, nz, **f64)
-        dlam = torch.empty(B, m, **f64)
-        dnu = torch.empty(B, neq, **f64) if neq > 0 else None
-        args = []
-        for t, s in tans:
-            args += [_ptr(t), s]
-        _lib.check(lib.qpb200_boxq_jvp(
-            ctypes.byref(plan), B, _ptr(st.q), st.sq, _ptr(st.A), st.sA, *args, _ptr(st.zhat), _ptr(st.lam),
-            _ptr(st.slacks), _ptr(st.nus), _ptr(rhs), _ptr(dz), _ptr(dlam), _ptr(dnu), _stream()))
-    return dz, dlam, dnu
-
-
 def solve_box_jvp(st, tangents):
     """The JVP of (zhat, lam, nu) at the returned point on the device. tangents: (dq, dp, dA, db, dlb, dub), each None
-    (zero), batched or un-batched as its input. Returns fp64 (dz (B,nz), dlam (B,nineq) in the [lb rows; ub rows]
-    layout, dnu (B,neq) or None); one qpb200_box_jvp call: the right-hand side kernel and the backward's solve."""
+    (zero), batched or un-batched as its input (with a dense Q, dQ first). Returns fp64 (dz (B,nz), dlam (B,nineq) in
+    the [lb rows; ub rows] layout, dnu (B,neq) or None); one qpb200_box_jvp / qpb200_boxq_jvp call: the right-hand side
+    kernel and the backward's solve."""
     if _qp._pending:
         _qp.flush_checks(wait=False)
     lib = _lib.load()
@@ -274,8 +183,8 @@ def solve_box_jvp(st, tangents):
     nz, neq, m = plan.nz, plan.neq, plan.nineq
     f64 = dict(dtype=torch.float64, device=device)
     with torch.cuda.device(device):
-        per = (nz, nz, neq * nz, neq, nz if plan.has_lb else 0, nz if plan.has_ub else 0)
-        tans = _qp.tangent_args(tangents, (2, 2, 3, 2, 2, 2), per, device)
+        per = (nz * nz if st.dense_Q else nz, nz, neq * nz, neq, nz if plan.has_lb else 0, nz if plan.has_ub else 0)
+        tans = _qp.tangent_args(tangents, (3 if st.dense_Q else 2, 2, 3, 2, 2, 2), per, device)
         rhs = torch.empty(B * (nz + m + neq), **f64)
         dz = torch.empty(B, nz, **f64)
         dlam = torch.empty(B, m, **f64)
@@ -283,7 +192,8 @@ def solve_box_jvp(st, tangents):
         args = []
         for t, s in tans:
             args += [_ptr(t), s]
-        _lib.check(lib.qpb200_box_jvp(
+        fn = lib.qpb200_boxq_jvp if st.dense_Q else lib.qpb200_box_jvp
+        _lib.check(fn(
             ctypes.byref(plan), B, _ptr(st.q), st.sq, _ptr(st.A), st.sA, *args, _ptr(st.zhat), _ptr(st.lam),
             _ptr(st.slacks), _ptr(st.nus), _ptr(rhs), _ptr(dz), _ptr(dlam), _ptr(dnu), _stream()))
     return dz, dlam, dnu
@@ -315,6 +225,7 @@ def solve_dense_forward(q_, p_, A_, b_, lb_, ub_, eps, verbose, notImprovedLim, 
                             check_Q_spd)
     st = _BoxSolved()
     st.plan, st.nBatch, st.device, st.dense = dst.plan, dst.nBatch, dst.device, (dst, h.dim() == 1)
+    st.dense_Q = dense_Q
     st.zhat, st.lam, st.slacks, st.nus = dst.zhat, dst.lam, dst.slacks, dst.nus
     st.iters, st.best_resid, st.trace = dst.iters, dst.best_resid, dst.trace
     st.q = st.A = None
@@ -383,10 +294,8 @@ def BoxQPFunction(eps=1e-12, verbose=0, notImprovedLim=3, maxIter=20, check_Q_sp
     class BoxQPFunctionFn(Function):
         @staticmethod
         def forward(ctx, q_, p_, A_, b_, lb_, ub_):
-            if dense_Q:
-                st = solve_boxq_forward(q_, p_, A_, b_, lb_, ub_, eps, verbose, notImprovedLim, maxIter, check_Q_spd)
-            else:
-                st = solve_box_forward(q_, p_, A_, b_, lb_, ub_, eps, verbose, notImprovedLim, maxIter, check_Q_spd)
+            st = solve_box_forward(q_, p_, A_, b_, lb_, ub_, eps, verbose, notImprovedLim, maxIter, check_Q_spd,
+                                   dense_Q)
             if st is None:
                 st = solve_dense_forward(q_, p_, A_, b_, lb_, ub_, eps, verbose, notImprovedLim, maxIter, check_Q_spd,
                                          dense_Q)
@@ -409,7 +318,7 @@ def BoxQPFunction(eps=1e-12, verbose=0, notImprovedLim=3, maxIter=20, check_Q_sp
             if st.dense is not None:
                 out = dense_jvp(st, tangents, *ctx.sides, dense_Q=dense_Q)
             else:
-                out = (solve_boxq_jvp if dense_Q else solve_box_jvp)(st, tangents)
+                out = solve_box_jvp(st, tangents)
             return _qp.jvp_outputs(*out, ctx.out, duals)
 
         @staticmethod
@@ -421,8 +330,7 @@ def BoxQPFunction(eps=1e-12, verbose=0, notImprovedLim=3, maxIter=20, check_Q_sp
             flags = [X is not None and X.nelement() > 0 and X.dim() == r - 1 for X, r in zip(ins, ranks)]
             want = list(ctx.needs_input_grad)
             if st.dense is None:
-                outs = (solve_boxq_backward if dense_Q else solve_box_backward)(st, dl_dzhat, flags, want, dl_dlam,
-                                                                                dl_dnu)
+                outs = solve_box_backward(st, dl_dzhat, flags, want, dl_dlam, dl_dnu)
             else:
                 outs = dense_backward(st, dl_dzhat, flags, want, q.size(-1) if lb is not None else 0, ub is not None,
                                       dl_dlam, dl_dnu, dense_Q)

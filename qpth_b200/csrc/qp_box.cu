@@ -16,12 +16,13 @@
 //            one that decides: (8, 136, lb) fits in 114 KB and is rejected by it alone.
 //   a cluster per QP (family Cluster): past that, a thread block cluster of 2, 4 or 8 CTAs (qpb200_box_plan.cl_ctas),
 //            each CTA holding a slice of the variables; M is summed and factored redundantly in every CTA.
-//   distributed M (k_box_*_dm): past neq_pad = 128, M is distributed over the cluster as well and A is read from
+//   distributed M (family Dm): past neq_pad = 128, M is distributed over the cluster as well and A is read from
 //            global memory.
 // BoxQPFunction runs the dense kernels on the dense equivalent only where none covers the shape. For the first two the
-// Mehrotra loop (k_box_forward<F>), the backward and KKT kernels and the structured solve (box_solve<F>) are written
-// once; a family supplies only what differs: its per-CTA context, its reductions, how A is staged, how M is formed and
-// solved.
+// Mehrotra loop (k_box_forward<F>), the backward and the KKT kernels are those of qp_box_loop.cuh, which the dense-Q
+// family of qp_boxq.cu shares, and the structured solve (box_solve<F>) is written once here; a family supplies whole
+// phases: its per-CTA context, its reductions, how A is staged, how M is formed and solved. The distributed-M kernels
+// keep their own copy of the loop (DESIGN.md, box kernels).
 #include <cooperative_groups.h>
 #include <cuda_runtime.h>
 #include <math.h>
@@ -41,17 +42,14 @@
 #define qpb qpb_box
 #include "qp_pf.cuh"
 #include "qp_jvp.cuh"
+#include "qp_box_loop.cuh"
 
-extern "C" void qpb200_internal_cuda_error(int err, const char* what);   // (qp_kernels.cu) records the message, per thread
 extern "C" int qpb200_internal_set_smem(const void* kernel, size_t bytes);   // (qp_kernels.cu) the kernels' smem limits
 
 namespace {
 
 using namespace qpb::pf;
 namespace cg = cooperative_groups;
-constexpr int kBoxNT = qpb::fast::kNT;
-constexpr int kClW = kBoxNT / 32;          // warps per CTA: scalar partials are published per warp
-constexpr int kBoxMaxSmem = 232448;        // H100: 227 KB of dynamic shared memory per CTA
 
 // ---- shared-memory layout (doubles; every offset a multiple of 8, i.e. 64-byte aligned) ------------------------------
 struct BoxDims {
@@ -64,8 +62,6 @@ struct BoxDims {
     int b, y, ry, rhs, t, dya, dy, by;                       // length ep
     int total;               // doubles
 };
-
-__host__ __device__ inline int r8(int v) { return (v + 7) & ~7; }
 
 // the n-, m- and ep-length vectors of D (counts set) from offset o; returns the end
 __host__ __device__ inline int box_vectors(BoxDims& D, int o) {
@@ -93,21 +89,6 @@ __host__ __device__ inline BoxDims box_dims(int n, int e, int has_lb, int has_ub
     D.total = box_vectors(D, o);
     return D;
 }
-
-// inequality row i is sign(i) * e_var(i)
-__device__ __forceinline__ int bvar(const BoxDims& D, int i) { return i < D.nlb ? i : i - D.nlb; }
-__device__ __forceinline__ double bsgn(const BoxDims& D, int i) { return i < D.nlb ? -1.0 : 1.0; }
-
-// G'v of a length-m shared vector at column j (the lb row and/or the ub row of variable j)
-__device__ __forceinline__ double gt_col(const BoxDims& D, const double* v, int j) {
-    double a = 0.0;
-    if (D.nlb) a -= v[j];
-    if (D.m > D.nlb) a += v[D.nlb + j];
-    return a;
-}
-
-__device__ __forceinline__ double box_step(double v, double dv) { return (dv > 0.0) ? INFINITY : (-v / dv); }
-__device__ __forceinline__ double box_step_fix(double v) { return (isinf(v) && v > 0.0) ? 1.0 : v; }
 
 // hinv = 1 / (q + G'DG) for the local variables and the d currently in shared memory (no barrier)
 __device__ __forceinline__ void form_hinv(const BoxDims& D) {
@@ -154,40 +135,81 @@ __device__ __forceinline__ void stair_solve(const BoxDims& D, bool fresh, int dy
     pf_bwd(D.S, D.ep, D.rhs, dy);
 }
 
-// ---- the families -------------------------------------------------------------------------------------------------------
-// Each is the per-CTA context of one layout, built in the kernel from its parameter (F::Dims), and supplies:
-//   qp(), j0() (first local variable), ng() / mg() (nz and inequality rows of the whole QP), grow(i) (global
-//   inequality row of local row i), leader() (rank 0: writes the length-neq outputs, iters, best_resid, the trace and
-//   spd_flag), a(i, j) (A at local column j), reduce_sum / reduce_min, any (the SPD test), stage, form (H^-1 and M),
-//   ry_step (ry = A x - b, |ry|^2 into acc, and the reduction of acc), solve_mid (rhs = ry - A H^-1 r, factor or forward
-//   sweep, pf_diag, backward sweep to dy) and sync() (the closing cluster barrier).
+// ---- the structured solve of OneCta and Cluster -----------------------------------------------------------------------
+// The structured KKT solve with the H / M of the last form:
+//   K [dx ds dz dy] = -[rx rs rz ry];  rs, rz, ry may be -1 (zero). fresh: M was just formed and is factored here
+// (with the right-hand side carried along), else the existing factor is reused. Ends with a block barrier.
+template <class F>
+__device__ __noinline__ void box_solve(F& f, bool fresh, int rx, int rs, int rz, int ry, int dx, int ds, int dz, int dy) {
+    QPB_SMEM;
+    const BoxDims& D = f.D;
+    const int tid = threadIdx.x;
+    const int n = D.n, m = D.m, e = D.e;
+    // r = rx + G'(D rz - rs), kept as H^-1 r in D.r
+    for (int j = tid; j < n; j += kBoxNT) {
+        double a = qsm[rx + j];
+        if (D.nlb) {
+            const double t = ((rz >= 0) ? qsm[D.d + j] * qsm[rz + j] : 0.0) - ((rs >= 0) ? qsm[rs + j] : 0.0);
+            a -= t;
+        }
+        if (m > D.nlb) {
+            const int i = D.nlb + j;
+            const double t = ((rz >= 0) ? qsm[D.d + i] * qsm[rz + i] : 0.0) - ((rs >= 0) ? qsm[rs + i] : 0.0);
+            a += t;
+        }
+        qsm[D.r + j] = a * qsm[D.hinv + j];
+    }
+    __syncthreads();
+    if (e > 0) f.solve_mid(fresh, ry, dy);
+    // dx = -H^-1 r - H^-1 A'dy
+    for (int j = tid; j < n; j += kBoxNT) {
+        double a = 0.0;
+        for (int i = 0; i < e; ++i) a = fma(f.a(i, j), qsm[dy + i], a);
+        qsm[dx + j] = -qsm[D.r + j] - a * qsm[D.hinv + j];
+    }
+    __syncthreads();
+    for (int i = tid; i < m; i += kBoxNT) {
+        const double di = qsm[D.d + i];
+        const double rsi = (rs >= 0) ? qsm[rs + i] : 0.0;
+        const double dzi = di * (bsgn(D, i) * qsm[dx + bvar(D, i)] + ((rz >= 0) ? qsm[rz + i] : 0.0)) - rsi;
+        qsm[dz + i] = dzi;
+        qsm[ds + i] = (-rsi - dzi) / di;
+    }
+    __syncthreads();
+}
+
+// ---- the families (qp_box_loop.cuh lists what each supplies) -----------------------------------------------------------
+
+// 1 where a q_j of this CTA's variables is not positive (no barrier)
+__device__ __forceinline__ int q_bad(const BoxDims& D) {
+    QPB_SMEM;
+    int bad = 0;
+    for (int j = threadIdx.x; j < D.n; j += kBoxNT) bad |= !(qsm[D.q + j] > 0.0);
+    return bad;
+}
 
 // One CTA per QP; j0 = 0 and leader() (rank 0) are compile-time facts.
-struct OneCta {
-    using Dims = BoxDims;
+struct OneCta : BoxCta<BoxDims> {
     static constexpr int kMinFwd = 3, kMinBwd = 4, kMinKkt = 0;     // CTAs per SM (0: no bound)
-    BoxDims D;
 
-    __device__ explicit OneCta(const BoxDims& P) : D(P) {}
-    __device__ static int qp() { return blockIdx.x; }
-    __host__ __device__ static constexpr int j0() { return 0; }
-    __device__ int ng() const { return D.n; }
-    __device__ int mg() const { return D.m; }
-    __device__ static int64_t grow(int i) { return i; }
-    __host__ __device__ static constexpr bool leader() { return true; }
-    __device__ double a(int i, int j) const { QPB_SMEM; return qsm[D.A + i * D.lda + j]; }
-    template <int N> __device__ void reduce_sum(double (&v)[N]) {
-        QPB_SMEM;
-        qpb::block_reduce<N, false>(v, qsm + D.red, threadIdx.x, kBoxNT);
+    __device__ explicit OneCta(const BoxDims& P) : BoxCta(P) {}
+    __device__ int spd_bad() const { return __syncthreads_or(q_bad(D)); }
+    template <class G> __device__ static void before_residuals(G) {}
+    __device__ double qx_p(int j) const { QPB_SMEM; return fma(qsm[D.q + j], qsm[D.x + j], qsm[D.p + j]); }
+    template <class G> __device__ void before_affine(G form_d) const {
+        form_d();
+        form();
     }
-    template <int N> __device__ void reduce_min(double (&v)[N]) {
-        QPB_SMEM;
-        qpb::block_reduce<N, true>(v, qsm + D.red, threadIdx.x, kBoxNT);
+    __device__ void solve(bool fresh, int rx, int rs, int rz, int ry, int dx, int ds, int dz, int dy) {
+        box_solve(*this, fresh, rx, rs, rz, ry, dx, ds, dz, dy);
     }
-    __device__ static int any(int v) { return __syncthreads_or(v); }
-    __device__ static void sync() {}
+    // dq = dx o z
+    __device__ void write_dq(double* dq, int qp, const double* __restrict__ zhat) const {
+        QPB_SMEM;
+        for (int j = threadIdx.x; j < D.n; j += kBoxNT) dq[(int64_t)qp * D.n + j] = qsm[D.dx + j] * zhat[(int64_t)qp * D.n + j];
+    }
 
-    // q, A, b (nullptr in the backward and KKT kernels) of this QP; the staircase tile table
+    // q, A, b of this QP; the staircase tile table
     __device__ void stage(const double* q, const double* A, const double* b) const {
         QPB_SMEM;
         const int tid = threadIdx.x;
@@ -216,21 +238,6 @@ struct OneCta {
             qsm[D.S + pf_rowoff(r) + c] = v;
         }
         __syncthreads();
-    }
-
-    // ry = A x - b, one warp per row; |ry|^2 per warp before the block reduction
-    __device__ void ry_step(double (&acc)[4]) {
-        QPB_SMEM;
-        const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-        for (int i = warp; i < D.ep; i += kClW) {
-            double a = 0.0;
-            if (i < D.e)
-                for (int k = lane; k < D.n; k += 32) a = fma(qsm[D.A + i * D.lda + k], qsm[D.x + k], a);
-            a = qpb::warp_sum(a);
-            const double r = (i < D.e) ? a - qsm[D.b + i] : 0.0;
-            if (lane == 0) { qsm[D.ry + i] = r; acc[0] = fma(r, r, acc[0]); }
-        }
-        reduce_sum(acc);
     }
 
     __device__ void solve_mid(bool fresh, int ry, int dy) {
@@ -361,14 +368,30 @@ struct Cluster {
     __device__ static bool leader() { return rank() == 0; }
     template <int N> __device__ void reduce_sum(double (&v)[N]) { cl_reduce<N, false>(X, v, ph, 0, 0); }
     template <int N> __device__ void reduce_min(double (&v)[N]) { cl_reduce<N, true>(X, v, ph, 0, 0); }
-    __device__ int any(int bad) {
-        double v[1] = {bad ? 1.0 : 0.0};
+    __device__ int spd_bad() {
+        double v[1] = {q_bad(D) ? 1.0 : 0.0};
         reduce_sum(v);
         return v[0] > 0.0;
     }
     // no CTA exits while another may still read its shared memory
     __device__ static void sync() { cg::this_cluster().sync(); }
     __device__ double a(int i, int j) const { QPB_SMEM; return qsm[D.A + i * D.lda + j]; }
+    template <class G> __device__ static void before_residuals(G) {}
+    __device__ double qx_p(int j) const { QPB_SMEM; return fma(qsm[D.q + j], qsm[D.x + j], qsm[D.p + j]); }
+    template <class G> __device__ void before_affine(G form_d) const {
+        form_d();
+        form();
+    }
+    __device__ void solve(bool fresh, int rx, int rs, int rz, int ry, int dx, int ds, int dz, int dy) {
+        box_solve(*this, fresh, rx, rs, rz, ry, dx, ds, dz, dy);
+    }
+    __device__ void write_dq(double* dq, int qp, const double* __restrict__ zhat) const {
+        QPB_SMEM;
+        for (int j = threadIdx.x; j < D.n; j += kBoxNT) {
+            const int64_t g = (int64_t)qp * X.ng + j0() + j;
+            dq[g] = qsm[D.dx + j] * zhat[g];
+        }
+    }
 
     // q and this CTA's columns of A; b replicated (forward only); the staircase tile table
     __device__ void stage(const double* q, const double* A, const double* b) const {
@@ -454,302 +477,6 @@ struct Cluster {
         stair_solve(D, fresh, dy);
     }
 };
-
-// ---- the solver, written once over the families ------------------------------------------------------------------------
-// The structured KKT solve with the H / M of the last form:
-//   K [dx ds dz dy] = -[rx rs rz ry];  rs, rz, ry may be -1 (zero). fresh: M was just formed and is factored here
-// (with the right-hand side carried along), else the existing factor is reused. Ends with a block barrier.
-template <class F>
-__device__ __noinline__ void box_solve(F& f, bool fresh, int rx, int rs, int rz, int ry, int dx, int ds, int dz, int dy) {
-    QPB_SMEM;
-    const BoxDims& D = f.D;
-    const int tid = threadIdx.x;
-    const int n = D.n, m = D.m, e = D.e;
-    // r = rx + G'(D rz - rs), kept as H^-1 r in D.r
-    for (int j = tid; j < n; j += kBoxNT) {
-        double a = qsm[rx + j];
-        if (D.nlb) {
-            const double t = ((rz >= 0) ? qsm[D.d + j] * qsm[rz + j] : 0.0) - ((rs >= 0) ? qsm[rs + j] : 0.0);
-            a -= t;
-        }
-        if (m > D.nlb) {
-            const int i = D.nlb + j;
-            const double t = ((rz >= 0) ? qsm[D.d + i] * qsm[rz + i] : 0.0) - ((rs >= 0) ? qsm[rs + i] : 0.0);
-            a += t;
-        }
-        qsm[D.r + j] = a * qsm[D.hinv + j];
-    }
-    __syncthreads();
-    if (e > 0) f.solve_mid(fresh, ry, dy);
-    // dx = -H^-1 r - H^-1 A'dy
-    for (int j = tid; j < n; j += kBoxNT) {
-        double a = 0.0;
-        for (int i = 0; i < e; ++i) a = fma(f.a(i, j), qsm[dy + i], a);
-        qsm[dx + j] = -qsm[D.r + j] - a * qsm[D.hinv + j];
-    }
-    __syncthreads();
-    for (int i = tid; i < m; i += kBoxNT) {
-        const double di = qsm[D.d + i];
-        const double rsi = (rs >= 0) ? qsm[rs + i] : 0.0;
-        const double dzi = di * (bsgn(D, i) * qsm[dx + bvar(D, i)] + ((rz >= 0) ? qsm[rz + i] : 0.0)) - rsi;
-        qsm[dz + i] = dzi;
-        qsm[ds + i] = (-rsi - dzi) / di;
-    }
-    __syncthreads();
-}
-
-// forward (batch.py:47-207) with the structured solve; the loop of k_forward_fast (qp_solve.cuh). Every CTA writes its
-// slice of zhat, lam and slacks; the leader nus, iters, best_resid, the trace rows and spd_flag. One CTA per QP: three
-// CTAs per SM (at most 168 registers; about 48 KB of shared memory per QP at nz = 64, neq = 40): four (128 registers)
-// spill.
-//
-// INVARIANT (Cluster, and the k_box_*_dm kernels, which repeat this loop): every CTA of a cluster executes the same
-// sequence of cluster.sync() calls. Every reduction leaves bit-identical sums and minima in every CTA, and so does every
-// solve (M is summed in rank order and factored redundantly, or dy is gathered from its owners), so y, mu, the residual
-// and the step lengths are bit-identical too. Every branch that reaches a cluster barrier (the exit tests, NaN and mu > 1e32 exits, best-iterate
-// tracking, notImprovedLim, e > 0, fresh) is decided from those values or from kernel arguments only; a CTA that branched
-// on a value of its own would deadlock its cluster.
-template <class F>
-__global__ void __launch_bounds__(kBoxNT, F::kMinFwd)
-k_box_forward(typename F::Dims P, const double* __restrict__ q, int64_t sq, const double* __restrict__ p, int64_t sp,
-              const double* __restrict__ A, int64_t sA, const double* __restrict__ b, int64_t sb,
-              const double* __restrict__ lb, int64_t slb, const double* __restrict__ ub, int64_t sub, double eps,
-              double stall_tol, double best_tie, int notImprovedLim, int maxIter, double* __restrict__ zhat,
-              double* __restrict__ lam, double* __restrict__ slacks, double* __restrict__ nus, int* __restrict__ iters_out,
-              double* __restrict__ resid_out, double* __restrict__ trace, int* __restrict__ spd_flag) {
-    QPB_SMEM;
-    F f(P);
-    const BoxDims& D = f.D;
-    const int tid = threadIdx.x, qp = f.qp(), j0 = f.j0();
-    const int n = D.n, m = D.m, e = D.e, ep = D.ep;
-    f.stage(q + (int64_t)qp * sq, A + (int64_t)qp * sA, (e > 0) ? b + (int64_t)qp * sb : nullptr);
-    {
-        int bad = 0;
-        for (int j = tid; j < n; j += kBoxNT) {
-            qsm[D.p + j] = p[(int64_t)qp * sp + j0 + j];
-            bad |= !(qsm[D.q + j] > 0.0);
-        }
-        bad = f.any(bad);
-        if (f.leader() && tid == 0 && spd_flag != nullptr) spd_flag[qp] = bad;
-    }
-    for (int i = tid; i < m; i += kBoxNT) {
-        qsm[D.h + i] = (i < D.nlb) ? -lb[(int64_t)qp * slb + j0 + i] : ub[(int64_t)qp * sub + j0 + i - D.nlb];
-        qsm[D.d + i] = 1.0;
-        qsm[D.rz + i] = -qsm[D.h + i];
-    }
-    for (int i = tid; i < ep; i += kBoxNT) { qsm[D.ry + i] = -qsm[D.b + i]; qsm[D.y + i] = 0.0; }
-    __syncthreads();
-
-    // ---- initial point: solve_kkt(p, 0, -h, -b) with d = 1   (batch.py:61-67)
-    f.form();
-    box_solve(f, true, D.p, -1, D.rz, D.ry, D.x, D.s, D.z, D.y);
-    {
-        double mn[2] = {INFINITY, INFINITY};
-        for (int i = tid; i < m; i += kBoxNT) { mn[0] = fmin(mn[0], qsm[D.s + i]); mn[1] = fmin(mn[1], qsm[D.z + i]); }
-        f.reduce_min(mn);
-        for (int i = tid; i < m; i += kBoxNT) {                  // slacks and duals >= 1 (batch.py:77-87)
-            if (mn[0] < 0.0) qsm[D.s + i] -= mn[0] - 1.0;
-            if (mn[1] < 0.0) qsm[D.z + i] -= mn[1] - 1.0;
-        }
-        __syncthreads();
-    }
-
-    double best = 0.0;
-    int nNot = 0, iters_run = 0;
-    const double dm = (double)f.mg();
-    for (int it = 0; it < maxIter; ++it) {
-        iters_run = it + 1;
-        // ---- residuals (batch.py:94-107)
-        double acc[4] = {0.0, 0.0, 0.0, 0.0};                   // |ry|^2, |rz|^2, |rx|^2, s.z
-        for (int j = tid; j < n; j += kBoxNT) {
-            double a = 0.0;
-            for (int i = 0; i < e; ++i) a = fma(f.a(i, j), qsm[D.y + i], a);
-            const double r = fma(qsm[D.q + j], qsm[D.x + j], qsm[D.p + j]) + gt_col(D, qsm + D.z, j) + a;
-            qsm[D.rx + j] = r;
-            acc[2] = fma(r, r, acc[2]);
-        }
-        for (int i = tid; i < m; i += kBoxNT) {
-            const double r = bsgn(D, i) * qsm[D.x + bvar(D, i)] + qsm[D.s + i] - qsm[D.h + i];
-            qsm[D.rz + i] = r;
-            acc[1] = fma(r, r, acc[1]);
-            acc[3] = fma(qsm[D.s + i], qsm[D.z + i], acc[3]);
-        }
-        f.ry_step(acc);
-        const double mu = fabs(acc[3] / dm);
-        const double resid = sqrt(acc[1]) + sqrt(acc[0]) + sqrt(acc[2]) + dm * mu;
-        if (trace != nullptr && f.leader() && tid == 0) {       // what verbose=1 prints (batch.py:115-117)
-            double* tr = trace + ((int64_t)qp * maxIter + it) * 4;
-            tr[0] = sqrt(acc[1]) + sqrt(acc[0]); tr[1] = sqrt(acc[2]); tr[2] = mu; tr[3] = resid;
-        }
-        // ---- best-iterate tracking and exit tests (batch.py:118-143), per QP: cluster-wide values only
-        const bool improved = (it == 0) || (resid < best);
-        if (improved) { best = resid; nNot = 0; } else { ++nNot; }
-        if (improved || resid < best_tie * best) {
-            for (int j = tid; j < n; j += kBoxNT) qsm[D.bx + j] = qsm[D.x + j];
-            for (int i = tid; i < m; i += kBoxNT) { qsm[D.bs + i] = qsm[D.s + i]; qsm[D.bz + i] = qsm[D.z + i]; }
-            for (int i = tid; i < e; i += kBoxNT) qsm[D.by + i] = qsm[D.y + i];
-        }
-        if ((nNot == notImprovedLim && best < stall_tol) || best < eps || mu > 1e32) break;
-        if (!(resid == resid) || isinf(resid)) break;
-        // ---- d = z/s, H, M; the affine direction (batch.py:109-113,150) factors M
-        for (int i = tid; i < m; i += kBoxNT) qsm[D.d + i] = qsm[D.z + i] / qsm[D.s + i];
-        __syncthreads();
-        f.form();
-        box_solve(f, true, D.rx, D.z, D.rz, D.ry, D.dxa, D.dsa, D.dza, D.dya);
-        // ---- affine step length and sigma (batch.py:160-168)
-        double mn[2] = {INFINITY, INFINITY};
-        for (int i = tid; i < m; i += kBoxNT) {
-            mn[0] = fmin(mn[0], box_step(qsm[D.z + i], qsm[D.dza + i]));
-            mn[1] = fmin(mn[1], box_step(qsm[D.s + i], qsm[D.dsa + i]));
-        }
-        f.reduce_min(mn);
-        {
-            const double alpha = fmin(fmin(box_step_fix(mn[0]), box_step_fix(mn[1])), 1.0);
-            double sm[2] = {0.0, 0.0};
-            for (int i = tid; i < m; i += kBoxNT) {
-                sm[0] = fma(qsm[D.s + i] + alpha * qsm[D.dsa + i], qsm[D.z + i] + alpha * qsm[D.dza + i], sm[0]);
-                sm[1] = fma(qsm[D.s + i], qsm[D.z + i], sm[1]);
-            }
-            f.reduce_sum(sm);
-            const double sr = sm[0] / sm[1];
-            const double sig = sr * sr * sr;
-            // ---- corrector right-hand side (batch.py:170-181): rs = (-mu sig + dsa dza) / s, rx = rz = ry = 0
-            for (int i = tid; i < m; i += kBoxNT)
-                qsm[D.rsc + i] = (-mu * sig + qsm[D.dsa + i] * qsm[D.dza + i]) / qsm[D.s + i];
-            for (int j = tid; j < n; j += kBoxNT) qsm[D.rx + j] = 0.0;
-            __syncthreads();
-        }
-        box_solve(f, false, D.rx, D.rsc, -1, -1, D.dx, D.ds, D.dz, D.dy);
-        // ---- combined direction, step length, update (batch.py:185-203)
-        mn[0] = INFINITY; mn[1] = INFINITY;
-        for (int i = tid; i < m; i += kBoxNT) {
-            const double dzi = qsm[D.dza + i] + qsm[D.dz + i], dsi = qsm[D.dsa + i] + qsm[D.ds + i];
-            qsm[D.dz + i] = dzi;
-            qsm[D.ds + i] = dsi;
-            mn[0] = fmin(mn[0], box_step(qsm[D.z + i], dzi));
-            mn[1] = fmin(mn[1], box_step(qsm[D.s + i], dsi));
-        }
-        f.reduce_min(mn);
-        const double alpha = fmin(0.999 * fmin(box_step_fix(mn[0]), box_step_fix(mn[1])), 1.0);
-        for (int j = tid; j < n; j += kBoxNT) qsm[D.x + j] = fma(alpha, qsm[D.dxa + j] + qsm[D.dx + j], qsm[D.x + j]);
-        for (int i = tid; i < m; i += kBoxNT) {
-            qsm[D.s + i] = fma(alpha, qsm[D.ds + i], qsm[D.s + i]);
-            qsm[D.z + i] = fma(alpha, qsm[D.dz + i], qsm[D.z + i]);
-        }
-        for (int i = tid; i < e; i += kBoxNT) qsm[D.y + i] = fma(alpha, qsm[D.dya + i] + qsm[D.dy + i], qsm[D.y + i]);
-        __syncthreads();
-    }
-    __syncthreads();
-    for (int j = tid; j < n; j += kBoxNT) zhat[(int64_t)qp * f.ng() + j0 + j] = qsm[D.bx + j];
-    for (int i = tid; i < m; i += kBoxNT) {
-        const int64_t g = (int64_t)qp * f.mg() + f.grow(i);
-        lam[g] = qsm[D.bz + i];
-        slacks[g] = qsm[D.bs + i];
-    }
-    if (f.leader()) {
-        if (nus != nullptr)
-            for (int i = tid; i < e; i += kBoxNT) nus[(int64_t)qp * e + i] = qsm[D.by + i];
-        if (tid == 0) { iters_out[qp] = iters_run; resid_out[qp] = best; }
-    }
-    f.sync();
-}
-
-// QPFunctionFn.backward (qp.py:128-182) for the box QP: d from the clamped duals (qp.py:148), one factor of M and one
-// solve per QP, then dq = dx o z, dp = dx, dlb = dlam_lb, dub = -dlam_ub, dA = dnu z' + nu dx', db = -dnu. dxv, dlamv
-// and dnuv always receive dx, dlam, dnu (the batch means read them); a gradient whose mean flag is set is skipped here.
-// Every CTA writes its slice of dx, dlam, dq, dp, dlb, dub and its columns of dA; the leader dnu and db. dl_dlam and dl_dnu
-// (NULL: zero) are the adjoints of the returned duals: they are the rz and ry of the solve, which rz / ry are not otherwise.
-struct BoxGrads {
-    double *dq, *dp, *dlb, *dub, *dA, *db;
-    int mq, mp, mlb, mub, mA, mb;
-};
-
-template <class F>
-__global__ void __launch_bounds__(kBoxNT, F::kMinBwd)
-k_box_backward(typename F::Dims P, const double* __restrict__ q, int64_t sq, const double* __restrict__ A, int64_t sA,
-               const double* __restrict__ dl, const double* __restrict__ dl_dlam, const double* __restrict__ dl_dnu,
-               const double* __restrict__ zhat, const double* __restrict__ lam,
-               const double* __restrict__ slacks, const double* __restrict__ nus, BoxGrads O,
-               double* __restrict__ dxv, double* __restrict__ dlamv, double* __restrict__ dnuv) {
-    QPB_SMEM;
-    F f(P);
-    const BoxDims& D = f.D;
-    const int tid = threadIdx.x, qp = f.qp(), j0 = f.j0();
-    const int n = D.n, m = D.m, e = D.e, N = f.ng();
-    f.stage(q + (int64_t)qp * sq, A + (int64_t)qp * sA, nullptr);
-    for (int j = tid; j < n; j += kBoxNT) qsm[D.rx + j] = dl[(int64_t)qp * N + j0 + j];
-    for (int i = tid; i < m; i += kBoxNT) {
-        const int64_t g = (int64_t)qp * f.mg() + f.grow(i);
-        qsm[D.d + i] = fmax(lam[g], 1e-8) / fmax(slacks[g], 1e-8);
-        if (dl_dlam != nullptr) qsm[D.rz + i] = dl_dlam[g];
-    }
-    // every CTA loads all of dl_dnu: the right-hand side of M stays bit-identical across the cluster (see k_box_forward)
-    if (dl_dnu != nullptr)
-        for (int i = tid; i < e; i += kBoxNT) qsm[D.ry + i] = dl_dnu[(int64_t)qp * e + i];
-    __syncthreads();
-    f.form();
-    box_solve(f, true, D.rx, -1, dl_dlam != nullptr ? D.rz : -1, dl_dnu != nullptr ? D.ry : -1, D.dx, D.ds, D.dz, D.dy);
-    for (int j = tid; j < n; j += kBoxNT) {
-        const int64_t g = (int64_t)qp * N + j0 + j;
-        const double dx = qsm[D.dx + j], z = zhat[g];
-        dxv[g] = dx;
-        if (O.dq && !O.mq) O.dq[g] = dx * z;
-        if (O.dp && !O.mp) O.dp[g] = dx;
-    }
-    for (int i = tid; i < m; i += kBoxNT) {
-        const double dz = qsm[D.dz + i];
-        dlamv[(int64_t)qp * f.mg() + f.grow(i)] = dz;
-        if (i < D.nlb) { if (O.dlb && !O.mlb) O.dlb[(int64_t)qp * N + j0 + i] = dz; }
-        else if (O.dub && !O.mub) O.dub[(int64_t)qp * N + j0 + i - D.nlb] = -dz;
-    }
-    if (f.leader())
-        for (int i = tid; i < e; i += kBoxNT) {
-            dnuv[(int64_t)qp * e + i] = qsm[D.dy + i];
-            if (O.db && !O.mb) O.db[(int64_t)qp * e + i] = -qsm[D.dy + i];
-        }
-    if (O.dA && !O.mA)
-        for (int t = tid; t < e * n; t += kBoxNT) {
-            const int i = t / n, j = t - i * n;
-            O.dA[((int64_t)qp * e + i) * N + j0 + j] = fma(qsm[D.dy + i], zhat[(int64_t)qp * N + j0 + j],
-                                                           nus[(int64_t)qp * e + i] * qsm[D.dx + j]);
-        }
-    f.sync();
-}
-
-// qpb200_box_solve_kkt: the structured factor and solve for caller-given d and right-hand sides (all vectors (B, len))
-template <class F>
-__global__ void __launch_bounds__(kBoxNT, F::kMinKkt)
-k_box_kkt(typename F::Dims P, const double* __restrict__ q, int64_t sq, const double* __restrict__ A, int64_t sA,
-          const double* __restrict__ d, const double* __restrict__ rx, const double* __restrict__ rs,
-          const double* __restrict__ rz, const double* __restrict__ ry, double* __restrict__ dx, double* __restrict__ ds,
-          double* __restrict__ dz, double* __restrict__ dy) {
-    QPB_SMEM;
-    F f(P);
-    const BoxDims& D = f.D;
-    const int tid = threadIdx.x, qp = f.qp(), j0 = f.j0();
-    const int n = D.n, m = D.m, e = D.e, N = f.ng();
-    f.stage(q + (int64_t)qp * sq, A + (int64_t)qp * sA, nullptr);
-    for (int j = tid; j < n; j += kBoxNT) qsm[D.rx + j] = rx[(int64_t)qp * N + j0 + j];
-    for (int i = tid; i < m; i += kBoxNT) {
-        const int64_t g = (int64_t)qp * f.mg() + f.grow(i);
-        qsm[D.d + i] = d[g];
-        qsm[D.rsc + i] = rs[g];
-        qsm[D.rz + i] = rz[g];
-    }
-    for (int i = tid; i < e; i += kBoxNT) qsm[D.ry + i] = ry[(int64_t)qp * e + i];
-    __syncthreads();
-    f.form();
-    box_solve(f, true, D.rx, D.rsc, D.rz, D.ry, D.dx, D.ds, D.dz, D.dy);
-    for (int j = tid; j < n; j += kBoxNT) dx[(int64_t)qp * N + j0 + j] = qsm[D.dx + j];
-    for (int i = tid; i < m; i += kBoxNT) {
-        const int64_t g = (int64_t)qp * f.mg() + f.grow(i);
-        ds[g] = qsm[D.ds + i];
-        dz[g] = qsm[D.dz + i];
-    }
-    if (dy != nullptr && f.leader())
-        for (int i = tid; i < e; i += kBoxNT) dy[(int64_t)qp * e + i] = qsm[D.dy + i];
-    f.sync();
-}
 
 // ---- distributed-M kernels: neq_pad > 128 on a cluster ---------------------------------------------------------------
 // Past neq_pad = 128 a full copy of M per CTA no longer fits (the staircase of order 256 alone is 272 KB). These kernels
@@ -1449,12 +1176,6 @@ k_box_jvp_rhs(int n, int e, int nlb, int m, const double* __restrict__ dq, int64
         if (m > nlb) rz[qp * m + nlb + i] = dub ? -dub[qp * sdub + i] : 0.0;
     }
     for (int i = tid; i < e; i += kJvpNT) ry[qp * e + i] = ay[i];
-}
-
-int box_check_launch(const char* what) {
-    cudaError_t err = cudaGetLastError();
-    if (err != cudaSuccess) { qpb200_internal_cuda_error((int)err, what); return QPB200_ERR_CUDA; }
-    return QPB200_OK;
 }
 
 int box_plan_check(const qpb200_box_plan* P) {
