@@ -127,6 +127,8 @@ int qpb200_plan_kernels(const qpb200_plan* plan, int64_t out[QPB200_ENTRY_COUNT]
 
 /* pre_factor_kkt (batch.py:375-429) + the SPD check of qp.py:81-85.
  * nsys systems (1 if Q, G, A are all shared, else nBatch); sQ/sG/sA strides as above.
+ * Only the lower triangle of Q is read: its strictly upper triangle may hold anything, NaN included, and the factors
+ * are those of the symmetric matrix tril(Q) + tril(Q, -1)^T. The same holds for qpb200_pre_factor_kkt_reg.
  * Writes Lfac (nsys*L_elems), Wfac (nsys*W_elems), Kfac (nsys*K_elems) and
  * spd_flag[nsys] (0 = SPD, 1 = a pivot of chol(Q) was not positive). */
 int qpb200_pre_factor_kkt(const qpb200_plan* plan, int nsys,
@@ -204,7 +206,9 @@ int qpb200_solve_kkt(const qpb200_plan* plan, int nbatch,
  * Here the regularised solve is the SAME pair of kernels with reg_eps threaded through: chol(Q + eps I); reduced matrix
  * W W^T + diag(eps on equality rows, 1/(d + eps) + eps on inequality rows), which is SPD whatever the rank of A. One
  * pre_factor_kkt_reg serves every refinement step (the reference refactors each time). reg_eps = 0 is the plain call.
- * The refinement loop itself (residual + correction) is host-side glue: qpth_b200/kkt.py. */
+ * The refinement loop itself (residual + correction) is host-side glue: qpth_b200/kkt.py.
+ * Only the lower triangle of Q is read, as by qpb200_pre_factor_kkt: the factors are those of tril(Q) + tril(Q, -1)^T
+ * (+ eps I), so a refinement residual must be formed with that symmetric matrix. */
 int qpb200_pre_factor_kkt_reg(const qpb200_plan* plan, int nsys,
                               const double* Q, int64_t sQ, const double* G, int64_t sG,
                               const double* A, int64_t sA, double reg_eps,
@@ -419,7 +423,9 @@ int qpb200_dfma_probe(int blocks, int threads, int iters, double* out, void* str
 
 /* Whole path on HOST buffers (pageable or pinned): H2D, pre_factor_kkt, forward,
  * backward, D2H, on `device`; synchronises before returning.  All six inputs
- * batched (nbatch leading dimension); gradients may be NULL to skip backward. */
+ * batched (nbatch leading dimension); gradients may be NULL to skip backward.
+ * Only the lower triangle of each Q is read: the result is that of tril(Q) + tril(Q, -1)^T, whatever the
+ * strictly upper triangle holds, NaN included. */
 int qpb200_qp_host(int device, int nbatch, int nz, int nineq, int neq,
                    const double* Q_host, const double* p_host, const double* G_host,
                    const double* h_host, const double* A_host, const double* b_host,
@@ -441,7 +447,9 @@ int qpb200_optnet_chain(int nz, int nineq, const double* L, const double* G, con
 /* Transfer helper for SYMMETRIC (nbatch, n, n) matrices - Q on its way in, dQ on its way out (qp.py:157-158 builds dQ
  * as 1/2 (dx z^T + z dx^T)): only the lower triangle crosses PCIe, as `band`-row strips (strip b = rows [b band, (b+1)
  * band) x columns [0, (b+1) band)), one strided 3-D copy per strip on `stream`. The part of the destination above the
- * strips is left untouched. direction 0: host -> device, 1: device -> host. The host buffer should be pinned. */
+ * strips is left untouched. direction 0: host -> device, 1: device -> host. The host buffer should be pinned. Every
+ * entry point that takes a dense Q reads only its lower triangle, so such a device buffer can be passed as Q whatever
+ * its upper part holds. */
 int qpb200_copy_lower(const double* src, double* dst, int nbatch, int n, int band, int direction, void* stream);
 
 #ifdef __cplusplus

@@ -285,7 +285,9 @@ def BoxQPFunction(eps=1e-12, verbose=0, notImprovedLim=3, maxIter=20, check_Q_sp
     to its dense equivalent, dQ = diag(dq), dh = [-dlb; dub]).
 
     dense_Q=True: the first argument is a dense Q, (nBatch, nz, nz) or (nz, nz) (a 2-D Q is un-batched), of which only
-    the lower triangle is read, as in QPFunction's kernels. Everything else is as above, with QPFunction's semantics on
+    the lower triangle is read, as in QPFunction's kernels (the dense fallback too): the strictly upper triangle may hold
+    anything, NaN included, and the result is that of the symmetric matrix tril(Q) + tril(Q, -1)^T. A tangent dQ is
+    read in full and enters as sym(dQ). Everything else is as above, with QPFunction's semantics on
     the dense equivalent (Q, G = [-I; I], h = [-lb; ub]): 'Q is not SPD.' where chol(Q) breaks down, the gradient
     dQ = 1/2 (dx z' + z dx') (the batch mean for an un-batched Q), and the tangent dQ enters forward mode as
     sym(dQ) z. Shapes past the dense-Q kernels (qpb200_boxq_plan.ok) run the dense kernels on the dense equivalent."""

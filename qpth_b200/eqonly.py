@@ -23,7 +23,8 @@ EQ_IR_STEPS = 2
 
 def _solve(F, Q, A, d, rx, rs, rz, ry, steps):
     """F.solve, then `steps` refinement steps against the true system [Q 0 0 A'; 0 d 1 0; 0 1 0 0; A 0 0 0] (the dummy
-    inequality row has G = 0): K~ dd = -(K [dx ds dz dy] + r), one factorization for all of them."""
+    inequality row has G = 0): K~ dd = -(K [dx ds dz dy] + r), one factorization for all of them. Q must be the symmetric
+    matrix the factor saw (the mirrored lower triangle of the caller's Q)."""
     dx, ds, dz, dy = F.solve(d, rx, rs, rz, ry)
     for _ in range(steps):
         resx = torch.bmm(Q, dx.unsqueeze(2)).squeeze(2) + torch.bmm(A.transpose(1, 2), dy.unsqueeze(2)).squeeze(2) + rx
@@ -60,9 +61,12 @@ class QPEqualityFn(Function):
             raise RuntimeError('Q is not positive semidefinite.' if reg else 'Q is not SPD.')
         one, zero = torch.ones(nBatch, 1, **f64), torch.zeros(nBatch, 1, **f64)
         steps = EQ_IR_STEPS if reg else 0
-        zhat, _, _, nus = _solve(F, Q, A, one, p, zero, -one, -b, steps)   # K [x s z y] = -[p 0 -h -b]
+        # the factor sees only the lower triangle of Q: refine against that matrix, tril(Q) + tril(Q, -1)', so that the
+        # strictly upper triangle is never read here either
+        Qr = (torch.tril(Q) + torch.tril(Q, -1).transpose(1, 2)) if steps else Q
+        zhat, _, _, nus = _solve(F, Qr, A, one, p, zero, -one, -b, steps)   # K [x s z y] = -[p 0 -h -b]
         ctx.F, ctx.flags, ctx.one, ctx.zero = F, flags, one, zero
-        ctx.QA, ctx.steps = (Q, A), steps
+        ctx.QA, ctx.steps = (Qr, A), steps
         ctx.zhat64, ctx.nus = zhat, nus
         ctx.meta = [(X.device, X.dtype) for X in (Q_, p_, A_, b_)]
         ctx.duals = duals

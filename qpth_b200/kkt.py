@@ -8,7 +8,11 @@ the correction loop are a handful of batched mat-vecs in torch on the device: gl
 
 All tensors fp64 on one CUDA device, batched: Q (B,nz,nz), D (B,nineq,nineq) diagonal (or its diagonal (B,nineq)),
 G (B,nineq,nz), A (B,neq,nz) or None / empty, rx (B,nz), rs, rz (B,nineq), ry (B,neq) or None.
-Returns (dx, ds, dz, dy) with dy None when neq == 0, like the reference."""
+Returns (dx, ds, dz, dy) with dy None when neq == 0, like the reference.
+
+These helpers keep the reference's signature and take a SYMMETRIC Q: the kernels read only its lower triangle, while the
+residual of kkt_resid_reg (and so the refinement of solve_kkt_ir) multiplies by the whole of Q. QPFunction and the
+equality-only path never call them with anything else."""
 import ctypes
 
 import torch

@@ -9,7 +9,11 @@ backward kernel reduces the per-sample gradients of the shared Q, G, h to their 
 no (B, nz, nz) tensor ever exists) and one launch maps them onto the parameters (`qpb200_optnet_chain`): dL, dG, dz0,
 ds0. The notebook's version runs ~8 torch kernels with (nz, nz) temporaries before and after every QPFunction call and
 materialises nothing different; results are identical to composing the same formulas with torch autograd around
-`qpth_b200.QPFunction` (tests/test_gpu_layers.py)."""
+`qpth_b200.QPFunction` (tests/test_gpu_layers.py).
+
+Only the lower triangle of L is read: its strictly upper triangle may hold anything, NaN included, the results are those
+of tril(L), and the gradient dL is exactly zero above the diagonal. The Q built from it reaches the QP kernels, which
+read only its lower triangle."""
 import ctypes
 
 import torch

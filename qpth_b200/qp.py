@@ -382,7 +382,12 @@ def QPFunction(eps=1e-12, verbose=0, notImprovedLim=3, maxIter=20, solver=QPSolv
     nineq >= 1: up to ms_pad = 8 ceil(neq / 8) + nineq rounded up to 8 of about 200 on the product-form kernels, beyond
     that on the generic global-scratch kernels. With linearly dependent equality rows the equality duals, and so the
     gradients dA and db, are not unique; z*, the inequality duals, the slacks and dQ, dp, dG, dh are. An unbounded or
-    infeasible problem gives the inaccurate-solution banner, as in the default mode."""
+    infeasible problem gives the inaccurate-solution banner, as in the default mode.
+
+    Only the lower triangle of Q is read, by every kernel and host path behind this function (the equality-only path
+    included): the strictly upper triangle may hold anything, NaN included, and the result - z*, the duals, the SPD
+    check, every gradient - is that of the symmetric matrix tril(Q) + tril(Q, -1)^T. A forward-mode tangent dQ is read
+    in full and enters as sym(dQ) = (dQ + dQ^T) / 2 (tests/test_gpu_q_lower_triangle.py)."""
     check_kkt_solver(kkt_solver)
     if solver == QPSolvers.CVXPY:
         # qp.py:97-120,142-143: per-sample CVXPY solve on the CPU, then pre_factor_kkt + the same backward.

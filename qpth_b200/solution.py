@@ -104,7 +104,11 @@ def QPSolutionFunction(check_Q_spd=True, kkt_solver=KKTSolvers.LU_PARTIAL, duals
 
     kkt_solver: KKTSolvers.LU_PARTIAL (the default) needs Q positive definite. KKTSolvers.IR_UNOPT differentiates with
     the regularised KKT solve of QPFunction(kkt_solver=IR_UNOPT), so an LP (Q = 0) or a low-rank Q solved by any solver
-    can be differentiated; check_Q_spd then checks that Q is positive semidefinite."""
+    can be differentiated; check_Q_spd then checks that Q is positive semidefinite.
+
+    Only the lower triangle of Q is read: its strictly upper triangle may hold anything, NaN included, and the gradients
+    and tangents are those of the symmetric matrix tril(Q) + tril(Q, -1)^T. A tangent dQ is read in full and enters as
+    sym(dQ) = (dQ + dQ^T) / 2."""
     check_kkt_solver(kkt_solver)
 
     class QPSolutionFn(Function):

@@ -121,3 +121,14 @@ def family_trajectory_jobs():
                             ("trajectory_on_gpu", dict(fam=fam, shape=s, B=TRAJ_B, unbatched=u, maxIter=it, eps=eps)),
                             {}, None))
     return out
+
+
+def lower_triangle_job_name(fam, shape):
+    return "lower_%s_%dx%dx%d" % ((fam,) + tuple(shape))
+
+
+def lower_triangle_jobs():
+    """tests/test_gpu_q_lower_triangle.py: kernel_families.lower_triangle_runs on every shape of the child families."""
+    from tests.kernel_families import cases
+    return [(lower_triangle_job_name(fam, s), "call", ("lower_triangle_runs", dict(fam=fam, shape=s)), {}, None)
+            for fam, s in cases(child=True, forward=True)]

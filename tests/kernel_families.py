@@ -299,9 +299,10 @@ def kkt_inputs(fam, shape, B, shared):
                 rs=rs.randn(B, nineq), rz=rs.randn(B, nineq), ry=rs.randn(B, neq))
 
 
-def kkt_on_gpu(fam, shape, B, shared, reg, dev="cuda:0"):
+def kkt_on_gpu(fam, shape, B, shared, reg, dev="cuda:0", Q=None, fill_L=None):
     """pre_factor_kkt[_reg] + solve_kkt[_reg] through the C ABI with the family's plan: batched systems (sF = 1) or one
-    system for the whole batch (nsys = 1, sF = 0). Returns dx, ds, dz, dy (B rows each) and the SPD flags."""
+    system for the whole batch (nsys = 1, sF = 0). Returns dx, ds, dz, dy (B rows each) and the SPD flags. Q: this Q
+    in place of the generator's. fill_L: the packed L buffer is filled with this value first and returned as "L"."""
     import torch
     from qpth_b200 import _lib
     lib = _lib.load()
@@ -313,8 +314,8 @@ def kkt_on_gpu(fam, shape, B, shared, reg, dev="cuda:0"):
     f64 = dict(dtype=torch.float64, device=dev)
     tt = lambda a: torch.tensor(np.ascontiguousarray(a), **f64)
     P = lambda t: ctypes.c_void_p(t.data_ptr()) if (t is not None and t.numel() > 0) else None
-    Q, G, A = tt(x["Q"]), tt(x["G"]), (tt(x["A"]) if neq else None)
-    L = torch.empty(nsys * plan.L_elems, **f64)
+    Q, G, A = tt(x["Q"] if Q is None else Q), tt(x["G"]), (tt(x["A"]) if neq else None)
+    L = torch.empty(nsys * plan.L_elems, **f64) if fill_L is None else torch.full((nsys * plan.L_elems,), fill_L, **f64)
     W = torch.empty(nsys * plan.W_elems, **f64)
     K = torch.empty(nsys * plan.K_elems, **f64)
     spd = torch.zeros(nsys, dtype=torch.int32, device=dev)
@@ -343,6 +344,8 @@ def kkt_on_gpu(fam, shape, B, shared, reg, dev="cuda:0"):
     out = dict(dx=dx.cpu().numpy(), ds=ds.cpu().numpy(), dz=dz.cpu().numpy(), spd=spd.cpu().numpy())
     if neq:
         out["dy"] = dy.cpu().numpy()
+    if fill_L is not None:
+        out["L"] = L.cpu().numpy()
     return out
 
 
@@ -435,3 +438,135 @@ def backward_on_gpu(fam, shape, B=BWD_B):
         plan = family_plan(fam, shape)
         got = solution_backward(pr, {k: True for k in "QpGhAb"}, plan)
     return {k: v for k, v in got.items() if v is not None}
+
+
+# ------------------------------------------------------------------------------------------------------------------
+# Only the lower triangle of Q is read (tests/test_gpu_q_lower_triangle.py, tests/test_q_lower_triangle_cpu.py).
+
+# the symmetric matrix twice (the control: a difference there is nondeterminism, not the poison), then the strictly upper
+# triangle set to NaN and to finite garbage
+VARIANTS = ("sym", "sym_again", "nan", "garbage")
+L_FILL = 0.375                   # the packed L buffer's contents before pre_factor_kkt, the same in every run
+
+
+def sym_lower(Q):
+    """The symmetric matrix of Q's lower triangle, tril(Q) + tril(Q, -1)^T: what the kernels solve with."""
+    Q = np.asarray(Q)
+    return np.tril(Q) + np.swapaxes(np.tril(Q, -1), -1, -2)
+
+
+def poison(Q, how, rs):
+    """Q with its strictly upper triangle replaced: NaN, or -1e3 times the transposed lower triangle plus N(0, 1) noise
+    (finite and unrelated to the lower triangle: what fmin / fmax or a comparison would hide from NaN)."""
+    Q = np.asarray(Q)
+    upper = np.triu(np.ones(Q.shape[-2:], dtype=bool), 1)
+    bad = np.full(Q.shape, np.nan) if how == "nan" else -1e3 * np.swapaxes(Q, -1, -2) + rs.randn(*Q.shape)
+    return np.where(upper, bad, Q)
+
+
+def q_variants(Q, seed):
+    """{variant: Q} of VARIANTS, built from sym_lower(Q)."""
+    Qs = sym_lower(Q)
+    rs = np.random.RandomState(seed)
+    return dict(sym=Qs, sym_again=Qs.copy(), nan=poison(Qs, "nan", rs), garbage=poison(Qs, "garbage", rs))
+
+
+def adjoints(pr, seed):
+    """Random adjoints of z, lam and nu for a problem dict with batched p, h, b."""
+    rs = np.random.RandomState(seed)
+    B = np.shape(pr["p"])[0]
+    return {k: rs.randn(B, np.shape(pr[i])[-1] if np.size(pr[i]) else 0) for k, i in (("z", "p"), ("lam", "h"), ("nu", "b"))}
+
+
+def leaf(x, dev, grad):
+    """An array or tensor as a new fp64 leaf tensor on `dev` (a device tensor is copied as it is, every byte of it)."""
+    import torch
+    x = x if torch.is_tensor(x) else torch.tensor(np.asarray(x))
+    return x.detach().to(device=dev, dtype=torch.float64).clone().requires_grad_(grad)
+
+
+def qp_outputs(pr, adj, kkt_solver=None, backward=True, dev="cuda:0"):
+    """QPFunction(duals=True, check_Q_spd=True) on `pr` with qp.TRACE on and deferred checks off, then a backward with
+    the adjoints `adj` on z, lam and nu: z, lam, slacks, nu, iters, best_resid, the trace and every gradient."""
+    import torch
+    from qpth_b200 import KKTSolvers, QPFunction, qp as qpmod
+    e = torch.Tensor().to(dev).double()
+    t = {k: leaf(pr[k], dev, backward) for k in ("Q", "p", "G", "h", "A", "b")}
+    t = {k: (v if v.numel() else e) for k, v in t.items()}
+    saved = qpmod.TRACE, qpmod.LAZY_CHECKS
+    qpmod.TRACE, qpmod.LAZY_CHECKS = True, False
+    try:
+        f = QPFunction(verbose=-1, check_Q_spd=True, kkt_solver=kkt_solver or KKTSolvers.LU_PARTIAL, duals=True)
+        z, lam, nu = f(*(t[k] for k in ("Q", "p", "G", "h", "A", "b")))
+        if backward:
+            outs = [(z, "z"), (lam, "lam")] + ([(nu, "nu")] if nu.numel() else [])
+            sum((o * torch.tensor(adj[k], dtype=torch.float64, device=dev)).sum() for o, k in outs).backward()
+    finally:
+        qpmod.TRACE, qpmod.LAZY_CHECKS = saved
+    st = f.last_solve()
+    out = dict(z=z.detach().cpu().numpy(), lam=lam.detach().cpu().numpy(), nu=nu.detach().cpu().numpy(),
+               slacks=st.slacks.cpu().numpy(), iters=st.iters.cpu().numpy(), best_resid=st.best_resid.cpu().numpy(),
+               trace=st.trace.cpu().numpy())
+    out.update({"d" + k: v.grad.cpu().numpy() for k, v in t.items() if v.grad is not None})
+    return out
+
+
+def lower_triangle_runs(fam, shape, B=2):
+    """Every VARIANT of Q on the family's plan: QPFunction's forward and backward with duals, with Q, G, A, h, b batched
+    (nsys = B) and un-batched (nsys = 1), and pre_factor_kkt + solve_kkt at reg 0 and 1e-7 with the packed L buffer.
+    Keys "<run>__<variant>__<output>"."""
+    fwd_only = FAMILIES[fam].get("forward_only", False)
+    out = {}
+    for unbatched in (False, True):
+        pr = trajectory_problem(fam, shape, B, unbatched)
+        adj = adjoints(pr, seed_for(fam, shape, 5))
+        with family_env(fam):
+            family_plan(fam, shape)
+            for v, Q in q_variants(pr["Q"], seed_for(fam, shape, 6)).items():
+                r = qp_outputs(dict(pr, Q=Q), adj, backward=not fwd_only)
+                out.update({"%s__%s__%s" % ("qp_unbatched" if unbatched else "qp_batched", v, k): a for k, a in r.items()})
+    if not fwd_only:
+        x = kkt_inputs(fam, shape, B, False)
+        for reg in (0.0, 1e-7):
+            for v, Q in q_variants(x["Q"], seed_for(fam, shape, 7)).items():
+                r = kkt_on_gpu(fam, shape, B, False, reg, Q=Q, fill_L=L_FILL)
+                out.update({"%s__%s__%s" % ("kkt_reg" if reg else "kkt", v, k): a for k, a in r.items()})
+    return out
+
+
+def compare_variants(rec):
+    """Group `rec` ("<run>__<variant>__<output>") by run, and assert every variant bit-identical to "sym", output by
+    output (NaN only where the trace has rows past a QP's last iteration). Returns the runs compared."""
+    runs = sorted({k.split("__")[0] for k in rec})
+    for run in runs:
+        outs = sorted({k.split("__")[2] for k in rec if k.startswith(run + "__")})
+        for o in outs:
+            ref = rec["%s__sym__%s" % (run, o)]
+            if o != "trace":
+                assert np.isfinite(ref).all(), (run, o)
+            for v in VARIANTS[1:]:
+                got = rec["%s__%s__%s" % (run, v, o)]
+                assert got.shape == ref.shape and np.array_equal(got, ref, equal_nan=(o == "trace")), \
+                    (run, v, o, np.nanmax(np.abs(got - ref)) if got.shape == ref.shape else got.shape)
+    return runs
+
+
+def eq_outputs(pr, adj, tan, kkt_solver, dev="cuda:0"):
+    """The equality-only path (Q, p, A, b; no inequality rows) of QPFunction(duals=True, check_Q_spd=True): z*, nu, the
+    gradients of <adj_z, z> + <adj_nu, nu>, and the JVP (dz, dnu) along the tangents `tan` of Q, p, A and b."""
+    import torch
+    import torch.autograd.forward_ad as fwAD
+    from qpth_b200 import QPFunction
+    t = {k: leaf(v, dev, True) for k, v in pr.items() if k in ("Q", "p", "A", "b")}
+    e = torch.Tensor().to(dev).double()
+    f = QPFunction(verbose=-1, check_Q_spd=True, kkt_solver=kkt_solver, duals=True)
+    z, lam, nu = f(t["Q"], t["p"], e, e, t["A"], t["b"])
+    assert lam.shape == (z.shape[0], 0)
+    T = lambda a: torch.tensor(a, dtype=torch.float64, device=dev)
+    ((z * T(adj["z"])).sum() + (nu * T(adj["nu"])).sum()).backward()
+    out = dict(z=z.detach().cpu().numpy(), nu=nu.detach().cpu().numpy(), **{"d" + k: v.grad.cpu().numpy() for k, v in t.items()})
+    with fwAD.dual_level():
+        zd, _, nud = f(*(fwAD.make_dual(t[k].detach(), T(tan[k])) if k in t else e for k in ("Q", "p", "G", "h", "A", "b")))
+        out["jvp_z"] = fwAD.unpack_dual(zd).tangent.cpu().numpy()
+        out["jvp_nu"] = fwAD.unpack_dual(nud).tangent.cpu().numpy()
+    return out
