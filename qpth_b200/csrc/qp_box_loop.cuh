@@ -2,7 +2,8 @@
 // with the bounds eliminated). Included by qp_box.cu (kNT = 128: diagonal Q, families OneCta and Cluster) and by
 // qp_boxq.cu (kNT = 256: dense Q, family DenseQ); each unit sets its own QPB_NT and its own `qpb` namespace first.
 //
-// A family is the per-CTA context of one layout, built in the kernel from its parameter (F::Dims), with
+// A family is the per-CTA context of one layout, built in the kernel from its parameter (F::Dims, __grid_constant__: a
+// family may hold a reference to it without ptxas copying the parameter into local memory), with
 //   D                     this CTA's layout: counts (n, m, e, ep, nlb: its local variables, inequality rows, neq,
 //                         neq_pad, lb rows) and the shared-memory offsets of the vectors below;
 //   kMinFwd / kMinBwd / kMinKkt   the CTAs per SM of each kernel's __launch_bounds__ (0: no bound);
@@ -106,19 +107,20 @@ struct BoxCta {
 // forward (batch.py:47-207); the loop of k_forward_fast (qp_solve.cuh). Every CTA writes its slice of zhat, lam and
 // slacks; the leader nus, iters, best_resid, the trace rows and spd_flag.
 //
-// INVARIANT (Cluster, and the k_box_*_dm kernels of qp_box.cu, which repeat this loop): every CTA of a cluster executes the same sequence of cluster.sync() calls. Every
-// reduction leaves bit-identical sums and minima in every CTA, and so does every solve (M is summed in rank order and
-// factored redundantly, or dy is gathered from its owners), so y, mu, the residual and the step lengths are
-// bit-identical too. Every branch that reaches a cluster barrier (the exit tests, NaN and mu > 1e32 exits, best-iterate
-// tracking, notImprovedLim, e > 0, fresh) is decided from those values or from kernel arguments only; a CTA that
-// branched on a value of its own would deadlock its cluster.
+// INVARIANT (Cluster, and the k_box_*_dm kernels of qp_box.cu, which repeat this loop): every CTA of a cluster executes
+// the same sequence of cluster.sync() calls. Every reduction leaves bit-identical sums and minima in every CTA, and so
+// does every solve (M is summed in rank order and factored redundantly, or dy is gathered from its owners), so y, mu,
+// the residual and the step lengths are bit-identical too. Every branch that reaches a cluster barrier (the exit
+// tests, NaN and mu > 1e32 exits, best-iterate tracking, notImprovedLim, e > 0, fresh) is decided from those values or
+// from kernel arguments only; a CTA that branched on a value of its own would deadlock its cluster.
 template <class F>
 __global__ void __launch_bounds__(kBoxNT, F::kMinFwd)
-k_box_forward(typename F::Dims P, const double* __restrict__ q, int64_t sq, const double* __restrict__ p, int64_t sp,
-              const double* __restrict__ A, int64_t sA, const double* __restrict__ b, int64_t sb,
-              const double* __restrict__ lb, int64_t slb, const double* __restrict__ ub, int64_t sub, double eps,
-              double stall_tol, double best_tie, int notImprovedLim, int maxIter, double* __restrict__ zhat,
-              double* __restrict__ lam, double* __restrict__ slacks, double* __restrict__ nus, int* __restrict__ iters_out,
+k_box_forward(const __grid_constant__ typename F::Dims P, const double* __restrict__ q, int64_t sq,
+              const double* __restrict__ p, int64_t sp, const double* __restrict__ A, int64_t sA,
+              const double* __restrict__ b, int64_t sb, const double* __restrict__ lb, int64_t slb,
+              const double* __restrict__ ub, int64_t sub, double eps, double stall_tol, double best_tie,
+              int notImprovedLim, int maxIter, double* __restrict__ zhat, double* __restrict__ lam,
+              double* __restrict__ slacks, double* __restrict__ nus, int* __restrict__ iters_out,
               double* __restrict__ resid_out, double* __restrict__ trace, int* __restrict__ spd_flag) {
     QPB_SMEM;
     F f(P);
@@ -270,11 +272,11 @@ struct BoxGrads {
 
 template <class F>
 __global__ void __launch_bounds__(kBoxNT, F::kMinBwd)
-k_box_backward(typename F::Dims P, const double* __restrict__ q, int64_t sq, const double* __restrict__ A, int64_t sA,
-               const double* __restrict__ dl, const double* __restrict__ dl_dlam, const double* __restrict__ dl_dnu,
-               const double* __restrict__ zhat, const double* __restrict__ lam,
-               const double* __restrict__ slacks, const double* __restrict__ nus, BoxGrads O,
-               double* __restrict__ dxv, double* __restrict__ dlamv, double* __restrict__ dnuv) {
+k_box_backward(const __grid_constant__ typename F::Dims P, const double* __restrict__ q, int64_t sq,
+               const double* __restrict__ A, int64_t sA, const double* __restrict__ dl,
+               const double* __restrict__ dl_dlam, const double* __restrict__ dl_dnu, const double* __restrict__ zhat,
+               const double* __restrict__ lam, const double* __restrict__ slacks, const double* __restrict__ nus,
+               BoxGrads O, double* __restrict__ dxv, double* __restrict__ dlamv, double* __restrict__ dnuv) {
     QPB_SMEM;
     F f(P);
     const auto& D = f.D;
@@ -324,10 +326,10 @@ k_box_backward(typename F::Dims P, const double* __restrict__ q, int64_t sq, con
 // vectors (B, len))
 template <class F>
 __global__ void __launch_bounds__(kBoxNT, F::kMinKkt)
-k_box_kkt(typename F::Dims P, const double* __restrict__ q, int64_t sq, const double* __restrict__ A, int64_t sA,
-          const double* __restrict__ d, const double* __restrict__ rx, const double* __restrict__ rs,
-          const double* __restrict__ rz, const double* __restrict__ ry, double* __restrict__ dx, double* __restrict__ ds,
-          double* __restrict__ dz, double* __restrict__ dy) {
+k_box_kkt(const __grid_constant__ typename F::Dims P, const double* __restrict__ q, int64_t sq,
+          const double* __restrict__ A, int64_t sA, const double* __restrict__ d, const double* __restrict__ rx,
+          const double* __restrict__ rs, const double* __restrict__ rz, const double* __restrict__ ry,
+          double* __restrict__ dx, double* __restrict__ ds, double* __restrict__ dz, double* __restrict__ dy) {
     QPB_SMEM;
     F f(P);
     const auto& D = f.D;

@@ -21,15 +21,15 @@ LIMITS = {
     r"k_box_forwardINS_6OneCta": (208, 60, 68),
     r"k_box_forwardINS_7Cluster": (368, 0, 0),
     r"k_box_forward_dm": (400, 0, 0),
-    r"k_box_forwardINS_6DenseQ": (392, 212, 632),
+    r"k_box_forwardINS_6DenseQ": (144, 128, 324),
     r"k_box_backwardINS_6OneCta": (168, 0, 0),
     r"k_box_backwardINS_7Cluster": (368, 0, 0),
     r"k_box_backward_dm": (400, 0, 0),
-    r"k_box_backwardINS_6DenseQ": (168, 0, 0),
+    r"k_box_backwardINS_6DenseQ": (0, 0, 0),
     r"k_box_kktINS_6OneCta": (168, 0, 0),
     r"k_box_kktINS_7Cluster": (368, 0, 0),
     r"k_box_kkt_dm": (400, 0, 0),
-    r"k_box_kktINS_6DenseQ": (168, 0, 0),
+    r"k_box_kktINS_6DenseQ": (0, 0, 0),
 }
 
 
