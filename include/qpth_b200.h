@@ -305,6 +305,21 @@ int qpb200_jvp_reg(const qpb200_plan* plan, int nbatch,
                    double* rhs, double* dz, double* dlam, double* dnu,
                    double* scratch, void* stream);
 
+/* Jacobians at the returned point (an extension): d(z*, lam, nu)/d(p, h, b) for every QP of the batch, the negated
+ * inverse of the backward's system [Q 0 G' A'; 0 D I 0; G I 0 0; A 0 0 0] with D = clamp(lam, 1e-8) / clamp(s, 1e-8):
+ *   J_z,p = -R_xx, J_z,h = R_x,lam, J_z,b = R_x,nu (likewise for the lam and nu rows), R = that matrix's inverse.
+ * One CTA per QP forms S = W W' + diag(0, 1/d) from Wfac, factors it once and solves for all the columns in blocks of 8.
+ * It reads Lfac and Wfac of qpb200_pre_factor_kkt (any qpb200_plan_init plan; not the regularised factors), never K. */
+/* Dynamic shared memory of qpb200_jacobian for a qpb200_plan_init plan; *smem_bytes = 0 where the kernel does not
+ * cover the shape (the caller then uses qpb200_jvp column by column). No device work. */
+int qpb200_jacobian_smem(const qpb200_plan* plan, int64_t* smem_bytes);
+/* d(z*, lam, nu)/d(p, h, b) at the point (lam, slacks), with the backward's clamped D. rows / cols: bit 0 z / p,
+ * bit 1 lam / h, bit 2 nu / b. J: nbatch row-major blocks of R x C doubles, the blocks in the order z, lam, nu and
+ * p, h, b. sF as in qpb200_backward. QPB200_ERR_BAD_ARG for a NULL pointer, an empty mask, a nu or b bit with
+ * neq == 0, or nbatch < 1; QPB200_ERR_TOO_LARGE where qpb200_jacobian_smem reports 0. */
+int qpb200_jacobian(const qpb200_plan* plan, int nbatch, int rows, int cols, const double* lam, const double* slacks,
+                    const double* Lfac, const double* Wfac, int sF, double* J, void* stream);
+
 /* ---- Box QPs (qpth_b200/box.py BoxQPFunction): min 1/2 z' diag(q) z + p'z  s.t.  A z = b,  lb <= z <= ub -------------
  * The dense equivalent is Q = diag(q), G = [-I; I] (only the sides given: lb rows first), h = [-lb; ub]; lam and slacks
  * are laid out as [lb rows; ub rows] (nineq = (has_lb + has_ub) * nz). The inequality block of the KKT system is

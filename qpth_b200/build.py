@@ -29,12 +29,13 @@ def up_to_date():
 
 # (source, extra defines, object suffix): the 256-thread build of every kernel + the 192- and 512-thread builds of the
 # product-form solve kernels (three QPs per SM; large orders) + the 128-thread box-QP kernels (BoxQPFunction) + the
-# 256-thread dense-Q box-QP kernels (BoxQPFunction(dense_Q=True))
+# 256-thread dense-Q box-QP kernels (BoxQPFunction(dense_Q=True)) + the 256-thread Jacobian kernel
 UNITS = [("qp_kernels.cu", [], "main"),
          ("qp_alt.cu", ["-DQPB_NT=192", "-DQPB_ALT_CTAS=3"], "alt192"),
          ("qp_alt.cu", ["-DQPB_NT=512", "-DQPB_ALT_CTAS=1"], "alt512"),
          ("qp_box.cu", ["-DQPB_NT=128"], "box"),
-         ("qp_boxq.cu", ["-DQPB_NT=256"], "boxq")]
+         ("qp_boxq.cu", ["-DQPB_NT=256"], "boxq"),
+         ("qp_jac.cu", ["-DQPB_NT=256"], "jac")]
 
 
 def build(force=False, verbose=False, extra=(), out=None):

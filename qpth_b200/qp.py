@@ -348,6 +348,108 @@ def jvp_outputs(dz, dlam, dnu, out, duals):
     return z, dlam.to(device=device, dtype=dtype), nu
 
 
+# Jacobians (jacobian() of QPFunction and QPSolutionFunction): rows z, lam, nu and columns p, h, b as bits 0, 1, 2
+JAC_WRT = ("p", "h", "b")
+
+
+def jacobian_covered(plan):
+    """True where qpb200_jacobian covers `plan` (qpb200_jacobian_smem reports its shared memory)."""
+    out = ctypes.c_int64(0)
+    _lib.check(_lib.load().qpb200_jacobian_smem(ctypes.byref(plan), ctypes.byref(out)))
+    return out.value > 0
+
+
+def _jacobian_kernel(st, rows, cols, J):
+    """qpb200_jacobian into J (B, R, C) fp64 on st.device."""
+    with torch.cuda.device(st.device):
+        _lib.check(_lib.load().qpb200_jacobian(
+            ctypes.byref(st.plan), st.nBatch, rows, cols, _ptr(st.lam), _ptr(st.slacks), _ptr(st.L), _ptr(st.W),
+            1 if st.nsys > 1 else 0, _ptr(J), _stream()))
+
+
+def _jacobian_columns(st, rows, cols, J):
+    """J column by column: one solve_jvp per column with an un-batched unit tangent of p, h or b (batch stride 0), which
+    gives that column for every QP at once (qpb200_jvp, or qpb200_jvp_reg with its refinement steps)."""
+    sizes = (st.plan.nz, st.plan.nineq, st.plan.neq)
+    c0 = 0
+    for k in range(3):
+        if not (cols >> k) & 1:
+            continue
+        for j in range(sizes[k]):
+            t = torch.zeros(sizes[k], dtype=torch.float64, device=st.device)
+            t[j] = 1.0
+            tans = [None] * 6
+            tans[2 * k + 1] = t                          # (dQ, dp, dG, dh, dA, db): dp, dh or db
+            outs = solve_jvp(st, tans)
+            r0 = 0
+            for i in range(3):
+                if (rows >> i) & 1:
+                    J[:, r0:r0 + sizes[i], c0 + j] = outs[i]
+                    r0 += sizes[i]
+        c0 += sizes[k]
+
+
+def solve_jacobian(st, rows, cols):
+    """d(zhat, lam, nu)/d(p, h, b) at the returned point of `st`, per QP: fp64 (B, R, C) on st.device, rows [z; lam; nu]
+    and columns [p, h, b] restricted to the bits of `rows` / `cols` (bit 0 z / p, bit 1 lam / h, bit 2 nu / b). One
+    qpb200_jacobian call where the kernel covers the plan (the default mode); otherwise, and always in the regularised
+    mode (IR_UNOPT), one solve_jvp per column."""
+    if _pending:
+        flush_checks(wait=False)
+    plan = st.plan
+    sizes = (plan.nz, plan.nineq, plan.neq)
+    if plan.neq == 0 and ((rows | cols) & 4):
+        raise ValueError("qpth_b200: a Jacobian with respect to b, or of nu, needs equality constraints (neq == 0)")
+    R = sum(sizes[i] for i in range(3) if (rows >> i) & 1)
+    C = sum(sizes[i] for i in range(3) if (cols >> i) & 1)
+    J = torch.empty(st.nBatch, R, C, dtype=torch.float64, device=st.device)
+    if not getattr(st, "reg", False) and jacobian_covered(plan):
+        _jacobian_kernel(st, rows, cols, J)
+    else:
+        _jacobian_columns(st, rows, cols, J)
+    return J
+
+
+def jacobian_of(st, out, wrt, duals):
+    """The `jacobian` attribute of QPFunction / QPSolutionFunction on the state `st` of their last forward, whose output
+    had out = (device, dtype). Returns {name: (B, rows, n_name)} for each name of `wrt`, rows z, or [z; lam; nu] with
+    duals."""
+    if st is None:
+        raise RuntimeError("qpth_b200: jacobian() needs a forward call of this function first")
+    names = (wrt,) if isinstance(wrt, str) else tuple(wrt)
+    if not names:
+        raise ValueError("qpth_b200: jacobian(wrt=...) needs at least one of %s" % (JAC_WRT,))
+    for nm in names:
+        if nm not in JAC_WRT:
+            raise ValueError("qpth_b200: jacobian(wrt=...) takes %s, not %r (Jacobians with respect to Q, G and A are "
+                             "not provided)" % (JAC_WRT, nm))
+    plan = st.plan
+    if "b" in names and plan.neq == 0:
+        raise ValueError("qpth_b200: jacobian(wrt='b') needs equality constraints (neq == 0)")
+    cols = sum(1 << JAC_WRT.index(nm) for nm in set(names))
+    rows = 1 | ((2 | (4 if plan.neq > 0 else 0)) if duals else 0)
+    J = solve_jacobian(st, rows, cols)
+    sizes = dict(zip(JAC_WRT, (plan.nz, plan.nineq, plan.neq)))
+    res, c0 = {}, 0
+    for nm in JAC_WRT:
+        if (cols >> JAC_WRT.index(nm)) & 1:
+            res[nm] = J[:, :, c0:c0 + sizes[nm]]
+            c0 += sizes[nm]
+    device, dtype = out
+    return {nm: res[nm].to(device=device, dtype=dtype).contiguous() for nm in names}
+
+
+JACOBIAN_DOC = """jacobian(wrt=("p", "h", "b"), duals=False) -> {name: tensor}: the Jacobians of the last forward's solution with
+    respect to p, h and b, per QP (also for an un-batched p, h or b: the true derivative, not a batch mean). J["p"] is
+    (nBatch, nz, nz) = dz*/dp, J["h"] (nBatch, nz, nineq), J["b"] (nBatch, nz, neq); duals=True gives the rows
+    [z; lam; nu], (nBatch, nz + nineq + neq, n). They are the negated inverse of the backward's system at the returned
+    point, [Q 0 G' A'; 0 D I 0; G I 0 0; A 0 0 0] with qpth's clamped D, so J t equals the forward-mode tangent for a
+    tangent t of p, h or b. One kernel call (qpb200_jacobian) factors S once per QP and solves for every column; where it
+    does not cover the shape, and with KKTSolvers.IR_UNOPT, one JVP per column. The result has the dtype and device of the
+    forward's output and is not differentiable. Jacobians with respect to Q, G and A are not provided: they are
+    contractions of these blocks with z, lam and nu (e.g. dz/dh_i lam_j gives the dG_ij column)."""
+
+
 def check_kkt_solver(kkt_solver):
     if kkt_solver == KKTSolvers.LU_FULL:
         raise ValueError("qpth_b200: KKTSolvers.LU_FULL is not provided; use KKTSolvers.LU_PARTIAL (Q positive definite) "
@@ -372,6 +474,9 @@ def QPFunction(eps=1e-12, verbose=0, notImprovedLim=3, maxIter=20, solver=QPSolv
     one solve of the backward's system with -[rx; 0; rz; ry], rx = sym(dQ) z + dp + dG' lam + dA' nu, rz = dG z - dh,
     ry = dA z - db (qpb200_jvp), the exact transpose of the backward pass. The tangent of an un-batched input applies
     to every QP and gives the true derivative, where the backward returns the batch mean.
+
+    The returned callable's `jacobian(wrt=("p", "h", "b"), duals=False)` gives the whole Jacobians of the last forward's
+    solution with respect to p, h and b, per QP (its docstring has the details).
 
     kkt_solver (an extension of the reference's signature): KKTSolvers.LU_PARTIAL, the default, needs Q positive definite.
     KKTSolvers.IR_UNOPT also solves QPs whose Q is only positive semidefinite (LPs with Q = 0, low-rank quadratic terms)
@@ -402,11 +507,17 @@ def QPFunction(eps=1e-12, verbose=0, notImprovedLim=3, maxIter=20, solver=QPSolv
                                                                                                           kkt_solver)
             return f(Q_, p_, G_, h_, A_, b_, zhats, lams, slacks, nus)
 
+        def no_jacobian(wrt=JAC_WRT, duals=False):
+            raise NotImplementedError("qpth_b200: jacobian() is not provided for solver=QPSolvers.CVXPY; solve with "
+                                      "CVXPY and call QPSolutionFunction's jacobian() instead")
+
+        apply_cvxpy.jacobian = no_jacobian
         return apply_cvxpy
     if solver != QPSolvers.PDIPM_BATCHED:
         assert False                                     # qp.py:121-122
 
     _last = [None]
+    _jac = [None, None, False]           # the state and (device, dtype) of the last forward; True: it was equality-only
 
     class QPFunctionFn(Function):
         @staticmethod
@@ -420,6 +531,7 @@ def QPFunction(eps=1e-12, verbose=0, notImprovedLim=3, maxIter=20, solver=QPSolv
             st = solve_forward(Q_, p_, G_, h_, A_, b_, eps, verbose, notImprovedLim, maxIter, check_Q_spd, kkt_solver)
             ctx.st = st
             _last[0] = st
+            _jac[0], _jac[1] = st, (Q_.device, Q_.dtype)
             ctx.neq, ctx.nineq, ctx.nz = st.plan.neq, st.plan.nineq, st.plan.nz
             zhats = st.zhat.to(device=Q_.device, dtype=Q_.dtype)
             ctx.save_for_backward(zhats, Q_, p_, G_, h_, A_, b_)
@@ -453,9 +565,19 @@ def QPFunction(eps=1e-12, verbose=0, notImprovedLim=3, maxIter=20, solver=QPSolv
         if G_.nelement() == 0 and h_.nelement() == 0 and A_.nelement() > 0:
             # equality-constrained QP: an extension (the reference cannot run nineq == 0); one KKT solve, eqonly.py
             from .eqonly import solve_equality_qp
+            _jac[:] = [None, None, True]
             return solve_equality_qp(Q_, p_, A_, b_, check_Q_spd, reg=kkt_solver == KKTSolvers.IR_UNOPT, duals=duals)
+        _jac[2] = False
         return QPFunctionFn.apply(Q_, p_, G_, h_, A_, b_)
 
+    def jacobian(wrt=JAC_WRT, duals=False):
+        if _jac[2]:
+            raise NotImplementedError("qpth_b200: jacobian() is not provided for the equality-only path (nineq == 0); "
+                                      "use forward-mode AD (torch.autograd.forward_ad) column by column")
+        return jacobian_of(_jac[0], _jac[1], wrt, duals)
+
+    jacobian.__doc__ = JACOBIAN_DOC
     # diagnostics the reference keeps on ctx (nus / lams / slacks) plus per-QP iteration counts
     apply.last_solve = lambda: _last[0]
+    apply.jacobian = jacobian
     return apply

@@ -100,7 +100,8 @@ def QPSolutionFunction(check_Q_spd=True, kkt_solver=KKTSolvers.LU_PARTIAL, duals
     without equality rows), as QPFunction(duals=True) does; a loss may use all three.
 
     Forward mode (torch.autograd.forward_ad) is supported as for QPFunction; the tangents of the four solution tensors
-    are ignored.
+    are ignored. f.jacobian(wrt, duals) gives the Jacobians with respect to p, h and b at the last solution passed, as
+    QPFunction's does.
 
     kkt_solver: KKTSolvers.LU_PARTIAL (the default) needs Q positive definite. KKTSolvers.IR_UNOPT differentiates with
     the regularised KKT solve of QPFunction(kkt_solver=IR_UNOPT), so an LP (Q = 0) or a low-rank Q solved by any solver
@@ -110,11 +111,13 @@ def QPSolutionFunction(check_Q_spd=True, kkt_solver=KKTSolvers.LU_PARTIAL, duals
     and tangents are those of the symmetric matrix tril(Q) + tril(Q, -1)^T. A tangent dQ is read in full and enters as
     sym(dQ) = (dQ + dQ^T) / 2."""
     check_kkt_solver(kkt_solver)
+    _last = [None, None]                 # the state and (device, dtype) of the last forward, for jacobian()
 
     class QPSolutionFn(Function):
         @staticmethod
         def forward(ctx, Q_, p_, G_, h_, A_, b_, zhat, lams, slacks, nus):
             ctx.st = pre_factor_state(Q_, p_, G_, h_, A_, b_, zhat, lams, slacks, nus, check_Q_spd, kkt_solver)
+            _last[0], _last[1] = ctx.st, (Q_.device, Q_.dtype)
             zhats = ctx.st.zhat.to(device=Q_.device, dtype=Q_.dtype)
             ctx.save_for_backward(zhats, Q_, p_, G_, h_, A_, b_)
             ctx.lams, ctx.slacks, ctx.nus = ctx.st.lam, ctx.st.slacks, ctx.st.nus
@@ -149,6 +152,13 @@ def QPSolutionFunction(check_Q_spd=True, kkt_solver=KKTSolvers.LU_PARTIAL, duals
         sol = [x.detach() if torch.is_tensor(x) else x for x in (zhat, lams, slacks, nus)]
         return QPSolutionFn.apply(Q_, p_, G_, h_, A_, b_, *sol)
 
+    def jacobian(wrt=("p", "h", "b"), duals=False):
+        from .qp import jacobian_of
+        return jacobian_of(_last[0], _last[1], wrt, duals)
+
+    from .qp import JACOBIAN_DOC
+    jacobian.__doc__ = JACOBIAN_DOC
+    apply.jacobian = jacobian
     return apply
 
 
