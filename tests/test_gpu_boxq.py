@@ -215,9 +215,18 @@ def test_duals_end_to_end_against_central_differences():
     assert rel_rows(p.grad.cpu().numpy(), num).max() < 1e-5
 
 
+def _box_G(n):
+    var, sgn = rows(n, True, True)
+    G = np.zeros((2 * n, n))
+    G[np.arange(2 * n), var] = sgn
+    return G
+
+
 def test_jvp_matches_model_and_transposes_the_backward():
     import torch.autograd.forward_ad as fwAD
     from qpth_b200 import BoxQPFunction
+    from tests import jvp_models as jm
+    from tests.test_gpu_boxq_edges import dlam_floor
     B, n, e = 3, 14, 3
     bx = random_boxq(88, B, n, e, "both")
     rs = np.random.RandomState(8)
@@ -237,6 +246,15 @@ def test_jvp_matches_model_and_transposes_the_backward():
         mz, ml, mn = qm.jvp_one(sol, dQ=tang["Q"][i], dp=tang["p"][i], dA=tang["A"][i], db=tang["b"][i],
                                 dlb=tang["lb"][i], dub=tang["ub"][i])
         assert rel_rows(dz[i], mz).max() < 1e-8 and rel_rows(dnu[i], mn).max() < 1e-8
+        # dlam = d (G dz + rz) carries d up to 1e8 at the converged point, so kernels and model both round it to ~1e-8:
+        # the refined dense solve decides, with the bound of tests/test_gpu_boxq_edges.py
+        G = _box_G(n)
+        dh = np.concatenate([-tang["lb"][i], tang["ub"][i]])
+        ref = jm.jvp_dense(qm.sym_lower(bx["Q"][i]), G, bx["A"][i], sol["x"], sol["lam"], sol["s"], sol["nu"],
+                           dict(Q=tang["Q"][i], p=tang["p"][i], h=dh, A=tang["A"][i], b=tang["b"][i]))
+        d = np.maximum(sol["lam"], 1e-8) / np.maximum(sol["s"], 1e-8)
+        bound = max(10 * dense_kkt.rel(ml, ref[1]), 1e-10, dlam_floor(d, G, ref[0], -dh, ref[1]))
+        assert dense_kkt.rel(dlam[i], ref[1]) <= bound, (i, dense_kkt.rel(dlam[i], ref[1]), bound)
     # transpose identity: <g, JVP(t)> = sum_X <grad_X, t_X> for batched inputs
     g = rs.randn(B, n)
     ins = {k: prim[k].clone().requires_grad_(True) for k in KEYS}
