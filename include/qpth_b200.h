@@ -382,6 +382,22 @@ int qpb200_box_jvp(const qpb200_box_plan* plan, int nbatch, const double* q, int
                    const double* zhat, const double* lam, const double* slacks, const double* nus, double* rhs,
                    double* dz, double* dlam, double* dnu, void* stream);
 
+/* Jacobians of a box QP at the returned point (an extension, csrc/qp_jac.cu): d(z*, lam, nu)/d(p, lb, ub, b) per QP,
+ * with the backward's clamped D = clamp(lam, 1e-8) / clamp(s, 1e-8) = [d_lb; d_ub]. With H = q + d_lb + d_ub and
+ * X = [H A'; A 0]^-1: the p columns are -X e_j (z and nu rows), the b columns X e_(nz + c), the lb / ub columns the p
+ * columns scaled by -d_lb_j / -d_ub_j, and the lam rows d_lb o (rz_lb - z) and d_ub o (rz_ub + z) (rz_lb = e_j in lb
+ * column j, rz_ub = -e_j in ub column j, zero otherwise). One CTA per QP factors M = A H^-1 A' once and solves for
+ * every column in blocks of 8; any qpb200_box_plan_init plan whose buffers fit is covered, whatever its layout. */
+/* Dynamic shared memory of qpb200_box_jacobian; *smem_bytes = 0 where the kernel does not cover the shape (the caller
+ * then uses qpb200_box_jvp column by column). No device work. */
+int qpb200_box_jacobian_smem(const qpb200_box_plan* plan, int64_t* smem_bytes);
+/* rows: bit 0/1/2 = z / lam / nu; cols: bit 0/1/2/3 = p / lb / ub / b. J: nbatch row-major blocks of R x C doubles,
+ * the blocks in that order. q, A with batch strides sq, sA (0 = shared). QPB200_ERR_BAD_ARG for a NULL pointer, an
+ * empty mask, an unknown bit, an lb / ub bit for an absent side, a nu / b bit with neq == 0, or nbatch < 1;
+ * QPB200_ERR_TOO_LARGE where qpb200_box_jacobian_smem reports 0. */
+int qpb200_box_jacobian(const qpb200_box_plan* plan, int nbatch, int rows, int cols, const double* q, int64_t sq,
+                        const double* A, int64_t sA, const double* lam, const double* slacks, double* J, void* stream);
+
 /* The structured factor and solve for caller-supplied d (B,nineq) and right-hand sides (the counterpart of
  * qpb200_solve_kkt):  [diag(q) 0 G' A'; 0 D I 0; G I 0 0; A 0 0 0] [dx ds dz dy] = -[rx rs rz ry].
  * ry / dy may be NULL when neq == 0. */
@@ -426,6 +442,13 @@ int qpb200_boxq_jvp(const qpb200_boxq_plan* plan, int nbatch, const double* Q, i
                     const double* db, int64_t sdb, const double* dlb, int64_t sdlb, const double* dub, int64_t sdub,
                     const double* zhat, const double* lam, const double* slacks, const double* nus, double* rhs,
                     double* dz, double* dlam, double* dnu, void* stream);
+/* As qpb200_box_jacobian with a dense Q (nz x nz, batch stride sQ; only its lower triangle is read): K = [H A'; A 0],
+ * H = Q + diag(d_lb + d_ub), is factored once per QP as the forward factors it (L diag(I, -I) L' on the bordered
+ * staircase) and every column is solved in blocks of 8. *smem_bytes = 0 where the kernel does not cover the plan (every
+ * qpb200_boxq_plan_init plan with ok = 1 is covered); the caller then uses qpb200_boxq_jvp column by column. */
+int qpb200_boxq_jacobian_smem(const qpb200_boxq_plan* plan, int64_t* smem_bytes);
+int qpb200_boxq_jacobian(const qpb200_boxq_plan* plan, int nbatch, int rows, int cols, const double* Q, int64_t sQ,
+                         const double* A, int64_t sA, const double* lam, const double* slacks, double* J, void* stream);
 /* As qpb200_box_solve_kkt: [Q 0 G' A'; 0 D I 0; G I 0 0; A 0 0 0] [dx ds dz dy] = -[rx rs rz ry]. */
 int qpb200_boxq_solve_kkt(const qpb200_boxq_plan* plan, int nbatch, const double* Q, int64_t sQ, const double* A,
                           int64_t sA, const double* d, const double* rx, const double* rs, const double* rz,

@@ -101,6 +101,8 @@ SIGNATURES = {
                             _P, _L, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     "qpb200_box_solve_kkt": (_I, [ctypes.POINTER(BoxPlan), _I, _P, _L, _P, _L, _P, _P, _P, _P, _P,
                                   _P, _P, _P, _P, _P]),
+    "qpb200_box_jacobian_smem": (_I, [ctypes.POINTER(BoxPlan), _P]),
+    "qpb200_box_jacobian": (_I, [ctypes.POINTER(BoxPlan), _I, _I, _I, _P, _L, _P, _L, _P, _P, _P, _P]),
     "qpb200_boxq_plan_init": (_I, [_I, _I, _I, _I, ctypes.POINTER(BoxQPlan)]),
     "qpb200_boxq_forward": (_I, [ctypes.POINTER(BoxQPlan), _I, _P, _L, _P, _L, _P, _L, _P, _L, _P, _L, _P, _L,
                                  _D, _D, _D, _I, _I, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
@@ -110,6 +112,8 @@ SIGNATURES = {
                              _P, _L, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     "qpb200_boxq_solve_kkt": (_I, [ctypes.POINTER(BoxQPlan), _I, _P, _L, _P, _L, _P, _P, _P, _P, _P,
                                    _P, _P, _P, _P, _P]),
+    "qpb200_boxq_jacobian_smem": (_I, [ctypes.POINTER(BoxQPlan), _P]),
+    "qpb200_boxq_jacobian": (_I, [ctypes.POINTER(BoxQPlan), _I, _I, _I, _P, _L, _P, _L, _P, _P, _P, _P]),
 }
 
 _lib = None

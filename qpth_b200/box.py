@@ -270,6 +270,131 @@ def dense_jvp(st, tangents, nlb, has_ub, dense_Q=False):
     return _qp.solve_jvp(dst, (dQ, dp, None, dh, dA, db))
 
 
+# ---- Jacobians (jacobian() of BoxQPFunction): rows z, lam, nu as bits 0, 1, 2 and columns p, lb, ub, b as bits 0..3 ---
+BOX_JAC_WRT = ("p", "lb", "ub", "b")
+
+
+def box_jacobian_covered(plan, dense_Q=False):
+    """True where qpb200_box_jacobian (dense_Q: qpb200_boxq_jacobian) covers a qpb200_box_plan (qpb200_boxq_plan): its
+    smem function reports the shared memory."""
+    out = ctypes.c_int64(0)
+    lib = _lib.load()
+    fn = lib.qpb200_boxq_jacobian_smem if dense_Q else lib.qpb200_box_jacobian_smem
+    _lib.check(fn(ctypes.byref(plan), ctypes.byref(out)))
+    return out.value > 0
+
+
+def _box_jacobian_kernel(st, rows, cols, J):
+    """qpb200_box_jacobian (a dense Q: qpb200_boxq_jacobian) into J (B, R, C) fp64 on st.device."""
+    lib = _lib.load()
+    with torch.cuda.device(st.device):
+        _lib.check((lib.qpb200_boxq_jacobian if st.dense_Q else lib.qpb200_box_jacobian)(
+            ctypes.byref(st.plan), st.nBatch, rows, cols, _ptr(st.q), st.sq, _ptr(st.A), st.sA, _ptr(st.lam),
+            _ptr(st.slacks), _ptr(J), _stream()))
+
+
+def _box_jacobian_columns(st, rows, cols, J):
+    """J column by column: one solve_box_jvp per column with an un-batched unit tangent of p, lb, ub or b (batch stride
+    0), which gives that column for every QP at once."""
+    plan = st.plan
+    sizes, rsizes = (plan.nz,) * 3 + (plan.neq,), (plan.nz, plan.nineq, plan.neq)
+    c0 = 0
+    for k in range(4):
+        if not (cols >> k) & 1:
+            continue
+        for j in range(sizes[k]):
+            t = torch.zeros(sizes[k], dtype=torch.float64, device=st.device)
+            t[j] = 1.0
+            tans = [None] * 6
+            tans[(1, 4, 5, 3)[k]] = t                    # (dq, dp, dA, db, dlb, dub): dp, dlb, dub or db
+            outs = solve_box_jvp(st, tans)
+            r0 = 0
+            for i in range(3):
+                if (rows >> i) & 1:
+                    J[:, r0:r0 + rsizes[i], c0 + j] = outs[i]
+                    r0 += rsizes[i]
+        c0 += sizes[k]
+
+
+def _box_jacobian_dense(st, rows, cols, nlb, J):
+    """The dense fallback: _qp.solve_jacobian on the dense equivalent, whose lam rows are already [lb rows; ub rows];
+    h = [-lb; ub] gives J_lb = -J_h[:, :, :nlb] and J_ub = J_h[:, :, nlb:]."""
+    dst, _ = st.dense
+    n, m, e = dst.plan.nz, dst.plan.nineq, dst.plan.neq
+    Jd = _qp.solve_jacobian(dst, rows, (cols & 1) | (2 if cols & 6 else 0) | (4 if cols & 8 else 0))
+    src, c0 = 0, 0
+    if cols & 1:
+        J[:, :, :n] = Jd[:, :, :n]
+        src, c0 = n, n
+    if cols & 6:
+        if cols & 2:
+            J[:, :, c0:c0 + n] = -Jd[:, :, src:src + nlb]
+            c0 += n
+        if cols & 4:
+            J[:, :, c0:c0 + n] = Jd[:, :, src + nlb:src + m]
+            c0 += n
+        src += m
+    if cols & 8:
+        J[:, :, c0:c0 + e] = Jd[:, :, src:src + e]
+
+
+def solve_box_jacobian(st, rows, cols, nlb):
+    """d(zhat, lam, nu)/d(p, lb, ub, b) at the returned point of `st`, per QP: fp64 (B, R, C) on st.device, rows
+    [z; lam; nu] and columns [p, lb, ub, b] restricted to the bits of `rows` / `cols`. nlb: nz if lb was given, else 0.
+    One qpb200_box_jacobian (dense Q: qpb200_boxq_jacobian) call where the kernel covers the plan; otherwise one
+    solve_box_jvp per column, and on the dense fallback the dense path's solve_jacobian."""
+    if _qp._pending:
+        _qp.flush_checks(wait=False)
+    plan = st.plan
+    n, m, e = plan.nz, plan.nineq, plan.neq
+    R = sum((n, m, e)[i] for i in range(3) if (rows >> i) & 1)
+    C = sum((n, n, n, e)[k] for k in range(4) if (cols >> k) & 1)
+    J = torch.empty(st.nBatch, R, C, dtype=torch.float64, device=st.device)
+    if st.dense is not None:
+        _box_jacobian_dense(st, rows, cols, nlb, J)
+    elif box_jacobian_covered(plan, st.dense_Q):
+        _box_jacobian_kernel(st, rows, cols, J)
+    else:
+        _box_jacobian_columns(st, rows, cols, J)
+    return J
+
+
+def box_jacobian_of(st, out, sides, wrt, duals):
+    """The `jacobian` attribute of BoxQPFunction on the state `st` of its last forward, whose output had
+    out = (device, dtype) and sides = (nlb, has_ub). Returns {name: (B, rows, n_name)} for each name of `wrt` (None:
+    every input the problem has), rows z, or [z; lam; nu] with duals."""
+    if st is None:
+        raise RuntimeError("qpth_b200: jacobian() needs a forward call of this function first")
+    nlb, has_ub = sides
+    n, e = st.plan.nz, st.plan.neq
+    present = ("p",) + (("lb",) if nlb else ()) + (("ub",) if has_ub else ()) + (("b",) if e > 0 else ())
+    names = present if wrt is None else ((wrt,) if isinstance(wrt, str) else tuple(wrt))
+    if not names:
+        raise ValueError("qpth_b200: jacobian(wrt=...) needs at least one of %s" % (present,))
+    for nm in names:
+        if nm in ("q", "Q", "A"):
+            raise ValueError(
+                "qpth_b200: jacobian(wrt=...) does not take %r; contract the blocks it does give: J_.,q = J_.,p diag(z) "
+                "for a diagonal q, J_.,Q_ik = J_.,p_i z_k for a dense Q (which enters as sym(dQ)), and "
+                "J_.,A_ck = J_.,p_k nu_c - J_.,b_c z_k" % nm)
+        if nm not in BOX_JAC_WRT:
+            raise ValueError("qpth_b200: jacobian(wrt=...) takes %s, not %r" % (BOX_JAC_WRT, nm))
+        if nm not in present:
+            raise ValueError("qpth_b200: jacobian(wrt=%r): this problem has no %s" % (
+                nm, "equality constraints (neq == 0)" if nm == "b" else "%s side" % nm))
+    cols = sum(1 << BOX_JAC_WRT.index(nm) for nm in set(names))
+    rows = 1 | ((2 | (4 if e > 0 else 0)) if duals else 0)
+    J = solve_box_jacobian(st, rows, cols, nlb)
+    res, c0 = {}, 0
+    for k, nm in enumerate(BOX_JAC_WRT):
+        if (cols >> k) & 1:
+            w = e if nm == "b" else n
+            res[nm] = J[:, :, c0:c0 + w]
+            c0 += w
+    device, dtype = out
+    return {nm: res[nm].to(device=device, dtype=dtype).contiguous() for nm in names}
+
+
 def BoxQPFunction(eps=1e-12, verbose=0, notImprovedLim=3, maxIter=20, check_Q_spd=True, duals=False, dense_Q=False):
     """Factory with QPFunction's options; returns f(q, p, A, b, lb, ub) -> z (nBatch, nz).
 
@@ -290,8 +415,24 @@ def BoxQPFunction(eps=1e-12, verbose=0, notImprovedLim=3, maxIter=20, check_Q_sp
     read in full and enters as sym(dQ). Everything else is as above, with QPFunction's semantics on
     the dense equivalent (Q, G = [-I; I], h = [-lb; ub]): 'Q is not SPD.' where chol(Q) breaks down, the gradient
     dQ = 1/2 (dx z' + z dx') (the batch mean for an un-batched Q), and the tangent dQ enters forward mode as
-    sym(dQ) z. Shapes past the dense-Q kernels (qpb200_boxq_plan.ok) run the dense kernels on the dense equivalent."""
+    sym(dQ) z. Shapes past the dense-Q kernels (qpb200_boxq_plan.ok) run the dense kernels on the dense equivalent.
+
+    f.jacobian(wrt=None, duals=False) -> {name: tensor}: the whole Jacobians of the last forward's solution with respect
+    to p, lb, ub and b, per QP (also for an un-batched input: the true derivative, not a batch mean). wrt=None means
+    every input the problem has: p, the sides given, and b when neq > 0. J["p"] is (nBatch, nz, nz) = dz*/dp, J["lb"]
+    and J["ub"] (nBatch, nz, nz), J["b"] (nBatch, nz, neq); duals=True gives the rows [z; lam; nu] (lam in the
+    [lb rows; ub rows] layout, nu only when neq > 0). They are taken at the returned point with the backward's clamped
+    D = [d_lb; d_ub], so J t equals the forward-mode tangent of t: with H = Q + diag(d_lb + d_ub) and
+    X = [H A'; A 0]^-1, J_z,p = -X_zz, J_z,b = X_zn, J_z,lb = -J_z,p diag(d_lb), J_z,ub = -J_z,p diag(d_ub), and the
+    lam rows are d_lb o (rz_lb - z) and d_ub o (rz_ub + z) of the same column (rz_lb = e_j in lb column j, rz_ub = -e_j
+    in ub column j). One kernel call factors once per QP and solves for every column: with a diagonal q
+    (qpb200_box_jacobian) M = A H^-1 A', with a dense Q (qpb200_boxq_jacobian) the bordered [H A'; A 0] as the forward
+    does. Shapes whose factor or column buffers do not fit one CTA take one JVP per column, and the dense fallback the
+    dense path's jacobian. Jacobians with respect to q, Q and A are contractions of these:
+    J_.,q = J_.,p diag(z), J_.,Q_ik = J_.,p_i z_k (sym(dQ) enters), J_.,A_ck = J_.,p_k nu_c - J_.,b_c z_k. The result has
+    the dtype and device of the forward's output and is not differentiable."""
     _last = [None]
+    _jac = [None, None, None]            # the state, (device, dtype) and (nlb, has_ub) of the last forward
 
     class BoxQPFunctionFn(Function):
         @staticmethod
@@ -308,6 +449,7 @@ def BoxQPFunction(eps=1e-12, verbose=0, notImprovedLim=3, maxIter=20, check_Q_sp
             ctx.lams, ctx.slacks, ctx.nus = st.lam, st.slacks, st.nus
             ctx.out = (q_.device, q_.dtype)
             ctx.sides = (q_.size(-1) if lb_ is not None else 0, ub_ is not None)
+            _jac[:] = [st, ctx.out, ctx.sides]
             ctx.set_materialize_grads(False)
             if not duals:
                 return zhats
@@ -342,5 +484,9 @@ def BoxQPFunction(eps=1e-12, verbose=0, notImprovedLim=3, maxIter=20, check_Q_sp
     def apply(q, p, A, b, lb, ub):
         return BoxQPFunctionFn.apply(q, p, A, b, lb, ub)
 
+    def jacobian(wrt=None, duals=False):
+        return box_jacobian_of(_jac[0], _jac[1], _jac[2], wrt, duals)
+
     apply.last_solve = lambda: _last[0]
+    apply.jacobian = jacobian
     return apply

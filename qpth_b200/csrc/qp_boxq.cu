@@ -38,6 +38,7 @@
 #include "qp_pf.cuh"
 #include "qp_jvp.cuh"
 #include "qp_box_loop.cuh"
+#include "qp_jac.cuh"
 
 extern "C" int qpb200_internal_set_smem(const void* kernel, size_t bytes);   // (qp_kernels.cu) the kernels' smem limits
 // (qp_kernels.cu) out = scale / B (U^T X + Y^T V) by k_mean_outer: the batch mean of dQ for an un-batched Q
@@ -331,6 +332,102 @@ int boxq_launch(const char* what, void (*kernel)(KArgs...), const qpb200_boxq_pl
     return box_check_launch(what);
 }
 
+// ---- Jacobians of z*, lam, nu with respect to p, lb, ub, b (qpb200_boxq_jacobian) ----------------------------------
+// At the returned point with the backward's clamped D, X = K^-1 for K = [H A'; A 0], H = Q + G'DG: p column j is
+// -X e_j (z and nu rows), b column c is X e_(nz_pad + c), the lb / ub columns and the lam rows are scalings of them
+// (box_jac_store). One CTA per QP builds K's staircase with boxq_fill, factors it as the forward does (pf_chol_setup,
+// the trailing block negated, pf_chol: K = L diag(I, -I) L'), and then each warp sweeps whole 8-column blocks with
+// jac_ssolve_bordered: the forward sweep from the block of the right-hand side's unit rows, T_k' T_k, the trailing block
+// rows negated, the backward sweep. Shared memory: the staircase, panel, tile table, pf_chol's vector (N) and d; then
+// the warps' N x 8 buffers, where A is staged for boxq_fill before the factorization (the staircase holds A after it).
+struct BQDims {
+    int aug, blk, per, nblk;       // pf_chol's vector, the buffers (A staged there first), doubles per buffer, buffers
+    int64_t smem;                  // dynamic shared memory, bytes; 0: not covered
+};
+
+// the layout of k_boxq_jacobian: the QDims fields boxq_fill reads (S, pan, tab, d, A), and the buffers
+BQDims boxq_jac_dims(const qpb200_boxq_plan* p, QDims& D) {
+    D = QDims{};
+    D.n = p->nz; D.e = p->neq; D.np = r8(D.n); D.ep = r8(D.e); D.N = D.np + D.ep;
+    D.nlb = p->has_lb ? D.n : 0; D.m = (p->has_lb + p->has_ub) * D.n;
+    D.lda = D.n | 1;
+    const int nts = D.N >> 3;
+    BQDims J{};
+    int o = 0;
+    D.S = o; o += r8(pf_elems(nts));
+    D.pan = o; o += r8((8 * nts + 8) * kPanLd);
+    D.tab = o; o += r8(pf_tab_doubles(nts));
+    J.aug = o; o += D.N;
+    D.d = o; o += r8(D.m);
+    J.blk = D.A = o;
+    J.per = 8 * D.N;
+    const int64_t cap = kBoxMaxSmem / 8, a_end = (int64_t)J.blk + r8(D.e * D.lda);
+    int64_t nb = (cap - J.blk) / J.per;
+    if (nb > kBoxNT / 32) nb = kBoxNT / 32;
+    if (D.N > kBoxNT || a_end > cap || nb < 1) nb = 0;     // the factorization's order bound of qpb200_boxq_plan.ok
+    J.nblk = (int)nb;
+    const int64_t end = (int64_t)J.blk + nb * J.per;
+    J.smem = nb ? 8 * (end > a_end ? end : a_end) : 0;
+    return J;
+}
+
+__global__ void __launch_bounds__(kBoxNT, 1)
+k_boxq_jacobian(const __grid_constant__ QDims D, BQDims J, BOut O, const double* __restrict__ Q, int64_t sQ, const double* __restrict__ A,
+                int64_t sA, const double* __restrict__ lam, const double* __restrict__ slk, double* __restrict__ Jg) {
+    QPB_SMEM;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int64_t qp = blockIdx.x;
+    const int n = D.n, m = D.m, e = D.e, np = D.np, N = D.N, nts = N >> 3, ntz = np >> 3;
+    // ---- 1. d = clamp(lam, 1e-8) / clamp(s, 1e-8), A staged, K's staircase, K = L diag(I, -I) L'
+    for (int i = tid; i < m; i += kBoxNT) qsm[D.d + i] = fmax(lam[qp * m + i], 1e-8) / fmax(slk[qp * m + i], 1e-8);
+    if (e > 0) {
+        const double* Aq = A + qp * sA;
+        for (int t = tid; t < e * n; t += kBoxNT) {
+            const int i = t / n, j = t - i * n;
+            qsm[D.A + i * D.lda + j] = Aq[t];
+        }
+    }
+    for (int i = tid; i < N; i += kBoxNT) qsm[J.aug + i] = 0.0;
+    pf_build_tab(D.tab, nts);
+    __syncthreads();
+    boxq_fill(D, Q + qp * sQ, true, true, -1);
+    if (e > 0) {
+        pf_chol_setup(D.S, nts, 0, ntz, J.aug, D.pan, D.tab, nullptr, 0);   // L11, L21; -M in the trailing block
+        for (int t = tid; t < D.ep * D.ep; t += kBoxNT) {
+            const int r = np + t / D.ep, c = np + t % D.ep;
+            if (c <= r) qsm[D.S + pf_rowoff(r) + c] = -qsm[D.S + pf_rowoff(r) + c];
+        }
+        __syncthreads();
+        pf_chol(D.S, nts, ntz, J.aug, D.pan, D.tab);                        // L22
+    } else {
+        pf_chol(D.S, nts, 0, J.aug, D.pan, D.tab);
+    }
+    __syncthreads();
+    // ---- 2. column blocks: p blocks (which also give the lb and ub columns), then the b tiles, one warp per block
+    if (warp >= J.nblk) return;
+    double* X = qsm + J.blk + (int64_t)warp * J.per;
+    const double* dv = qsm + D.d;
+    const int npb = (O.cp >= 0 || O.clb >= 0 || O.cub >= 0) ? ntz : 0;
+    const int nblocks = npb + ((O.cb >= 0) ? (D.ep >> 3) : 0);
+    double* Jq = Jg + qp * (int64_t)O.R * O.C;
+#pragma unroll 1
+    for (int t = warp; t < nblocks; t += J.nblk) {
+        const bool pblk = t < npb;
+        const int j0 = 8 * (pblk ? t : t - npb), row0 = pblk ? j0 : np + j0;
+        // X = K^-1 E (p) or -K^-1 E (b): then U = X's z rows and Y = its nu rows are -z and -nu of the column
+        const double one = pblk ? 1.0 : -1.0;
+        for (int i = lane; i < 8 * N; i += 32) X[i] = ((i >> 3) == row0 + (i & 7)) ? one : 0.0;
+        __syncwarp();
+        jac_ssolve_bordered(qsm + D.S, nts, row0 >> 3, ntz, X);
+#pragma unroll 1
+        for (int kind = 0; kind < (pblk ? 3 : 1); ++kind) {
+            const int c0 = pblk ? (kind == 0 ? O.cp : (kind == 1 ? O.clb : O.cub)) : O.cb;
+            if (c0 >= 0) box_jac_store(Jq, O, n, D.nlb, m, e, dv, X, X + 8 * np, kind, c0 + j0, j0, min(8, (pblk ? n : e) - j0));
+        }
+        __syncwarp();
+    }
+}
+
 }  // namespace
 
 extern "C" {
@@ -430,6 +527,48 @@ int qpb200_boxq_solve_kkt(const qpb200_boxq_plan* plan, int nbatch, const double
     if (nbatch <= 0 || !Q || !d || !rx || !rs || !rz || !dx || !ds || !dz) return QPB200_ERR_BAD_ARG;
     if (plan->neq > 0 && (!A || !ry || !dy)) return QPB200_ERR_BAD_ARG;
     return boxq_launch("k_boxq_kkt", k_box_kkt<DenseQ>, plan, nbatch, stream, Q, sQ, A, sA, d, rx, rs, rz, ry, dx, ds, dz, dy);
+}
+
+
+int qpb200_boxq_jacobian_smem(const qpb200_boxq_plan* plan, int64_t* smem_bytes) {
+    if (!plan || !smem_bytes) return QPB200_ERR_BAD_ARG;
+    if (plan->nz <= 0 || plan->neq < 0 || plan->neq_pad != r8(plan->neq) ||
+        plan->nineq != (plan->has_lb + plan->has_ub) * plan->nz || plan->nineq <= 0)
+        return QPB200_ERR_BAD_ARG;
+    QDims D;
+    *smem_bytes = boxq_jac_dims(plan, D).smem;
+    return QPB200_OK;
+}
+
+int qpb200_boxq_jacobian(const qpb200_boxq_plan* plan, int nbatch, int rows, int cols, const double* Q, int64_t sQ,
+                         const double* A, int64_t sA, const double* lam, const double* slacks, double* J, void* stream) {
+    int64_t smem = 0;
+    int rc = qpb200_boxq_jacobian_smem(plan, &smem);
+    if (rc) return rc;
+    if (!Q || !lam || !slacks || !J || nbatch < 1 || sQ < 0 || sA < 0) return QPB200_ERR_BAD_ARG;
+    if (rows <= 0 || cols <= 0 || (rows & ~7) || (cols & ~15)) return QPB200_ERR_BAD_ARG;
+    if (plan->neq == 0 && ((rows & 4) || (cols & 8))) return QPB200_ERR_BAD_ARG;
+    if (plan->neq > 0 && !A) return QPB200_ERR_BAD_ARG;
+    if (((cols & 2) && !plan->has_lb) || ((cols & 4) && !plan->has_ub)) return QPB200_ERR_BAD_ARG;
+    if (smem == 0) return QPB200_ERR_TOO_LARGE;
+    QDims D;
+    const BQDims Jd = boxq_jac_dims(plan, D);
+    const int n = D.n, m = D.m, e = D.e;
+    BOut O;
+    int off = 0;
+    O.rz = (rows & 1) ? off : -1; off += (rows & 1) ? n : 0;
+    O.rl = (rows & 2) ? off : -1; off += (rows & 2) ? m : 0;
+    O.rn = (rows & 4) ? off : -1; off += (rows & 4) ? e : 0;
+    O.R = off; off = 0;
+    O.cp = (cols & 1) ? off : -1; off += (cols & 1) ? n : 0;
+    O.clb = (cols & 2) ? off : -1; off += (cols & 2) ? n : 0;
+    O.cub = (cols & 4) ? off : -1; off += (cols & 4) ? n : 0;
+    O.cb = (cols & 8) ? off : -1; off += (cols & 8) ? e : 0;
+    O.C = off;
+    rc = qpb200_internal_set_smem((const void*)k_boxq_jacobian, (size_t)Jd.smem);
+    if (rc) return rc;
+    k_boxq_jacobian<<<nbatch, kBoxNT, (size_t)Jd.smem, (cudaStream_t)stream>>>(D, Jd, O, Q, sQ, A, sA, lam, slacks, J);
+    return box_check_launch("k_boxq_jacobian");
 }
 
 }  // extern "C"

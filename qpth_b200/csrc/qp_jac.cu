@@ -1,4 +1,5 @@
-// qp_jac.cu - Jacobians of (z*, lam, nu) with respect to (p, h, b) at a returned point (qpb200_jacobian).
+// qp_jac.cu - Jacobians of (z*, lam, nu) with respect to (p, h, b) at a returned point (qpb200_jacobian), and of box QPs
+// with respect to (p, lb, ub, b) (qpb200_box_jacobian, below k_jacobian).
 //
 // The Jacobian is the negated inverse of the backward's symmetric system K = [Q 0 G' A'; 0 D I 0; G I 0 0; A 0 0 0],
 // D = clamp(lam, 1e-8) / clamp(s, 1e-8). In the whitened form of DESIGN section 3, with V = W L^-1 (L = chol(Q),
@@ -26,6 +27,7 @@
 // the device functions of the headers have external linkage (host stubs): give this build its own namespace
 #define qpb qpb_jac
 #include "qp_pf.cuh"
+#include "qp_jac.cuh"
 
 extern "C" int qpb200_internal_set_smem(const void* kernel, size_t bytes);   // (qp_kernels.cu) the kernels' smem limits
 extern "C" void qpb200_internal_cuda_error(int err, const char* what);     // (qp_kernels.cu) qpb200_last_cuda_error
@@ -158,105 +160,6 @@ __device__ __noinline__ void jac_ltsolve(const double* __restrict__ Lg, int n, i
     }
 }
 
-// Y = W U (ms_pad x 8; rows >= ms zero), W rows of stride ldw, columns < n read
-__device__ __noinline__ void jac_wu(const double* __restrict__ Wg, int ldw, int n, int ms, int nts, int np,
-                                   const double* U, double* Y) {
-    const int lane = threadIdx.x & 31, g = lane >> 2, q = lane & 3;
-#pragma unroll 1
-    for (int i = 0; i < nts; ++i) {
-        const int r = 8 * i + g;
-        const bool ok = r < ms;
-        const double* Wr = Wg + (int64_t)(ok ? r : 0) * ldw;
-        double c0 = 0.0, c1 = 0.0, e0 = 0.0, e1 = 0.0;       // two accumulator chains
-#pragma unroll 4
-        for (int k = 0; k < np; k += 8) {
-            const double a0 = (ok && k + q < n) ? Wr[k + q] : 0.0, a1 = (ok && k + q + 4 < n) ? Wr[k + q + 4] : 0.0;
-            dmma884(c0, c1, a0, U[(k + q) * 8 + g]);
-            dmma884(e0, e1, a1, U[(k + q + 4) * 8 + g]);
-        }
-        *reinterpret_cast<double2*>(Y + r * 8 + 2 * q) = make_double2(c0 + e0, c1 + e1);
-    }
-    __syncwarp();
-}
-
-// U -= W' Y (nz_pad x 8)
-__device__ __noinline__ void jac_u_minus_wty(const double* __restrict__ Wg, int ldw, int n, int ms, int ntz, int msp,
-                                            const double* Y, double* U) {
-    const int lane = threadIdx.x & 31, g = lane >> 2, q = lane & 3;
-#pragma unroll 1
-    for (int i = 0; i < ntz; ++i) {
-        const int cidx = 8 * i + g;                          // A[g][q] = W[k + q][cidx]
-        const bool ok = cidx < n;
-        double2 cv = *reinterpret_cast<const double2*>(U + cidx * 8 + 2 * q);
-        double e0 = 0.0, e1 = 0.0;
-#pragma unroll 4
-        for (int k = 0; k < msp; k += 8) {
-            const double a0 = (ok && k + q < ms) ? Wg[(int64_t)(k + q) * ldw + cidx] : 0.0;
-            const double a1 = (ok && k + q + 4 < ms) ? Wg[(int64_t)(k + q + 4) * ldw + cidx] : 0.0;
-            dmma884(cv.x, cv.y, -a0, Y[(k + q) * 8 + g]);
-            dmma884(e0, e1, -a1, Y[(k + q + 4) * 8 + g]);
-        }
-        *reinterpret_cast<double2*>(U + cidx * 8 + 2 * q) = make_double2(cv.x + e0, cv.y + e1);
-    }
-    __syncwarp();
-}
-
-// Y = S^-1 Y with the product-form factor at M (T_k on the diagonal tiles, P_ik below): Y's block rows < kf are zero.
-//     forward  Y_i -= P_ik Y_k (k ascending),  diagonal  Y_k = T_k' T_k Y_k,  backward  Y_k -= P_ik' Y_i (i descending)
-__device__ __noinline__ void jac_ssolve(const double* M, int nts, int kf, double* Y) {
-    const int lane = threadIdx.x & 31, g = lane >> 2, q = lane & 3;
-#pragma unroll 1
-    for (int k = kf; k < nts - 1; ++k) {
-        const int k0 = 8 * k;
-        const double b0 = Y[(k0 + q) * 8 + g], b1 = Y[(k0 + q + 4) * 8 + g];
-#pragma unroll 2
-        for (int i = k + 1; i < nts; ++i) {
-            const double* Pr = M + pf_rowoff(8 * i + g) + k0;
-            double2* cp = reinterpret_cast<double2*>(Y + (8 * i + g) * 8 + 2 * q);
-            double2 cv = *cp;
-            dmma884(cv.x, cv.y, -Pr[q], b0);
-            dmma884(cv.x, cv.y, -Pr[q + 4], b1);
-            *cp = cv;
-        }
-        __syncwarp();
-    }
-#pragma unroll 1
-    for (int k = kf; k < nts; ++k) {
-        const int k0 = 8 * k;
-        const double* Tg = M + pf_rowoff(k0 + g) + k0;       // row g of T_k (entries above the diagonal are not T)
-        double z0 = 0.0, z1 = 0.0;
-        dmma884(z0, z1, (q <= g) ? Tg[q] : 0.0, Y[(k0 + q) * 8 + g]);
-        dmma884(z0, z1, (q + 4 <= g) ? Tg[q + 4] : 0.0, Y[(k0 + q + 4) * 8 + g]);
-        __syncwarp();
-        *reinterpret_cast<double2*>(Y + (k0 + g) * 8 + 2 * q) = make_double2(z0, z1);
-        __syncwarp();
-        const double t0 = (g <= q) ? M[pf_rowoff(k0 + q) + k0 + g] : 0.0;          // T'[g][q] = T[q][g]
-        const double t1 = (g <= q + 4) ? M[pf_rowoff(k0 + q + 4) + k0 + g] : 0.0;
-        double c0 = 0.0, c1 = 0.0;
-        dmma884(c0, c1, t0, Y[(k0 + q) * 8 + g]);
-        dmma884(c0, c1, t1, Y[(k0 + q + 4) * 8 + g]);
-        __syncwarp();
-        *reinterpret_cast<double2*>(Y + (k0 + g) * 8 + 2 * q) = make_double2(c0, c1);
-    }
-    __syncwarp();
-#pragma unroll 1
-    for (int i = nts - 1; i > 0; --i) {
-        const int i0 = 8 * i;
-        const double b0 = Y[(i0 + q) * 8 + g], b1 = Y[(i0 + q + 4) * 8 + g];
-        const double* P0 = M + pf_rowoff(i0 + q) + g;        // A[g][q] = P_ik[q][g]
-        const double* P1 = M + pf_rowoff(i0 + q + 4) + g;
-#pragma unroll 2
-        for (int k = 0; k < i; ++k) {
-            double2* cp = reinterpret_cast<double2*>(Y + (8 * k + g) * 8 + 2 * q);
-            double2 cv = *cp;
-            dmma884(cv.x, cv.y, -P0[8 * k], b0);
-            dmma884(cv.x, cv.y, -P1[8 * k], b1);
-            *cp = cv;
-        }
-        __syncwarp();
-    }
-}
-
 // J rows [row0, row0 + cnt) <- -B[src0 + ..] (8 columns at column col0, the first ncol of them valid)
 __device__ __forceinline__ void jac_store(double* Jq, const JOut& O, int row0, int cnt, const double* B, int src0,
                                           int col0, int ncol) {
@@ -355,6 +258,137 @@ k_jacobian(JDims D, JOut O, const double* __restrict__ lam, const double* __rest
     }
 }
 
+// ---- BoxQPFunction, diagonal Q (qpb200_box_jacobian) -----------------------------------------------------------------
+// With Q = diag(q) and G = [-I; I] the inequality block is eliminated as in the box kernels: H = q + d_lb + d_ub
+// (diagonal), M = A H^-1 A' (order neq), and with K_b = [H A'; A 0]
+//     p block j:  U = H^-1 E_j, Y = M^-1 (A U),   z = -H^-1 (E_j - A'Y),   nu = -Y
+//     b block c:  Y = M^-1 E_c,                     z =  H^-1 A'Y,           nu = -Y
+// i.e. the steps of k_jacobian with W = A and L = H^(1/2), whose triangular solves become a diagonal scaling. The lb and
+// ub columns are the p columns scaled by -d_lb_j / -d_ub_j, and the lam rows d_lb o (rz_lb - z), d_ub o (rz_ub + z), so
+// they are written from the p blocks' solves (box_jac_store). One CTA of 256 threads per QP; A (row stride nz) is read
+// from global memory (L2); M's staircase, H^-1, d and the warps' column buffers (nz_pad x 8 and neq_pad x 8) live in
+// shared memory. It does not use the forward's layout: any box plan whose buffers fit is covered.
+struct BDims {
+    int n, m, e, ep, nlb, nts, np, ntz;       // nz, nineq, neq, neq_pad, nz if lb given else 0, neq_pad / 8, nz_pad, / 8
+    int pan, tab, aug, hv, dv, blk, per;      // M at 0; panel, tile table, pf_chol's vector, H^-1, d, buffers
+    int nblk;                                 // column blocks in flight, 0: not covered
+    int64_t smem;                             // dynamic shared memory, bytes
+};
+
+BDims box_jac_dims(const qpb200_box_plan* p) {
+    BDims D{};
+    D.n = p->nz; D.m = p->nineq; D.e = p->neq; D.ep = p->neq_pad; D.nlb = p->has_lb ? p->nz : 0;
+    D.nts = D.ep >> 3; D.np = (D.n + 7) & ~7; D.ntz = D.np >> 3;
+    D.pan = pf_elems(D.nts);
+    D.tab = D.pan + (8 * D.nts + 8) * kPanLd;
+    D.aug = D.tab + ((pf_tab_doubles(D.nts) + 7) & ~7);
+    D.hv = D.aug + 8 * D.nts;
+    D.dv = D.hv + D.np;
+    D.blk = D.dv + ((D.m + 7) & ~7);
+    D.per = 8 * (D.np + D.ep);
+    const int64_t left = kJacMaxSmem - 8 * (int64_t)D.blk;
+    int64_t nb = left > 0 ? left / (8 * (int64_t)D.per) : 0;
+    if (nb > kNT / 32) nb = kNT / 32;
+    D.nblk = (int)nb;
+    D.smem = D.nblk ? 8 * ((int64_t)D.blk + (int64_t)D.nblk * D.per) : 0;
+    return D;
+}
+
+__global__ void __launch_bounds__(kNT, 1)
+k_box_jacobian(BDims D, BOut O, const double* __restrict__ q, int64_t sq, const double* __restrict__ A, int64_t sA,
+               const double* __restrict__ lam, const double* __restrict__ slk, double* __restrict__ J) {
+    QPB_SMEM;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int g = lane >> 2, q4 = lane & 3;
+    const int64_t qp = blockIdx.x;
+    const int n = D.n, m = D.m, e = D.e, nts = D.nts, np = D.np;
+    const double* qv = q + qp * sq;
+    const double* Ag = (e > 0) ? A + qp * sA : nullptr;
+    double* hv = qsm + D.hv;
+    double* dv = qsm + D.dv;
+    // ---- 1. d = clamp(lam, 1e-8) / clamp(s, 1e-8) as the backward forms it, H^-1 (0 past nz)
+    for (int i = tid; i < m; i += kNT) dv[i] = fmax(lam[qp * m + i], 1e-8) / fmax(slk[qp * m + i], 1e-8);
+    __syncthreads();
+    for (int j = tid; j < np; j += kNT) {
+        double h = 0.0;
+        if (j < n) {
+            h = qv[j];
+            if (D.nlb) h += dv[j];
+            if (m > D.nlb) h += dv[D.nlb + j];
+            h = 1.0 / h;
+        }
+        hv[j] = h;
+    }
+    __syncthreads();
+    // ---- 2. M = A H^-1 A' (identity past neq) -> staircase (lower tiles), M = L_M L_M' in product form
+    if (e > 0) {
+        const int T2 = nts * (nts + 1) / 2;
+#pragma unroll 1
+        for (int t = warp; t < T2; t += kNT / 32) {
+            int ti = (int)((sqrtf(8.0f * (float)t + 1.0f) - 1.0f) * 0.5f);
+            while (ti * (ti + 1) / 2 > t) --ti;
+            while ((ti + 1) * (ti + 2) / 2 <= t) ++ti;
+            const int tj = t - ti * (ti + 1) / 2;
+            const int ra = 8 * ti + g, rb = 8 * tj + g;
+            const bool oka = ra < e, okb = rb < e;
+            const double* pa = Ag + (int64_t)(oka ? ra : 0) * n;
+            const double* pb = Ag + (int64_t)(okb ? rb : 0) * n;
+            double c0 = 0.0, c1 = 0.0, e0 = 0.0, e1 = 0.0;   // two accumulator chains
+#pragma unroll 4
+            for (int kk = 0; kk < np; kk += 8) {
+                const bool k0 = kk + q4 < n, k1 = kk + q4 + 4 < n;
+                dmma884(c0, c1, (oka && k0) ? pa[kk + q4] * hv[kk + q4] : 0.0, (okb && k0) ? pb[kk + q4] : 0.0);
+                dmma884(e0, e1, (oka && k1) ? pa[kk + q4 + 4] * hv[kk + q4 + 4] : 0.0, (okb && k1) ? pb[kk + q4 + 4] : 0.0);
+            }
+            const int rr = 8 * ti + g, cc = 8 * tj + 2 * q4;
+            double v0 = c0 + e0, v1 = c1 + e1;
+            if (rr >= e) {                                   // padding rows: identity
+                if (rr == cc) v0 = 1.0;
+                if (rr == cc + 1) v1 = 1.0;
+            }
+            *reinterpret_cast<double2*>(qsm + pf_rowoff(rr) + cc) = make_double2(v0, v1);
+        }
+        for (int i = tid; i < 8 * nts; i += kNT) qsm[D.aug + i] = 0.0;
+        pf_build_tab(D.tab, nts);
+        __syncthreads();
+        pf_chol(0, nts, 0, D.aug, D.pan, D.tab);
+        __syncthreads();
+    }
+    // ---- 3. column blocks: p blocks (which also give the lb and ub columns), then the b tiles, one warp per block
+    if (warp >= D.nblk) return;
+    double* U = qsm + D.blk + (int64_t)warp * D.per;
+    double* Y = U + 8 * np;
+    const int npb = (O.cp >= 0 || O.clb >= 0 || O.cub >= 0) ? D.ntz : 0;
+    const int nblocks = npb + ((O.cb >= 0) ? nts : 0);
+    double* Jq = J + qp * (int64_t)O.R * O.C;
+#pragma unroll 1
+    for (int t = warp; t < nblocks; t += D.nblk) {
+        const bool pblk = t < npb;
+        const int j0 = 8 * (pblk ? t : t - npb);
+        if (pblk) {                                          // Y = A H^-1 E_t, then U = E_t
+            for (int i = lane; i < 8 * np; i += 32) U[i] = ((i >> 3) == j0 + (i & 7)) ? hv[i >> 3] : 0.0;
+            __syncwarp();
+            jac_wu(Ag, n, n, e, nts, np, U, Y);
+            for (int i = lane; i < 8 * np; i += 32) U[i] = ((i >> 3) == j0 + (i & 7)) ? 1.0 : 0.0;
+        } else {                                             // U = 0, Y = E_c
+            for (int i = lane; i < 8 * np; i += 32) U[i] = 0.0;
+            for (int i = lane; i < 8 * D.ep; i += 32) Y[i] = ((i >> 3) == j0 + (i & 7)) ? 1.0 : 0.0;
+        }
+        __syncwarp();
+        jac_ssolve(qsm, nts, pblk ? 0 : (j0 >> 3), Y);
+        jac_u_minus_wty(Ag, n, n, e, D.ntz, D.ep, Y, U);
+        for (int i = lane; i < 8 * np; i += 32) U[i] *= hv[i >> 3];
+        __syncwarp();
+        // a p block: its p, lb and ub columns (kind 0, 1, 2); a b tile: its b columns
+#pragma unroll 1
+        for (int kind = 0; kind < (pblk ? 3 : 1); ++kind) {
+            const int c0 = pblk ? (kind == 0 ? O.cp : (kind == 1 ? O.clb : O.cub)) : O.cb;
+            if (c0 >= 0) box_jac_store(Jq, O, D.n, D.nlb, D.m, D.e, dv, U, Y, kind, c0 + j0, j0, min(8, (pblk ? n : e) - j0));
+        }
+        __syncwarp();
+    }
+}
+
 }  // namespace
 
 extern "C" {
@@ -389,6 +423,46 @@ int qpb200_jacobian(const qpb200_plan* plan, int nbatch, int rows, int cols, con
     k_jacobian<<<nbatch, kNT, (size_t)D.smem, (cudaStream_t)stream>>>(D, O, lam, slacks, Lfac, Wfac, sF, J);
     const cudaError_t err = cudaGetLastError();
     if (err != cudaSuccess) { qpb200_internal_cuda_error((int)err, "k_jacobian"); return QPB200_ERR_CUDA; }
+    return QPB200_OK;
+}
+
+int qpb200_box_jacobian_smem(const qpb200_box_plan* plan, int64_t* smem_bytes) {
+    if (!plan || !smem_bytes) return QPB200_ERR_BAD_ARG;
+    if (plan->nz <= 0 || plan->neq < 0 || plan->neq_pad != ((plan->neq + 7) & ~7) ||
+        plan->nineq != (plan->has_lb + plan->has_ub) * plan->nz || plan->nineq <= 0)
+        return QPB200_ERR_BAD_ARG;
+    *smem_bytes = box_jac_dims(plan).smem;
+    return QPB200_OK;
+}
+
+int qpb200_box_jacobian(const qpb200_box_plan* plan, int nbatch, int rows, int cols, const double* q, int64_t sq,
+                        const double* A, int64_t sA, const double* lam, const double* slacks, double* J, void* stream) {
+    int64_t smem = 0;
+    int rc = qpb200_box_jacobian_smem(plan, &smem);
+    if (rc) return rc;
+    if (!q || !lam || !slacks || !J || nbatch < 1 || sq < 0 || sA < 0) return QPB200_ERR_BAD_ARG;
+    if (rows <= 0 || cols <= 0 || (rows & ~7) || (cols & ~15)) return QPB200_ERR_BAD_ARG;
+    if (plan->neq == 0 && ((rows & 4) || (cols & 8))) return QPB200_ERR_BAD_ARG;
+    if (plan->neq > 0 && !A) return QPB200_ERR_BAD_ARG;
+    if (((cols & 2) && !plan->has_lb) || ((cols & 4) && !plan->has_ub)) return QPB200_ERR_BAD_ARG;
+    if (smem == 0) return QPB200_ERR_TOO_LARGE;
+    const BDims D = box_jac_dims(plan);
+    BOut O;
+    int off = 0;
+    O.rz = (rows & 1) ? off : -1; off += (rows & 1) ? D.n : 0;
+    O.rl = (rows & 2) ? off : -1; off += (rows & 2) ? D.m : 0;
+    O.rn = (rows & 4) ? off : -1; off += (rows & 4) ? D.e : 0;
+    O.R = off; off = 0;
+    O.cp = (cols & 1) ? off : -1; off += (cols & 1) ? D.n : 0;
+    O.clb = (cols & 2) ? off : -1; off += (cols & 2) ? D.n : 0;
+    O.cub = (cols & 4) ? off : -1; off += (cols & 4) ? D.n : 0;
+    O.cb = (cols & 8) ? off : -1; off += (cols & 8) ? D.e : 0;
+    O.C = off;
+    rc = qpb200_internal_set_smem((const void*)k_box_jacobian, (size_t)D.smem);
+    if (rc) return rc;
+    k_box_jacobian<<<nbatch, kNT, (size_t)D.smem, (cudaStream_t)stream>>>(D, O, q, sq, A, sA, lam, slacks, J);
+    const cudaError_t err = cudaGetLastError();
+    if (err != cudaSuccess) { qpb200_internal_cuda_error((int)err, "k_box_jacobian"); return QPB200_ERR_CUDA; }
     return QPB200_OK;
 }
 

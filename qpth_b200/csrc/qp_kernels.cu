@@ -1225,7 +1225,7 @@ int qpb200_internal_mean_outer(int B, int rows, int cols, const double* u, const
     return QPB200_OK;
 }
 
-int qpb200_version(void) { return 101; }
+int qpb200_version(void) { return 102; }
 
 const char* qpb200_error_string(int code) {
     switch (code) {
