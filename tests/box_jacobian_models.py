@@ -10,6 +10,8 @@ blocked_box_jacobian: the arithmetic of qpb200_box_jacobian (csrc/qp_jac.cu, dia
     with the lb / ub columns the p columns scaled by -d_lb_j / -d_ub_j and the lam rows d_lb o (rz_lb - z),
     d_ub o (rz_ub + z) (rz_lb = e_j in lb column j, rz_ub = -e_j in ub column j).
 Both return rows [z; lam; nu] and columns [p, lb, ub, b] (the sides given; b only when neq > 0).
+diagonal_box_jacobian: a diagonal q and no equality rows, one long-double KKT block per variable (the reference at
+    widths whose dense model is too large to form).
 """
 import numpy as np
 
@@ -174,6 +176,46 @@ def dense_box_jacobian_refined(Q, A, lam, s, nlb, has_ub, steps=3):
     Jd = np.concatenate([-R[rows][:, :n], R[rows][:, n + m:n + 2 * m], R[rows][:, n + 2 * m:]], axis=1)
     cols = [Jd[:, :n]] + ([-Jd[:, n:n + nlb]] if nlb else []) + ([Jd[:, n + nlb:n + m]] if has_ub else [])
     return np.concatenate(cols + ([Jd[:, n + m:]] if e else []), axis=1)
+
+
+def diagonal_box_jacobian(q, lam, s, nlb, has_ub):
+    """dense_box_jacobian of a diagonal q without equality rows, from one KKT block per variable: with A empty the
+    backward's system decouples into [q_j 0 g'; 0 D_j I; g I 0] over (z_j, the slacks and the duals of its sides),
+    g = -1 for lb and +1 for ub. Each block (order 3 or 5) is inverted by Gauss-Jordan elimination in np.longdouble
+    (pivots q_j, d, then the negative definite -(g g' / q_j + D_j^-1): no pivoting needed), and J is assembled from them:
+    rows [z; lam], columns [p, lb, ub] of the sides given. The reference for widths whose dense model is too large."""
+    n = q.shape[0]
+    sides = ([-1.0] if nlb else []) + ([1.0] if has_ub else [])
+    k = len(sides)
+    d = jm.clamped_d(lam, s).astype(np.longdouble).reshape(k, n).T            # (n, k): d of variable j's sides
+    o = 1 + 2 * k
+    K = np.zeros((n, o, o), dtype=np.longdouble)
+    K[:, 0, 0] = q
+    for a, g in enumerate(sides):
+        K[:, 0, 1 + k + a] = K[:, 1 + k + a, 0] = g
+        K[:, 1 + a, 1 + a] = d[:, a]
+        K[:, 1 + a, 1 + k + a] = K[:, 1 + k + a, 1 + a] = 1.0
+    R = np.broadcast_to(np.eye(o, dtype=np.longdouble), (n, o, o)).copy()
+    for c in range(o):
+        piv = K[:, c, c].copy()
+        K[:, c] /= piv[:, None]
+        R[:, c] /= piv[:, None]
+        for r in range(o):
+            if r != c:
+                f = K[:, r, c].copy()
+                K[:, r] -= f[:, None] * K[:, c]
+                R[:, r] -= f[:, None] * R[:, c]
+    R = R.astype(np.float64)
+    m = k * n
+    J = np.zeros((n + m, n * (1 + k)))
+    j = np.arange(n)
+    rows = [j] + [n + a * n + j for a in range(k)]                             # z_j, then lam_j of each side
+    for ri, r in enumerate(rows):
+        slot = 0 if ri == 0 else 1 + k + (ri - 1)
+        J[r, j] = -R[:, slot, 0]                                               # p: -R_.,x
+        for a, g in enumerate(sides):                                          # h: R_.,(G x + s) of that side,
+            J[r, n + a * n + j] = g * R[:, slot, 1 + k + a]                    # lb = -h, ub = h
+    return J
 
 
 def split(J, n, m, e, nlb, has_ub):
