@@ -305,6 +305,55 @@ int qpb200_jvp_reg(const qpb200_plan* plan, int nbatch,
                    double* rhs, double* dz, double* dlam, double* dnu,
                    double* scratch, void* stream);
 
+/* Double backward (an extension): the derivative of phi = sum_X <w_X, grad_X> for cotangents w_X on the six outputs
+ * grad_X of qpb200_backward_duals, with respect to its adjoints (g_z, g_lam, g_nu) and to Q, p, G, h, A, b, treating
+ * that backward as computed (the 1e-8 clamps of D included). v = (dxv, dlamv, dnuv) is the first backward's solve at
+ * the same point. The call runs
+ *   1. qpb200_jvp with tangents w_X: u = (gg_z, gg_lam, gg_nu), the gradients of g_z, g_lam and g_nu;
+ *   2. a kernel forming the cotangents of the solution, cz = sym(wQ) vx + wG' vlam + wA' vnu - G' c_s,
+ *      clam = wG vx + c_lam, cnu = wA vx, from the cotangent c_D = (ulam / D)(vlam / D) of D = clamp(lam) / clamp(s):
+ *      c_lam = c_D / clamp(s) where lam >= 1e-8, c_s = -c_D D / clamp(s) where s >= 1e-8 (0 elsewhere; s = h - G z);
+ *   3. qpb200_backward_duals with (cz, clam, cnu): w = (wx, wlam, wnu);
+ *   4. a kernel writing dQ = sym(wx z' + ux vx'), dp = wx, dG = (wlam - c_s) z' + lam wx' + vlam ux' + ulam vx',
+ *      dh = c_s - wlam, dA = wnu z' + nu wx' + vnu ux' + unu vx', db = -wnu.
+ * w_X: pointer and batch stride in elements (0: one cotangent for every QP); each may be NULL (zero), wG and wh must be
+ * NULL when nineq == 0 and wA, wb when neq == 0. G (stride sG) is the constraint matrix of the forward. The cotangent of
+ * a batch-mean gradient (an un-batched input) is the caller's w_X / nbatch. dQ .. db may be NULL (skipped); sum_X = 1
+ * writes the batch sum (one un-batched tensor, the exact derivative for an un-batched input), 0 the per-QP gradients.
+ * gg_z (B,nz), gg_lam (B,nineq), gg_nu (B,neq) are always written. work: QPB200_DOUBLE_BACKWARD_WORK doubles. Arguments
+ * are checked as qpb200_jvp checks them, before anything is launched. */
+#define QPB200_DOUBLE_BACKWARD_WORK(nbatch, nz, nineq, neq) \
+    ((int64_t)(nbatch) * (2 * (int64_t)(nz) + 3 * (int64_t)(nineq) + 2 * (int64_t)(neq)))
+int qpb200_double_backward(const qpb200_plan* plan, int nbatch,
+                           const double* wQ, int64_t swQ, const double* wp, int64_t swp,
+                           const double* wG, int64_t swG, const double* wh, int64_t swh,
+                           const double* wA, int64_t swA, const double* wb, int64_t swb,
+                           const double* G, int64_t sG,
+                           const double* dxv, const double* dlamv, const double* dnuv,
+                           const double* zhat, const double* lam, const double* slacks, const double* nus,
+                           const double* Lfac, const double* Wfac, const double* Kfac, int sF,
+                           double* gg_z, double* gg_lam, double* gg_nu,
+                           double* dQ, int sum_Q, double* dp, int sum_p,
+                           double* dG, int sum_G, double* dh, int sum_h,
+                           double* dA, int sum_A, double* db, int sum_b,
+                           double* work, double* scratch, void* stream);
+/* qpb200_double_backward for the regularised mode: qpb200_jvp_reg and qpb200_backward_reg_duals with their ir_steps
+ * refinement steps (plan, reg_eps and ir_steps as there). */
+int qpb200_double_backward_reg(const qpb200_plan* plan, int nbatch,
+                               const double* wQ, int64_t swQ, const double* wp, int64_t swp,
+                               const double* wG, int64_t swG, const double* wh, int64_t swh,
+                               const double* wA, int64_t swA, const double* wb, int64_t swb,
+                               const double* G, int64_t sG,
+                               const double* dxv, const double* dlamv, const double* dnuv,
+                               const double* zhat, const double* lam, const double* slacks, const double* nus,
+                               const double* Lfac, const double* Wfac, const double* Kfac, int sF,
+                               double reg_eps, int ir_steps,
+                               double* gg_z, double* gg_lam, double* gg_nu,
+                               double* dQ, int sum_Q, double* dp, int sum_p,
+                               double* dG, int sum_G, double* dh, int sum_h,
+                               double* dA, int sum_A, double* db, int sum_b,
+                               double* work, double* scratch, void* stream);
+
 /* Jacobians at the returned point (an extension): d(z*, lam, nu)/d(p, h, b) for every QP of the batch, the negated
  * inverse of the backward's system [Q 0 G' A'; 0 D I 0; G I 0 0; A 0 0 0] with D = clamp(lam, 1e-8) / clamp(s, 1e-8):
  *   J_z,p = -R_xx, J_z,h = R_x,lam, J_z,b = R_x,nu (likewise for the lam and nu rows), R = that matrix's inverse.

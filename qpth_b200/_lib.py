@@ -82,6 +82,12 @@ SIGNATURES = {
                         _P, _P, _P, _P, _P, _P, _P, _I, _P, _P, _P, _P, _P, _P]),
     "qpb200_jvp_reg": (_I, [ctypes.POINTER(Plan), _I, _P, _L, _P, _L, _P, _L, _P, _L, _P, _L, _P, _L,
                             _P, _P, _P, _P, _P, _P, _P, _I, _D, _I, _P, _P, _P, _P, _P, _P]),
+    "qpb200_double_backward": (_I, [ctypes.POINTER(Plan), _I, _P, _L, _P, _L, _P, _L, _P, _L, _P, _L, _P, _L, _P, _L,
+                                    _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _I, _P, _P, _P,
+                                    _P, _I, _P, _I, _P, _I, _P, _I, _P, _I, _P, _I, _P, _P, _P]),
+    "qpb200_double_backward_reg": (_I, [ctypes.POINTER(Plan), _I, _P, _L, _P, _L, _P, _L, _P, _L, _P, _L, _P, _L,
+                                        _P, _L, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _I, _D, _I, _P, _P, _P,
+                                        _P, _I, _P, _I, _P, _I, _P, _I, _P, _I, _P, _I, _P, _P, _P]),
     "qpb200_jacobian_smem": (_I, [ctypes.POINTER(Plan), _P]),
     "qpb200_jacobian": (_I, [ctypes.POINTER(Plan), _I, _I, _I, _P, _P, _P, _P, _I, _P, _P]),
     "qpb200_optnet_construct": (_I, [_I, _I, _P, _P, _P, _P, _D, _P, _P, _P]),

@@ -860,6 +860,197 @@ k_jvp_rhs(int n, int m, int e, const double* __restrict__ dQ, int64_t sdQ, const
     for (int i = tid; i < e; i += kThreads) ry[qp * e + i] = ay[i];
 }
 
+// Double backward (qpb200_double_backward). The first backward solved K v = -[g_z; 0; g_lam; g_nu]; v = (vx, vlam, vnu)
+// are its dxv, dlamv, dnuv. With cotangents w_X on its six outputs, u = (ux, ulam, unu) is the JVP of the solution for
+// tangents w_X (the gradient of g), and k_ggrad_rhs forms the cotangents of the solution (z, lam, nu) that go through the
+// dual backward:
+//   cz = sym(wQ) vx + wG' vlam + wA' vnu - G' c_s,   clam = wG vx + c_lam,   cnu = wA vx,
+// where c_D = (ulam / D)(vlam / D) is the cotangent of D = clamp(lam) / clamp(s) (1e-8 clamps) and
+//   c_lam = c_D / clamp(s) where lam >= 1e-8 (else 0),   c_s = -c_D D / clamp(s) where s >= 1e-8 (else 0)
+// (torch's clamp passes the gradient at the bound). c_s is also written: s = h - G z, so it enters h and G. Each of wQ,
+// wG, wA and G is read once with jvp::contract (row and column pass together). Shared memory: vx and cz (n), one m
+// buffer holding c_s during the G pass and vlam after it, the clam accumulator (m), vnu and cnu (e), and the column
+// partials: the layout of k_jvp_rhs, jvp_smem_bytes(n, m, e), 200 KB at n = m = e = 4096.
+// Algorithmic bytes per QP: 8 (n^2 + 2 m n + e n) of matrices, 8 (n + 5 m + e) of vectors read, 8 (n + 2 m + e) written.
+__global__ void __launch_bounds__(kThreads)
+k_ggrad_rhs(int n, int m, int e, const double* __restrict__ wQ, int64_t swQ, const double* __restrict__ wG,
+            int64_t swG, const double* __restrict__ wA, int64_t swA, const double* __restrict__ G, int64_t sG,
+            const double* __restrict__ dxv, const double* __restrict__ dlamv, const double* __restrict__ dnuv,
+            const double* __restrict__ ulam, const double* __restrict__ lam, const double* __restrict__ slacks,
+            double* __restrict__ cz, double* __restrict__ clam, double* __restrict__ cnu, double* __restrict__ cs) {
+    QPB_SMEM;
+    const int64_t qp = blockIdx.x;
+    const int tid = threadIdx.x;
+    double* vx = qsm;
+    double* az = vx + jvp_r8(n);
+    double* r1 = az + jvp_r8(n);        // c_s, then vlam
+    double* al = r1 + jvp_r8(m);
+    double* vn = al + jvp_r8(m);
+    double* an = vn + jvp_r8(e);
+    double* part = an + jvp_r8(e);
+    for (int i = tid; i < n; i += kThreads) {
+        vx[i] = dxv[qp * n + i];
+        az[i] = 0.0;
+    }
+    for (int i = tid; i < m; i += kThreads) {
+        const double l = lam[qp * m + i], s = slacks[qp * m + i];
+        const double sc = fmax(s, 1e-8), d = fmax(l, 1e-8) / sc;
+        const double cd = (ulam[qp * m + i] / d) * (dlamv[qp * m + i] / d);
+        al[i] = l >= 1e-8 ? cd / sc : 0.0;
+        const double c = s >= 1e-8 ? -cd * d / sc : 0.0;
+        r1[i] = c;
+        cs[qp * m + i] = c;
+    }
+    for (int i = tid; i < e; i += kThreads) {
+        vn[i] = dnuv[qp * e + i];
+        an[i] = 0.0;
+    }
+    __syncthreads();
+    if (m > 0) {
+        jvp::contract<kThreads>(G + qp * sG, m, n, vx, r1, part, [&](int, double) {},
+                                [&](int c, double s) { az[c] -= s; });
+        for (int i = tid; i < m; i += kThreads) r1[i] = dlamv[qp * m + i];
+        __syncthreads();
+    }
+    if (wG && m > 0)
+        jvp::contract<kThreads>(wG + qp * swG, m, n, vx, r1, part, [&](int r, double s) { al[r] += s; },
+                                [&](int c, double s) { az[c] += s; });
+    if (wA && e > 0)
+        jvp::contract<kThreads>(wA + qp * swA, e, n, vx, vn, part, [&](int r, double s) { an[r] += s; },
+                                [&](int c, double s) { az[c] += s; });
+    if (wQ)
+        jvp::contract<kThreads>(wQ + qp * swQ, n, n, vx, vx, part, [&](int r, double s) { az[r] += 0.5 * s; },
+                                [&](int c, double s) { az[c] += 0.5 * s; });
+    __syncthreads();
+    for (int i = tid; i < n; i += kThreads) cz[qp * n + i] = az[i];
+    for (int i = tid; i < m; i += kThreads) clam[qp * m + i] = al[i];
+    for (int i = tid; i < e; i += kThreads) cnu[qp * e + i] = an[i];
+}
+
+// The second-order gradients from the three solves: v (first backward), u (JVP, the gradient of g), w (dual backward
+// with k_ggrad_rhs's cotangents), and c_s, with t = wlam - c_s:
+//   dQ = sym(wx z' + ux vx'),   dp = wx,   dG = t z' + lam wx' + vlam ux' + ulam vx',   dh = -t,
+//   dA = wnu z' + nu wx' + vnu ux' + unu vx',   db = -wnu.
+// Every term is rounded on its own and the four added as (a + b) + (c + d), so dQ is symmetric bit for bit.
+struct GgTerms {
+    const double *z, *lam, *nu, *vx, *vl, *vn, *ux, *ul, *un, *wx, *wl, *wn, *cs;
+};
+__device__ __forceinline__ double gg4(double a0, double b0, double a1, double b1, double a2, double b2, double a3,
+                                      double b3) {
+    return __dadd_rn(__dadd_rn(__dmul_rn(a0, b0), __dmul_rn(a1, b1)), __dadd_rn(__dmul_rn(a2, b2), __dmul_rn(a3, b3)));
+}
+
+// Per-QP gradients (an output is NULL here when it is not wanted or is reduced over the batch by k_ggrad_sum*): one
+// pass over each, QP blockIdx.x, its elements strided over blockIdx.y and the threads. The vectors are read through L1.
+struct GgOut { double *dQ, *dp, *dG, *dh, *dA, *db; };
+__global__ void __launch_bounds__(256)
+k_ggrad_out(int n, int m, int e, GgTerms T, GgOut O) {
+    const int64_t qp = blockIdx.x;
+    const int64_t i0 = (int64_t)blockIdx.y * blockDim.x + threadIdx.x, step = (int64_t)gridDim.y * blockDim.x;
+    const double* z = T.z + qp * n;
+    const double* vx = T.vx + qp * n;
+    const double* ux = T.ux + qp * n;
+    const double* wx = T.wx + qp * n;
+    if (O.dQ) {
+        double* o = O.dQ + qp * n * n;
+        for (int64_t i = i0; i < (int64_t)n * n; i += step) {
+            const int r = (int)(i / n), c = (int)(i - (int64_t)r * n);
+            o[i] = 0.5 * gg4(wx[r], z[c], z[r], wx[c], ux[r], vx[c], vx[r], ux[c]);
+        }
+    }
+    if (O.dp) for (int64_t i = i0; i < n; i += step) O.dp[qp * n + i] = wx[i];
+    if (m > 0) {
+        const double* l = T.lam + qp * m;
+        const double* vl = T.vl + qp * m;
+        const double* ul = T.ul + qp * m;
+        const double* wl = T.wl + qp * m;
+        const double* cs = T.cs + qp * m;
+        if (O.dG) {
+            double* o = O.dG + qp * m * n;
+            for (int64_t i = i0; i < (int64_t)m * n; i += step) {
+                const int r = (int)(i / n), c = (int)(i - (int64_t)r * n);
+                o[i] = gg4(wl[r] - cs[r], z[c], l[r], wx[c], vl[r], ux[c], ul[r], vx[c]);
+            }
+        }
+        if (O.dh) for (int64_t i = i0; i < m; i += step) O.dh[qp * m + i] = cs[i] - wl[i];
+    }
+    if (e > 0) {
+        const double* nu = T.nu + qp * e;
+        const double* vn = T.vn + qp * e;
+        const double* un = T.un + qp * e;
+        const double* wn = T.wn + qp * e;
+        if (O.dA) {
+            double* o = O.dA + qp * e * n;
+            for (int64_t i = i0; i < (int64_t)e * n; i += step) {
+                const int r = (int)(i / n), c = (int)(i - (int64_t)r * n);
+                o[i] = gg4(wn[r], z[c], nu[r], wx[c], vn[r], ux[c], un[r], vx[c]);
+            }
+        }
+        if (O.db) for (int64_t i = i0; i < e; i += step) O.db[qp * e + i] = -wn[i];
+    }
+}
+
+// Batch sums for un-batched inputs (the exact derivative of the first backward's batch mean), in the style of
+// k_mean_outer: out[r][c] = scale sum_b sum_k u_k[b][r] x_k[b][c], four (u, x) pairs, u_0 - usub in place of u_0 where
+// usub is given. One CTA per 32 x 64 tile, the batch walked in chunks of 8 QPs in ascending order: a fixed summation
+// order, so the result does not depend on the launch.
+constexpr int kGsB = 8;
+struct GgPairs { const double* u[4]; const double* x[4]; const double* usub; };
+__global__ void __launch_bounds__(256)
+k_ggrad_sum(int B, int rows, int cols, GgPairs P, double scale, double* __restrict__ out) {
+    __shared__ double su[4][kGsB][kMoR], sx[4][kGsB][kMoC];
+    const int tid = threadIdx.x;
+    const int r0 = blockIdx.y * kMoR, c0 = blockIdx.x * kMoC;
+    const int tr = (tid >> 4) * 2, tc = (tid & 15) * 4;
+    double acc[2][4] = {{0.0, 0.0, 0.0, 0.0}, {0.0, 0.0, 0.0, 0.0}};
+    for (int b0 = 0; b0 < B; b0 += kGsB) {
+        for (int i = tid; i < kGsB * kMoR; i += 256) {
+            const int bb = i / kMoR, rr = i - bb * kMoR;
+            const bool ok = (b0 + bb < B) && (r0 + rr < rows);
+            const int64_t at = (int64_t)(b0 + bb) * rows + r0 + rr;
+#pragma unroll
+            for (int k = 0; k < 4; ++k) su[k][bb][rr] = ok ? P.u[k][at] : 0.0;
+            if (ok && P.usub) su[0][bb][rr] -= P.usub[at];
+        }
+        for (int i = tid; i < kGsB * kMoC; i += 256) {
+            const int bb = i / kMoC, cc = i - bb * kMoC;
+            const bool ok = (b0 + bb < B) && (c0 + cc < cols);
+            const int64_t at = (int64_t)(b0 + bb) * cols + c0 + cc;
+#pragma unroll
+            for (int k = 0; k < 4; ++k) sx[k][bb][cc] = ok ? P.x[k][at] : 0.0;
+        }
+        __syncthreads();
+        for (int bb = 0; bb < kGsB; ++bb) {
+#pragma unroll
+            for (int i = 0; i < 2; ++i)
+#pragma unroll
+                for (int j = 0; j < 4; ++j)
+                    acc[i][j] += gg4(su[0][bb][tr + i], sx[0][bb][tc + j], su[1][bb][tr + i], sx[1][bb][tc + j],
+                                     su[2][bb][tr + i], sx[2][bb][tc + j], su[3][bb][tr + i], sx[3][bb][tc + j]);
+        }
+        __syncthreads();
+    }
+#pragma unroll
+    for (int i = 0; i < 2; ++i)
+#pragma unroll
+        for (int j = 0; j < 4; ++j)
+            if (r0 + tr + i < rows && c0 + tc + j < cols)
+                out[(int64_t)(r0 + tr + i) * cols + c0 + tc + j] = acc[i][j] * scale;
+}
+// out[i] = scale sum_b (u[b][i] - usub[b][i]) (usub may be NULL), the batch in ascending order
+__global__ void __launch_bounds__(256)
+k_ggrad_sum_vec(int B, int len, const double* __restrict__ u, const double* __restrict__ usub, double scale,
+                double* __restrict__ out) {
+    const int idx = blockIdx.x * blockDim.x + threadIdx.x;
+    if (idx >= len) return;
+    double s = 0.0;
+    for (int b = 0; b < B; ++b) {
+        const int64_t at = (int64_t)b * len + idx;
+        s += usub ? u[at] - usub[at] : u[at];
+    }
+    out[idx] = s * scale;
+}
+
 
 }  // namespace
 #include "qp_solve.cuh"
@@ -1225,7 +1416,7 @@ int qpb200_internal_mean_outer(int B, int rows, int cols, const double* u, const
     return QPB200_OK;
 }
 
-int qpb200_version(void) { return 102; }
+int qpb200_version(void) { return 103; }
 
 const char* qpb200_error_string(int code) {
     switch (code) {
@@ -1700,6 +1891,134 @@ int qpb200_jvp_reg(const qpb200_plan* plan, int nbatch, const double* dQ, int64_
                                      ir_steps, nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0,
                                      dz, dlam, dnu, scratch, stream);
 }
+
+// ---- double backward: the JVP, k_ggrad_rhs, the dual backward, then k_ggrad_out / k_ggrad_sum* --------------------
+// work: the JVP's right-hand side, then cz, clam, cnu (B (n + m + e)); c_s (B m); wx, wlam, wnu (B (n + m + e)).
+struct GgArgs {
+    const double *wQ, *wp, *wG, *wh, *wA, *wb; int64_t swQ, swp, swG, swh, swA, swb;
+    const double* G; int64_t sG;
+    const double *dxv, *dlamv, *dnuv;
+    double *gg_z, *gg_lam, *gg_nu;
+    double *dQ, *dp, *dG, *dh, *dA, *db; int sumQ, sump, sumG, sumh, sumA, sumb;    // 1: the batch sum
+    double* work;
+};
+
+static int check_ggrad_args(const qpb200_plan* plan, int nbatch, const GgArgs& g, const double* zhat,
+                            const double* lam, const double* slacks, const double* nus, const double* Lfac,
+                            const double* Wfac, const double* Kfac, const double* scratch) {
+    const int rc = check_jvp_args(plan, nbatch, g.swQ, g.swp, g.swG, g.swh, g.swA, g.swb, g.wG, g.wh, g.wA, g.wb, zhat,
+                                  lam, slacks, nus, Lfac, Wfac, Kfac, g.work, g.gg_z, g.gg_lam, g.gg_nu, scratch);
+    if (rc) return rc;
+    if (!g.dxv || !g.dlamv || g.sG < 0) return QPB200_ERR_BAD_ARG;
+    if (plan->nineq > 0 && !g.G) return QPB200_ERR_BAD_ARG;
+    if (plan->neq > 0 && !g.dnuv) return QPB200_ERR_BAD_ARG;
+    if (plan->neq == 0 && (g.dA || g.db)) return QPB200_ERR_BAD_ARG;
+    return QPB200_OK;
+}
+
+static void gg_sum(int B, int rows, int cols, GgPairs P, double scale, double* out, cudaStream_t st) {
+    k_ggrad_sum<<<dim3((cols + kMoC - 1) / kMoC, (rows + kMoR - 1) / kMoR), 256, 0, st>>>(B, rows, cols, P, scale, out);
+}
+
+static void gg_sum_vec(int B, int len, const double* u, const double* usub, double scale, double* out,
+                       cudaStream_t st) {
+    k_ggrad_sum_vec<<<(len + 255) / 256, 256, 0, st>>>(B, len, u, usub, scale, out);
+}
+
+// After the JVP (into gg_*): k_ggrad_rhs, the dual backward (`reg`: the regularised one), then the gradients.
+static int double_backward_tail(const qpb200_plan* plan, int nbatch, const GgArgs& g, const double* zhat,
+                                const double* lam, const double* slacks, const double* nus, const double* Lfac,
+                                const double* Wfac, const double* Kfac, int sF, bool reg, double reg_eps, int ir_steps,
+                                double* scratch, cudaStream_t st) {
+    const int n = plan->nz, m = plan->nineq, e = plan->neq;
+    const int64_t B = nbatch;
+    double* cz = g.work;
+    double* clam = cz + B * n;
+    double* cnu = clam + B * m;
+    double* cs = cnu + B * e;
+    double* wx = cs + B * m;
+    double* wl = wx + B * n;
+    double* wn = wl + B * m;
+    int rc = launch(k_ggrad_rhs, nbatch, kThreads, jvp_smem_bytes(n, m, e), st, n, m, e, g.wQ, g.swQ, g.wG, g.swG, g.wA,
+                    g.swA, g.G, g.sG, g.dxv, g.dlamv, g.dnuv, g.gg_lam, lam, slacks, cz, clam, cnu, cs);
+    if (rc) return rc;
+    const double* rnu = (e > 0 && g.wA) ? cnu : nullptr;       // cnu = wA vx: NULL when there is no wA
+    rc = reg ? qpb200_backward_reg_duals(plan, nbatch, cz, clam, rnu, zhat, lam, slacks, nus, Lfac, Wfac, Kfac, sF,
+                                         reg_eps, ir_steps, nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0,
+                                         nullptr, 0, wx, wl, e > 0 ? wn : nullptr, scratch, st)
+             : qpb200_backward_duals(plan, nbatch, cz, clam, rnu, zhat, lam, slacks, nus, Lfac, Wfac, Kfac, sF, nullptr,
+                                     0, nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0, wx, wl,
+                                     e > 0 ? wn : nullptr, scratch, st);
+    if (rc) return rc;
+    const GgTerms T{zhat, lam, nus, g.dxv, g.dlamv, g.dnuv, g.gg_z, g.gg_lam, g.gg_nu, wx, wl, wn, cs};
+    const GgOut O{g.sumQ ? nullptr : g.dQ, g.sump ? nullptr : g.dp, g.sumG ? nullptr : g.dG, g.sumh ? nullptr : g.dh,
+                  (g.sumA || e == 0) ? nullptr : g.dA, (g.sumb || e == 0) ? nullptr : g.db};
+    if (O.dQ || O.dp || O.dG || O.dh || O.dA || O.db) {
+        const int64_t most = (int64_t)n * (n > m ? (n > e ? n : e) : (m > e ? m : e));
+        const int64_t chunks = (most + 256 * 8 - 1) / (256 * 8);
+        k_ggrad_out<<<dim3(nbatch, (unsigned)(chunks < 64 ? chunks : 64)), 256, 0, st>>>(n, m, e, T, O);
+    }
+    if (g.dQ && g.sumQ)
+        gg_sum(nbatch, n, n, GgPairs{{wx, zhat, g.gg_z, g.dxv}, {zhat, wx, g.dxv, g.gg_z}, nullptr}, 0.5, g.dQ, st);
+    if (g.dp && g.sump) gg_sum_vec(nbatch, n, wx, nullptr, 1.0, g.dp, st);
+    if (m > 0) {
+        if (g.dG && g.sumG)
+            gg_sum(nbatch, m, n, GgPairs{{wl, lam, g.dlamv, g.gg_lam}, {zhat, wx, g.gg_z, g.dxv}, cs}, 1.0, g.dG, st);
+        if (g.dh && g.sumh) gg_sum_vec(nbatch, m, wl, cs, -1.0, g.dh, st);
+    }
+    if (e > 0) {
+        if (g.dA && g.sumA)
+            gg_sum(nbatch, e, n, GgPairs{{wn, nus, g.dnuv, g.gg_nu}, {zhat, wx, g.gg_z, g.dxv}, nullptr}, 1.0, g.dA,
+                   st);
+        if (g.db && g.sumb) gg_sum_vec(nbatch, e, wn, nullptr, -1.0, g.db, st);
+    }
+    CK(cudaGetLastError());
+    return QPB200_OK;
+}
+
+#define QPB_GG_ARGS                                                                                                    \
+    GgArgs g{wQ, wp, wG, wh, wA, wb, swQ, swp, swG, swh, swA, swb, G, sG, dxv, dlamv, dnuv, gg_z, gg_lam, gg_nu,        \
+             dQ, dp, dG, dh, dA, db, sum_Q, sum_p, sum_G, sum_h, sum_A, sum_b, work}
+
+int qpb200_double_backward(const qpb200_plan* plan, int nbatch, const double* wQ, int64_t swQ, const double* wp,
+                           int64_t swp, const double* wG, int64_t swG, const double* wh, int64_t swh, const double* wA,
+                           int64_t swA, const double* wb, int64_t swb, const double* G, int64_t sG, const double* dxv,
+                           const double* dlamv, const double* dnuv, const double* zhat, const double* lam,
+                           const double* slacks, const double* nus, const double* Lfac, const double* Wfac,
+                           const double* Kfac, int sF, double* gg_z, double* gg_lam, double* gg_nu, double* dQ,
+                           int sum_Q, double* dp, int sum_p, double* dG, int sum_G, double* dh, int sum_h, double* dA,
+                           int sum_A, double* db, int sum_b, double* work, double* scratch, void* stream) {
+    QPB_GG_ARGS;
+    int rc = check_ggrad_args(plan, nbatch, g, zhat, lam, slacks, nus, Lfac, Wfac, Kfac, scratch);
+    if (rc) return rc;
+    rc = qpb200_jvp(plan, nbatch, wQ, swQ, wp, swp, wG, swG, wh, swh, wA, swA, wb, swb, zhat, lam, slacks, nus, Lfac,
+                    Wfac, Kfac, sF, work, gg_z, gg_lam, gg_nu, scratch, stream);
+    if (rc) return rc;
+    return double_backward_tail(plan, nbatch, g, zhat, lam, slacks, nus, Lfac, Wfac, Kfac, sF, false, 0.0, 0, scratch,
+                                (cudaStream_t)stream);
+}
+
+int qpb200_double_backward_reg(const qpb200_plan* plan, int nbatch, const double* wQ, int64_t swQ, const double* wp,
+                               int64_t swp, const double* wG, int64_t swG, const double* wh, int64_t swh,
+                               const double* wA, int64_t swA, const double* wb, int64_t swb, const double* G,
+                               int64_t sG, const double* dxv, const double* dlamv, const double* dnuv,
+                               const double* zhat, const double* lam, const double* slacks, const double* nus,
+                               const double* Lfac, const double* Wfac, const double* Kfac, int sF, double reg_eps,
+                               int ir_steps, double* gg_z, double* gg_lam, double* gg_nu, double* dQ, int sum_Q,
+                               double* dp, int sum_p, double* dG, int sum_G, double* dh, int sum_h, double* dA,
+                               int sum_A, double* db, int sum_b, double* work, double* scratch, void* stream) {
+    QPB_GG_ARGS;
+    int rc = check_ggrad_args(plan, nbatch, g, zhat, lam, slacks, nus, Lfac, Wfac, Kfac, scratch);
+    if (rc) return rc;
+    rc = check_reg_plan(plan, reg_eps, ir_steps, scratch);
+    if (rc) return rc;
+    rc = qpb200_jvp_reg(plan, nbatch, wQ, swQ, wp, swp, wG, swG, wh, swh, wA, swA, wb, swb, zhat, lam, slacks, nus,
+                        Lfac, Wfac, Kfac, sF, reg_eps, ir_steps, work, gg_z, gg_lam, gg_nu, scratch, stream);
+    if (rc) return rc;
+    return double_backward_tail(plan, nbatch, g, zhat, lam, slacks, nus, Lfac, Wfac, Kfac, sF, true, reg_eps, ir_steps,
+                                scratch, (cudaStream_t)stream);
+}
+#undef QPB_GG_ARGS
 
 #ifdef QPB_TIMING
 int qpb200_debug_timing(long long* host64, int reset) {

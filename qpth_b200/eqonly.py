@@ -70,6 +70,7 @@ class QPEqualityFn(Function):
         ctx.zhat64, ctx.nus = zhat, nus
         ctx.meta = [(X.device, X.dtype) for X in (Q_, p_, A_, b_)]
         ctx.duals = duals
+        ctx.save_for_backward(Q_, p_, A_, b_)
         ctx.set_materialize_grads(False)
         zhat_out = zhat.to(device=Q_.device, dtype=Q_.dtype)
         if not duals:
@@ -103,24 +104,95 @@ class QPEqualityFn(Function):
 
     @staticmethod
     def backward(ctx, dl_dzhat, dl_dlam=None, dl_dnu=None):
-        z, nus = ctx.zhat64, ctx.nus
-        dl = (torch.zeros_like(z) if dl_dzhat is None
-              else dl_dzhat.detach().to(device=z.device, dtype=torch.float64).contiguous().view_as(z))
-        # dl/dnu is the ry of the solve: K [dx ds dz dnu] = -[dl 0 0 dl/dnu]
-        ry = (torch.zeros_like(nus) if dl_dnu is None
-              else dl_dnu.detach().to(device=z.device, dtype=torch.float64).contiguous().view_as(nus))
-        dx, _, _, dnu = _solve(ctx.F, *ctx.QA, ctx.one, dl, ctx.zero, ctx.zero, ry, ctx.steps)
-        grads = [0.5 * (bger(dx, z) + bger(z, dx)),         # qp.py:175-177
-                 dx,                                        # qp.py:150
-                 bger(dnu, z) + bger(nus, dx),              # qp.py:166-167
-                 -dnu]                                      # qp.py:168
-        out = []
-        for g, unb, (dev, dt), need in zip(grads, ctx.flags, ctx.meta, ctx.needs_input_grad[:4]):
-            if not need:
-                out.append(None)
-                continue
-            out.append((g.mean(0) if unb else g).to(device=dev, dtype=dt))
-        return tuple(out) + (None, None, None)
+        if torch.is_grad_enabled():          # create_graph=True: gradients that can be differentiated again
+            return QPEqualityBackwardFn.apply(ctx, ctx.needs_input_grad[:4], dl_dzhat, dl_dnu,
+                                              *ctx.saved_tensors) + (None, None, None)
+        return _first_order(ctx, dl_dzhat, dl_dnu, ctx.needs_input_grad[:4])[0] + (None, None, None)
+
+
+def _first_order(ctx, dl_dzhat, dl_dnu, want):
+    """QPEqualityFn's backward at the state `ctx` of its forward: (the gradients of Q, p, A, b, (dx, dnu))."""
+    z, nus = ctx.zhat64, ctx.nus
+    dl = (torch.zeros_like(z) if dl_dzhat is None
+          else dl_dzhat.detach().to(device=z.device, dtype=torch.float64).contiguous().view_as(z))
+    # dl/dnu is the ry of the solve: K [dx ds dz dnu] = -[dl 0 0 dl/dnu]
+    ry = (torch.zeros_like(nus) if dl_dnu is None
+          else dl_dnu.detach().to(device=z.device, dtype=torch.float64).contiguous().view_as(nus))
+    dx, _, _, dnu = _solve(ctx.F, *ctx.QA, ctx.one, dl, ctx.zero, ctx.zero, ry, ctx.steps)
+    grads = [0.5 * (bger(dx, z) + bger(z, dx)),         # qp.py:175-177
+             dx,                                        # qp.py:150
+             bger(dnu, z) + bger(nus, dx),              # qp.py:166-167
+             -dnu]                                      # qp.py:168
+    out = []
+    for g, unb, (dev, dt), need in zip(grads, ctx.flags, ctx.meta, want):
+        if not need:
+            out.append(None)
+            continue
+        out.append((g.mean(0) if unb else g).to(device=dev, dtype=dt))
+    return tuple(out), (dx, dnu)
+
+
+def _mv(M, x):
+    return torch.matmul(M, x.unsqueeze(-1)).squeeze(-1)
+
+
+class QPEqualityBackwardFn(Function):
+    """QPEqualityFn's backward as a differentiable function of (g_z, g_nu, Q, p, A, b), under create_graph=True. Its
+    backward is the double backward of qpb200_double_backward without inequality rows (no D, c_lam or c_s terms), with
+    the same solves as the first order: u = the JVP for tangents w (the gradients of g_z, g_nu), then the solve of the
+    cotangents cz = sym(wQ) vx + wA' vnu, cnu = wA vx of (z, nu), w; dQ = sym(wx z' + ux vx'), dp = wx,
+    dA = wnu z' + nu wx' + vnu ux' + unu vx', db = -wnu. The cotangent of a batch mean is w / nBatch per QP, and the
+    gradient of an un-batched input the batch sum."""
+    @staticmethod
+    def forward(ctx, eq, want, g_z, g_nu, Q_, p_, A_, b_):
+        out, ctx.v = _first_order(eq, g_z, g_nu, want)
+        ctx.eq = eq
+        ctx.like = (g_z, g_nu, Q_, p_, A_, b_)
+        ctx.set_materialize_grads(False)
+        return out
+
+    @staticmethod
+    def backward(ctx, wQ, wp, wA, wb):
+        from .qp import THIRD_ORDER_ERR
+        if torch.is_grad_enabled():
+            raise RuntimeError(THIRD_ORDER_ERR)
+        need = ctx.needs_input_grad[2:]
+        if all(w is None for w in (wQ, wp, wA, wb)) or not any(need):
+            return (None,) * 8
+        eq = ctx.eq
+        z, nus = eq.zhat64, eq.nus
+        vx, vn = ctx.v
+        B = z.shape[0]
+        om = []
+        for w, unb in zip((wQ, wp, wA, wb), eq.flags):
+            w = None if w is None else w.detach().to(device=z.device, dtype=torch.float64)
+            om.append(None if w is None else (w / B if unb else w))
+        wQ, wp, wA, wb = om
+        rx, ry, cz, cn = torch.zeros_like(z), torch.zeros_like(nus), torch.zeros_like(z), torch.zeros_like(nus)
+        if wQ is not None:
+            rx = rx + 0.5 * (_mv(wQ, z) + _mv(wQ.transpose(-1, -2), z))
+            cz = cz + 0.5 * (_mv(wQ, vx) + _mv(wQ.transpose(-1, -2), vx))
+        if wp is not None:
+            rx = rx + wp
+        if wA is not None:
+            rx = rx + _mv(wA.transpose(-1, -2), nus)
+            ry = ry + _mv(wA, z)
+            cz = cz + _mv(wA.transpose(-1, -2), vn)
+            cn = cn + _mv(wA, vx)
+        if wb is not None:
+            ry = ry - wb
+        ux, _, _, un = _solve(eq.F, *eq.QA, eq.one, rx.contiguous(), eq.zero, eq.zero, ry.contiguous(), eq.steps)
+        wx, _, _, wn = _solve(eq.F, *eq.QA, eq.one, cz.contiguous(), eq.zero, eq.zero, cn.contiguous(), eq.steps)
+        grads = [ux, un,
+                 0.5 * ((bger(wx, z) + bger(z, wx)) + (bger(ux, vx) + bger(vx, ux))),
+                 wx,
+                 bger(wn, z) + bger(nus, wx) + bger(vn, ux) + bger(un, vx),
+                 -wn]
+        unb = (False, False) + tuple(eq.flags)
+        res = []
+        for g, X, u, n in zip(grads, ctx.like, unb, need):
+            res.append((g.sum(0) if u else g).to(device=X.device, dtype=X.dtype) if (n and X is not None) else None)
+        return (None, None) + tuple(res)
 
 
 def solve_equality_qp(Q_, p_, A_, b_, check_Q_spd=True, reg=False, duals=False):

@@ -256,9 +256,10 @@ def dual_outputs(st, like):
     return lam, nu
 
 
-def solve_backward(st, dl_dzhat, mean_flags, want, dl_dlam=None, dl_dnu=None):
+def solve_backward(st, dl_dzhat, mean_flags, want, dl_dlam=None, dl_dnu=None, keep=False):
     """QPFunctionFn.backward on the device. mean_flags / want: 6-tuples for (Q,p,G,h,A,b). dl_dlam / dl_dnu: the
-    gradients of the loss with respect to the returned duals (None: zero); dl_dzhat None: zero."""
+    gradients of the loss with respect to the returned duals (None: zero); dl_dzhat None: zero. keep: also return the
+    solve (dxv, dlamv, dnuv), which the double backward reads."""
     if _pending:
         flush_checks(wait=False)
     lib = _lib.load()
@@ -291,7 +292,86 @@ def solve_backward(st, dl_dzhat, mean_flags, want, dl_dlam=None, dl_dnu=None):
             ctypes.byref(plan), B, _ptr(dl), *adj, _ptr(st.zhat), _ptr(st.lam), _ptr(st.slacks), _ptr(st.nus),
             _ptr(st.L), _ptr(st.W), _ptr(st.K), 1 if st.nsys > 1 else 0, *((float(kkt.IR_EPS), int(kkt.IR_STEPS)) if reg else ()),
             *args, _ptr(dxv), _ptr(dlamv), _ptr(dnuv), _ptr(st.scratch), _stream()))
+    if keep:
+        return outs, (dxv, dlamv, dnuv)
     return outs
+
+
+def solve_double_backward(st, v, omegas, flags, want, G):
+    """The double backward on the device (qpb200_double_backward(_reg)): v = (dxv, dlamv, dnuv) of the first backward at
+    the point of `st`; omegas: the cotangents of its six outputs (Q, p, G, h, A, b), each None or shaped as that output;
+    flags: the first backward's mean flags (an un-batched input: its cotangent is divided by nBatch, and its second-order
+    gradient is the batch sum); want: which of the six gradients to write; G: the forward's G. Returns fp64
+    (gg_z, gg_lam, gg_nu, dQ, dp, dG, dh, dA, db): the gradients of g_z, g_lam, g_nu (gg_nu None without equality rows)
+    and of the six inputs (None where not wanted)."""
+    if _pending:
+        flush_checks(wait=False)
+    lib = _lib.load()
+    plan, B, device = st.plan, st.nBatch, st.device
+    nz, nineq, neq = plan.nz, plan.nineq, plan.neq
+    f64 = dict(dtype=torch.float64, device=device)
+    with torch.cuda.device(device):
+        om = [None if (w is None or (k >= 4 and neq == 0)) else (_dev64(w, device) / B if flags[k] else w)
+              for k, w in enumerate(omegas)]
+        tans = tangent_args(om, (3, 2, 3, 2, 3, 2), (nz * nz, nz, nineq * nz, nineq, neq * nz, neq), device)
+        G64 = _dev64(G, device)
+        sG = nineq * nz if G64.dim() == 3 else 0
+        shapes = [(nz, nz), (nz,), (nineq, nz), (nineq,), (neq, nz), (neq,)]
+        outs = []
+        for k in range(6):
+            if not want[k] or (k >= 4 and neq == 0):
+                outs.append(None)
+            else:
+                outs.append(torch.empty(*(shapes[k] if flags[k] else (B,) + shapes[k]), **f64))
+        gz = torch.empty(B, nz, **f64)
+        glam = torch.empty(B, nineq, **f64)
+        gnu = torch.empty(B, neq, **f64) if neq > 0 else None
+        work = torch.empty(B * (2 * nz + 3 * nineq + 2 * neq), **f64)
+        args = []
+        for t, s in tans:
+            args += [_ptr(t), s]
+        grads = []
+        for k in range(6):
+            grads += [_ptr(outs[k]), 1 if flags[k] else 0]
+        reg = getattr(st, "reg", False)
+        _lib.check((lib.qpb200_double_backward_reg if reg else lib.qpb200_double_backward)(
+            ctypes.byref(plan), B, *args, _ptr(G64), sG, *(_ptr(x) for x in v),
+            _ptr(st.zhat), _ptr(st.lam), _ptr(st.slacks), _ptr(st.nus), _ptr(st.L), _ptr(st.W), _ptr(st.K),
+            1 if st.nsys > 1 else 0, *((float(kkt.IR_EPS), int(kkt.IR_STEPS)) if reg else ()),
+            _ptr(gz), _ptr(glam), _ptr(gnu), *grads, _ptr(work), _ptr(st.scratch), _stream()))
+    return [gz, glam, gnu] + outs
+
+
+THIRD_ORDER_ERR = ("qpth_b200: third-order derivatives through the QP layer are not provided: the double backward is not "
+                   "differentiable (call the second torch.autograd.grad without create_graph=True)")
+
+
+def _cast(g, like):
+    return None if (g is None or like is None) else g.to(device=like.device, dtype=like.dtype)
+
+
+class QPBackwardFn(Function):
+    """The first-order backward of QPFunction / QPSolutionFunction as a differentiable function of the incoming gradients
+    (g_z, g_lam, g_nu) and of (Q, p, G, h, A, b): what their backward runs under create_graph=True. Its forward is the
+    first backward's own solve_backward call; its backward is solve_double_backward."""
+    @staticmethod
+    def forward(ctx, st, flags, want, g_z, g_lam, g_nu, Q, p, G, h, A, b):
+        outs, v = solve_backward(st, g_z, flags, want, g_lam, g_nu, keep=True)
+        ctx.st, ctx.v, ctx.flags = st, v, flags
+        ctx.like = (g_z, g_lam, g_nu, Q, p, G, h, A, b)
+        ctx.set_materialize_grads(False)
+        return tuple(_cast(g, X) for X, g in zip((Q, p, G, h, A, b), outs))
+
+    @staticmethod
+    def backward(ctx, *omegas):
+        if torch.is_grad_enabled():
+            raise RuntimeError(THIRD_ORDER_ERR)
+        need = ctx.needs_input_grad[3:]
+        if all(w is None for w in omegas) or not any(need):
+            return (None,) * 12
+        G = ctx.like[5]
+        res = solve_double_backward(ctx.st, ctx.v, omegas, ctx.flags, need[3:], G)
+        return (None, None, None) + tuple(_cast(g, X) if n else None for g, X, n in zip(res, ctx.like, need))
 
 
 def tangent_args(tangents, ranks, per, device):
@@ -478,6 +558,13 @@ def QPFunction(eps=1e-12, verbose=0, notImprovedLim=3, maxIter=20, solver=QPSolv
     The returned callable's `jacobian(wrt=("p", "h", "b"), duals=False)` gives the whole Jacobians of the last forward's
     solution with respect to p, h and b, per QP (its docstring has the details).
 
+    Second order: under `torch.autograd.grad(..., create_graph=True)` the gradients are differentiable again, in the
+    incoming gradients of z, lam, nu and in Q, p, G, h, A, b (Hessian-vector products, `torch.autograd.functional.hessian`,
+    gradient penalties, meta-learning through the layer). The double backward is the exact derivative of the backward as
+    computed (qpth's clamped D included): one JVP solve, one dual backward solve and two bandwidth-bound kernels
+    (qpb200_double_backward). The cotangent of an un-batched input's gradient (a batch mean) is shared by every QP, and
+    that input's second-order gradient is the batch sum. Without create_graph nothing changes. Third order raises.
+
     kkt_solver (an extension of the reference's signature): KKTSolvers.LU_PARTIAL, the default, needs Q positive definite.
     KKTSolvers.IR_UNOPT also solves QPs whose Q is only positive semidefinite (LPs with Q = 0, low-rank quadratic terms)
     and QPs whose equality rows are linearly dependent: every KKT solve factors the system regularised with kkt.IR_EPS
@@ -555,6 +642,8 @@ def QPFunction(eps=1e-12, verbose=0, notImprovedLim=3, maxIter=20, solver=QPSolv
             flags = [expandParam(X, nBatch, nd)[1]
                      for X, nd in ((Q, 3), (p, 2), (G, 3), (h, 2), (A, 3), (b, 2))]   # qp.py:131-136
             want = list(ctx.needs_input_grad)
+            if torch.is_grad_enabled():          # create_graph=True: gradients that can be differentiated again
+                return QPBackwardFn.apply(ctx.st, flags, want, dl_dzhat, dl_dlam, dl_dnu, Q, p, G, h, A, b)
             outs = solve_backward(ctx.st, dl_dzhat, flags, want, dl_dlam, dl_dnu)
             grads = []
             for X, g in zip((Q, p, G, h, A, b), outs):

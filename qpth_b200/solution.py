@@ -101,7 +101,8 @@ def QPSolutionFunction(check_Q_spd=True, kkt_solver=KKTSolvers.LU_PARTIAL, duals
 
     Forward mode (torch.autograd.forward_ad) is supported as for QPFunction; the tangents of the four solution tensors
     are ignored. f.jacobian(wrt, duals) gives the Jacobians with respect to p, h and b at the last solution passed, as
-    QPFunction's does.
+    QPFunction's does. Under create_graph=True the gradients are differentiable again, as QPFunction's are (the solution
+    tensors stay constants); third order raises.
 
     kkt_solver: KKTSolvers.LU_PARTIAL (the default) needs Q positive definite. KKTSolvers.IR_UNOPT differentiates with
     the regularised KKT solve of QPFunction(kkt_solver=IR_UNOPT), so an LP (Q = 0) or a low-rank Q solved by any solver
@@ -142,6 +143,10 @@ def QPSolutionFunction(check_Q_spd=True, kkt_solver=KKTSolvers.LU_PARTIAL, duals
             flags = [expandParam(X, nBatch, nd)[1]
                      for X, nd in ((Q, 3), (p, 2), (G, 3), (h, 2), (A, 3), (b, 2))]   # qp.py:131-136
             want = list(ctx.needs_input_grad[:6])
+            if torch.is_grad_enabled():          # create_graph=True: gradients that can be differentiated again
+                from .qp import QPBackwardFn
+                return QPBackwardFn.apply(ctx.st, flags, want, dl_dzhat, dl_dlam, dl_dnu, Q, p, G, h, A,
+                                          b) + (None, None, None, None)
             outs = solve_backward(ctx.st, dl_dzhat, flags, want, dl_dlam, dl_dnu)
             grads = [None if g is None else g.to(device=X.device, dtype=X.dtype)
                      for X, g in zip((Q, p, G, h, A, b), outs)]
