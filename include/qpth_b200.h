@@ -430,6 +430,31 @@ int qpb200_box_jvp(const qpb200_box_plan* plan, int nbatch, const double* q, int
                    const double* db, int64_t sdb, const double* dlb, int64_t sdlb, const double* dub, int64_t sdub,
                    const double* zhat, const double* lam, const double* slacks, const double* nus, double* rhs,
                    double* dz, double* dlam, double* dnu, void* stream);
+/* Double backward (an extension), qpb200_double_backward with Q = diag(q) and the constant G = [-I; I]: the derivative
+ * of phi = sum_X <w_X, grad_X> for cotangents w_X on the outputs of qpb200_box_backward_duals, with respect to its
+ * adjoints (g_z, g_lam, g_nu) and to q, p, A, b, lb, ub, treating that backward as computed (the 1e-8 clamps of D
+ * included). v = (dxv, dlamv, dnuv) is the first backward's solve at the same point. The call runs
+ *   1. qpb200_box_jvp with tangents w_X: u = (gg_z, gg_lam, gg_nu), the gradients of g_z, g_lam and g_nu;
+ *   2. a kernel forming cz = wq o vx + wA' vnu + c_s_lb - c_s_ub, clam = c_lam, cnu = wA vx from the cotangent
+ *      c_D = (ulam / D)(vlam / D) of D: c_lam = c_D / clamp(s) where lam >= 1e-8, c_s = -c_D D / clamp(s) where
+ *      s >= 1e-8 (0 elsewhere);
+ *   3. qpb200_box_backward_duals with (cz, clam, cnu): w = (wx, wlam, wnu);
+ *   4. a kernel writing dq = wx o z + ux o vx, dp = wx, dlb = wlam_lb - c_s_lb, dub = c_s_ub - wlam_ub,
+ *      dA = wnu z' + nu wx' + vnu ux' + unu vx', db = -wnu.
+ * w_X in qpb200_box_jvp's tangent order, each with a batch stride (0: one cotangent for every QP) and NULL allowed
+ * (zero); wA, wb must be NULL when neq == 0, wlb / wub when that side is absent. The cotangent of a batch-mean gradient
+ * (an un-batched input) is the caller's w_X / nbatch. dq .. db may be NULL (skipped); sum_X = 1 writes the batch sum
+ * (one un-batched tensor, the exact derivative for an un-batched input), 0 the per-QP gradients. gg_z (B,nz), gg_lam
+ * (B,nineq), gg_nu (B,neq) are always written. work: QPB200_DOUBLE_BACKWARD_WORK(nbatch, nz, nineq, neq) doubles. Every
+ * argument is checked before anything is launched. */
+int qpb200_box_double_backward(const qpb200_box_plan* plan, int nbatch, const double* q, int64_t sq, const double* A,
+                               int64_t sA, const double* wq, int64_t swq, const double* wp, int64_t swp,
+                               const double* wA, int64_t swA, const double* wb, int64_t swb, const double* wlb,
+                               int64_t swlb, const double* wub, int64_t swub, const double* dxv, const double* dlamv,
+                               const double* dnuv, const double* zhat, const double* lam, const double* slacks,
+                               const double* nus, double* gg_z, double* gg_lam, double* gg_nu, double* dq, int sum_q,
+                               double* dp, int sum_p, double* dlb, int sum_lb, double* dub, int sum_ub, double* dA,
+                               int sum_A, double* db, int sum_b, double* work, void* stream);
 
 /* Jacobians of a box QP at the returned point (an extension, csrc/qp_jac.cu): d(z*, lam, nu)/d(p, lb, ub, b) per QP,
  * with the backward's clamped D = clamp(lam, 1e-8) / clamp(s, 1e-8) = [d_lb; d_ub]. With H = q + d_lb + d_ub and
@@ -491,6 +516,16 @@ int qpb200_boxq_jvp(const qpb200_boxq_plan* plan, int nbatch, const double* Q, i
                     const double* db, int64_t sdb, const double* dlb, int64_t sdlb, const double* dub, int64_t sdub,
                     const double* zhat, const double* lam, const double* slacks, const double* nus, double* rhs,
                     double* dz, double* dlam, double* dnu, void* stream);
+/* As qpb200_box_double_backward, with the cotangent wQ (nz x nz, stride swQ, read in full) in place of wq: cz gains
+ * sym(wQ) vx, and dQ = sym(wx z' + ux vx') (B,nz,nz), or its batch sum (nz,nz) with sum_Q = 1, replaces dq. */
+int qpb200_boxq_double_backward(const qpb200_boxq_plan* plan, int nbatch, const double* Q, int64_t sQ,
+                                const double* A, int64_t sA, const double* wQ, int64_t swQ, const double* wp,
+                                int64_t swp, const double* wA, int64_t swA, const double* wb, int64_t swb,
+                                const double* wlb, int64_t swlb, const double* wub, int64_t swub, const double* dxv,
+                                const double* dlamv, const double* dnuv, const double* zhat, const double* lam,
+                                const double* slacks, const double* nus, double* gg_z, double* gg_lam, double* gg_nu,
+                                double* dQ, int sum_Q, double* dp, int sum_p, double* dlb, int sum_lb, double* dub,
+                                int sum_ub, double* dA, int sum_A, double* db, int sum_b, double* work, void* stream);
 /* As qpb200_box_jacobian with a dense Q (nz x nz, batch stride sQ; only its lower triangle is read): K = [H A'; A 0],
  * H = Q + diag(d_lb + d_ub), is factored once per QP as the forward factors it (L diag(I, -I) L' on the bordered
  * staircase) and every column is solved in blocks of 8. *smem_bytes = 0 where the kernel does not cover the plan (every

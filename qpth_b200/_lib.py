@@ -105,6 +105,9 @@ SIGNATURES = {
                                        _P, _I, _P, _I, _P, _I, _P, _I, _P, _I, _P, _I, _P, _P, _P, _P]),
     "qpb200_box_jvp": (_I, [ctypes.POINTER(BoxPlan), _I, _P, _L, _P, _L, _P, _L, _P, _L, _P, _L, _P, _L, _P, _L,
                             _P, _L, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
+    "qpb200_box_double_backward": (_I, [ctypes.POINTER(BoxPlan), _I, _P, _L, _P, _L, _P, _L, _P, _L, _P, _L, _P, _L,
+                                        _P, _L, _P, _L, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P,
+                                        _P, _I, _P, _I, _P, _I, _P, _I, _P, _I, _P, _I, _P, _P]),
     "qpb200_box_solve_kkt": (_I, [ctypes.POINTER(BoxPlan), _I, _P, _L, _P, _L, _P, _P, _P, _P, _P,
                                   _P, _P, _P, _P, _P]),
     "qpb200_box_jacobian_smem": (_I, [ctypes.POINTER(BoxPlan), _P]),
@@ -116,6 +119,9 @@ SIGNATURES = {
                                         _P, _I, _P, _I, _P, _I, _P, _I, _P, _I, _P, _I, _P, _P, _P, _P]),
     "qpb200_boxq_jvp": (_I, [ctypes.POINTER(BoxQPlan), _I, _P, _L, _P, _L, _P, _L, _P, _L, _P, _L, _P, _L, _P, _L,
                              _P, _L, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
+    "qpb200_boxq_double_backward": (_I, [ctypes.POINTER(BoxQPlan), _I, _P, _L, _P, _L, _P, _L, _P, _L, _P, _L, _P, _L,
+                                         _P, _L, _P, _L, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P,
+                                         _P, _I, _P, _I, _P, _I, _P, _I, _P, _I, _P, _I, _P, _P]),
     "qpb200_boxq_solve_kkt": (_I, [ctypes.POINTER(BoxQPlan), _I, _P, _L, _P, _L, _P, _P, _P, _P, _P,
                                    _P, _P, _P, _P, _P]),
     "qpb200_boxq_jacobian_smem": (_I, [ctypes.POINTER(BoxQPlan), _P]),

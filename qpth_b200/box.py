@@ -132,10 +132,11 @@ def solve_box_forward(q_, p_, A_, b_, lb_, ub_, eps=1e-12, verbose=0, notImprove
     return st
 
 
-def solve_box_backward(st, dl_dzhat, mean_flags, want, dl_dlam=None, dl_dnu=None):
+def solve_box_backward(st, dl_dzhat, mean_flags, want, dl_dlam=None, dl_dnu=None, keep=False):
     """Gradients (dq, dp, dA, db, dlb, dub) on the device; mean_flags / want: 6-tuples in that order. dl_dlam ([lb rows;
     ub rows]) / dl_dnu: the gradients with respect to the returned duals (None: zero); dl_dzhat None: zero. With a
-    dense Q the first is dQ, (B, nz, nz) or (nz, nz) with its mean flag."""
+    dense Q the first is dQ, (B, nz, nz) or (nz, nz) with its mean flag. keep: also return the solve (dxv, dlamv,
+    dnuv), which the double backward reads."""
     if _qp._pending:
         _qp.flush_checks(wait=False)
     lib = _lib.load()
@@ -168,7 +169,77 @@ def solve_box_backward(st, dl_dzhat, mean_flags, want, dl_dlam=None, dl_dnu=None
             ctypes.byref(plan), B, _ptr(st.q), st.sq, _ptr(st.A), st.sA, _ptr(dl), *adj, _ptr(st.zhat), _ptr(st.lam),
             _ptr(st.slacks), _ptr(st.nus), _ptr(dq), mq, _ptr(dp), mp, _ptr(dlb), mlb, _ptr(dub), mub,
             _ptr(dA), mA, _ptr(db), mb, _ptr(dxv), _ptr(dlamv), _ptr(dnuv), _stream()))
+    if keep:
+        return outs, (dxv, dlamv, dnuv)
     return outs
+
+
+def solve_box_double_backward(st, v, omegas, flags, want):
+    """The double backward on the device (qpb200_box_double_backward / qpb200_boxq_double_backward): v = (dxv, dlamv,
+    dnuv) of the first backward at the point of `st`; omegas: the cotangents of its six outputs (dq, dp, dA, db, dlb,
+    dub; dQ with a dense Q), each None or shaped as that output; flags: the first backward's mean flags (an un-batched
+    input: its cotangent is divided by nBatch, and its second-order gradient is the batch sum); want: which of the six
+    gradients to write. Returns fp64 (gg_z, gg_lam, gg_nu, dq, dp, dA, db, dlb, dub): the gradients of g_z, g_lam, g_nu
+    (gg_nu None without equality rows) and of the six inputs (None where not wanted or absent)."""
+    if _qp._pending:
+        _qp.flush_checks(wait=False)
+    lib = _lib.load()
+    plan, B, device = st.plan, st.nBatch, st.device
+    nz, neq, m = plan.nz, plan.neq, plan.nineq
+    f64 = dict(dtype=torch.float64, device=device)
+    absent = (False, False, neq == 0, neq == 0, not plan.has_lb, not plan.has_ub)
+    with torch.cuda.device(device):
+        om = [None if (w is None or absent[k]) else (_dev64(w, device) / B if flags[k] else w)
+              for k, w in enumerate(omegas)]
+        per = (nz * nz if st.dense_Q else nz, nz, neq * nz, neq, nz, nz)
+        tans = _qp.tangent_args(om, (3 if st.dense_Q else 2, 2, 3, 2, 2, 2), per, device)
+        shapes = [(nz, nz) if st.dense_Q else (nz,), (nz,), (neq, nz), (neq,), (nz,), (nz,)]
+        outs = []
+        for k in range(6):
+            if not want[k] or absent[k]:
+                outs.append(None)
+            else:
+                outs.append(torch.empty(*(shapes[k] if flags[k] else (B,) + shapes[k]), **f64))
+        gz = torch.empty(B, nz, **f64)
+        glam = torch.empty(B, m, **f64)
+        gnu = torch.empty(B, neq, **f64) if neq > 0 else None
+        work = torch.empty(B * (2 * nz + 3 * m + 2 * neq), **f64)      # QPB200_DOUBLE_BACKWARD_WORK
+        args = []
+        for t, s in tans:
+            args += [_ptr(t), s]
+        dq, dp, dA, db, dlb, dub = outs
+        grads = []
+        for g, k in zip((dq, dp, dlb, dub, dA, db), (0, 1, 4, 5, 2, 3)):   # the ABI's order
+            grads += [_ptr(g), 1 if flags[k] else 0]
+        fn = lib.qpb200_boxq_double_backward if st.dense_Q else lib.qpb200_box_double_backward
+        _lib.check(fn(
+            ctypes.byref(plan), B, _ptr(st.q), st.sq, _ptr(st.A), st.sA, *args, *(_ptr(x) for x in v),
+            _ptr(st.zhat), _ptr(st.lam), _ptr(st.slacks), _ptr(st.nus), _ptr(gz), _ptr(glam), _ptr(gnu), *grads,
+            _ptr(work), _stream()))
+    return [gz, glam, gnu] + outs
+
+
+class BoxQPBackwardFn(Function):
+    """The first-order backward of BoxQPFunction (the box kernels) as a differentiable function of the incoming
+    gradients (g_z, g_lam, g_nu) and of (q, p, A, b, lb, ub): what its backward runs under create_graph=True. Its
+    forward is the first backward's own solve_box_backward call; its backward is solve_box_double_backward."""
+    @staticmethod
+    def forward(ctx, st, flags, want, g_z, g_lam, g_nu, q, p, A, b, lb, ub):
+        outs, v = solve_box_backward(st, g_z, flags, want, g_lam, g_nu, keep=True)
+        ctx.st, ctx.v, ctx.flags = st, v, flags
+        ctx.like = (g_z, g_lam, g_nu, q, p, A, b, lb, ub)
+        ctx.set_materialize_grads(False)
+        return tuple(_qp._cast(g, X) for X, g in zip((q, p, A, b, lb, ub), outs))
+
+    @staticmethod
+    def backward(ctx, *omegas):
+        if torch.is_grad_enabled():
+            raise RuntimeError(_qp.THIRD_ORDER_ERR)
+        need = ctx.needs_input_grad[3:]
+        if all(w is None for w in omegas) or not any(need):
+            return (None,) * 12
+        res = solve_box_double_backward(ctx.st, ctx.v, omegas, ctx.flags, need[3:])
+        return (None, None, None) + tuple(_qp._cast(g, X) if n else None for g, X, n in zip(res, ctx.like, need))
 
 
 def solve_box_jvp(st, tangents):
@@ -250,6 +321,35 @@ def dense_backward(st, dl, mean_flags, want, nlb, has_ub, dl_dlam=None, dl_dnu=N
             dub = dh[..., nlb:]
             dub = dub.mean(0) if (mub and dub.dim() == 2) else dub
     return [dq, dp, dA, db, dlb, dub]
+
+
+def dense_backward_graph(st, dl, mean_flags, want, ins, dl_dlam=None, dl_dnu=None, dense_Q=False):
+    """dense_backward under create_graph=True: (Q, h) of the dense equivalent built from the inputs with torch ops, the
+    first backward through qp.QPBackwardFn on the dense state (G constant), and the map back to (dq, dp, dA, db, dlb,
+    dub) again with torch ops, so that the gradients can be differentiated once more. Returns them cast to the inputs."""
+    dst, h_shared = st.dense
+    q, p, A, b, lb, ub = ins
+    mq, mp, mA, mb, mlb, mub = mean_flags
+    Q, G, h = dense_equivalent(q, lb, ub, dense_Q)
+    empty = torch.empty(0, dtype=q.dtype, device=q.device)
+    A_ = A if (A is not None and A.nelement() > 0) else empty
+    b_ = b if (b is not None and b.nelement() > 0) else empty
+    dQ, dp, _, dh, dA, db = _qp.QPBackwardFn.apply(
+        dst, (mq, mp, True, h_shared, mA, mb), (want[0], want[1], False, want[4] or want[5], want[2], want[3]),
+        dl, dl_dlam, dl_dnu, Q, p, G, h, A_, b_)
+    nlb = q.size(-1) if lb is not None else 0
+    dq = dQ if (dQ is None or dense_Q) else torch.diagonal(dQ, dim1=-2, dim2=-1)
+    dlb = dub = None
+    if dh is not None:
+        if want[4] and lb is not None:
+            dlb = -dh[..., :nlb]
+            dlb = dlb.mean(0) if (mlb and dlb.dim() == 2) else dlb
+        if want[5] and ub is not None:
+            dub = dh[..., nlb:]
+            dub = dub.mean(0) if (mub and dub.dim() == 2) else dub
+    outs = (dq, dp, dA, db, dlb, dub)
+    return tuple(None if (g is None or X is None or not w) else g.to(device=X.device, dtype=X.dtype)
+                 for X, g, w in zip(ins, outs, want))
 
 
 def dense_jvp(st, tangents, nlb, has_ub, dense_Q=False):
@@ -430,7 +530,17 @@ def BoxQPFunction(eps=1e-12, verbose=0, notImprovedLim=3, maxIter=20, check_Q_sp
     does. Shapes whose factor or column buffers do not fit one CTA take one JVP per column, and the dense fallback the
     dense path's jacobian. Jacobians with respect to q, Q and A are contractions of these:
     J_.,q = J_.,p diag(z), J_.,Q_ik = J_.,p_i z_k (sym(dQ) enters), J_.,A_ck = J_.,p_k nu_c - J_.,b_c z_k. The result has
-    the dtype and device of the forward's output and is not differentiable."""
+    the dtype and device of the forward's output and is not differentiable.
+
+    Second order: under `torch.autograd.grad(..., create_graph=True)` the gradients are differentiable again, in the
+    incoming gradients of z, lam, nu and in q (Q), p, A, b, lb, ub (Hessian-vector products,
+    `torch.autograd.functional.hessian`, gradient penalties, meta-learning through a sudoku layer or a projection). The
+    double backward is the exact derivative of the backward as computed (the clamped D included), on the layout that
+    solved the forward: one box JVP solve, one dual backward solve and two bandwidth-bound kernels
+    (qpb200_box_double_backward; a dense Q: qpb200_boxq_double_backward). The cotangent of an un-batched input's
+    gradient (a batch mean) is shared by every QP, and that input's second-order gradient is the batch sum. The dense
+    fallback goes through QPFunction's double backward on the dense equivalent. Without create_graph nothing changes.
+    Third order raises."""
     _last = [None]
     _jac = [None, None, None]            # the state, (device, dtype) and (nlb, has_ub) of the last forward
 
@@ -473,6 +583,10 @@ def BoxQPFunction(eps=1e-12, verbose=0, notImprovedLim=3, maxIter=20, check_Q_sp
             ranks = (3 if dense_Q else 2, 2, 3, 2, 2, 2)
             flags = [X is not None and X.nelement() > 0 and X.dim() == r - 1 for X, r in zip(ins, ranks)]
             want = list(ctx.needs_input_grad)
+            if torch.is_grad_enabled():          # create_graph=True: gradients that can be differentiated again
+                if st.dense is None:
+                    return BoxQPBackwardFn.apply(st, flags, want, dl_dzhat, dl_dlam, dl_dnu, *ins)
+                return dense_backward_graph(st, dl_dzhat, flags, want, ins, dl_dlam, dl_dnu, dense_Q)
             if st.dense is None:
                 outs = solve_box_backward(st, dl_dzhat, flags, want, dl_dlam, dl_dnu)
             else:

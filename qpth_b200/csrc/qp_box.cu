@@ -45,6 +45,9 @@
 #include "qp_box_loop.cuh"
 
 extern "C" int qpb200_internal_set_smem(const void* kernel, size_t bytes);   // (qp_kernels.cu) the kernels' smem limits
+// (qp_kernels.cu) out = scale sum_b sum_k u_k[b] x_k[b]' by k_ggrad_sum: the double backward's batch sums of dA and dQ
+extern "C" int qpb200_internal_ggrad_sum(int B, int rows, int cols, const double* const* u, const double* const* x,
+                                         double scale, double* out, void* stream);
 
 namespace {
 
@@ -1178,6 +1181,125 @@ k_box_jvp_rhs(int n, int e, int nlb, int m, const double* __restrict__ dq, int64
     for (int i = tid; i < e; i += kJvpNT) ry[qp * e + i] = ay[i];
 }
 
+// Double backward (qpb200_box_double_backward): the cotangents of the solution (z, lam, nu) that go through the dual
+// backward, for cotangents w on the first backward's outputs, v = (vx, vlam, vnu) its solve and ulam the lam part of
+// the JVP with tangents w (qp_kernels.cu's k_ggrad_rhs with Q = diag(q), G = [-I; I] constant, no wG):
+//   cz = wq o vx + wA' vnu + c_s_lb - c_s_ub,   clam = c_lam,   cnu = wA vx,
+// and c_s itself (the lb and ub gradients need it), from jvp::clamp_cotangents. wA is read once with jvp::contract; cz is
+// written straight from its column pass, as k_box_jvp_rhs writes rx. Shared memory: vx (n), vnu and the cnu
+// accumulator (e), the column partials: box_jvp_smem_bytes(n, e), 200 KB at the plan's limits n = 16384, e = 4096.
+// Algorithmic bytes per QP: 8 e n of wA, 8 (2 n + 4 m + e) of vectors read, 8 (n + 2 m + e) written.
+__global__ void __launch_bounds__(kJvpNT)
+k_box_ggrad_rhs(int n, int e, int nlb, int m, const double* __restrict__ wq, int64_t swq, const double* __restrict__ wA,
+                int64_t swA, const double* __restrict__ dxv, const double* __restrict__ dlamv,
+                const double* __restrict__ dnuv, const double* __restrict__ ulam, const double* __restrict__ lam,
+                const double* __restrict__ slacks, double* __restrict__ cz, double* __restrict__ clam,
+                double* __restrict__ cnu, double* __restrict__ cs) {
+    QPB_SMEM;
+    const int64_t qp = blockIdx.x;
+    const int tid = threadIdx.x;
+    double* vx = qsm;
+    double* vn = vx + r8(n);
+    double* an = vn + r8(e);
+    double* part = an + r8(e);
+    const int64_t o = qp * m;
+    auto c_s = [&](int i) {                        // row i's c_s, and its c_lam into clam
+        double cl, c;
+        qpb::jvp::clamp_cotangents(lam[o + i], slacks[o + i], ulam[o + i], dlamv[o + i], cl, c);
+        clam[o + i] = cl;
+        cs[o + i] = c;
+        return c;
+    };
+    for (int i = tid; i < n; i += kJvpNT) vx[i] = dxv[qp * n + i];
+    for (int i = tid; i < e; i += kJvpNT) {
+        vn[i] = dnuv[qp * e + i];
+        an[i] = 0.0;
+    }
+    __syncthreads();
+    auto x_part = [&](int c) {                   // wq o vx + c_s_lb - c_s_ub
+        const double a = nlb ? c_s(c) : 0.0, b = m > nlb ? c_s(nlb + c) : 0.0;
+        return wq ? fma(wq[qp * swq + c], vx[c], a - b) : a - b;
+    };
+    if (wA && e > 0) {
+        qpb::jvp::contract<kJvpNT>(wA + qp * swA, e, n, vx, vn, part, [&](int r, double s) { an[r] += s; },
+                                   [&](int c, double s) { cz[qp * n + c] = x_part(c) + s; });
+    } else {
+        for (int c = tid; c < n; c += kJvpNT) cz[qp * n + c] = x_part(c);
+        __syncthreads();
+    }
+    for (int i = tid; i < e; i += kJvpNT) cnu[qp * e + i] = an[i];
+}
+
+// The per-QP second-order gradients of both box units (qpb200_internal_box_ggrad_out) from v, u (the JVP), w (the dual
+// backward of k_box_ggrad_rhs's cotangents) and c_s:
+//   dq = wx o z + ux o vx (dense: dQ = sym(wx z' + ux vx')),   dp = wx,   dlb = wlam_lb - c_s_lb,
+//   dub = c_s_ub - wlam_ub,   dA = wnu z' + nu wx' + vnu ux' + unu vx',   db = -wnu.
+// Every product is rounded on its own and the terms added as (a + b) + (c + d), so dQ is symmetric bit for bit. One
+// pass over each output, QP blockIdx.x, its elements strided over blockIdx.y and the threads.
+struct BoxGgTerms { const double *z, *nu, *vx, *vn, *ux, *un, *wx, *wl, *wn, *cs; };
+struct BoxGgOut { double *dq, *dp, *dlb, *dub, *dA, *db; };
+__device__ __forceinline__ double box_gg2(double a0, double b0, double a1, double b1) {
+    return __dadd_rn(__dmul_rn(a0, b0), __dmul_rn(a1, b1));
+}
+__device__ __forceinline__ double box_gg4(double a0, double b0, double a1, double b1, double a2, double b2, double a3,
+                                          double b3) {
+    return __dadd_rn(box_gg2(a0, b0, a1, b1), box_gg2(a2, b2, a3, b3));
+}
+__global__ void __launch_bounds__(256)
+k_box_ggrad_out(int n, int e, int nlb, int m, int dense, BoxGgTerms T, BoxGgOut O) {
+    const int64_t qp = blockIdx.x;
+    const int64_t i0 = (int64_t)blockIdx.y * blockDim.x + threadIdx.x, step = (int64_t)gridDim.y * blockDim.x;
+    const double* z = T.z + qp * n;
+    const double* vx = T.vx + qp * n;
+    const double* ux = T.ux + qp * n;
+    const double* wx = T.wx + qp * n;
+    if (O.dq && dense) {
+        double* o = O.dq + qp * n * n;
+        for (int64_t i = i0; i < (int64_t)n * n; i += step) {
+            const int r = (int)(i / n), c = (int)(i - (int64_t)r * n);
+            o[i] = 0.5 * box_gg4(wx[r], z[c], z[r], wx[c], ux[r], vx[c], vx[r], ux[c]);
+        }
+    } else if (O.dq) {
+        for (int64_t i = i0; i < n; i += step) O.dq[qp * n + i] = box_gg2(wx[i], z[i], ux[i], vx[i]);
+    }
+    if (O.dp) for (int64_t i = i0; i < n; i += step) O.dp[qp * n + i] = wx[i];
+    const double* wl = T.wl + qp * m;
+    const double* cs = T.cs + qp * m;
+    if (O.dlb) for (int64_t i = i0; i < n; i += step) O.dlb[qp * n + i] = wl[i] - cs[i];
+    if (O.dub) for (int64_t i = i0; i < n; i += step) O.dub[qp * n + i] = cs[nlb + i] - wl[nlb + i];
+    if (e > 0) {
+        const double* nu = T.nu + qp * e;
+        const double* vn = T.vn + qp * e;
+        const double* un = T.un + qp * e;
+        const double* wn = T.wn + qp * e;
+        if (O.dA) {
+            double* o = O.dA + qp * e * n;
+            for (int64_t i = i0; i < (int64_t)e * n; i += step) {
+                const int r = (int)(i / n), c = (int)(i - (int64_t)r * n);
+                o[i] = box_gg4(wn[r], z[c], nu[r], wx[c], vn[r], ux[c], un[r], vx[c]);
+            }
+        }
+        if (O.db) for (int64_t i = i0; i < e; i += step) O.db[qp * e + i] = -wn[i];
+    }
+}
+
+// Batch sums of the box vectors for un-batched inputs: out[i] = scale sum_b t_b[i], the batch in ascending order (no
+// atomics, so the result does not depend on the launch), every array at batch stride s:
+//   t = u0 o x0 + u1 o x1 (x0 given: dq),   t = u0 - u1 (u1 given, x0 NULL: wlam - c_s),   t = u0 (dp, db).
+__global__ void __launch_bounds__(256)
+k_box_ggrad_sum_vec(int B, int len, int64_t s, const double* __restrict__ u0, const double* __restrict__ x0,
+                    const double* __restrict__ u1, const double* __restrict__ x1, double scale,
+                    double* __restrict__ out) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= len) return;
+    double acc = 0.0;
+    for (int b = 0; b < B; ++b) {
+        const int64_t at = (int64_t)b * s + i;
+        acc += x0 ? box_gg2(u0[at], x0[at], u1[at], x1[at]) : (u1 ? u0[at] - u1[at] : u0[at]);
+    }
+    out[i] = acc * scale;
+}
+
 int box_plan_check(const qpb200_box_plan* P) {
     if (P == nullptr) return QPB200_ERR_BAD_ARG;
     if (P->cl_ctas != 0 && P->cl_ctas != 2 && P->cl_ctas != 4 && P->cl_ctas != 8) return QPB200_ERR_BAD_ARG;
@@ -1419,6 +1541,94 @@ int qpb200_box_jvp(const qpb200_box_plan* plan, int nbatch, const double* q, int
     return qpb200_box_backward_duals(plan, nbatch, q, sq, A, sA, rx, (dlb || dub) ? rz : nullptr, (dA || db) ? ry : nullptr,
                                      zhat, lam, slacks, nus, nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0,
                                      nullptr, 0, dz, dlam, dnu, stream);
+}
+
+// The second-order gradients of both box units (here and in qpb200_boxq_double_backward, qp_boxq.cu) after the dual
+// backward: k_box_ggrad_out for the per-QP ones (dense: dq is a dense dQ), the batch sums of the un-batched ones
+// (sum_X) with k_box_ggrad_sum_vec and, for dA and a dense dQ, qp_kernels.cu's k_ggrad_sum.
+int qpb200_internal_box_ggrad_out(int nbatch, int n, int m, int e, int nlb, int dense, const double* zhat,
+                                  const double* nus, const double* dxv, const double* dnuv, const double* gg_z,
+                                  const double* gg_nu, const double* wx, const double* wl, const double* wn,
+                                  const double* cs, double* dq, int sum_q, double* dp, int sum_p, double* dlb,
+                                  int sum_lb, double* dub, int sum_ub, double* dA, int sum_A, double* db, int sum_b,
+                                  void* stream) {
+    cudaStream_t st = (cudaStream_t)stream;
+    const BoxGgTerms T{zhat, nus, dxv, dnuv, gg_z, gg_nu, wx, wl, wn, cs};
+    const BoxGgOut O{sum_q ? nullptr : dq, sum_p ? nullptr : dp, sum_lb ? nullptr : dlb, sum_ub ? nullptr : dub,
+                     (sum_A || e == 0) ? nullptr : dA, (sum_b || e == 0) ? nullptr : db};
+    if (O.dq || O.dp || O.dlb || O.dub || O.dA || O.db) {
+        const int64_t most = (int64_t)n * (dense ? (n > e ? n : e) : (e > 1 ? e : 1));
+        const int64_t chunks = (most + 256 * 8 - 1) / (256 * 8);
+        k_box_ggrad_out<<<dim3(nbatch, (unsigned)(chunks < 64 ? chunks : 64)), 256, 0, st>>>(n, e, nlb, m, dense, T, O);
+    }
+    const int TB = 256;
+    auto vsum = [&](int len, int64_t s, const double* u0, const double* x0, const double* u1, const double* x1,
+                    double scale, double* out) {
+        k_box_ggrad_sum_vec<<<(len + TB - 1) / TB, TB, 0, st>>>(nbatch, len, s, u0, x0, u1, x1, scale, out);
+    };
+    if (dq && sum_q && dense) {
+        const double* u[4] = {wx, zhat, gg_z, dxv};
+        const double* x[4] = {zhat, wx, dxv, gg_z};
+        const int rc = qpb200_internal_ggrad_sum(nbatch, n, n, u, x, 0.5, dq, stream);
+        if (rc) return rc;
+    } else if (dq && sum_q) {
+        vsum(n, n, wx, zhat, gg_z, dxv, 1.0, dq);
+    }
+    if (dp && sum_p) vsum(n, n, wx, nullptr, nullptr, nullptr, 1.0, dp);
+    if (dlb && sum_lb) vsum(n, m, wl, nullptr, cs, nullptr, 1.0, dlb);
+    if (dub && sum_ub) vsum(n, m, wl + nlb, nullptr, cs + nlb, nullptr, -1.0, dub);
+    if (e > 0) {
+        if (dA && sum_A) {
+            const double* u[4] = {wn, nus, dnuv, gg_nu};
+            const double* x[4] = {zhat, wx, gg_z, dxv};
+            const int rc = qpb200_internal_ggrad_sum(nbatch, e, n, u, x, 1.0, dA, stream);
+            if (rc) return rc;
+        }
+        if (db && sum_b) vsum(e, e, wn, nullptr, nullptr, nullptr, -1.0, db);
+    }
+    return box_check_launch("k_box_ggrad_out");
+}
+
+int qpb200_box_double_backward(const qpb200_box_plan* plan, int nbatch, const double* q, int64_t sq, const double* A,
+                               int64_t sA, const double* wq, int64_t swq, const double* wp, int64_t swp,
+                               const double* wA, int64_t swA, const double* wb, int64_t swb, const double* wlb,
+                               int64_t swlb, const double* wub, int64_t swub, const double* dxv, const double* dlamv,
+                               const double* dnuv, const double* zhat, const double* lam, const double* slacks,
+                               const double* nus, double* gg_z, double* gg_lam, double* gg_nu, double* dq, int sum_q,
+                               double* dp, int sum_p, double* dlb, int sum_lb, double* dub, int sum_ub, double* dA,
+                               int sum_A, double* db, int sum_b, double* work, void* stream) {
+    // the checks beyond qpb200_box_jvp's, which that call runs before its first launch
+    int rc = box_plan_check(plan);
+    if (rc) return rc;
+    if (!dxv || !dlamv || !work || (plan->neq > 0 && !dnuv)) return QPB200_ERR_BAD_ARG;
+    if (plan->neq == 0 && (dA || db)) return QPB200_ERR_BAD_ARG;
+    if ((dlb && !plan->has_lb) || (dub && !plan->has_ub)) return QPB200_ERR_BAD_ARG;
+    const int n = plan->nz, m = plan->nineq, e = plan->neq, nlb = plan->has_lb ? n : 0;
+    rc = qpb200_box_jvp(plan, nbatch, q, sq, A, sA, wq, swq, wp, swp, wA, swA, wb, swb, wlb, swlb, wub, swub, zhat, lam,
+                        slacks, nus, work, gg_z, gg_lam, gg_nu, stream);
+    if (rc) return rc;
+    // work: the JVP's right-hand side, then cz, clam, cnu (B (n + m + e)); c_s (B m); wx, wlam, wnu (B (n + m + e))
+    const int64_t B = nbatch;
+    double* cz = work;
+    double* clam = cz + B * n;
+    double* cnu = clam + B * m;
+    double* cs = cnu + B * e;
+    double* wx = cs + B * m;
+    double* wl = wx + B * n;
+    double* wn = wl + B * m;
+    const size_t bytes = box_jvp_smem_bytes(n, e);
+    rc = qpb200_internal_set_smem((const void*)k_box_ggrad_rhs, bytes);
+    if (rc) return rc;
+    k_box_ggrad_rhs<<<nbatch, kJvpNT, bytes, (cudaStream_t)stream>>>(n, e, nlb, m, wq, swq, wA, swA, dxv, dlamv, dnuv,
+                                                                     gg_lam, lam, slacks, cz, clam, cnu, cs);
+    rc = box_check_launch("k_box_ggrad_rhs");
+    if (rc) return rc;
+    rc = qpb200_box_backward_duals(plan, nbatch, q, sq, A, sA, cz, clam, (e > 0 && wA) ? cnu : nullptr, zhat, lam, slacks,
+                                   nus, nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0, wx, wl,
+                                   e > 0 ? wn : nullptr, stream);
+    if (rc) return rc;
+    return qpb200_internal_box_ggrad_out(nbatch, n, m, e, nlb, 0, zhat, nus, dxv, dnuv, gg_z, gg_nu, wx, wl, wn, cs, dq,
+                                         sum_q, dp, sum_p, dlb, sum_lb, dub, sum_ub, dA, sum_A, db, sum_b, stream);
 }
 
 int qpb200_box_solve_kkt(const qpb200_box_plan* plan, int nbatch, const double* q, int64_t sq, const double* A,

@@ -49,6 +49,13 @@ extern "C" int qpb200_internal_box_means(int nbatch, int n, int m, int e, int nl
                                          const double* dlamv, const double* dnuv, const double* zhat, const double* nus,
                                          double* dp, int mean_p, double* dlb, int mean_lb, double* dub, int mean_ub,
                                          double* dA, int mean_A, double* db, int mean_b, void* stream);
+// (qp_box.cu) the double backward's per-QP gradients and batch sums, as in qpb200_box_double_backward (dense: dQ)
+extern "C" int qpb200_internal_box_ggrad_out(int nbatch, int n, int m, int e, int nlb, int dense, const double* zhat,
+                                             const double* nus, const double* dxv, const double* dnuv,
+                                             const double* gg_z, const double* gg_nu, const double* wx,
+                                             const double* wl, const double* wn, const double* cs, double* dq,
+                                             int sum_q, double* dp, int sum_p, double* dlb, int sum_lb, double* dub,
+                                             int sum_ub, double* dA, int sum_A, double* db, int sum_b, void* stream);
 
 namespace {
 
@@ -315,6 +322,52 @@ k_boxq_jvp_rhs(int n, int e, int nlb, int m, const double* __restrict__ dQ, int6
     for (int i = tid; i < e; i += kBoxNT) ry[qp * e + i] = ay[i];
 }
 
+// Double backward (qpb200_boxq_double_backward): k_box_ggrad_rhs (qp_box.cu) with the cotangent wQ of a dense Q,
+//   cz = sym(wQ) vx + wA' vnu + c_s_lb - c_s_ub,   clam = c_lam,   cnu = wA vx,
+// one jvp::contract pass over wQ (into the n accumulator of cz) and one over wA. Shared memory: vx and cz (n), vnu and
+// cnu (e), the column partials: boxq_jvp_smem_bytes(n, e).
+__global__ void __launch_bounds__(kBoxNT)
+k_boxq_ggrad_rhs(int n, int e, int nlb, int m, const double* __restrict__ wQ, int64_t swQ, const double* __restrict__ wA,
+                 int64_t swA, const double* __restrict__ dxv, const double* __restrict__ dlamv,
+                 const double* __restrict__ dnuv, const double* __restrict__ ulam, const double* __restrict__ lam,
+                 const double* __restrict__ slacks, double* __restrict__ cz, double* __restrict__ clam,
+                 double* __restrict__ cnu, double* __restrict__ cs) {
+    QPB_SMEM;
+    const int64_t qp = blockIdx.x;
+    const int tid = threadIdx.x;
+    double* vx = qsm;
+    double* az = vx + r8(n);
+    double* vn = az + r8(n);
+    double* an = vn + r8(e);
+    double* part = an + r8(e);
+    const int64_t o = qp * m;
+    auto c_s = [&](int i) {                        // row i's c_s, and its c_lam into clam
+        double cl, c;
+        qpb::jvp::clamp_cotangents(lam[o + i], slacks[o + i], ulam[o + i], dlamv[o + i], cl, c);
+        clam[o + i] = cl;
+        cs[o + i] = c;
+        return c;
+    };
+    for (int i = tid; i < n; i += kBoxNT) {
+        vx[i] = dxv[qp * n + i];
+        az[i] = (nlb ? c_s(i) : 0.0) - (m > nlb ? c_s(nlb + i) : 0.0);
+    }
+    for (int i = tid; i < e; i += kBoxNT) {
+        vn[i] = dnuv[qp * e + i];
+        an[i] = 0.0;
+    }
+    __syncthreads();
+    if (wQ)
+        qpb::jvp::contract<kBoxNT>(wQ + qp * swQ, n, n, vx, vx, part, [&](int r, double s) { az[r] += 0.5 * s; },
+                                 [&](int c, double s) { az[c] += 0.5 * s; });
+    if (wA && e > 0)
+        qpb::jvp::contract<kBoxNT>(wA + qp * swA, e, n, vx, vn, part, [&](int r, double s) { an[r] += s; },
+                                 [&](int c, double s) { az[c] += s; });
+    __syncthreads();
+    for (int i = tid; i < n; i += kBoxNT) cz[qp * n + i] = az[i];
+    for (int i = tid; i < e; i += kBoxNT) cnu[qp * e + i] = an[i];
+}
+
 int boxq_plan_check(const qpb200_boxq_plan* P) {
     if (P == nullptr) return QPB200_ERR_BAD_ARG;
     if (!P->ok) return QPB200_ERR_TOO_LARGE;
@@ -517,6 +570,48 @@ int qpb200_boxq_jvp(const qpb200_boxq_plan* plan, int nbatch, const double* Q, i
     return qpb200_boxq_backward_duals(plan, nbatch, Q, sQ, A, sA, rx, (dlb || dub) ? rz : nullptr,
                                       (dA || db) ? ry : nullptr, zhat, lam, slacks, nus, nullptr, 0, nullptr, 0, nullptr,
                                       0, nullptr, 0, nullptr, 0, nullptr, 0, dz, dlam, dnu, stream);
+}
+
+int qpb200_boxq_double_backward(const qpb200_boxq_plan* plan, int nbatch, const double* Q, int64_t sQ,
+                                const double* A, int64_t sA, const double* wQ, int64_t swQ, const double* wp,
+                                int64_t swp, const double* wA, int64_t swA, const double* wb, int64_t swb,
+                                const double* wlb, int64_t swlb, const double* wub, int64_t swub, const double* dxv,
+                                const double* dlamv, const double* dnuv, const double* zhat, const double* lam,
+                                const double* slacks, const double* nus, double* gg_z, double* gg_lam, double* gg_nu,
+                                double* dQ, int sum_Q, double* dp, int sum_p, double* dlb, int sum_lb, double* dub,
+                                int sum_ub, double* dA, int sum_A, double* db, int sum_b, double* work, void* stream) {
+    // the checks beyond qpb200_boxq_jvp's, which that call runs before its first launch
+    int rc = boxq_plan_check(plan);
+    if (rc) return rc;
+    if (!dxv || !dlamv || !work || (plan->neq > 0 && !dnuv)) return QPB200_ERR_BAD_ARG;
+    if (plan->neq == 0 && (dA || db)) return QPB200_ERR_BAD_ARG;
+    if ((dlb && !plan->has_lb) || (dub && !plan->has_ub)) return QPB200_ERR_BAD_ARG;
+    const int n = plan->nz, m = plan->nineq, e = plan->neq, nlb = plan->has_lb ? n : 0;
+    rc = qpb200_boxq_jvp(plan, nbatch, Q, sQ, A, sA, wQ, swQ, wp, swp, wA, swA, wb, swb, wlb, swlb, wub, swub, zhat, lam,
+                         slacks, nus, work, gg_z, gg_lam, gg_nu, stream);
+    if (rc) return rc;
+    // work as in qpb200_box_double_backward
+    const int64_t B = nbatch;
+    double* cz = work;
+    double* clam = cz + B * n;
+    double* cnu = clam + B * m;
+    double* cs = cnu + B * e;
+    double* wx = cs + B * m;
+    double* wl = wx + B * n;
+    double* wn = wl + B * m;
+    const size_t bytes = boxq_jvp_smem_bytes(n, e);
+    rc = qpb200_internal_set_smem((const void*)k_boxq_ggrad_rhs, bytes);
+    if (rc) return rc;
+    k_boxq_ggrad_rhs<<<nbatch, kBoxNT, bytes, (cudaStream_t)stream>>>(n, e, nlb, m, wQ, swQ, wA, swA, dxv, dlamv, dnuv,
+                                                                      gg_lam, lam, slacks, cz, clam, cnu, cs);
+    rc = box_check_launch("k_boxq_ggrad_rhs");
+    if (rc) return rc;
+    rc = qpb200_boxq_backward_duals(plan, nbatch, Q, sQ, A, sA, cz, clam, (e > 0 && wA) ? cnu : nullptr, zhat, lam,
+                                    slacks, nus, nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0,
+                                    wx, wl, e > 0 ? wn : nullptr, stream);
+    if (rc) return rc;
+    return qpb200_internal_box_ggrad_out(nbatch, n, m, e, nlb, 1, zhat, nus, dxv, dnuv, gg_z, gg_nu, wx, wl, wn, cs, dQ,
+                                         sum_Q, dp, sum_p, dlb, sum_lb, dub, sum_ub, dA, sum_A, db, sum_b, stream);
 }
 
 int qpb200_boxq_solve_kkt(const qpb200_boxq_plan* plan, int nbatch, const double* Q, int64_t sQ, const double* A,

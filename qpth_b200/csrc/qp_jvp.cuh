@@ -68,5 +68,15 @@ __device__ __forceinline__ void contract(const double* __restrict__ M, int R, in
     }
 }
 
+// The double backward's cotangents of the backward's clamped D = clamp(lam, 1e-8) / clamp(s, 1e-8) at one inequality
+// row (k_box_ggrad_rhs, k_boxq_ggrad_rhs): with c_D = (ulam / D)(vlam / D), c_lam = c_D / clamp(s) where lam >= 1e-8
+// and c_s = -c_D D / clamp(s) where s >= 1e-8, each 0 elsewhere (torch's clamp passes the gradient at the bound).
+__device__ __forceinline__ void clamp_cotangents(double l, double s, double ul, double vl, double& c_lam, double& c_s) {
+    const double sc = fmax(s, 1e-8), d = fmax(l, 1e-8) / sc;
+    const double cd = (ul / d) * (vl / d);
+    c_lam = l >= 1e-8 ? cd / sc : 0.0;
+    c_s = s >= 1e-8 ? -cd * d / sc : 0.0;
+}
+
 }  // namespace jvp
 }  // namespace qpb

@@ -2020,6 +2020,15 @@ int qpb200_double_backward_reg(const qpb200_plan* plan, int nbatch, const double
 }
 #undef QPB_GG_ARGS
 
+// (qp_box.cu) the batch sums of the box double backward's dA and dense dQ: k_ggrad_sum with the pairs (u_k, x_k)
+int qpb200_internal_ggrad_sum(int B, int rows, int cols, const double* const* u, const double* const* x, double scale,
+                              double* out, void* stream) {
+    gg_sum(B, rows, cols, GgPairs{{u[0], u[1], u[2], u[3]}, {x[0], x[1], x[2], x[3]}, nullptr}, scale, out,
+           (cudaStream_t)stream);
+    CK(cudaGetLastError());
+    return QPB200_OK;
+}
+
 #ifdef QPB_TIMING
 int qpb200_debug_timing(long long* host64, int reset) {
     if (reset) {                          // 1: clear the slots; 2 + qp: clear and export QP `qp`'s slots from now on
