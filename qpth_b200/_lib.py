@@ -6,6 +6,8 @@ present when a solve is requested, the call fails loudly.
 import ctypes
 import os
 
+import torch
+
 _HERE = os.path.dirname(os.path.abspath(__file__))
 # QPB200_LIB: development override (A/B builds of the kernels); the product is the in-tree libqpth_b200.so
 LIB_PATH = os.environ.get("QPB200_LIB") or os.path.join(_HERE, "libqpth_b200.so")
@@ -162,6 +164,44 @@ def check(rc):
         raise QpthB200Error("qpth_b200: " + msg)
 
 
+def ptr(t):
+    """A tensor's data as a C pointer; None and empty tensors are NULL."""
+    return ctypes.c_void_p(t.data_ptr()) if t is not None and t.numel() > 0 else ctypes.c_void_p(0)
+
+
+def stream():
+    """The current CUDA stream of the current device, for the C calls."""
+    return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
+
+
+def dev64(t, device):
+    """fp64, contiguous, on `device`; un-batched tensors stay un-batched (stride 0 is passed to C)."""
+    return t.detach().to(device=device, dtype=torch.float64).contiguous()
+
+
+def pre_factor(plan, nsys, nBatch, Q, sQ, G, sG, A, sA, reg_eps, device, cu_stream):
+    """qpb200_pre_factor_kkt of nsys systems (batch strides sQ, sG, sA), or qpb200_pre_factor_kkt_reg with reg_eps
+    unless it is None, into new buffers sized by `plan`; the scratch also serves the solves of nBatch QPs. cu_stream:
+    the stream argument of the C call, from the caller's stream helper. Call it under torch.cuda.device(device).
+    Returns (L, W, K, scratch, spd): scratch is None where the plan needs none, and spd (nsys,) int32 flags the systems
+    whose Cholesky factorization broke down."""
+    f64 = dict(dtype=torch.float64, device=device)
+    L = torch.empty(nsys * plan.L_elems, **f64)
+    W = torch.empty(nsys * plan.W_elems, **f64)
+    K = torch.empty(nsys * plan.K_elems, **f64)
+    spd = torch.zeros(nsys, dtype=torch.int32, device=device)
+    nscr = max(nsys * plan.setup_scratch_elems, nBatch * plan.solve_scratch_elems)
+    scratch = torch.empty(nscr, **f64) if nscr > 0 else None
+    lib = load()
+    args = (ctypes.byref(plan), nsys, ptr(Q), sQ, ptr(G), sG, ptr(A), sA)
+    out = (ptr(L), ptr(W), ptr(K), ptr(spd), ptr(scratch), cu_stream)
+    if reg_eps is None:
+        check(lib.qpb200_pre_factor_kkt(*args, *out))
+    else:
+        check(lib.qpb200_pre_factor_kkt_reg(*args, float(reg_eps), *out))
+    return L, W, K, scratch, spd
+
+
 _plans = {}
 
 
@@ -248,6 +288,5 @@ _sm_count = {}
 
 def sm_count(device_index):
     if device_index not in _sm_count:
-        import torch
         _sm_count[device_index] = torch.cuda.get_device_properties(device_index).multi_processor_count
     return _sm_count[device_index]

@@ -85,7 +85,7 @@ def solve_box_forward(q_, p_, A_, b_, lb_, ub_, eps=1e-12, verbose=0, notImprove
     if _qp._pending:
         _qp.flush_checks(wait=False)
     assert maxIter >= 1
-    lib = _lib.load()
+    _lib.load()
     if not torch.cuda.is_available():
         raise _lib.QpthB200Error("qpth_b200: no CUDA device available (there is no CPU fallback).")
     if dense_Q:
@@ -121,8 +121,7 @@ def solve_box_forward(q_, p_, A_, b_, lb_, ub_, eps=1e-12, verbose=0, notImprove
         st.best_resid = torch.empty(nBatch, **f64)
         st.trace = torch.full((nBatch, int(maxIter), 4), float('nan'), **f64) if (verbose == 1 or _qp.TRACE) else None
         spd = torch.zeros(nBatch, dtype=torch.int32, device=device)
-        fn = lib.qpb200_boxq_forward if dense_Q else lib.qpb200_box_forward
-        _lib.check(fn(
+        _lib.check(_entry(st, "forward")(
             ctypes.byref(plan), nBatch, _ptr(q), st.sq, _ptr(p), stride(p, 2, nz), _ptr(A), st.sA,
             _ptr(b), stride(b, 2, neq), _ptr(lb), stride(lb, 2, nz), _ptr(ub), stride(ub, 2, nz),
             float(eps), float(_qp.STALL_TOL), float(_qp.BEST_TIE), int(notImprovedLim), int(maxIter),
@@ -132,6 +131,31 @@ def solve_box_forward(q_, p_, A_, b_, lb_, ub_, eps=1e-12, verbose=0, notImprove
     return st
 
 
+def _entry(st, name):
+    """The C entry point `name` of the layout of `st`: qpb200_boxq_<name> with a dense Q, else qpb200_box_<name>."""
+    return getattr(_lib.load(), ("qpb200_boxq_" if st.dense_Q else "qpb200_box_") + name)
+
+
+def _call(st, name, middle, tail):
+    """Check the C call `name` of the layout of `st` with its arguments: plan, nBatch, (q, sq, A, sA), `middle`, the
+    returned point (zhat, lam, slacks, nus), `tail`, the stream."""
+    _lib.check(_entry(st, name)(ctypes.byref(st.plan), st.nBatch, _ptr(st.q), st.sq, _ptr(st.A), st.sA, *middle,
+                                _ptr(st.zhat), _ptr(st.lam), _ptr(st.slacks), _ptr(st.nus), *tail, _stream()))
+
+
+def _grads(st, flags, want):
+    """The gradient outputs of the box layouts and their C arguments, in the ABI's order (dq, dp, dlb, dub, dA, db)."""
+    plan = st.plan
+    nz, neq = plan.nz, plan.neq
+    shapes = [(nz, nz) if st.dense_Q else (nz,), (nz,), (neq, nz), (neq,), (nz,), (nz,)]
+    absent = (False, False, neq == 0, neq == 0, not plan.has_lb, not plan.has_ub)
+    return _qp.grad_buffers(shapes, flags, want, absent, st.nBatch, st.device, (0, 1, 4, 5, 2, 3))
+
+
+def _ranks(st):
+    return (3 if st.dense_Q else 2, 2, 3, 2, 2, 2)
+
+
 def solve_box_backward(st, dl_dzhat, mean_flags, want, dl_dlam=None, dl_dnu=None, keep=False):
     """Gradients (dq, dp, dA, db, dlb, dub) on the device; mean_flags / want: 6-tuples in that order. dl_dlam ([lb rows;
     ub rows]) / dl_dnu: the gradients with respect to the returned duals (None: zero); dl_dzhat None: zero. With a
@@ -139,39 +163,19 @@ def solve_box_backward(st, dl_dzhat, mean_flags, want, dl_dlam=None, dl_dnu=None
     dnuv), which the double backward reads."""
     if _qp._pending:
         _qp.flush_checks(wait=False)
-    lib = _lib.load()
     plan, B, device = st.plan, st.nBatch, st.device
     nz, neq, m = plan.nz, plan.neq, plan.nineq
-    f64 = dict(dtype=torch.float64, device=device)
     with torch.cuda.device(device):
-        dl = _qp._adjoint(dl_dzhat, B, nz, device) if dl_dzhat is not None else torch.zeros(B, nz, **f64)
+        dl = (_qp._adjoint(dl_dzhat, B, nz, device) if dl_dzhat is not None
+              else torch.zeros(B, nz, dtype=torch.float64, device=device))
         glam, gnu = _qp._adjoint(dl_dlam, B, m, device), _qp._adjoint(dl_dnu, B, neq, device)
-        shapes = [(nz, nz) if st.dense_Q else (nz,), (nz,), (neq, nz), (neq,), (nz,), (nz,)]
-        outs = []
-        for k in range(6):
-            absent = (k in (2, 3) and neq == 0) or (k == 4 and not plan.has_lb) or (k == 5 and not plan.has_ub)
-            if not want[k] or absent:
-                outs.append(None)
-            else:
-                outs.append(torch.empty(*(shapes[k] if mean_flags[k] else (B,) + shapes[k]), **f64))
-        dxv = torch.empty(B, nz, **f64)
-        dlamv = torch.empty(B, m, **f64)
-        dnuv = torch.empty(B, neq, **f64) if neq > 0 else None
-        dq, dp, dA, db, dlb, dub = outs
-        mq, mp, mA, mb, mlb, mub = (1 if f else 0 for f in mean_flags)
-        if st.dense_Q:
-            fn, adj = lib.qpb200_boxq_backward_duals, (_ptr(glam), _ptr(gnu))
-        elif glam is None and gnu is None:          # no dual was used: the entry point of a zhat-only loss
-            fn, adj = lib.qpb200_box_backward, ()
+        outs, grads = _grads(st, mean_flags, want)
+        v = _qp.solve_triple(B, nz, m, neq, device)
+        if glam is None and gnu is None and not st.dense_Q:     # no dual was used: the entry point of a zhat-only loss
+            _call(st, "backward", (_ptr(dl),), (*grads, *(_ptr(x) for x in v)))
         else:
-            fn, adj = lib.qpb200_box_backward_duals, (_ptr(glam), _ptr(gnu))
-        _lib.check(fn(
-            ctypes.byref(plan), B, _ptr(st.q), st.sq, _ptr(st.A), st.sA, _ptr(dl), *adj, _ptr(st.zhat), _ptr(st.lam),
-            _ptr(st.slacks), _ptr(st.nus), _ptr(dq), mq, _ptr(dp), mp, _ptr(dlb), mlb, _ptr(dub), mub,
-            _ptr(dA), mA, _ptr(db), mb, _ptr(dxv), _ptr(dlamv), _ptr(dnuv), _stream()))
-    if keep:
-        return outs, (dxv, dlamv, dnuv)
-    return outs
+            _call(st, "backward_duals", (_ptr(dl), _ptr(glam), _ptr(gnu)), (*grads, *(_ptr(x) for x in v)))
+    return (outs, v) if keep else outs
 
 
 def solve_box_double_backward(st, v, omegas, flags, want):
@@ -183,63 +187,19 @@ def solve_box_double_backward(st, v, omegas, flags, want):
     (gg_nu None without equality rows) and of the six inputs (None where not wanted or absent)."""
     if _qp._pending:
         _qp.flush_checks(wait=False)
-    lib = _lib.load()
     plan, B, device = st.plan, st.nBatch, st.device
     nz, neq, m = plan.nz, plan.neq, plan.nineq
-    f64 = dict(dtype=torch.float64, device=device)
     absent = (False, False, neq == 0, neq == 0, not plan.has_lb, not plan.has_ub)
     with torch.cuda.device(device):
-        om = [None if (w is None or absent[k]) else (_dev64(w, device) / B if flags[k] else w)
+        om = [None if (w is None or absent[k]) else (_dev64(w, device) / B if flags[k] else _dev64(w, device))
               for k, w in enumerate(omegas)]
-        per = (nz * nz if st.dense_Q else nz, nz, neq * nz, neq, nz, nz)
-        tans = _qp.tangent_args(om, (3 if st.dense_Q else 2, 2, 3, 2, 2, 2), per, device)
-        shapes = [(nz, nz) if st.dense_Q else (nz,), (nz,), (neq, nz), (neq,), (nz,), (nz,)]
-        outs = []
-        for k in range(6):
-            if not want[k] or absent[k]:
-                outs.append(None)
-            else:
-                outs.append(torch.empty(*(shapes[k] if flags[k] else (B,) + shapes[k]), **f64))
-        gz = torch.empty(B, nz, **f64)
-        glam = torch.empty(B, m, **f64)
-        gnu = torch.empty(B, neq, **f64) if neq > 0 else None
-        work = torch.empty(B * (2 * nz + 3 * m + 2 * neq), **f64)      # QPB200_DOUBLE_BACKWARD_WORK
-        args = []
-        for t, s in tans:
-            args += [_ptr(t), s]
-        dq, dp, dA, db, dlb, dub = outs
-        grads = []
-        for g, k in zip((dq, dp, dlb, dub, dA, db), (0, 1, 4, 5, 2, 3)):   # the ABI's order
-            grads += [_ptr(g), 1 if flags[k] else 0]
-        fn = lib.qpb200_boxq_double_backward if st.dense_Q else lib.qpb200_box_double_backward
-        _lib.check(fn(
-            ctypes.byref(plan), B, _ptr(st.q), st.sq, _ptr(st.A), st.sA, *args, *(_ptr(x) for x in v),
-            _ptr(st.zhat), _ptr(st.lam), _ptr(st.slacks), _ptr(st.nus), _ptr(gz), _ptr(glam), _ptr(gnu), *grads,
-            _ptr(work), _stream()))
-    return [gz, glam, gnu] + outs
-
-
-class BoxQPBackwardFn(Function):
-    """The first-order backward of BoxQPFunction (the box kernels) as a differentiable function of the incoming
-    gradients (g_z, g_lam, g_nu) and of (q, p, A, b, lb, ub): what its backward runs under create_graph=True. Its
-    forward is the first backward's own solve_box_backward call; its backward is solve_box_double_backward."""
-    @staticmethod
-    def forward(ctx, st, flags, want, g_z, g_lam, g_nu, q, p, A, b, lb, ub):
-        outs, v = solve_box_backward(st, g_z, flags, want, g_lam, g_nu, keep=True)
-        ctx.st, ctx.v, ctx.flags = st, v, flags
-        ctx.like = (g_z, g_lam, g_nu, q, p, A, b, lb, ub)
-        ctx.set_materialize_grads(False)
-        return tuple(_qp._cast(g, X) for X, g in zip((q, p, A, b, lb, ub), outs))
-
-    @staticmethod
-    def backward(ctx, *omegas):
-        if torch.is_grad_enabled():
-            raise RuntimeError(_qp.THIRD_ORDER_ERR)
-        need = ctx.needs_input_grad[3:]
-        if all(w is None for w in omegas) or not any(need):
-            return (None,) * 12
-        res = solve_box_double_backward(ctx.st, ctx.v, omegas, ctx.flags, need[3:])
-        return (None, None, None) + tuple(_qp._cast(g, X) if n else None for g, X, n in zip(res, ctx.like, need))
+        tans = _qp.tangent_args(om, _ranks(st), (nz * nz if st.dense_Q else nz, nz, neq * nz, neq, nz, nz))
+        outs, grads = _grads(st, flags, want)
+        gg = _qp.solve_triple(B, nz, m, neq, device)
+        # QPB200_DOUBLE_BACKWARD_WORK
+        work = torch.empty(B * (2 * nz + 3 * m + 2 * neq), dtype=torch.float64, device=device)
+        _call(st, "double_backward", (*tans, *(_ptr(x) for x in v)), (*(_ptr(x) for x in gg), *grads, _ptr(work)))
+    return list(gg) + outs
 
 
 def solve_box_jvp(st, tangents):
@@ -249,28 +209,28 @@ def solve_box_jvp(st, tangents):
     kernel and the backward's solve."""
     if _qp._pending:
         _qp.flush_checks(wait=False)
-    lib = _lib.load()
     plan, B, device = st.plan, st.nBatch, st.device
     nz, neq, m = plan.nz, plan.neq, plan.nineq
-    f64 = dict(dtype=torch.float64, device=device)
     with torch.cuda.device(device):
+        tans = [None if t is None else _dev64(t, device) for t in tangents]
         per = (nz * nz if st.dense_Q else nz, nz, neq * nz, neq, nz if plan.has_lb else 0, nz if plan.has_ub else 0)
-        tans = _qp.tangent_args(tangents, (3 if st.dense_Q else 2, 2, 3, 2, 2, 2), per, device)
-        rhs = torch.empty(B * (nz + m + neq), **f64)
-        dz = torch.empty(B, nz, **f64)
-        dlam = torch.empty(B, m, **f64)
-        dnu = torch.empty(B, neq, **f64) if neq > 0 else None
-        args = []
-        for t, s in tans:
-            args += [_ptr(t), s]
-        fn = lib.qpb200_boxq_jvp if st.dense_Q else lib.qpb200_box_jvp
-        _lib.check(fn(
-            ctypes.byref(plan), B, _ptr(st.q), st.sq, _ptr(st.A), st.sA, *args, _ptr(st.zhat), _ptr(st.lam),
-            _ptr(st.slacks), _ptr(st.nus), _ptr(rhs), _ptr(dz), _ptr(dlam), _ptr(dnu), _stream()))
+        args = _qp.tangent_args(tans, _ranks(st), per)
+        rhs = torch.empty(B * (nz + m + neq), dtype=torch.float64, device=device)
+        dz, dlam, dnu = _qp.solve_triple(B, nz, m, neq, device)
+        _call(st, "jvp", args, (_ptr(rhs), _ptr(dz), _ptr(dlam), _ptr(dnu)))
     return dz, dlam, dnu
 
 
 # ---- shapes beyond the box kernels: the dense kernels on the dense equivalent ---------------------------------------
+def _side_rows(lo, hi):
+    """The right-hand side h = [lo; hi] of the sides given (None: absent), batched where either side is."""
+    sides = [s for s in (lo, hi) if s is not None]
+    if any(s.dim() == 2 for s in sides):
+        B = next(s.size(0) for s in sides if s.dim() == 2)
+        sides = [s if s.dim() == 2 else s.unsqueeze(0).expand(B, s.size(-1)) for s in sides]
+    return torch.cat(sides, -1)
+
+
 def dense_equivalent(q, lb, ub, dense_Q=False):
     """(Q, G, h) of QPFunction for a box QP: Q = diag(q) (dense_Q: q itself), G = [-I; I] (sides given),
     h = [-lb; ub]. Batched where q (for Q) or either bound (for h) is batched."""
@@ -278,13 +238,7 @@ def dense_equivalent(q, lb, ub, dense_Q=False):
     Q = q if dense_Q else torch.diag_embed(q)
     eye = torch.eye(nz, dtype=q.dtype, device=q.device)
     G = torch.cat(([-eye] if lb is not None else []) + ([eye] if ub is not None else []), 0)
-    sides = [(-lb) if lb is not None else None, ub]
-    sides = [s for s in sides if s is not None]
-    if any(s.dim() == 2 for s in sides):
-        B = next(s.size(0) for s in sides if s.dim() == 2)
-        sides = [s if s.dim() == 2 else s.unsqueeze(0).expand(B, nz) for s in sides]
-    h = torch.cat(sides, -1)
-    return Q, G, h
+    return Q, G, _side_rows(None if lb is None else -lb, ub)
 
 
 def solve_dense_forward(q_, p_, A_, b_, lb_, ub_, eps, verbose, notImprovedLim, maxIter, check_Q_spd, dense_Q=False):
@@ -304,52 +258,35 @@ def solve_dense_forward(q_, p_, A_, b_, lb_, ub_, eps, verbose, notImprovedLim, 
     return st
 
 
-def dense_backward(st, dl, mean_flags, want, nlb, has_ub, dl_dlam=None, dl_dnu=None, dense_Q=False):
+def dense_backward(st, dl, mean_flags, want, ins, dl_dlam=None, dl_dnu=None, dense_Q=False):
+    """The backward on the dense equivalent, mapped back to (dq, dp, dA, db, dlb, dub). The dense equivalent's rows are
+    lam's [lb rows; ub rows]: the dual adjoints pass through as they are. Without create_graph: qp.solve_backward on
+    the stored state. Under create_graph=True: (Q, h) built from the inputs with torch ops, qp.backward_graph on them
+    (G constant) and the map back in torch ops, so that the gradients can be differentiated once more."""
     dst, h_shared = st.dense
+    q, p, A, b, lb, ub = ins
     mq, mp, mA, mb, mlb, mub = mean_flags
-    # the dense equivalent's rows are lam's [lb rows; ub rows]: the dual adjoints pass through as they are
-    outs = _qp.solve_backward(dst, dl, (mq, mp, True, h_shared, mA, mb),
-                              (want[0], want[1], False, want[4] or want[5], want[2], want[3]), dl_dlam, dl_dnu)
-    dQ, dp, _, dh, dA, db = outs
+    flags = (mq, mp, True, h_shared, mA, mb)
+    dwant = (want[0], want[1], False, want[4] or want[5], want[2], want[3])
+    if torch.is_grad_enabled():
+        Q, G, h = dense_equivalent(q, lb, ub, dense_Q)
+        empty = torch.empty(0, dtype=q.dtype, device=q.device)
+        A_ = A if (A is not None and A.nelement() > 0) else empty
+        b_ = b if (b is not None and b.nelement() > 0) else empty
+        dQ, dp, _, dh, dA, db = _qp.backward_graph(dst, flags, dwant, dl, dl_dlam, dl_dnu, Q, p, G, h, A_, b_)
+    else:
+        dQ, dp, _, dh, dA, db = _qp.solve_backward(dst, dl, flags, dwant, dl_dlam, dl_dnu)
+    nlb = q.size(-1) if lb is not None else 0
     dq = dQ if (dQ is None or dense_Q) else torch.diagonal(dQ, dim1=-2, dim2=-1).contiguous()
     dlb = dub = None
     if dh is not None:
         if want[4] and nlb:
             dlb = -dh[..., :nlb]
             dlb = dlb.mean(0) if (mlb and dlb.dim() == 2) else dlb
-        if want[5] and has_ub:
-            dub = dh[..., nlb:]
-            dub = dub.mean(0) if (mub and dub.dim() == 2) else dub
-    return [dq, dp, dA, db, dlb, dub]
-
-
-def dense_backward_graph(st, dl, mean_flags, want, ins, dl_dlam=None, dl_dnu=None, dense_Q=False):
-    """dense_backward under create_graph=True: (Q, h) of the dense equivalent built from the inputs with torch ops, the
-    first backward through qp.QPBackwardFn on the dense state (G constant), and the map back to (dq, dp, dA, db, dlb,
-    dub) again with torch ops, so that the gradients can be differentiated once more. Returns them cast to the inputs."""
-    dst, h_shared = st.dense
-    q, p, A, b, lb, ub = ins
-    mq, mp, mA, mb, mlb, mub = mean_flags
-    Q, G, h = dense_equivalent(q, lb, ub, dense_Q)
-    empty = torch.empty(0, dtype=q.dtype, device=q.device)
-    A_ = A if (A is not None and A.nelement() > 0) else empty
-    b_ = b if (b is not None and b.nelement() > 0) else empty
-    dQ, dp, _, dh, dA, db = _qp.QPBackwardFn.apply(
-        dst, (mq, mp, True, h_shared, mA, mb), (want[0], want[1], False, want[4] or want[5], want[2], want[3]),
-        dl, dl_dlam, dl_dnu, Q, p, G, h, A_, b_)
-    nlb = q.size(-1) if lb is not None else 0
-    dq = dQ if (dQ is None or dense_Q) else torch.diagonal(dQ, dim1=-2, dim2=-1)
-    dlb = dub = None
-    if dh is not None:
-        if want[4] and lb is not None:
-            dlb = -dh[..., :nlb]
-            dlb = dlb.mean(0) if (mlb and dlb.dim() == 2) else dlb
         if want[5] and ub is not None:
             dub = dh[..., nlb:]
             dub = dub.mean(0) if (mub and dub.dim() == 2) else dub
-    outs = (dq, dp, dA, db, dlb, dub)
-    return tuple(None if (g is None or X is None or not w) else g.to(device=X.device, dtype=X.dtype)
-                 for X, g, w in zip(ins, outs, want))
+    return [dq, dp, dA, db, dlb, dub]
 
 
 def dense_jvp(st, tangents, nlb, has_ub, dense_Q=False):
@@ -360,18 +297,15 @@ def dense_jvp(st, tangents, nlb, has_ub, dense_Q=False):
     dQ = dq if (dq is None or dense_Q) else torch.diag_embed(dq)
     dh = None
     if dlb is not None or dub is not None:
-        sides = ([None if dlb is None else -dlb] if nlb else []) + ([dub] if has_ub else [])
-        like = next(s for s in sides if s is not None)
-        sides = [torch.zeros_like(like) if s is None else s for s in sides]
-        if any(s.dim() == 2 for s in sides):
-            B = next(s.size(0) for s in sides if s.dim() == 2)
-            sides = [s if s.dim() == 2 else s.unsqueeze(0).expand(B, s.size(-1)) for s in sides]
-        dh = torch.cat(sides, -1)
+        like = dlb if dlb is not None else dub
+        dh = _side_rows((torch.zeros_like(like) if dlb is None else -dlb) if nlb else None,
+                        (torch.zeros_like(like) if dub is None else dub) if has_ub else None)
     return _qp.solve_jvp(dst, (dQ, dp, None, dh, dA, db))
 
 
 # ---- Jacobians (jacobian() of BoxQPFunction): rows z, lam, nu as bits 0, 1, 2 and columns p, lb, ub, b as bits 0..3 ---
 BOX_JAC_WRT = ("p", "lb", "ub", "b")
+BOX_JAC_SLOTS = (1, 4, 5, 3)      # their tangents' slots in (dq, dp, dA, db, dlb, dub)
 
 
 def box_jacobian_covered(plan, dense_Q=False):
@@ -386,34 +320,15 @@ def box_jacobian_covered(plan, dense_Q=False):
 
 def _box_jacobian_kernel(st, rows, cols, J):
     """qpb200_box_jacobian (a dense Q: qpb200_boxq_jacobian) into J (B, R, C) fp64 on st.device."""
-    lib = _lib.load()
     with torch.cuda.device(st.device):
-        _lib.check((lib.qpb200_boxq_jacobian if st.dense_Q else lib.qpb200_box_jacobian)(
+        _lib.check(_entry(st, "jacobian")(
             ctypes.byref(st.plan), st.nBatch, rows, cols, _ptr(st.q), st.sq, _ptr(st.A), st.sA, _ptr(st.lam),
             _ptr(st.slacks), _ptr(J), _stream()))
 
 
 def _box_jacobian_columns(st, rows, cols, J):
-    """J column by column: one solve_box_jvp per column with an un-batched unit tangent of p, lb, ub or b (batch stride
-    0), which gives that column for every QP at once."""
-    plan = st.plan
-    sizes, rsizes = (plan.nz,) * 3 + (plan.neq,), (plan.nz, plan.nineq, plan.neq)
-    c0 = 0
-    for k in range(4):
-        if not (cols >> k) & 1:
-            continue
-        for j in range(sizes[k]):
-            t = torch.zeros(sizes[k], dtype=torch.float64, device=st.device)
-            t[j] = 1.0
-            tans = [None] * 6
-            tans[(1, 4, 5, 3)[k]] = t                    # (dq, dp, dA, db, dlb, dub): dp, dlb, dub or db
-            outs = solve_box_jvp(st, tans)
-            r0 = 0
-            for i in range(3):
-                if (rows >> i) & 1:
-                    J[:, r0:r0 + rsizes[i], c0 + j] = outs[i]
-                    r0 += rsizes[i]
-        c0 += sizes[k]
+    """qp.jacobian_columns for the columns p, lb, ub and b: unit tangents through solve_box_jvp."""
+    _qp.jacobian_columns(st, rows, cols, J, (st.plan.nz,) * 3 + (st.plan.neq,), BOX_JAC_SLOTS, solve_box_jvp)
 
 
 def _box_jacobian_dense(st, rows, cols, nlb, J):
@@ -443,56 +358,33 @@ def solve_box_jacobian(st, rows, cols, nlb):
     [z; lam; nu] and columns [p, lb, ub, b] restricted to the bits of `rows` / `cols`. nlb: nz if lb was given, else 0.
     One qpb200_box_jacobian (dense Q: qpb200_boxq_jacobian) call where the kernel covers the plan; otherwise one
     solve_box_jvp per column, and on the dense fallback the dense path's solve_jacobian."""
-    if _qp._pending:
-        _qp.flush_checks(wait=False)
-    plan = st.plan
-    n, m, e = plan.nz, plan.nineq, plan.neq
-    R = sum((n, m, e)[i] for i in range(3) if (rows >> i) & 1)
-    C = sum((n, n, n, e)[k] for k in range(4) if (cols >> k) & 1)
-    J = torch.empty(st.nBatch, R, C, dtype=torch.float64, device=st.device)
+    n = st.plan.nz
     if st.dense is not None:
-        _box_jacobian_dense(st, rows, cols, nlb, J)
-    elif box_jacobian_covered(plan, st.dense_Q):
-        _box_jacobian_kernel(st, rows, cols, J)
+        fill = lambda st_, rows_, cols_, J: _box_jacobian_dense(st_, rows_, cols_, nlb, J)   # noqa: E731
     else:
-        _box_jacobian_columns(st, rows, cols, J)
-    return J
+        fill = _box_jacobian_kernel if box_jacobian_covered(st.plan, st.dense_Q) else _box_jacobian_columns
+    return _qp.jacobian_matrix(st, rows, cols, (n, n, n, st.plan.neq), fill)
+
+
+def _box_refusal(nm):
+    if nm in ("q", "Q", "A"):
+        return ("qpth_b200: jacobian(wrt=...) does not take %r; contract the blocks it does give: "
+                "J_.,q = J_.,p diag(z) for a diagonal q, J_.,Q_ik = J_.,p_i z_k for a dense Q (which enters as sym(dQ)), "
+                "and J_.,A_ck = J_.,p_k nu_c - J_.,b_c z_k" % nm)
+    if nm not in BOX_JAC_WRT:
+        return "qpth_b200: jacobian(wrt=...) takes %s, not %r" % (BOX_JAC_WRT, nm)
+    return "qpth_b200: jacobian(wrt=%r): this problem has no %s" % (
+        nm, "equality constraints (neq == 0)" if nm == "b" else "%s side" % nm)
 
 
 def box_jacobian_of(st, out, sides, wrt, duals):
     """The `jacobian` attribute of BoxQPFunction on the state `st` of its last forward, whose output had
-    out = (device, dtype) and sides = (nlb, has_ub). Returns {name: (B, rows, n_name)} for each name of `wrt` (None:
-    every input the problem has), rows z, or [z; lam; nu] with duals."""
-    if st is None:
-        raise RuntimeError("qpth_b200: jacobian() needs a forward call of this function first")
-    nlb, has_ub = sides
-    n, e = st.plan.nz, st.plan.neq
-    present = ("p",) + (("lb",) if nlb else ()) + (("ub",) if has_ub else ()) + (("b",) if e > 0 else ())
-    names = present if wrt is None else ((wrt,) if isinstance(wrt, str) else tuple(wrt))
-    if not names:
-        raise ValueError("qpth_b200: jacobian(wrt=...) needs at least one of %s" % (present,))
-    for nm in names:
-        if nm in ("q", "Q", "A"):
-            raise ValueError(
-                "qpth_b200: jacobian(wrt=...) does not take %r; contract the blocks it does give: J_.,q = J_.,p diag(z) "
-                "for a diagonal q, J_.,Q_ik = J_.,p_i z_k for a dense Q (which enters as sym(dQ)), and "
-                "J_.,A_ck = J_.,p_k nu_c - J_.,b_c z_k" % nm)
-        if nm not in BOX_JAC_WRT:
-            raise ValueError("qpth_b200: jacobian(wrt=...) takes %s, not %r" % (BOX_JAC_WRT, nm))
-        if nm not in present:
-            raise ValueError("qpth_b200: jacobian(wrt=%r): this problem has no %s" % (
-                nm, "equality constraints (neq == 0)" if nm == "b" else "%s side" % nm))
-    cols = sum(1 << BOX_JAC_WRT.index(nm) for nm in set(names))
-    rows = 1 | ((2 | (4 if e > 0 else 0)) if duals else 0)
-    J = solve_box_jacobian(st, rows, cols, nlb)
-    res, c0 = {}, 0
-    for k, nm in enumerate(BOX_JAC_WRT):
-        if (cols >> k) & 1:
-            w = e if nm == "b" else n
-            res[nm] = J[:, :, c0:c0 + w]
-            c0 += w
-    device, dtype = out
-    return {nm: res[nm].to(device=device, dtype=dtype).contiguous() for nm in names}
+    out = (device, dtype) and sides = (nlb, has_ub): qp.jacobian_of on the columns p, lb, ub, b (wrt=None: every input
+    the problem has)."""
+    return _qp.jacobian_of(
+        st, out, wrt, duals,
+        lambda plan: tuple(zip(BOX_JAC_WRT, (plan.nz, sides[0], plan.nz if sides[1] else 0, plan.neq))),
+        lambda st_, rows, cols: solve_box_jacobian(st_, rows, cols, sides[0]), _box_refusal)
 
 
 def BoxQPFunction(eps=1e-12, verbose=0, notImprovedLim=3, maxIter=20, check_Q_spd=True, duals=False, dense_Q=False):
@@ -552,18 +444,11 @@ def BoxQPFunction(eps=1e-12, verbose=0, notImprovedLim=3, maxIter=20, check_Q_sp
             if st is None:
                 st = solve_dense_forward(q_, p_, A_, b_, lb_, ub_, eps, verbose, notImprovedLim, maxIter, check_Q_spd,
                                          dense_Q)
-            ctx.st = st
             _last[0] = st
-            zhats = st.zhat.to(device=q_.device, dtype=q_.dtype)
-            ctx.save_for_backward(zhats, q_, p_, A_, b_, lb_, ub_)
-            ctx.lams, ctx.slacks, ctx.nus = st.lam, st.slacks, st.nus
-            ctx.out = (q_.device, q_.dtype)
             ctx.sides = (q_.size(-1) if lb_ is not None else 0, ub_ is not None)
+            out = _qp.layer_outputs(ctx, st, (q_, p_, A_, b_, lb_, ub_), duals)
             _jac[:] = [st, ctx.out, ctx.sides]
-            ctx.set_materialize_grads(False)
-            if not duals:
-                return zhats
-            return (zhats,) + _qp.dual_outputs(st, q_)
+            return out
 
         @staticmethod
         def jvp(ctx, dq, dp, dA, db, dlb, dub):
@@ -583,17 +468,14 @@ def BoxQPFunction(eps=1e-12, verbose=0, notImprovedLim=3, maxIter=20, check_Q_sp
             ranks = (3 if dense_Q else 2, 2, 3, 2, 2, 2)
             flags = [X is not None and X.nelement() > 0 and X.dim() == r - 1 for X, r in zip(ins, ranks)]
             want = list(ctx.needs_input_grad)
-            if torch.is_grad_enabled():          # create_graph=True: gradients that can be differentiated again
-                if st.dense is None:
-                    return BoxQPBackwardFn.apply(st, flags, want, dl_dzhat, dl_dlam, dl_dnu, *ins)
-                return dense_backward_graph(st, dl_dzhat, flags, want, ins, dl_dlam, dl_dnu, dense_Q)
-            if st.dense is None:
-                outs = solve_box_backward(st, dl_dzhat, flags, want, dl_dlam, dl_dnu)
+            if st.dense is not None:
+                outs = dense_backward(st, dl_dzhat, flags, want, ins, dl_dlam, dl_dnu, dense_Q)
+            elif torch.is_grad_enabled():        # create_graph=True: gradients that can be differentiated again
+                return _qp.BackwardFn.apply(lambda *a: solve_box_backward(*a, keep=True), solve_box_double_backward,
+                                            st, flags, want, dl_dzhat, dl_dlam, dl_dnu, *ins)
             else:
-                outs = dense_backward(st, dl_dzhat, flags, want, q.size(-1) if lb is not None else 0, ub is not None,
-                                      dl_dlam, dl_dnu, dense_Q)
-            return tuple(None if (g is None or X is None or not w) else g.to(device=X.device, dtype=X.dtype)
-                         for X, g, w in zip(ins, outs, want))
+                outs = solve_box_backward(st, dl_dzhat, flags, want, dl_dlam, dl_dnu)
+            return tuple(_qp._cast(g, X) for X, g in zip(ins, outs))
 
     def apply(q, p, A, b, lb, ub):
         return BoxQPFunctionFn.apply(q, p, A, b, lb, ub)

@@ -32,10 +32,6 @@ IR_EPS = 1e-7          # batch.py:247
 IR_STEPS = 1
 
 
-def _ptr(t):
-    return ctypes.c_void_p(t.data_ptr()) if (t is not None and t.numel() > 0) else None
-
-
 def _diag(D):
     return D if D.dim() == 2 else torch.diagonal(D, dim1=1, dim2=2)
 
@@ -50,35 +46,22 @@ class _Factored:
         self.reg = float(reg)
         self.dev = Q.device
         self.plan = _lib.plan_for(self.nz, self.nineq, self.neq, two=False)
-        lib, plan, B = _lib.load(), self.plan, self.B
-        f64 = dict(dtype=torch.float64, device=self.dev)
-        self.L = torch.empty(B * plan.L_elems, **f64)
-        self.W = torch.empty(B * plan.W_elems, **f64)
-        self.K = torch.empty(B * plan.K_elems, **f64)
-        self.spd = torch.zeros(B, dtype=torch.int32, device=self.dev)
-        nscr = B * max(plan.setup_scratch_elems, plan.solve_scratch_elems)
-        self.scratch = torch.empty(nscr, **f64) if nscr > 0 else None
-        Qc, Gc = Q.contiguous(), G.contiguous()
-        Ac = A.contiguous() if self.neq else None
         with torch.cuda.device(self.dev):
-            st = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
-            _lib.check(lib.qpb200_pre_factor_kkt_reg(
-                ctypes.byref(plan), B, _ptr(Qc), self.nz * self.nz, _ptr(Gc), self.nineq * self.nz, _ptr(Ac),
-                self.neq * self.nz, self.reg, _ptr(self.L), _ptr(self.W), _ptr(self.K), _ptr(self.spd),
-                _ptr(self.scratch), st))
+            self.L, self.W, self.K, self.scratch, self.spd = _lib.pre_factor(
+                self.plan, self.B, self.B, Q.contiguous(), self.nz * self.nz, G.contiguous(), self.nineq * self.nz,
+                A.contiguous() if self.neq else None, self.neq * self.nz, self.reg, self.dev, _lib.stream())
 
     def solve(self, d, rx, rs, rz, ry):
-        lib, plan, B = _lib.load(), self.plan, self.B
+        B = self.B
         f64 = dict(dtype=torch.float64, device=self.dev)
         dx = torch.empty(B, self.nz, **f64); ds = torch.empty(B, self.nineq, **f64); dz = torch.empty(B, self.nineq, **f64)
         dy = torch.empty(B, self.neq, **f64) if self.neq else None
         args = [t.contiguous() for t in (d, rx, rs, rz)] + [ry.contiguous() if self.neq else None]
+        P = _lib.ptr
         with torch.cuda.device(self.dev):
-            st = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
-            _lib.check(lib.qpb200_solve_kkt_reg(
-                ctypes.byref(plan), B, _ptr(args[0]), _ptr(args[1]), _ptr(args[2]), _ptr(args[3]), _ptr(args[4]),
-                self.reg, _ptr(self.L), _ptr(self.W), _ptr(self.K), 1, _ptr(dx), _ptr(ds), _ptr(dz), _ptr(dy),
-                _ptr(self.scratch), st))
+            _lib.check(_lib.load().qpb200_solve_kkt_reg(
+                ctypes.byref(self.plan), B, *(P(t) for t in args), self.reg, P(self.L), P(self.W), P(self.K), 1,
+                P(dx), P(ds), P(dz), P(dy), P(self.scratch), _lib.stream()))
         return dx, ds, dz, dy
 
 

@@ -14,16 +14,11 @@ materialises nothing different; results are identical to composing the same form
 Only the lower triangle of L is read: its strictly upper triangle may hold anything, NaN included, the results are those
 of tril(L), and the gradient dL is exactly zero above the diagonal. The Q built from it reaches the QP kernels, which
 read only its lower triangle."""
-import ctypes
-
 import torch
 
 from . import _lib
+from ._lib import ptr
 from .qp import solve_forward, solve_backward
-
-
-def _p(t):
-    return ctypes.c_void_p(t.data_ptr())
 
 
 def OptNetQP(eps=1e-4, qp_eps=1e-12, notImprovedLim=3, maxIter=20):
@@ -37,8 +32,8 @@ def OptNetQP(eps=1e-4, qp_eps=1e-12, notImprovedLim=3, maxIter=20):
             Q = torch.empty(n, n, dtype=torch.float64, device=L.device)
             h = torch.empty(m, dtype=torch.float64, device=L.device)
             with torch.cuda.device(L.device):
-                st_ = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
-                _lib.check(lib.qpb200_optnet_construct(n, m, _p(Lc), _p(Gc), _p(z0c), _p(s0c), float(eps), _p(Q), _p(h), st_))
+                _lib.check(lib.qpb200_optnet_construct(n, m, ptr(Lc), ptr(Gc), ptr(z0c), ptr(s0c), float(eps), ptr(Q),
+                                                       ptr(h), _lib.stream()))
             e = torch.empty(0, dtype=torch.float64, device=L.device)
             st = solve_forward(Q, p.detach(), Gc, h, e, e, eps=qp_eps, verbose=-1, notImprovedLim=notImprovedLim,
                                maxIter=maxIter, check_Q_spd=False)
@@ -55,9 +50,8 @@ def OptNetQP(eps=1e-4, qp_eps=1e-12, notImprovedLim=3, maxIter=20):
             f64 = dict(dtype=torch.float64, device=Lc.device)
             dL = torch.empty(n, n, **f64); dG = torch.empty(m, n, **f64); dz0 = torch.empty(n, **f64); ds0 = torch.empty(m, **f64)
             with torch.cuda.device(Lc.device):
-                st_ = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
-                _lib.check(lib.qpb200_optnet_chain(n, m, _p(Lc), _p(Gc), _p(z0c), _p(dQ), _p(dGq), _p(dh),
-                                                   _p(dL), _p(dG), _p(dz0), _p(ds0), st_))
+                _lib.check(lib.qpb200_optnet_chain(n, m, ptr(Lc), ptr(Gc), ptr(z0c), ptr(dQ), ptr(dGq), ptr(dh),
+                                                   ptr(dL), ptr(dG), ptr(dz0), ptr(ds0), _lib.stream()))
             return dL, dG, dz0, ds0, dp
 
     return OptNetQPFn.apply

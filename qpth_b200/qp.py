@@ -24,6 +24,7 @@ import torch
 from torch.autograd import Function
 
 from . import _lib, kkt
+from ._lib import dev64 as _dev64, ptr as _ptr, stream as _stream
 from .util import check_shapes, expandParam, extract_nBatch
 
 INACC_ERR = """
@@ -110,19 +111,6 @@ class KKTSolvers(Enum):
     IR_UNOPT = 3
 
 
-def _ptr(t):
-    return ctypes.c_void_p(t.data_ptr()) if t is not None and t.numel() > 0 else ctypes.c_void_p(0)
-
-
-def _stream():
-    return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
-
-
-def _dev64(t, device):
-    """fp64, contiguous, on `device`; un-batched tensors stay un-batched (stride 0 is passed to C)."""
-    return t.detach().to(device=device, dtype=torch.float64).contiguous()
-
-
 class _Solved:
     """State carried from forward to backward (the reference's ctx.Q_LU / S_LU / R / nus / lams / slacks)."""
     __slots__ = ("plan", "nBatch", "nsys", "L", "W", "K", "zhat", "lam", "slacks", "nus",
@@ -141,7 +129,7 @@ def solve_forward(Q_, p_, G_, h_, A_, b_, eps=1e-12, verbose=0, notImprovedLim=3
     if nineq == 0:
         raise RuntimeError('qpth_b200: nineq == 0 is not supported (the reference unpacks G.size() at qp.py:87)')
     assert maxIter >= 1
-    lib = _lib.load()
+    _lib.load()
     if not torch.cuda.is_available():
         raise _lib.QpthB200Error("qpth_b200: no CUDA device available (there is no CPU fallback).")
     device = Q_.device if Q_.is_cuda else torch.device("cuda", torch.cuda.current_device())
@@ -167,21 +155,9 @@ def solve_forward(Q_, p_, G_, h_, A_, b_, eps=1e-12, verbose=0, notImprovedLim=3
         nsys = nBatch if (sQ or sG or sA) else 1
         st = _Solved()
         st.plan, st.nBatch, st.nsys, st.device, st.reg = plan, nBatch, nsys, device, reg
+        st.L, st.W, st.K, st.scratch, spd = _lib.pre_factor(plan, nsys, nBatch, Q, sQ, G, sG, A, sA,
+                                                             kkt.IR_EPS if reg else None, device, _stream())
         f64 = dict(dtype=torch.float64, device=device)
-        st.L = torch.empty(nsys * plan.L_elems, **f64)
-        st.W = torch.empty(nsys * plan.W_elems, **f64)
-        st.K = torch.empty(nsys * plan.K_elems, **f64)
-        spd = torch.zeros(nsys, dtype=torch.int32, device=device)
-        nscr = max(nsys * plan.setup_scratch_elems, nBatch * plan.solve_scratch_elems)
-        st.scratch = torch.empty(nscr, **f64) if nscr > 0 else None
-        if reg:
-            _lib.check(lib.qpb200_pre_factor_kkt_reg(
-                ctypes.byref(plan), nsys, _ptr(Q), sQ, _ptr(G), sG, _ptr(A), sA, float(kkt.IR_EPS),
-                _ptr(st.L), _ptr(st.W), _ptr(st.K), _ptr(spd), _ptr(st.scratch), _stream()))
-        else:
-            _lib.check(lib.qpb200_pre_factor_kkt(
-                ctypes.byref(plan), nsys, _ptr(Q), sQ, _ptr(G), sG, _ptr(A), sA,
-                _ptr(st.L), _ptr(st.W), _ptr(st.K), _ptr(spd), _ptr(st.scratch), _stream()))
         st.zhat = torch.empty(nBatch, nz, **f64)
         st.lam = torch.empty(nBatch, nineq, **f64)
         st.slacks = torch.empty(nBatch, nineq, **f64)
@@ -189,12 +165,11 @@ def solve_forward(Q_, p_, G_, h_, A_, b_, eps=1e-12, verbose=0, notImprovedLim=3
         st.iters = torch.empty(nBatch, dtype=torch.int32, device=device)
         st.best_resid = torch.empty(nBatch, **f64)
         st.trace = torch.full((nBatch, int(maxIter), 4), float('nan'), **f64) if (verbose == 1 or TRACE) else None
-        common = (float(eps), float(STALL_TOL), float(BEST_TIE), int(notImprovedLim), int(maxIter))
-        if reg:
-            common += (float(kkt.IR_EPS), int(kkt.IR_STEPS))
-        _lib.check((lib.qpb200_forward_reg if reg else lib.qpb200_forward)(
+        fn, ir = _entry(st, "qpb200_forward", "qpb200_forward_reg")
+        _lib.check(fn(
             ctypes.byref(plan), nBatch, _ptr(p), sp, _ptr(h), sh, _ptr(b), sb,
-            _ptr(st.L), _ptr(st.W), _ptr(st.K), 1 if nsys > 1 else 0, *common,
+            _ptr(st.L), _ptr(st.W), _ptr(st.K), 1 if nsys > 1 else 0,
+            float(eps), float(STALL_TOL), float(BEST_TIE), int(notImprovedLim), int(maxIter), *ir,
             _ptr(st.zhat), _ptr(st.lam), _ptr(st.slacks), _ptr(st.nus),
             _ptr(st.iters), _ptr(st.best_resid), _ptr(st.trace), _ptr(st.scratch), _stream()))
         diagnostics(spd, st, check_Q_spd, verbose, SPD_ERR_REG if reg else SPD_ERR)
@@ -256,45 +231,81 @@ def dual_outputs(st, like):
     return lam, nu
 
 
+# ---- pieces of the device wrappers of QPFunction and BoxQPFunction ---------------------------------------------------
+def grad_buffers(shapes, flags, want, absent, B, device, order=range(6)):
+    """The six input gradients a backward writes: None where not wanted or absent, else fp64 of the input's shape, with
+    a batch dimension unless its mean flag is set (an un-batched input). Returns them and the flat (pointer, mean flag)
+    argument list of the C ABI in `order`."""
+    outs = [None if (not w or a) else torch.empty(*(s if f else (B,) + s), dtype=torch.float64, device=device)
+            for s, f, w, a in zip(shapes, flags, want, absent)]
+    args = []
+    for k in order:
+        args += [_ptr(outs[k]), 1 if flags[k] else 0]
+    return outs, args
+
+
+def tangent_args(tangents, ranks, per):
+    """Input tangents (fp64 device tensors, which the caller keeps alive) as the flat (pointer, batch stride) argument
+    list of the C ABI: None (no tangent) is NULL with stride 0, an un-batched tangent (rank - 1 dimensions) gets stride
+    0, a batched one `per` elements."""
+    args = []
+    for t, r, n in zip(tangents, ranks, per):
+        if t is None or t.numel() == 0 or n == 0:
+            args += [_ptr(None), 0]
+        else:
+            args += [_ptr(t), n if t.dim() == r else 0]
+    return args
+
+
+def solve_triple(B, nz, nineq, neq, device):
+    """Fresh fp64 (B, nz), (B, nineq) and (B, neq) outputs of a KKT solve; the last is None without equality rows."""
+    f64 = dict(dtype=torch.float64, device=device)
+    return torch.empty(B, nz, **f64), torch.empty(B, nineq, **f64), torch.empty(B, neq, **f64) if neq > 0 else None
+
+
+def _entry(st, plain, reg):
+    """The C entry point for the mode of `st` and the arguments that follow its nsys flag: `reg` with
+    (IR_EPS, IR_STEPS) in the regularised mode (IR_UNOPT), else `plain` and none."""
+    lib = _lib.load()
+    if getattr(st, "reg", False):                   # (states built outside solve_forward may lack it: the default path)
+        return getattr(lib, reg), (float(kkt.IR_EPS), int(kkt.IR_STEPS))
+    return getattr(lib, plain), ()
+
+
+def _point(st):
+    """The arguments of the returned point and its factors: zhat, lam, slacks, nus, L, W, K and the nsys flag."""
+    return (_ptr(st.zhat), _ptr(st.lam), _ptr(st.slacks), _ptr(st.nus), _ptr(st.L), _ptr(st.W), _ptr(st.K),
+            1 if st.nsys > 1 else 0)
+
+
+def _shapes(plan):
+    return [(plan.nz, plan.nz), (plan.nz,), (plan.nineq, plan.nz), (plan.nineq,), (plan.neq, plan.nz), (plan.neq,)]
+
+
+RANKS = (3, 2, 3, 2, 3, 2)        # of (Q, p, G, h, A, b) batched
+
+
 def solve_backward(st, dl_dzhat, mean_flags, want, dl_dlam=None, dl_dnu=None, keep=False):
     """QPFunctionFn.backward on the device. mean_flags / want: 6-tuples for (Q,p,G,h,A,b). dl_dlam / dl_dnu: the
     gradients of the loss with respect to the returned duals (None: zero); dl_dzhat None: zero. keep: also return the
     solve (dxv, dlamv, dnuv), which the double backward reads."""
     if _pending:
         flush_checks(wait=False)
-    lib = _lib.load()
     plan, B, device = st.plan, st.nBatch, st.device
     nz, nineq, neq = plan.nz, plan.nineq, plan.neq
-    f64 = dict(dtype=torch.float64, device=device)
     with torch.cuda.device(device):
-        dl = _adjoint(dl_dzhat, B, nz, device) if dl_dzhat is not None else torch.zeros(B, nz, **f64)
+        dl = (_adjoint(dl_dzhat, B, nz, device) if dl_dzhat is not None
+              else torch.zeros(B, nz, dtype=torch.float64, device=device))
         glam, gnu = _adjoint(dl_dlam, B, nineq, device), _adjoint(dl_dnu, B, neq, device)
-        shapes = [(nz, nz), (nz,), (nineq, nz), (nineq,), (neq, nz), (neq,)]
-        outs = []
-        for k in range(6):
-            if not want[k] or (k >= 4 and neq == 0):
-                outs.append(None)
-            else:
-                shp = shapes[k] if mean_flags[k] else (B,) + shapes[k]
-                outs.append(torch.empty(*shp, **f64))
-        dxv = torch.empty(B, nz, **f64)
-        dlamv = torch.empty(B, nineq, **f64)
-        dnuv = torch.empty(B, neq, **f64) if neq > 0 else None
-        args = []
-        for k in range(6):
-            args += [_ptr(outs[k]), 1 if mean_flags[k] else 0]
-        reg = getattr(st, "reg", False)             # (solution.py builds _Solved without it: the default path)
+        outs, grads = grad_buffers(_shapes(plan), mean_flags, want, (False,) * 4 + (neq == 0,) * 2, B, device)
+        v = solve_triple(B, nz, nineq, neq, device)
         if glam is None and gnu is None:            # no dual was used: the entry point of a zhat-only loss
-            fn, adj = (lib.qpb200_backward_reg if reg else lib.qpb200_backward), ()
+            (fn, ir), adj = _entry(st, "qpb200_backward", "qpb200_backward_reg"), ()
         else:
-            fn, adj = (lib.qpb200_backward_reg_duals if reg else lib.qpb200_backward_duals), (_ptr(glam), _ptr(gnu))
-        _lib.check(fn(
-            ctypes.byref(plan), B, _ptr(dl), *adj, _ptr(st.zhat), _ptr(st.lam), _ptr(st.slacks), _ptr(st.nus),
-            _ptr(st.L), _ptr(st.W), _ptr(st.K), 1 if st.nsys > 1 else 0, *((float(kkt.IR_EPS), int(kkt.IR_STEPS)) if reg else ()),
-            *args, _ptr(dxv), _ptr(dlamv), _ptr(dnuv), _ptr(st.scratch), _stream()))
-    if keep:
-        return outs, (dxv, dlamv, dnuv)
-    return outs
+            (fn, ir), adj = _entry(st, "qpb200_backward_duals", "qpb200_backward_reg_duals"), (_ptr(glam), _ptr(gnu))
+        _lib.check(fn(ctypes.byref(plan), B, _ptr(dl), *adj, *_point(st), *ir, *grads, *(_ptr(x) for x in v),
+                      _ptr(st.scratch), _stream()))
+    return (outs, v) if keep else outs
 
 
 def solve_double_backward(st, v, omegas, flags, want, G):
@@ -306,40 +317,22 @@ def solve_double_backward(st, v, omegas, flags, want, G):
     and of the six inputs (None where not wanted)."""
     if _pending:
         flush_checks(wait=False)
-    lib = _lib.load()
     plan, B, device = st.plan, st.nBatch, st.device
     nz, nineq, neq = plan.nz, plan.nineq, plan.neq
-    f64 = dict(dtype=torch.float64, device=device)
+    absent = (False,) * 4 + (neq == 0,) * 2
     with torch.cuda.device(device):
-        om = [None if (w is None or (k >= 4 and neq == 0)) else (_dev64(w, device) / B if flags[k] else w)
+        om = [None if (w is None or absent[k]) else (_dev64(w, device) / B if flags[k] else _dev64(w, device))
               for k, w in enumerate(omegas)]
-        tans = tangent_args(om, (3, 2, 3, 2, 3, 2), (nz * nz, nz, nineq * nz, nineq, neq * nz, neq), device)
+        tans = tangent_args(om, RANKS, (nz * nz, nz, nineq * nz, nineq, neq * nz, neq))
         G64 = _dev64(G, device)
         sG = nineq * nz if G64.dim() == 3 else 0
-        shapes = [(nz, nz), (nz,), (nineq, nz), (nineq,), (neq, nz), (neq,)]
-        outs = []
-        for k in range(6):
-            if not want[k] or (k >= 4 and neq == 0):
-                outs.append(None)
-            else:
-                outs.append(torch.empty(*(shapes[k] if flags[k] else (B,) + shapes[k]), **f64))
-        gz = torch.empty(B, nz, **f64)
-        glam = torch.empty(B, nineq, **f64)
-        gnu = torch.empty(B, neq, **f64) if neq > 0 else None
-        work = torch.empty(B * (2 * nz + 3 * nineq + 2 * neq), **f64)
-        args = []
-        for t, s in tans:
-            args += [_ptr(t), s]
-        grads = []
-        for k in range(6):
-            grads += [_ptr(outs[k]), 1 if flags[k] else 0]
-        reg = getattr(st, "reg", False)
-        _lib.check((lib.qpb200_double_backward_reg if reg else lib.qpb200_double_backward)(
-            ctypes.byref(plan), B, *args, _ptr(G64), sG, *(_ptr(x) for x in v),
-            _ptr(st.zhat), _ptr(st.lam), _ptr(st.slacks), _ptr(st.nus), _ptr(st.L), _ptr(st.W), _ptr(st.K),
-            1 if st.nsys > 1 else 0, *((float(kkt.IR_EPS), int(kkt.IR_STEPS)) if reg else ()),
-            _ptr(gz), _ptr(glam), _ptr(gnu), *grads, _ptr(work), _ptr(st.scratch), _stream()))
-    return [gz, glam, gnu] + outs
+        outs, grads = grad_buffers(_shapes(plan), flags, want, absent, B, device)
+        gg = solve_triple(B, nz, nineq, neq, device)
+        work = torch.empty(B * (2 * nz + 3 * nineq + 2 * neq), dtype=torch.float64, device=device)
+        fn, ir = _entry(st, "qpb200_double_backward", "qpb200_double_backward_reg")
+        _lib.check(fn(ctypes.byref(plan), B, *tans, _ptr(G64), sG, *(_ptr(x) for x in v), *_point(st), *ir,
+                      *(_ptr(x) for x in gg), *grads, _ptr(work), _ptr(st.scratch), _stream()))
+    return list(gg) + outs
 
 
 THIRD_ORDER_ERR = ("qpth_b200: third-order derivatives through the QP layer are not provided: the double backward is not "
@@ -350,40 +343,35 @@ def _cast(g, like):
     return None if (g is None or like is None) else g.to(device=like.device, dtype=like.dtype)
 
 
-class QPBackwardFn(Function):
-    """The first-order backward of QPFunction / QPSolutionFunction as a differentiable function of the incoming gradients
-    (g_z, g_lam, g_nu) and of (Q, p, G, h, A, b): what their backward runs under create_graph=True. Its forward is the
-    first backward's own solve_backward call; its backward is solve_double_backward."""
+class BackwardFn(Function):
+    """The first-order backward of a QP layer as a differentiable function of the incoming gradients (g_z, g_lam, g_nu)
+    and of the layer's six inputs: what its backward runs under create_graph=True. Its forward is
+    first(st, g_z, flags, want, g_lam, g_nu), the layer's first-order backward returning (grads, v); its backward is
+    second(st, v, omegas, flags, want), the layer's double backward."""
     @staticmethod
-    def forward(ctx, st, flags, want, g_z, g_lam, g_nu, Q, p, G, h, A, b):
-        outs, v = solve_backward(st, g_z, flags, want, g_lam, g_nu, keep=True)
-        ctx.st, ctx.v, ctx.flags = st, v, flags
-        ctx.like = (g_z, g_lam, g_nu, Q, p, G, h, A, b)
+    def forward(ctx, first, second, st, flags, want, g_z, g_lam, g_nu, *ins):
+        outs, v = first(st, g_z, flags, want, g_lam, g_nu)
+        ctx.second, ctx.st, ctx.v, ctx.flags = second, st, v, flags
+        ctx.like = (g_z, g_lam, g_nu) + ins
         ctx.set_materialize_grads(False)
-        return tuple(_cast(g, X) for X, g in zip((Q, p, G, h, A, b), outs))
+        return tuple(_cast(g, X) for X, g in zip(ins, outs))
 
     @staticmethod
     def backward(ctx, *omegas):
         if torch.is_grad_enabled():
             raise RuntimeError(THIRD_ORDER_ERR)
-        need = ctx.needs_input_grad[3:]
+        need = ctx.needs_input_grad[5:]
         if all(w is None for w in omegas) or not any(need):
-            return (None,) * 12
-        G = ctx.like[5]
-        res = solve_double_backward(ctx.st, ctx.v, omegas, ctx.flags, need[3:], G)
-        return (None, None, None) + tuple(_cast(g, X) if n else None for g, X, n in zip(res, ctx.like, need))
+            return (None,) * 14
+        res = ctx.second(ctx.st, ctx.v, omegas, ctx.flags, need[3:])
+        return (None,) * 5 + tuple(_cast(g, X) if n else None for g, X, n in zip(res, ctx.like, need))
 
 
-def tangent_args(tangents, ranks, per, device):
-    """Forward-mode input tangents as (fp64 device tensor, batch stride) pairs for the C ABI: None (no tangent) stays
-    None with stride 0, an un-batched tangent (rank - 1 dimensions) gets stride 0, a batched one `per` elements."""
-    out = []
-    for t, r, n in zip(tangents, ranks, per):
-        if t is None or t.numel() == 0 or n == 0:
-            out.append((None, 0))
-        else:
-            out.append((_dev64(t, device), n if t.dim() == r else 0))
-    return out
+def backward_graph(st, flags, want, g_z, g_lam, g_nu, Q, p, G, h, A, b):
+    """solve_backward under create_graph=True: gradients of (Q, p, G, h, A, b) that can be differentiated again."""
+    return BackwardFn.apply(lambda *a: solve_backward(*a, keep=True),
+                            lambda st_, v, om, fl, w: solve_double_backward(st_, v, om, fl, w, G),
+                            st, flags, want, g_z, g_lam, g_nu, Q, p, G, h, A, b)
 
 
 def solve_jvp(st, tangents):
@@ -392,26 +380,16 @@ def solve_jvp(st, tangents):
     qpb200_jvp(_reg) call: the right-hand side kernel and the backward's KKT solve."""
     if _pending:
         flush_checks(wait=False)
-    lib = _lib.load()
     plan, B, device = st.plan, st.nBatch, st.device
     nz, nineq, neq = plan.nz, plan.nineq, plan.neq
-    f64 = dict(dtype=torch.float64, device=device)
     with torch.cuda.device(device):
-        tans = tangent_args(tangents, (3, 2, 3, 2, 3, 2),
-                            (nz * nz, nz, nineq * nz, nineq, neq * nz, neq), device)
-        rhs = torch.empty(B * (nz + nineq + neq), **f64)
-        dz = torch.empty(B, nz, **f64)
-        dlam = torch.empty(B, nineq, **f64)
-        dnu = torch.empty(B, neq, **f64) if neq > 0 else None
-        args = []
-        for t, s in tans:
-            args += [_ptr(t), s]
-        reg = getattr(st, "reg", False)             # (solution.py builds _Solved without it: the default path)
-        _lib.check((lib.qpb200_jvp_reg if reg else lib.qpb200_jvp)(
-            ctypes.byref(plan), B, *args, _ptr(st.zhat), _ptr(st.lam), _ptr(st.slacks), _ptr(st.nus),
-            _ptr(st.L), _ptr(st.W), _ptr(st.K), 1 if st.nsys > 1 else 0,
-            *((float(kkt.IR_EPS), int(kkt.IR_STEPS)) if reg else ()),
-            _ptr(rhs), _ptr(dz), _ptr(dlam), _ptr(dnu), _ptr(st.scratch), _stream()))
+        tans = [None if t is None else _dev64(t, device) for t in tangents]
+        args = tangent_args(tans, RANKS, (nz * nz, nz, nineq * nz, nineq, neq * nz, neq))
+        rhs = torch.empty(B * (nz + nineq + neq), dtype=torch.float64, device=device)
+        dz, dlam, dnu = solve_triple(B, nz, nineq, neq, device)
+        fn, ir = _entry(st, "qpb200_jvp", "qpb200_jvp_reg")
+        _lib.check(fn(ctypes.byref(plan), B, *args, *_point(st), *ir, _ptr(rhs), _ptr(dz), _ptr(dlam), _ptr(dnu),
+                      _ptr(st.scratch), _stream()))
     return dz, dlam, dnu
 
 
@@ -428,8 +406,46 @@ def jvp_outputs(dz, dlam, dnu, out, duals):
     return z, dlam.to(device=device, dtype=dtype), nu
 
 
-# Jacobians (jacobian() of QPFunction and QPSolutionFunction): rows z, lam, nu and columns p, h, b as bits 0, 1, 2
+def layer_outputs(ctx, st, ins, duals):
+    """The end of a QP layer's forward: keep `st` and the inputs for backward and jvp, and return zhat, or (zhat, lam,
+    nu) with duals, with the dtype and device of the first input."""
+    X = ins[0]
+    ctx.st, ctx.duals = st, duals
+    zhats = st.zhat.to(device=X.device, dtype=X.dtype)
+    ctx.save_for_backward(zhats, *ins)
+    # parity with the reference's ctx attributes (device fp64 views)
+    ctx.lams, ctx.slacks, ctx.nus = st.lam, st.slacks, st.nus
+    ctx.out = (X.device, X.dtype)
+    # an unused output's gradient, and an input without a tangent, arrive as None: nothing zero-filled is read
+    ctx.set_materialize_grads(False)
+    return (zhats,) + dual_outputs(st, X) if duals else zhats
+
+
+class QPLayerFn(Function):
+    """backward and jvp of QPFunction and QPSolutionFunction, whose forward(ctx, Q, p, G, h, A, b, ...) ends with
+    layer_outputs; inputs after the sixth (QPSolutionFunction's solution) are constants."""
+    @staticmethod
+    def jvp(ctx, *tangents):
+        return jvp_outputs(*solve_jvp(ctx.st, tangents[:6]), ctx.out, ctx.duals)
+
+    @staticmethod
+    def backward(ctx, dl_dzhat, dl_dlam=None, dl_dnu=None):
+        zhats, Q, p, G, h, A, b = ctx.saved_tensors
+        nBatch = extract_nBatch(Q, p, G, h, A, b)
+        flags = [expandParam(X, nBatch, nd)[1]
+                 for X, nd in ((Q, 3), (p, 2), (G, 3), (h, 2), (A, 3), (b, 2))]   # qp.py:131-136
+        want = list(ctx.needs_input_grad[:6])
+        if torch.is_grad_enabled():          # create_graph=True: gradients that can be differentiated again
+            grads = backward_graph(ctx.st, flags, want, dl_dzhat, dl_dlam, dl_dnu, Q, p, G, h, A, b)
+        else:
+            outs = solve_backward(ctx.st, dl_dzhat, flags, want, dl_dlam, dl_dnu)
+            grads = tuple(_cast(g, X) for X, g in zip((Q, p, G, h, A, b), outs))
+        return grads + (None,) * (len(ctx.needs_input_grad) - 6)
+
+
+# ---- Jacobians: rows z, lam, nu as bits 0, 1, 2; columns one bit per input of the layer's table ---------------------
 JAC_WRT = ("p", "h", "b")
+JAC_SLOTS = (1, 3, 5)             # their tangents' slots in (dQ, dp, dG, dh, dA, db)
 
 
 def jacobian_covered(plan):
@@ -447,26 +463,45 @@ def _jacobian_kernel(st, rows, cols, J):
             1 if st.nsys > 1 else 0, _ptr(J), _stream()))
 
 
-def _jacobian_columns(st, rows, cols, J):
-    """J column by column: one solve_jvp per column with an un-batched unit tangent of p, h or b (batch stride 0), which
-    gives that column for every QP at once (qpb200_jvp, or qpb200_jvp_reg with its refinement steps)."""
-    sizes = (st.plan.nz, st.plan.nineq, st.plan.neq)
+def jacobian_columns(st, rows, cols, J, csizes, slots, jvp):
+    """J column by column: for column block k (csizes[k] columns), one jvp(st, tangents) per column with an un-batched
+    unit tangent (batch stride 0) in slot slots[k] of the six tangents, which gives that column for every QP at once
+    (qpb200_jvp, or qpb200_jvp_reg with its refinement steps; the box layouts' JVPs)."""
+    rsizes = (st.plan.nz, st.plan.nineq, st.plan.neq)
     c0 = 0
-    for k in range(3):
+    for k, (n, slot) in enumerate(zip(csizes, slots)):
         if not (cols >> k) & 1:
             continue
-        for j in range(sizes[k]):
-            t = torch.zeros(sizes[k], dtype=torch.float64, device=st.device)
+        for j in range(n):
+            t = torch.zeros(n, dtype=torch.float64, device=st.device)
             t[j] = 1.0
             tans = [None] * 6
-            tans[2 * k + 1] = t                          # (dQ, dp, dG, dh, dA, db): dp, dh or db
-            outs = solve_jvp(st, tans)
+            tans[slot] = t
+            outs = jvp(st, tans)
             r0 = 0
             for i in range(3):
                 if (rows >> i) & 1:
-                    J[:, r0:r0 + sizes[i], c0 + j] = outs[i]
-                    r0 += sizes[i]
-        c0 += sizes[k]
+                    J[:, r0:r0 + rsizes[i], c0 + j] = outs[i]
+                    r0 += rsizes[i]
+        c0 += n
+
+
+def _jacobian_columns(st, rows, cols, J):
+    """jacobian_columns for the columns p, h and b: unit tangents through solve_jvp."""
+    jacobian_columns(st, rows, cols, J, (st.plan.nz, st.plan.nineq, st.plan.neq), JAC_SLOTS, solve_jvp)
+
+
+def jacobian_matrix(st, rows, cols, csizes, fill):
+    """J (B, R, C) fp64 on st.device: rows [z; lam; nu] and column blocks of csizes, restricted to the bits of `rows` /
+    `cols`, written by fill(st, rows, cols, J): the family's kernel or its column path."""
+    if _pending:
+        flush_checks(wait=False)
+    rsizes = (st.plan.nz, st.plan.nineq, st.plan.neq)
+    R = sum(n for i, n in enumerate(rsizes) if (rows >> i) & 1)
+    C = sum(n for k, n in enumerate(csizes) if (cols >> k) & 1)
+    J = torch.empty(st.nBatch, R, C, dtype=torch.float64, device=st.device)
+    fill(st, rows, cols, J)
+    return J
 
 
 def solve_jacobian(st, rows, cols):
@@ -474,47 +509,49 @@ def solve_jacobian(st, rows, cols):
     and columns [p, h, b] restricted to the bits of `rows` / `cols` (bit 0 z / p, bit 1 lam / h, bit 2 nu / b). One
     qpb200_jacobian call where the kernel covers the plan (the default mode); otherwise, and always in the regularised
     mode (IR_UNOPT), one solve_jvp per column."""
-    if _pending:
-        flush_checks(wait=False)
     plan = st.plan
-    sizes = (plan.nz, plan.nineq, plan.neq)
     if plan.neq == 0 and ((rows | cols) & 4):
         raise ValueError("qpth_b200: a Jacobian with respect to b, or of nu, needs equality constraints (neq == 0)")
-    R = sum(sizes[i] for i in range(3) if (rows >> i) & 1)
-    C = sum(sizes[i] for i in range(3) if (cols >> i) & 1)
-    J = torch.empty(st.nBatch, R, C, dtype=torch.float64, device=st.device)
-    if not getattr(st, "reg", False) and jacobian_covered(plan):
-        _jacobian_kernel(st, rows, cols, J)
-    else:
-        _jacobian_columns(st, rows, cols, J)
-    return J
+    fill = _jacobian_kernel if not getattr(st, "reg", False) and jacobian_covered(plan) else _jacobian_columns
+    return jacobian_matrix(st, rows, cols, (plan.nz, plan.nineq, plan.neq), fill)
 
 
-def jacobian_of(st, out, wrt, duals):
-    """The `jacobian` attribute of QPFunction / QPSolutionFunction on the state `st` of their last forward, whose output
-    had out = (device, dtype). Returns {name: (B, rows, n_name)} for each name of `wrt`, rows z, or [z; lam; nu] with
-    duals."""
+def _qp_table(plan):
+    return tuple(zip(JAC_WRT, (plan.nz, plan.nineq, plan.neq)))
+
+
+def _qp_refusal(nm):
+    if nm not in JAC_WRT:
+        return ("qpth_b200: jacobian(wrt=...) takes %s, not %r (Jacobians with respect to Q, G and A are not provided)"
+                % (JAC_WRT, nm))
+    return "qpth_b200: jacobian(wrt='b') needs equality constraints (neq == 0)"
+
+
+def jacobian_of(st, out, wrt, duals, table=_qp_table, solve=None, refusal=_qp_refusal):
+    """The `jacobian` attribute of a QP layer on the state `st` of its last forward, whose output had
+    out = (device, dtype). table(st.plan): ((name, columns), ...) of the inputs in column-bit order, columns 0 for one
+    the problem lacks; solve(st, rows, cols) -> J; refusal(name): the error for a name the problem does not take. The
+    defaults are QPFunction's and QPSolutionFunction's (p, h, b; solve_jacobian). Returns {name: (B, rows, columns)}
+    for each name of `wrt` (None: every input the problem has), rows z, or [z; lam; nu] with duals."""
     if st is None:
         raise RuntimeError("qpth_b200: jacobian() needs a forward call of this function first")
-    names = (wrt,) if isinstance(wrt, str) else tuple(wrt)
+    table = table(st.plan)
+    present = tuple(nm for nm, n in table if n)
+    names = present if wrt is None else ((wrt,) if isinstance(wrt, str) else tuple(wrt))
     if not names:
-        raise ValueError("qpth_b200: jacobian(wrt=...) needs at least one of %s" % (JAC_WRT,))
+        raise ValueError("qpth_b200: jacobian(wrt=...) needs at least one of %s" % (present,))
     for nm in names:
-        if nm not in JAC_WRT:
-            raise ValueError("qpth_b200: jacobian(wrt=...) takes %s, not %r (Jacobians with respect to Q, G and A are "
-                             "not provided)" % (JAC_WRT, nm))
-    plan = st.plan
-    if "b" in names and plan.neq == 0:
-        raise ValueError("qpth_b200: jacobian(wrt='b') needs equality constraints (neq == 0)")
-    cols = sum(1 << JAC_WRT.index(nm) for nm in set(names))
-    rows = 1 | ((2 | (4 if plan.neq > 0 else 0)) if duals else 0)
-    J = solve_jacobian(st, rows, cols)
-    sizes = dict(zip(JAC_WRT, (plan.nz, plan.nineq, plan.neq)))
+        if nm not in present:
+            raise ValueError(refusal(nm))
+    known = [nm for nm, _ in table]
+    cols = sum(1 << known.index(nm) for nm in set(names))
+    rows = 1 | ((2 | (4 if st.plan.neq > 0 else 0)) if duals else 0)
+    J = (solve or solve_jacobian)(st, rows, cols)
     res, c0 = {}, 0
-    for nm in JAC_WRT:
-        if (cols >> JAC_WRT.index(nm)) & 1:
-            res[nm] = J[:, :, c0:c0 + sizes[nm]]
-            c0 += sizes[nm]
+    for k, (nm, n) in enumerate(table):
+        if (cols >> k) & 1:
+            res[nm] = J[:, :, c0:c0 + n]
+            c0 += n
     device, dtype = out
     return {nm: res[nm].to(device=device, dtype=dtype).contiguous() for nm in names}
 
@@ -606,7 +643,7 @@ def QPFunction(eps=1e-12, verbose=0, notImprovedLim=3, maxIter=20, solver=QPSolv
     _last = [None]
     _jac = [None, None, False]           # the state and (device, dtype) of the last forward; True: it was equality-only
 
-    class QPFunctionFn(Function):
+    class QPFunctionFn(QPLayerFn):
         @staticmethod
         def forward(ctx, Q_, p_, G_, h_, A_, b_):
             """Solve a batch of QPs  argmin_z 1/2 z^T Q z + p^T z  s.t. Gz <= h, Az = b.
@@ -616,39 +653,10 @@ def QPFunction(eps=1e-12, verbose=0, notImprovedLim=3, maxIter=20, solver=QPSolv
             Returns zhat (nBatch, nz).  (qp.py:23-125)
             """
             st = solve_forward(Q_, p_, G_, h_, A_, b_, eps, verbose, notImprovedLim, maxIter, check_Q_spd, kkt_solver)
-            ctx.st = st
             _last[0] = st
             _jac[0], _jac[1] = st, (Q_.device, Q_.dtype)
             ctx.neq, ctx.nineq, ctx.nz = st.plan.neq, st.plan.nineq, st.plan.nz
-            zhats = st.zhat.to(device=Q_.device, dtype=Q_.dtype)
-            ctx.save_for_backward(zhats, Q_, p_, G_, h_, A_, b_)
-            # parity with the reference's ctx attributes (device fp64 views)
-            ctx.lams, ctx.slacks, ctx.nus = st.lam, st.slacks, st.nus
-            ctx.out = (Q_.device, Q_.dtype)
-            # an unused output's gradient, and an input without a tangent, arrive as None: nothing zero-filled is read
-            ctx.set_materialize_grads(False)
-            if not duals:
-                return zhats
-            return (zhats,) + dual_outputs(st, Q_)
-
-        @staticmethod
-        def jvp(ctx, dQ, dp, dG, dh, dA, db):
-            return jvp_outputs(*solve_jvp(ctx.st, (dQ, dp, dG, dh, dA, db)), ctx.out, duals)
-
-        @staticmethod
-        def backward(ctx, dl_dzhat, dl_dlam=None, dl_dnu=None):
-            zhats, Q, p, G, h, A, b = ctx.saved_tensors
-            nBatch = extract_nBatch(Q, p, G, h, A, b)
-            flags = [expandParam(X, nBatch, nd)[1]
-                     for X, nd in ((Q, 3), (p, 2), (G, 3), (h, 2), (A, 3), (b, 2))]   # qp.py:131-136
-            want = list(ctx.needs_input_grad)
-            if torch.is_grad_enabled():          # create_graph=True: gradients that can be differentiated again
-                return QPBackwardFn.apply(ctx.st, flags, want, dl_dzhat, dl_dlam, dl_dnu, Q, p, G, h, A, b)
-            outs = solve_backward(ctx.st, dl_dzhat, flags, want, dl_dlam, dl_dnu)
-            grads = []
-            for X, g in zip((Q, p, G, h, A, b), outs):
-                grads.append(None if g is None else g.to(device=X.device, dtype=X.dtype))
-            return tuple(grads)
+            return layer_outputs(ctx, st, (Q_, p_, G_, h_, A_, b_), duals)
 
     def apply(Q_, p_, G_, h_, A_, b_):
         if G_.nelement() == 0 and h_.nelement() == 0 and A_.nelement() > 0:

@@ -19,14 +19,13 @@ commercial solver, a solution cached from a previous step):
 
 There is no CPU fallback for the backward: without the library or a CUDA device the call raises.
 """
-import ctypes
-
 import torch
-from torch.autograd import Function
 
-from . import _lib
-from .qp import KKTSolvers, check_kkt_solver
-from .util import expandParam, extract_nBatch
+from . import _lib, kkt
+from . import qp as _qp
+from .qp import (JACOBIAN_DOC, SPD_ERR, SPD_ERR_REG, KKTSolvers, QPLayerFn, _Solved, check_kkt_solver, jacobian_of,
+                 layer_outputs)
+from .util import check_shapes
 
 
 def pre_factor_state(Q_, p_, G_, h_, A_, b_, zhat, lams, slacks, nus, check_Q_spd=True,
@@ -34,20 +33,17 @@ def pre_factor_state(Q_, p_, G_, h_, A_, b_, zhat, lams, slacks, nus, check_Q_sp
     """`pre_factor_kkt` on the device + the given solution, packaged as the state `solve_backward` consumes.
     kkt_solver=KKTSolvers.IR_UNOPT: the regularised factors (`qpb200_pre_factor_kkt_reg`), so that the backward pass is
     `qpb200_backward_reg` and Q need only be positive semidefinite."""
-    from . import kkt
-    from .qp import SPD_ERR, SPD_ERR_REG, _Solved, _dev64, _ptr, _stream
-    from .util import check_shapes
     nBatch, nz, nineq, neq = check_shapes(Q_, p_, G_, h_, A_, b_)
     assert neq > 0 or nineq > 0                         # qp.py:89
     if nineq == 0:
         raise RuntimeError('qpth_b200: nineq == 0 is not supported (the reference unpacks G.size() at qp.py:87)')
-    lib = _lib.load()
+    _lib.load()
     if not torch.cuda.is_available():
         raise _lib.QpthB200Error("qpth_b200: no CUDA device available (there is no CPU fallback).")
     device = Q_.device if Q_.is_cuda else torch.device("cuda", torch.cuda.current_device())
     with torch.cuda.device(device):
-        Q, G = _dev64(Q_, device), _dev64(G_, device)
-        A = _dev64(A_, device) if neq > 0 else None
+        Q, G = _qp._dev64(Q_, device), _qp._dev64(G_, device)
+        A = _qp._dev64(A_, device) if neq > 0 else None
         reg = kkt_solver == KKTSolvers.IR_UNOPT
         plan = _lib.plan_for_ir(nz, nineq, neq) if reg else _lib.plan_for(nz, nineq, neq)
         sQ = nz * nz if Q.dim() == 3 else 0
@@ -56,21 +52,8 @@ def pre_factor_state(Q_, p_, G_, h_, A_, b_, zhat, lams, slacks, nus, check_Q_sp
         nsys = nBatch if (sQ or sG or sA) else 1
         st = _Solved()
         st.plan, st.nBatch, st.nsys, st.device, st.reg = plan, nBatch, nsys, device, reg
-        f64 = dict(dtype=torch.float64, device=device)
-        st.L = torch.empty(nsys * plan.L_elems, **f64)
-        st.W = torch.empty(nsys * plan.W_elems, **f64)
-        st.K = torch.empty(nsys * plan.K_elems, **f64)
-        spd = torch.zeros(nsys, dtype=torch.int32, device=device)
-        nscr = max(nsys * plan.setup_scratch_elems, nBatch * plan.solve_scratch_elems)
-        st.scratch = torch.empty(nscr, **f64) if nscr > 0 else None
-        if reg:
-            _lib.check(lib.qpb200_pre_factor_kkt_reg(
-                ctypes.byref(plan), nsys, _ptr(Q), sQ, _ptr(G), sG, _ptr(A), sA, float(kkt.IR_EPS),
-                _ptr(st.L), _ptr(st.W), _ptr(st.K), _ptr(spd), _ptr(st.scratch), _stream()))
-        else:
-            _lib.check(lib.qpb200_pre_factor_kkt(
-                ctypes.byref(plan), nsys, _ptr(Q), sQ, _ptr(G), sG, _ptr(A), sA,
-                _ptr(st.L), _ptr(st.W), _ptr(st.K), _ptr(spd), _ptr(st.scratch), _stream()))
+        st.L, st.W, st.K, st.scratch, spd = _lib.pre_factor(plan, nsys, nBatch, Q, sQ, G, sG, A, sA,
+                                                             kkt.IR_EPS if reg else None, device, _qp._stream())
         if check_Q_spd and bool(spd.any()):
             raise RuntimeError(SPD_ERR_REG if reg else SPD_ERR)
 
@@ -88,7 +71,7 @@ def pre_factor_state(Q_, p_, G_, h_, A_, b_, zhat, lams, slacks, nus, check_Q_sp
         st.slacks = sol(slacks, nineq)
         st.nus = sol(nus, neq) if neq > 0 else None
         st.iters = torch.zeros(nBatch, dtype=torch.int32, device=device)
-        st.best_resid = torch.zeros(nBatch, **f64)
+        st.best_resid = torch.zeros(nBatch, dtype=torch.float64, device=device)
         st.trace = None
     return st
 
@@ -114,43 +97,12 @@ def QPSolutionFunction(check_Q_spd=True, kkt_solver=KKTSolvers.LU_PARTIAL, duals
     check_kkt_solver(kkt_solver)
     _last = [None, None]                 # the state and (device, dtype) of the last forward, for jacobian()
 
-    class QPSolutionFn(Function):
+    class QPSolutionFn(QPLayerFn):
         @staticmethod
         def forward(ctx, Q_, p_, G_, h_, A_, b_, zhat, lams, slacks, nus):
-            ctx.st = pre_factor_state(Q_, p_, G_, h_, A_, b_, zhat, lams, slacks, nus, check_Q_spd, kkt_solver)
-            _last[0], _last[1] = ctx.st, (Q_.device, Q_.dtype)
-            zhats = ctx.st.zhat.to(device=Q_.device, dtype=Q_.dtype)
-            ctx.save_for_backward(zhats, Q_, p_, G_, h_, A_, b_)
-            ctx.lams, ctx.slacks, ctx.nus = ctx.st.lam, ctx.st.slacks, ctx.st.nus
-            ctx.out = (Q_.device, Q_.dtype)
-            ctx.set_materialize_grads(False)
-            if not duals:
-                return zhats
-            from .qp import dual_outputs
-            return (zhats,) + dual_outputs(ctx.st, Q_)
-
-        @staticmethod
-        def jvp(ctx, dQ, dp, dG, dh, dA, db, *solution_tangents):
-            # the solution tensors are constants of this node: their tangents are ignored
-            from .qp import jvp_outputs, solve_jvp
-            return jvp_outputs(*solve_jvp(ctx.st, (dQ, dp, dG, dh, dA, db)), ctx.out, duals)
-
-        @staticmethod
-        def backward(ctx, dl_dzhat, dl_dlam=None, dl_dnu=None):
-            from .qp import solve_backward
-            zhats, Q, p, G, h, A, b = ctx.saved_tensors
-            nBatch = extract_nBatch(Q, p, G, h, A, b)
-            flags = [expandParam(X, nBatch, nd)[1]
-                     for X, nd in ((Q, 3), (p, 2), (G, 3), (h, 2), (A, 3), (b, 2))]   # qp.py:131-136
-            want = list(ctx.needs_input_grad[:6])
-            if torch.is_grad_enabled():          # create_graph=True: gradients that can be differentiated again
-                from .qp import QPBackwardFn
-                return QPBackwardFn.apply(ctx.st, flags, want, dl_dzhat, dl_dlam, dl_dnu, Q, p, G, h, A,
-                                          b) + (None, None, None, None)
-            outs = solve_backward(ctx.st, dl_dzhat, flags, want, dl_dlam, dl_dnu)
-            grads = [None if g is None else g.to(device=X.device, dtype=X.dtype)
-                     for X, g in zip((Q, p, G, h, A, b), outs)]
-            return tuple(grads) + (None, None, None, None)
+            st = pre_factor_state(Q_, p_, G_, h_, A_, b_, zhat, lams, slacks, nus, check_Q_spd, kkt_solver)
+            _last[0], _last[1] = st, (Q_.device, Q_.dtype)
+            return layer_outputs(ctx, st, (Q_, p_, G_, h_, A_, b_), duals)
 
     def apply(Q_, p_, G_, h_, A_, b_, zhat, lams, slacks, nus):
         # the solution is a constant of this node: detach it, or autograd would walk back into whatever produced it
@@ -158,10 +110,8 @@ def QPSolutionFunction(check_Q_spd=True, kkt_solver=KKTSolvers.LU_PARTIAL, duals
         return QPSolutionFn.apply(Q_, p_, G_, h_, A_, b_, *sol)
 
     def jacobian(wrt=("p", "h", "b"), duals=False):
-        from .qp import jacobian_of
         return jacobian_of(_last[0], _last[1], wrt, duals)
 
-    from .qp import JACOBIAN_DOC
     jacobian.__doc__ = JACOBIAN_DOC
     apply.jacobian = jacobian
     return apply
